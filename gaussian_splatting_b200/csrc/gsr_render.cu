@@ -71,7 +71,7 @@ constexpr int CTA_WARPS = CTA_THREADS / 32;
 #define GSR_BWD_UNROLL 1
 #endif
 #ifndef GSR_BWD_MINB
-// 8 CTAs per SM = 64 registers per thread: the walk fits (one 4-byte spill per batch, outside the inner loop) and
+// 8 CTAs per SM = 64 registers per thread: the walk fits (the masked build uses no local memory at all) and
 // the eighth CTA hides more of the shared-memory / shuffle latencies than a 72-register build gains.  An H100 SM has
 // 64 K registers, 2048 threads and 228 KB of shared memory, so 8 CTAs of 128 threads and ~25 KB are resident
 #define GSR_BWD_MINB 8
@@ -94,14 +94,17 @@ static_assert(GROUPS == 2 || GROUPS == 4, "GROUPS must be 2 or 4");
 // end of their list read (the walks are branch-free and must not re-read a real entry: the forward MARKS entries)
 constexpr int LIST_BYTES = GROUPS * BATCH + 16;
 constexpr int LIST_DUMMY = GROUPS * BATCH;
-// Contribution masks (forward -> backward): for every (tile, batch, warp, lane group) one BATCH-bit mask over the
-// POSITIONS of the group's candidate list (build_lists: ascending record order, identical in both kernels) that
-// contributed to at least one pixel of the group's block.  Slot of batch b of a tile whose
+// Contribution masks (forward -> backward): for every (tile, batch, warp, lane group) one BATCH-bit mask whose bit j
+// is set when staged record j of the batch contributed to at least one pixel of the group's block.  The backward
+// walks exactly the set bits, in ascending record order.  Slot of batch b of a tile whose
 // records start at stream position `start`: start / BATCH + tile + b (unique: a tile has at most total / BATCH + 1
 // batches), i.e. at most P / BATCH + n_tiles + 1 slots of MASK_WORDS_PER_SLOT 32-bit words.
 constexpr int MASK_WORDS = BATCH / 32;
 constexpr int MASK_WORDS_PER_SLOT = CTA_WARPS * GROUPS * MASK_WORDS;
 static_assert(BATCH == 128, "contribution masks are laid out for 128-record batches");
+// per-warp record flags of the forward's marking: GROUPS x BATCH bytes, cleared by 32 lanes x 16 bytes
+constexpr int FLAG_BYTES = 32 * 16;
+static_assert(GROUPS * BATCH <= FLAG_BYTES, "record flags must fit the per-warp flag area");
 
 // pixel blocks: warp w owns the 16x4 band of rows 4w..4w+3, lane group g its g-th GROUP_W x 4 block;
 // lane l of a group handles the pixel pair (2*(l % PAIRS_X) + {0,1}, l / PAIRS_X) of that block
@@ -305,14 +308,21 @@ __device__ __forceinline__ bool blend_hazard(float e, float w) {
     return (d & 0xff7fffffu) == 0u;
 }
 
-// MARK: the walk also records, per lane group, WHICH list positions contributed to at least one pixel of the group
-// (a 32-bit word per 32 list positions, OR-reduced over the group's lanes and stored to gm_warp[group][word]).
-// The marks live in a register — a store inside the loop costs ptxas's register-pair coalescing (+11 instructions
-// per iteration, measured) — so the walk is split into runs of 32 positions; the inner loop stays one basic block.
+__device__ __forceinline__ void sts_u8(uint32_t addr, uint32_t v) {
+    asm volatile("st.shared.u8 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+
+// MARK: the walk also records, per lane group, WHICH staged records contributed to at least one pixel of the group.
+// Inside the loop the marks are list positions in a register — a store inside the loop costs ptxas's register-pair
+// coalescing (+11 instructions per iteration, measured) — so the walk is split into runs of 32 positions and the
+// inner loop stays one basic block.  After each run the positions are OR-reduced over each group and lane l turns
+// position t0 + l of every group into a byte flag per record (flag_addr: this warp's [GROUPS][BATCH] bytes, zero on
+// entry); after the walk one ballot per 32 records turns the flags into the group's 128-bit record mask, stored to
+// gm_warp[group][word], and the flags are cleared again.
 template <bool CHECK, bool MARK>
 __device__ __forceinline__ void fwd_walk(const float4* __restrict__ rec4, uint32_t list_addr, uint32_t dummy_addr,
                                          int my_cnt, int iters, int next_base, F2 fpx, float fpy, FwdState& st,
-                                         uint32_t* __restrict__ gm_warp, int lane) {
+                                         uint32_t* __restrict__ gm_warp, uint32_t flag_addr, int lane) {
     const float neg_sat = -GSR_SAT_THRESH;
     int lj0 = -1, lj1 = -1;  // record (within this batch) of the last contribution
     for (int t0 = 0; t0 < iters; t0 += (MARK ? 32 : BATCH)) {
@@ -366,16 +376,31 @@ __device__ __forceinline__ void fwd_walk(const float4* __restrict__ rec4, uint32
             pbit <<= 1;
         }
     }
-    if (MARK) {  // OR over each lane group (two full-warp reductions: both halves execute the same instructions)
-        uint32_t gsum[GROUPS];
+    if (MARK) {  // OR over each lane group (full-warp reductions: all groups execute the same instructions)
 #pragma unroll
-        for (int g = 0; g < GROUPS; ++g)
-            gsum[g] = __reduce_or_sync(0xffffffffu, (lane / GROUP_LANES == g) ? pmask : 0u);
-        uint32_t mine = gsum[0];
-#pragma unroll
-        for (int g = 1; g < GROUPS; ++g) mine = (lane == g) ? gsum[g] : mine;
-        if (lane < GROUPS) gm_warp[lane * MASK_WORDS + (t0 >> 5)] = mine;
+        for (int g = 0; g < GROUPS; ++g) {
+            const uint32_t gsum = __reduce_or_sync(0xffffffffu, (lane / GROUP_LANES == g) ? pmask : 0u);
+            if ((gsum >> lane) & 1u) {  // list position t0 + lane of group g contributed: flag its record
+                const uint32_t j = lds_u8(list_addr + (g - lane / GROUP_LANES) * BATCH + t0 + lane);
+                sts_u8(flag_addr + g * BATCH + j, 1u);
+            }
+        }
     }
+    }
+    if (MARK) {
+        __syncwarp();
+        uint32_t mine = 0u;
+#pragma unroll
+        for (int g = 0; g < GROUPS; ++g) {
+#pragma unroll
+            for (int w = 0; w < MASK_WORDS; ++w) {
+                const uint32_t m = __ballot_sync(0xffffffffu, lds_u8(flag_addr + g * BATCH + w * 32 + lane) != 0u);
+                mine = (lane == g * MASK_WORDS + w) ? m : mine;
+            }
+        }
+        if (lane < GROUPS * MASK_WORDS) gm_warp[lane] = mine;
+        __syncwarp();
+        asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(flag_addr + lane * 16), "r"(0u) : "memory");
     }
     if (lj0 >= 0) st.last0 = next_base + lj0;
     if (lj1 >= 0) st.last1 = next_base + lj1;
@@ -446,6 +471,7 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     __shared__ __align__(8) uint64_t s_full[STAGES];
     __shared__ int s_cnt[STAGES];
     __shared__ __align__(16) uint8_t s_list[CTA_WARPS][LIST_BYTES];
+    __shared__ __align__(16) uint8_t s_flag[CTA_WARPS][MARK ? FLAG_BYTES : 16];  // MARK: per-record flags (fwd_walk)
 
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
@@ -461,6 +487,8 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     const uint32_t list_addr = smem_u32(list + (lane / GROUP_LANES) * BATCH);
     const uint32_t dummy_addr = smem_u32(list + LIST_DUMMY);
     if (lane == 0) list[LIST_DUMMY] = 0;  // made visible to the warp by the __syncwarp that ends build_lists
+    const uint32_t flag_addr = smem_u32(&s_flag[warp][0]);
+    if (MARK) reinterpret_cast<uint4*>(&s_flag[warp][0])[lane] = make_uint4(0u, 0u, 0u, 0u);  // likewise
     // this warp's mask words of batch 0 (the slot advances by one per batch)
     uint32_t* gm = MARK ? masks + ((size_t)(start / BATCH + tile) * MASK_WORDS_PER_SLOT + warp * GROUPS * MASK_WORDS)
                         : nullptr;
@@ -518,11 +546,11 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
             if (__any_sync(0xffffffffu, small)) {
                 if (lane == 0) STAT(0, iters);
                 fwd_walk<true, MARK>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
-                                     MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, lane);
+                                     MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane);
             } else {
                 if (lane == 0) STAT(1, iters);
                 fwd_walk<false, MARK>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
-                                      MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, lane);
+                                      MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane);
             }
             if (lane == 0) { STAT(5, cnts[0] + cnts[1]); STAT(6, 2 * cnt); }
         }
@@ -685,36 +713,36 @@ __device__ __forceinline__ F2 recip_one_minus2(F2 alpha) {
     return fma2(r0, fma2(nl, r0, e), r0);
 }
 
-// Keep, in every group's list, only the positions the forward marked as contributing (its position masks):
-// lane L handles list positions 4L .. 4L+3, in place (compaction only moves entries towards the front; every
-// lane reads its four entries before anybody writes).  gm: this warp's [GROUPS][MASK_WORDS] words of the batch.
-__device__ __forceinline__ void filter_lists(const uint32_t* __restrict__ gm, int lane, uint8_t* __restrict__ list,
-                                             int (&cnts)[GROUPS]) {
+// Each group's list is the set bits of its record mask from the forward (ascending record order): lane L handles
+// records 4L .. 4L+3 and writes the set ones at their popc-prefix positions.  gm: this warp's [GROUPS][MASK_WORDS]
+// words of the batch.  Bits at or beyond cnt are dropped: the backward's last batch can be shorter than the forward's
+// (it ends at the deepest splat any pixel consumed), and the stage holds no record there.
+__device__ __forceinline__ void mask_lists(const uint32_t* __restrict__ gm, int cnt, int lane,
+                                           uint8_t* __restrict__ list, int (&cnts)[GROUPS]) {
     const int wsel = lane >> 3, shift = (lane & 7) * 4;
-    uint32_t ent[GROUPS], nib[GROUPS];
-    int off[GROUPS];
+    const uint32_t ent = 0x03020100u + 0x04040404u * (uint32_t)lane;  // the four record indices of this lane
+    uint4 lim = make_uint4(~0u, ~0u, ~0u, ~0u);
+    if (cnt < BATCH) {  // warp-uniform; the first batch the backward walks, at most
+        auto low = [cnt](int w) { const int n = cnt - 32 * w; return n >= 32 ? ~0u : n <= 0 ? 0u : (1u << n) - 1u; };
+        lim = make_uint4(low(0), low(1), low(2), low(3));
+    }
 #pragma unroll
     for (int g = 0; g < GROUPS; ++g) {
-        const uint4 m = __ldg(reinterpret_cast<const uint4*>(gm + g * MASK_WORDS));  // same address for all lanes
+        uint4 m = __ldg(reinterpret_cast<const uint4*>(gm + g * MASK_WORDS));  // same address for all lanes
+        m.x &= lim.x; m.y &= lim.y; m.z &= lim.z; m.w &= lim.w;
         const int p0 = __popc(m.x), p1 = __popc(m.y), p2 = __popc(m.z), p3 = __popc(m.w);
         uint32_t wv = m.x;
         wv = (wsel == 1) ? m.y : wv;
         wv = (wsel == 2) ? m.z : wv;
         wv = (wsel == 3) ? m.w : wv;
-        off[g] = ((wsel > 0) ? p0 : 0) + ((wsel > 1) ? p1 : 0) + ((wsel > 2) ? p2 : 0) + __popc(wv & ((1u << shift) - 1u));
-        nib[g] = (wv >> shift) & 0xfu;
-        ent[g] = *reinterpret_cast<const uint32_t*>(list + g * BATCH + lane * 4);
+        int o = ((wsel > 0) ? p0 : 0) + ((wsel > 1) ? p1 : 0) + ((wsel > 2) ? p2 : 0) + __popc(wv & ((1u << shift) - 1u));
+        const uint32_t nib = (wv >> shift) & 0xfu;
         cnts[g] = p0 + p1 + p2 + p3;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int g = 0; g < GROUPS; ++g) {
         uint8_t* dst = list + g * BATCH;
-        int o = off[g];
-        if (nib[g] & 1u) dst[o++] = (uint8_t)(ent[g] & 0xffu);
-        if (nib[g] & 2u) dst[o++] = (uint8_t)((ent[g] >> 8) & 0xffu);
-        if (nib[g] & 4u) dst[o++] = (uint8_t)((ent[g] >> 16) & 0xffu);
-        if (nib[g] & 8u) dst[o] = (uint8_t)(ent[g] >> 24);
+        if (nib & 1u) dst[o++] = (uint8_t)(ent & 0xffu);
+        if (nib & 2u) dst[o++] = (uint8_t)((ent >> 8) & 0xffu);
+        if (nib & 4u) dst[o++] = (uint8_t)((ent >> 16) & 0xffu);
+        if (nib & 8u) dst[o] = (uint8_t)(ent >> 24);
     }
     __syncwarp();
 }
@@ -836,8 +864,10 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
         uint32_t acc_cell = smem_u32(acc) + my_slot * 4;  // this lane's moment cell of record 0
         asm volatile("" : "+r"(acc_cell));                // kept in a register: not re-derived inside the walk
         int cnts[GROUPS];
-        build_lists(rec4, cnt, lane, pm.bx0, pm.by0, list, cnts);  // the same lists the forward walked ...
-        if (MASKS) filter_lists(gm + (size_t)b * MASK_WORDS_PER_SLOT, lane, list, cnts);  // ... minus the idle entries
+        if (MASKS)  // exactly the records that contributed to some pixel of the group
+            mask_lists(gm + (size_t)b * MASK_WORDS_PER_SLOT, cnt, lane, list, cnts);
+        else  // the same candidate lists the forward walked
+            build_lists(rec4, cnt, lane, pm.bx0, pm.by0, list, cnts);
         const int my_cnt = group_select(cnts, lane / GROUP_LANES);
         const int iters = group_max(cnts);
         const int chunk_base1 = (b * BATCH) % CHUNK_REF + 1;  // tile_splat_idx % CHUNK of record 0 of this batch, + 1

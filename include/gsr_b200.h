@@ -131,9 +131,9 @@ int gsr_pack_records(int P, const int32_t* sorted_gaussian_idx, const float* uvs
                      void* stream);
 
 /* Number of 32-bit words of the forward -> backward contribution masks for P (gaussian, tile) pairs on an H x W
- * image: per (tile, 128-record batch, warp, lane group) one 128-bit mask over the POSITIONS of the group's candidate
- * list (the batch's records that pass the footprint test of the group's 4x4 pixel block, in batch order) that
- * contributed to at least one pixel of the block.  Forward and backward must come from the same build. */
+ * image: per (tile, 128-record batch, warp, lane group) one 128-bit mask whose bit j is set when record j of the
+ * batch contributed to at least one pixel of the group's 4x4 pixel block.  Forward and backward must come from the
+ * same build. */
 size_t gsr_contribution_mask_words(int64_t P, int H, int W);
 
 /* records [P,12], tile_ranges [n_tiles+1], background [3] ->
