@@ -30,6 +30,7 @@ CU_SOURCES = [
     "gsr_render_generic.cu",
     "gsr_adam.cu",
     "gsr_densify.cu",
+    "gsr_loss.cu",
 ]
 HEADERS = [
     CSRC / "gsr_common.cuh",

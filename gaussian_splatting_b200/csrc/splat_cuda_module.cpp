@@ -858,6 +858,83 @@ torch::Tensor camera_centre(torch::Tensor camera_T_world) {
     return out;
 }
 
+// ---------------------------------------------------------------------------------------------
+// photometric loss (gsr_photometric_loss_*): [H,W,C] (the renderer's image, B = 1) or [B,C,H,W], any strides
+// ---------------------------------------------------------------------------------------------
+struct LossShape {
+    int B, C, H, W;
+    std::vector<int64_t> strides;  // (B, C, H, W) element strides
+};
+
+LossShape loss_shape(const torch::Tensor& t, const char* name) {
+    TORCH_CHECK(t.is_cuda(), name, " is not a CUDA tensor");
+    TORCH_CHECK(t.dim() == 3 || t.dim() == 4, name, " must be [H,W,C] or [B,C,H,W]");
+    LossShape s;
+    if (t.dim() == 3) {
+        s.B = 1;
+        s.H = t.size(0);
+        s.W = t.size(1);
+        s.C = t.size(2);
+        s.strides = {t.size(0) * t.stride(0), t.stride(2), t.stride(0), t.stride(1)};
+    } else {
+        s.B = t.size(0);
+        s.C = t.size(1);
+        s.H = t.size(2);
+        s.W = t.size(3);
+        s.strides = {t.stride(0), t.stride(1), t.stride(2), t.stride(3)};
+    }
+    return s;
+}
+
+LossShape check_loss_inputs(const torch::Tensor& pred, const torch::Tensor& target, const std::vector<double>& window,
+                            int* dt) {
+    LossShape s = loss_shape(pred, "pred");
+    LossShape ts = loss_shape(target, "target");
+    TORCH_CHECK(pred.sizes() == target.sizes(), "pred and target must have the same shape");
+    TORCH_CHECK(pred.device() == target.device(), "pred and target must be on the same device");
+    TORCH_CHECK(window.size() == 11, "window must have 11 taps");
+    TORCH_CHECK(s.H >= 11 && s.W >= 11, "H and W must be at least 11");
+    *dt = common_dtype(pred, {&target});
+    return s;
+}
+
+// returns out [3] = (loss, L1, SSIM) in pred's dtype
+torch::Tensor photometric_loss_forward(torch::Tensor pred, torch::Tensor target, std::vector<double> window,
+                                       double c1, double c2, double l1_weight, double ssim_weight) {
+    int dt = 0;
+    const LossShape s = check_loss_inputs(pred, target, window, &dt);
+    const LossShape ts = loss_shape(target, "target");
+    c10::cuda::CUDAGuard guard(pred.device());
+    torch::Tensor out = torch::empty({3}, pred.options());
+    const size_t tb = gsr_photometric_loss_temp_bytes(s.B, s.C, s.H, s.W);
+    torch::Tensor temp = torch::empty({(int64_t)tb}, pred.options().dtype(torch::kUInt8));
+    check_rc(gsr_photometric_loss_forward(dt, s.B, s.C, s.H, s.W, pred.data_ptr(), s.strides.data(),
+                                          target.data_ptr(), ts.strides.data(), window.data(), c1, c2, l1_weight,
+                                          ssim_weight, out.data_ptr(), temp.data_ptr(), tb, cur_stream()),
+             "gsr_photometric_loss_forward");
+    return out;
+}
+
+// returns grad_loss * d loss / d pred, allocated with empty_like(pred) (a permuted view keeps its strides)
+torch::Tensor photometric_loss_backward(torch::Tensor pred, torch::Tensor target, std::vector<double> window,
+                                        double c1, double c2, double l1_weight, double ssim_weight,
+                                        torch::Tensor grad_loss) {
+    int dt = 0;
+    const LossShape s = check_loss_inputs(pred, target, window, &dt);
+    const LossShape ts = loss_shape(target, "target");
+    TORCH_CHECK(grad_loss.is_cuda() && grad_loss.device() == pred.device(), "grad_loss must be on pred's device");
+    TORCH_CHECK(grad_loss.numel() == 1 && grad_loss.dtype() == pred.dtype(), "grad_loss must be a scalar of pred's dtype");
+    c10::cuda::CUDAGuard guard(pred.device());
+    torch::Tensor grad = torch::empty_like(pred);
+    const LossShape gs = loss_shape(grad, "grad");
+    check_rc(gsr_photometric_loss_backward(dt, s.B, s.C, s.H, s.W, pred.data_ptr(), s.strides.data(),
+                                           target.data_ptr(), ts.strides.data(), window.data(), c1, c2, l1_weight,
+                                           ssim_weight, grad_loss.data_ptr(), grad.data_ptr(), gs.strides.data(),
+                                           cur_stream()),
+             "gsr_photometric_loss_backward");
+    return grad;
+}
+
 std::string version() { return gsr_version(); }
 
 }  // namespace
@@ -897,5 +974,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("densify_accumulate", &densify_accumulate, "per-step densification statistics");
     m.def("densify_apply", &densify_apply, "clone / split / delete applied to the flat parameter + Adam buffers");
     m.def("camera_centre", &camera_centre, "inverse(camera_T_world)[:3, 3] with torch's bits, one kernel");
+    m.def("photometric_loss_forward", &photometric_loss_forward,
+          "(1 - ssim_frac) * L1 + ssim_frac * (1 - SSIM) forward -> (loss, L1, SSIM)");
+    m.def("photometric_loss_backward", &photometric_loss_backward, "photometric loss backward -> gradient on pred");
     m.def("version", &version, "library version string");
 }

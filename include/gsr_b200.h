@@ -357,6 +357,29 @@ int gsr_densify_apply(int n_in, int n_out, int n_sh_rest, const float* p_in, con
                       const float* xyz_add, const float* q_set, const float* scale_set, float* p_out, float* m_out,
                       float* v_out, void* stream);
 
+/* ---- photometric loss of the training step (splat_py/trainer.py:363-374) ------------------------------------
+ * loss = l1_weight * L1 + ssim_weight * (1 - SSIM), with L1 = mean |pred - target| over all B*C*H*W elements and
+ * SSIM the mean over B*C*(H-10)*(W-10) valid window origins of the 11x11 separable Gaussian-window SSIM map
+ * S = (2 mu_p mu_t + c1)(2 s_pt + c2) / ((mu_p^2 + mu_t^2 + c1)(s_pp + s_tt + c2)) (no clamping).
+ * pred, target, grad_pred: base pointer + element strides (B, C, H, W) in *_strides_host[4], any layout (the
+ * [H,W,C] image of the renderer is B = 1 with strides (H*W*C, 1, W*C, C)); window_host [11]: the window taps;
+ * c1 = (0.01 * data_range)^2, c2 = (0.03 * data_range)^2.  H and W must be >= 11.  Results do not depend on the
+ * strides, bit for bit, and are identical from run to run. */
+size_t gsr_photometric_loss_temp_bytes(int B, int C, int H, int W);
+/* out [3] (device, dtype) <- {loss, L1, SSIM}; temp: gsr_photometric_loss_temp_bytes(B, C, H, W) bytes. */
+int gsr_photometric_loss_forward(int dtype, int B, int C, int H, int W, const void* pred,
+                                 const int64_t* pred_strides_host, const void* target,
+                                 const int64_t* target_strides_host, const double* window_host, double c1, double c2,
+                                 double l1_weight, double ssim_weight, void* out, void* temp, size_t temp_bytes,
+                                 void* stream);
+/* grad_pred <- grad_loss[0] * d loss / d pred (grad_loss: a device scalar of the same dtype); recomputes the
+ * moments, stores no intermediate maps.  No gradient with respect to target. */
+int gsr_photometric_loss_backward(int dtype, int B, int C, int H, int W, const void* pred,
+                                  const int64_t* pred_strides_host, const void* target,
+                                  const int64_t* target_strides_host, const double* window_host, double c1, double c2,
+                                  double l1_weight, double ssim_weight, const void* grad_loss, void* grad_pred,
+                                  const int64_t* grad_strides_host, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,6 +49,10 @@ def main():
                     help="flat: one NCCL all-reduce(avg) of the flat gradient bucket + gsr_adam_step on the replicated "
                          "flat buffer; sharded: ONE kernel per rank doing reduce-scatter + Adam + all-gather over NVLink "
                          "peer memory (gsr_adam_step_sharded), Adam state sharded over the ranks (needs >= 2 ranks)")
+    ap.add_argument("--loss", choices=["shim", "fused"], default="shim",
+                    help="shim: L1 + the SSIM stand-in through permuted NCHW views, like run_trainer.py's reference arm; "
+                         "fused: gaussian_splatting_b200.loss.photometric_loss in the step and its ssim() in evaluate() "
+                         "(one forward and one backward kernel)")
     a = ap.parse_args()
 
     real_stdout = os.fdopen(os.dup(1), "w")
@@ -67,6 +71,7 @@ def main():
     import gaussian_splatting_b200 as gsb
     from gaussian_splatting_b200.densify import AdaptiveDensityControl, DensificationStats
     from gaussian_splatting_b200.flat_adam import REFERENCE_LR_MULTIPLIERS as mult, FlatAdam
+    from gaussian_splatting_b200.loss import photometric_loss, ssim as fused_ssim
     from gaussian_splatting_b200.rasterize import rasterize
     from gaussian_splatting_b200.structs import Camera
     from gaussian_splatting_b200.view_parallel import GradientBucket, all_reduce_statistics
@@ -163,8 +168,11 @@ def main():
                                        torch.zeros(3, device=dev))
                 l2 = torch.nn.functional.mse_loss(pred.clip(0, 1), im.image)
                 psnrs.append(-10 * torch.log10(l2).item())
-                ssims.append(ssim(pred.unsqueeze(0).permute(0, 3, 1, 2).clip(0, 1),
-                                  im.image.unsqueeze(0).permute(0, 3, 1, 2)).item())
+                if a.loss == "fused":
+                    ssims.append(fused_ssim(pred.clip(0, 1), im.image).item())
+                else:
+                    ssims.append(ssim(pred.unsqueeze(0).permute(0, 3, 1, 2).clip(0, 1),
+                                      im.image.unsqueeze(0).permute(0, 3, 1, 2)).item())
         return float(np.mean(psnrs)), float(np.mean(ssims))
 
     fields = ("xyz", "quaternion", "scale", "opacity", "rgb", "sh")
@@ -200,9 +208,12 @@ def main():
         uv.retain_grad()
         if timed:
             ev[1].record()
-        l1 = torch.nn.functional.l1_loss(image, im.image)
-        ssim_loss = 1.0 - ssim(image.unsqueeze(0).permute(0, 3, 1, 2), im.image.unsqueeze(0).permute(0, 3, 1, 2))
-        loss = (1.0 - config.ssim_frac) * l1 + config.ssim_frac * ssim_loss
+        if a.loss == "fused":
+            loss = photometric_loss(image, im.image, config.ssim_frac)
+        else:
+            l1 = torch.nn.functional.l1_loss(image, im.image)
+            ssim_loss = 1.0 - ssim(image.unsqueeze(0).permute(0, 3, 1, 2), im.image.unsqueeze(0).permute(0, 3, 1, 2))
+            loss = (1.0 - config.ssim_frac) * l1 + config.ssim_frac * ssim_loss
         loss.backward()
         if timed:
             ev[2].record()
@@ -262,6 +273,8 @@ def main():
                           "memory in one kernel, Adam state sharded)") if sharded else
                          ("FlatAdam (gsr_adam_step) after one NCCL all-reduce(avg) of the flat gradient bucket"
                           if world > 1 else "FlatAdam (gsr_adam_step)"),
+            "loss": ("fused: photometric_loss (gsr_photometric_loss_forward / _backward), ssim() in evaluation"
+                     if a.loss == "fused" else "shim: l1_loss + SSIM stand-in (tools/e2e/shims) through NCHW views"),
             "device": torch.cuda.get_device_name(local),
         }
         real_stdout.write("E2E " + json.dumps(line) + "\n")
