@@ -21,6 +21,12 @@ def np_scene(n, res, sh_degree=3, seed=0, view=0, n_views=3, dtype=np.float32, s
                 sh=a(g.sh), T=a(T), K=a(cam.K), H=cam.height, W=cam.width)
 
 
+def sh12_scene(sh_degree):
+    """20 000 gaussians at SH degree 1 or 2, 320x192: the scenes of tests/golden/sh12_reference.npz."""
+    return np_scene(20_000, "small", sh_degree=sh_degree, seed=20 + sh_degree, view=1, n_views=3,
+                    sigma_px=(2.5, 0.5, 0.5, 10.0))
+
+
 def reference_fixture(dtype=np.float32):
     """The reference's own unit-test scene: 6 gaussians, 640x480 camera, tilted pose."""
     xyz = np.array([[1, 2, -4], [4, 5, 6], [7, 8, -9], [1, 2, 15], [2.5, -1, 4], [-1, -2, 10]], dtype)

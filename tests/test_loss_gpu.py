@@ -61,7 +61,9 @@ def _rel(x, ref):
     return float((x.double() - ref.double()).abs().max() / ref.double().abs().max().clamp_min(1e-300))
 
 
-@pytest.mark.parametrize("shape", [(11, 11, 3), (37, 53, 3), (96, 128, 3), (1080, 1920, 3), (2, 3, 40, 50)])
+# C = 1, 4 and 40: the kernels stage channels three at a time, so these exercise partial and many channel groups
+@pytest.mark.parametrize("shape", [(11, 11, 3), (37, 53, 3), (96, 128, 3), (1080, 1920, 3), (2, 3, 40, 50), (20, 30, 1),
+                                   (37, 53, 4), (2, 5, 40, 50)])
 @pytest.mark.parametrize("frac", FRACS)
 def test_fp32_kernels_against_fp64_oracle(shape, frac):
     a, b = _pair(shape, 1)
@@ -95,10 +97,10 @@ def _permuted_nchw(shape, seed):
     return base.permute(0, 3, 1, 2)
 
 
-@pytest.mark.parametrize("case", ["hwc", "permuted"])
+@pytest.mark.parametrize("case", ["hwc", "hwc4", "permuted"])
 def test_gradcheck_fp64(case):
-    if case == "hwc":
-        a, b = _pair((13, 17, 3), 3, torch.float64)
+    if case in ("hwc", "hwc4"):
+        a, b = _pair((13, 17, 3 if case == "hwc" else 4), 3, torch.float64)
     else:
         a = _permuted_nchw((2, 3, 12, 15), 4)
         b = (a + 0.2 * torch.randn(a.shape, device=dev(), dtype=torch.float64)).clamp(0, 1)

@@ -18,7 +18,7 @@ def _loss(sc, G, **over):
     return float((o.image * G).sum()), o
 
 
-@pytest.mark.parametrize("sh_degree", [0, 3])
+@pytest.mark.parametrize("sh_degree", [0, 1, 2, 3])
 def test_fp64_backward_matches_finite_differences(sh_degree):
     sc = np_scene(128, "tiny", sh_degree=sh_degree, dtype=np.float64, sigma_px=(3.0, 0.4, 1.0, 6.0))
     rng = np.random.default_rng(1)

@@ -331,6 +331,28 @@ def test_live_reference_per_pixel_sh_backward_fp32():
         assert_grad_close(mine[k], gd, f"perpixel_{k}")
 
 
+@pytest.mark.parametrize("mode,path", [("precompute", "fused"), ("precompute", "unfused"), ("perpixel", "unfused")])
+@pytest.mark.parametrize("deg", [1, 2])
+def test_sh_degrees_1_and_2_against_the_reference(deg, mode, path):
+    """SH degrees 1 and 2 (the densifier's add_sh_band passes through both) against the compiled reference
+    (tools/make_golden.py --sh12): forward bit for bit (the per-pixel image, which has no bit contract, to 1e-5),
+    gradients within max(1e-4, 10 x the reference's own run-to-run noise)."""
+    gd = load_golden("sh12_reference.npz")
+    sc = scenes.sh12_scene(deg)
+    assert sc["sh"].shape[2] == (deg + 1) ** 2 - 1
+    mine = run_b200(sc, fn=rasterize if path == "fused" else rasterize_unfused,
+                    G=synth.make_upstream_grad("small").numpy(), sh_precompute=(mode == "precompute"))
+    p = f"sh{deg}_{mode}"
+    assert_digest(mine["culling_mask"], gd, f"{p}_mask", "culling_mask")
+    assert_digest(mine["uv"], gd, f"{p}_uv", "uv")
+    if mode == "precompute":
+        assert_digest(mine["image"], gd, f"{p}_image", "image")
+    else:
+        assert_grad_close(mine["image"].reshape(-1, 3), gd, f"{p}_image_px", 1e-5)
+    for k in GRAD_KEYS:
+        assert_grad_close(mine[k], gd, f"{p}_{k}", max(REL_TOL, 10.0 * float(gd[f"{p}_{k}_noise"])))
+
+
 def test_contribution_masks_do_not_change_the_gradients():
     """The forward records which (8x4 pixel block, splat) pairs contributed and the backward visits only those;
     without the masks (GSR_NO_MASKS=1) the backward walks the forward's conservative candidate lists.  Same

@@ -3,6 +3,7 @@ its splat_py package) on the GPU:
 
     python tools/make_golden.py --out <dir>          # the operator / small-scene fixtures
     python tools/make_golden.py --live --out <dir>   # live_reference.npz: the larger scenes, as digests + samples
+    python tools/make_golden.py --sh12 --out <dir>   # sh12_reference.npz: SH degrees 1 and 2, both SH modes
 
 then copy the files into tests/golden/.  Scenes are regenerated from seeds by the tests
 (gaussian_splatting_b200.synth / tests/scenes.py); the fixtures hold only the reference's OUTPUTS.  Nothing here
@@ -177,6 +178,32 @@ def live(out, dev):
     print({k: v for k, v in rec.items() if k.endswith("_noise")})
 
 
+def sh12(out, dev):
+    """The reference at SH degrees 1 and 2 (tests/scenes.py sh12_scene), with the SH colour precomputed per gaussian
+    and per pixel: forward outputs as digests (the per-pixel image as a sample, it has no bit contract), gradients as
+    samples + column sums, and the reference's own run-to-run noise of each gradient."""
+    ref_loader.load_reference()
+    rec = {}
+    G = synth.make_upstream_grad("small").numpy()
+    for deg in (1, 2):
+        sc = scenes.sh12_scene(deg)
+        for mode in ("precompute", "perpixel"):
+            a, b = (run_rasterize(None, sc, dev, mode == "precompute", 0.5, G) for _ in range(2))
+            p = f"sh{deg}_{mode}"
+            rec.update({f"{p}_mask": scenes.digest(a["culling_mask"]), f"{p}_uv": scenes.digest(a["uv"])})
+            if mode == "precompute":
+                rec[f"{p}_image"] = scenes.digest(a["image"])
+            else:
+                rec.update(grad_summary(f"{p}_image_px", torch.from_numpy(a["image"].reshape(-1, 3))))
+            for k in [k for k in a if k.startswith("g_")]:
+                rec.update(grad_summary(f"{p}_{k}", torch.from_numpy(a[k])))
+                x, y = a[k].astype(np.float64), b[k].astype(np.float64)
+                rec[f"{p}_{k}_noise"] = np.abs(y - x).max() / max(np.abs(x).max(), 1e-30)
+    rec["gpu"] = torch.cuda.get_device_name(0)
+    np.savez_compressed(out / "sh12_reference.npz", **{k: np.asarray(v) for k, v in rec.items()})
+    print({k: float(v) for k, v in rec.items() if k.endswith("_noise")})
+
+
 def adc_reference(dev):
     """The reference trainer's adaptive_density_control (splat_py/trainer.py + optimizer_manager.py on
     torch.optim.Adam), two consecutive passes on the 100k-gaussian case of tests/test_densify_gpu.py: digests of
@@ -245,12 +272,15 @@ def main():
     ap.add_argument("--out", default="golden_out")
     ap.add_argument("--live", action="store_true")
     ap.add_argument("--fixture6-only", action="store_true")
+    ap.add_argument("--sh12", action="store_true")
     args = ap.parse_args()
     out = Path(args.out)
     out.mkdir(parents=True, exist_ok=True)
     dev = torch.device("cuda")
     if args.live:
         return live(out, dev)
+    if args.sh12:
+        return sh12(out, dev)
     if args.fixture6_only:
         return fixture6(out, dev)
     ref_ext, _ = ref_loader.load_reference()
