@@ -283,9 +283,10 @@ __global__ void __launch_bounds__(PRE_THREADS, 7)
 #ifndef GSR_PRE_BWD_MINB
 #define GSR_PRE_BWD_MINB 6
 #endif
-template <int N_SH, bool HAS_SH>
-__global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB)
-    k_preprocess_bwd(int N, const float* __restrict__ xyz, const float* __restrict__ quat,
+// DEPTH: the interleaved rows carry the render backward's camera-frame z gradient in slot 9 (conic2 z pad2); it joins
+// the z component of the camera-frame position gradient before grad_xyz = W^T grad_xyz_cam
+template <int N_SH, bool HAS_SH, bool DEPTH>
+__device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ xyz, const float* __restrict__ quat,
                      const float* __restrict__ scale, const float* __restrict__ opa_logit,
                      const float* __restrict__ Tdev, const float* __restrict__ Kdev,
                      const float* __restrict__ camdev, const uint8_t* __restrict__ visible,
@@ -319,7 +320,7 @@ __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB)
     // every thread fetches its gaussian's inputs before the view constants are fetched (cooperatively): the
     // memory latencies overlap instead of queueing up behind one thread's 28 loads
     float x = 0.f, y = 0.f, z = 0.f, qw = 1.f, qx = 0.f, qy = 0.f, qz = 0.f, s0 = 0.f, s1 = 0.f, s2 = 0.f, opl = 0.f,
-          gcv[3] = {0.f, 0.f, 0.f}, guv[2] = {0.f, 0.f}, gov = 0.f, grv[3] = {0.f, 0.f, 0.f};
+          gcv[3] = {0.f, 0.f, 0.f}, guv[2] = {0.f, 0.f}, gov = 0.f, grv[3] = {0.f, 0.f, 0.f}, gzc = 0.f;
     if (vis) {
         x = xyz[i * 3 + 0]; y = xyz[i * 3 + 1]; z = xyz[i * 3 + 2];
         qw = quat[i * 4 + 0]; qx = quat[i * 4 + 1]; qy = quat[i * 4 + 2]; qz = quat[i * 4 + 3];
@@ -330,7 +331,14 @@ __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB)
             const float4 r0 = row[0], r1 = row[1];
             grv[0] = r0.x; grv[1] = r0.y; grv[2] = r0.z; gov = r0.w;
             if (rows_uv) { guv[0] = r1.x; guv[1] = r1.y; }
-            gcv[0] = r1.z; gcv[1] = r1.w; gcv[2] = g_rows[(size_t)i * GSR_GRAD_ROW_FLOATS + 8];
+            gcv[0] = r1.z; gcv[1] = r1.w;
+            if (DEPTH) {
+                const float2 r2 = *reinterpret_cast<const float2*>(g_rows + (size_t)i * GSR_GRAD_ROW_FLOATS + 8);
+                gcv[2] = r2.x;
+                gzc = r2.y;
+            } else {
+                gcv[2] = g_rows[(size_t)i * GSR_GRAD_ROW_FLOATS + 8];
+            }
         } else {
         gcv[0] = g_conic[i * 3 + 0]; gcv[1] = g_conic[i * 3 + 1]; gcv[2] = g_conic[i * 3 + 2];
         // gradient on the projected mean = the render backward's sum (g_uv, by gaussian; may be absent) + whatever
@@ -366,7 +374,8 @@ __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB)
         float gp_j[3], gp_uv[3] = {0.f, 0.f, 0.f};
         proj_jacobian_bwd<float>(px, py, pz, vc.K[0], vc.K[4], gJ, gp_j);
         project_uv_bwd<float>(px, py, pz, vc.K[0], vc.K[4], guv[0], guv[1], gp_uv);
-        const float gp[3] = {gp_j[0] + gp_uv[0], gp_j[1] + gp_uv[1], gp_j[2] + gp_uv[2]};
+        float gp[3] = {gp_j[0] + gp_uv[0], gp_j[1] + gp_uv[1], gp_j[2] + gp_uv[2]};
+        if (DEPTH) gp[2] += gzc;
         // xyz_cam = W xyz + t  =>  grad_xyz = W^T grad_xyz_cam
 #pragma unroll
         for (int k = 0; k < 3; ++k) gx[k] = W[0 + k] * gp[0] + W[3 + k] * gp[1] + W[6 + k] * gp[2];
@@ -420,6 +429,29 @@ __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB)
         if (HAS_SH) coop_copy(o_sh + (size_t)i0 * NR3, s_sh, cnt * NR3);
     }
 }
+
+#define GSR_PRE_BWD_PARAMS                                                                                          \
+    int N, const float* __restrict__ xyz, const float* __restrict__ quat, const float* __restrict__ scale,          \
+        const float* __restrict__ opa_logit, const float* __restrict__ Tdev, const float* __restrict__ Kdev,        \
+        const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rgb,     \
+        const float* __restrict__ g_opa, const float* __restrict__ g_uv, const float* __restrict__ g_conic,         \
+        const float* __restrict__ g_rows, int rows_uv, const float* __restrict__ g_uv_compact,                      \
+        const uint64_t* __restrict__ scan, float* __restrict__ o_xyz, float* __restrict__ o_quat,                   \
+        float* __restrict__ o_scale, float* __restrict__ o_opa, float* __restrict__ o_dc, float* __restrict__ o_sh, \
+        int use_tma
+#define GSR_PRE_BWD_FORWARD                                                                                      \
+    N, xyz, quat, scale, opa_logit, Tdev, Kdev, camdev, visible, g_rgb, g_opa, g_uv, g_conic, g_rows, rows_uv, \
+        g_uv_compact, scan, o_xyz, o_quat, o_scale, o_opa, o_dc, o_sh, use_tma
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB) k_preprocess_bwd(GSR_PRE_BWD_PARAMS) {
+    preprocess_bwd<N_SH, HAS_SH, false>(GSR_PRE_BWD_FORWARD);
+}
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB) k_preprocess_bwd_depth(GSR_PRE_BWD_PARAMS) {
+    preprocess_bwd<N_SH, HAS_SH, true>(GSR_PRE_BWD_FORWARD);
+}
+#undef GSR_PRE_BWD_PARAMS
+#undef GSR_PRE_BWD_FORWARD
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
@@ -480,7 +512,7 @@ int gsr_preprocess_forward(int N, int n_sh_rest, const float* xyz, const float* 
     return (int)cudaGetLastError();
 }
 
-int gsr_preprocess_backward(int N, int n_sh_rest, const float* xyz, const float* quaternion,
+static int preprocess_backward(bool depth, int N, int n_sh_rest, const float* xyz, const float* quaternion,
                             const float* scale, const float* opacity_logit, const float* camera_T_world,
                             const float* K, const float* camera_centre, const uint8_t* visible,
                             const float* grad_rgb,
@@ -501,15 +533,51 @@ int gsr_preprocess_backward(int N, int n_sh_rest, const float* xyz, const float*
     N, xyz, quaternion, scale, opacity_logit, camera_T_world, K, camera_centre, visible, grad_rgb,         \
         grad_opacity, grad_uv,                                                                             \
         grad_conic, grad_rows, use_rows_uv, grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, use_tma
-    switch (n_sh_rest) {
-        case 0: k_preprocess_bwd<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        case 3: k_preprocess_bwd<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        case 8: k_preprocess_bwd<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        case 15: k_preprocess_bwd<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        default: return GSR_ERR_UNSUPPORTED;
+    if (depth) {
+        switch (n_sh_rest) {
+            case 0: k_preprocess_bwd_depth<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 3: k_preprocess_bwd_depth<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 8: k_preprocess_bwd_depth<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 15: k_preprocess_bwd_depth<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            default: return GSR_ERR_UNSUPPORTED;
+        }
+    } else {
+        switch (n_sh_rest) {
+            case 0: k_preprocess_bwd<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 3: k_preprocess_bwd<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 8: k_preprocess_bwd<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 15: k_preprocess_bwd<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            default: return GSR_ERR_UNSUPPORTED;
+        }
     }
 #undef GSR_PRE_ARGS
     return (int)cudaGetLastError();
+}
+
+int gsr_preprocess_backward(int N, int n_sh_rest, const float* xyz, const float* quaternion, const float* scale,
+                            const float* opacity_logit, const float* camera_T_world, const float* K,
+                            const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
+                            const float* grad_opacity, const float* grad_uv, const float* grad_conic,
+                            const float* grad_rows, int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
+                            float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                            float* g_sh_rest, void* stream) {
+    return preprocess_backward(false, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
+                               camera_centre, visible, grad_rgb, grad_opacity, grad_uv, grad_conic, grad_rows,
+                               use_rows_uv, grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit,
+                               g_rgb_dc, g_sh_rest, stream);
+}
+
+int gsr_preprocess_backward_depth(int N, int n_sh_rest, const float* xyz, const float* quaternion, const float* scale,
+                                  const float* opacity_logit, const float* camera_T_world, const float* K,
+                                  const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                                  int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
+                                  float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                                  float* g_sh_rest, void* stream) {
+    if (N > 0 && (grad_rows == nullptr || (reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0)) return GSR_ERR_BAD_ARG;
+    return preprocess_backward(true, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
+                               camera_centre, visible, nullptr, nullptr, nullptr, nullptr, grad_rows, use_rows_uv,
+                               grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc,
+                               g_sh_rest, stream);
 }
 
 }  // extern "C"

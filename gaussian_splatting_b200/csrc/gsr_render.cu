@@ -168,14 +168,56 @@ __device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gmem_s
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// whole warp: fetch records [p0, p0 + cnt) of the sorted pair list into a stage
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {  // release: this thread's earlier shared stores
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
+// Depth/alpha mode: camera-frame z of every pair, decoded from the depth field of its sort key (the record stays
+// 48 bytes).  Keys carry bits(z) - depth_base, or depth_key()'s order-preserving transform of bits(z) when
+// depth_base == 0; with the id in the key the field sits above the id bits.  In the key/value fallback (sorted id
+// array, no keys) the per-gaussian depth keys are read instead.
+struct DepthSource {
+    const uint32_t* zkey;  // per-gaussian depth keys [N] (read only when the tile kernels get a sorted id array)
+    uint32_t depth_base;
+    uint32_t depth_mask;   // (1 << depth_bits) - 1
+    int id_bits;
+};
+__device__ __forceinline__ float decode_depth_key(uint32_t dk, uint32_t base) {
+    const uint32_t b = base != 0u ? dk + base : ((dk & 0x80000000u) ? (dk & 0x7fffffffu) : ~dk);
+    return __uint_as_float(b);
+}
+__device__ __forceinline__ uint32_t source_id_z(const RecSource& src, const DepthSource& ds, int p, float& z) {
+    uint32_t id, dk;
+    if (src.keys != nullptr) {
+        const uint64_t key = __ldg(src.keys + p);
+        id = (uint32_t)(key & src.id_mask);
+        dk = (uint32_t)(key >> ds.id_bits) & ds.depth_mask;
+    } else {
+        id = (uint32_t)__ldg(src.ids + p);
+        dk = __ldg(ds.zkey + id);
+    }
+    z = decode_depth_key(dk, ds.depth_base);
+    return id;
+}
+
+// whole warp: fetch records [p0, p0 + cnt) of the sorted pair list into a stage.  DEPTH: also the z of each
+// record into zstage; those are plain shared stores, released to the waiting warps by a second (ordinary) arrival
+// of every lane on the stage's barrier (the barrier then counts 64 arrivals)
+template <bool DEPTH = false>
 __device__ __forceinline__ void gather_batch(const RecSource& src, int p0, int cnt, float* __restrict__ stage,
-                                             uint64_t* bar, int lane) {
+                                             uint64_t* bar, int lane, const DepthSource* ds = nullptr,
+                                             float* __restrict__ zstage = nullptr) {
     uint32_t id[BATCH / 32];
+    float z[BATCH / 32];
 #pragma unroll
     for (int k = 0; k < BATCH / 32; ++k) {
         const int r = k * 32 + lane;
-        id[k] = (r < cnt) ? source_id(src, p0 + r) : 0u;
+        if (DEPTH) {
+            z[k] = 0.0f;
+            id[k] = (r < cnt) ? source_id_z(src, *ds, p0 + r, z[k]) : 0u;
+        } else {
+            id[k] = (r < cnt) ? source_id(src, p0 + r) : 0u;
+        }
     }
 #pragma unroll
     for (int k = 0; k < BATCH / 32; ++k) {
@@ -186,14 +228,19 @@ __device__ __forceinline__ void gather_batch(const RecSource& src, int p0, int c
             cp_async16(d, g);
             cp_async16(d + 16u, g + 4);
             cp_async16(d + 32u, g + 8);
+            if (DEPTH) zstage[r] = z[k];
         }
     }
     cp_async_mbar_arrive_noinc(bar);  // fires when this lane's copies have landed (at once if it issued none)
+    if (DEPTH) mbar_arrive(bar);
 }
 
 constexpr int GRAD_ROW = GSR_GRAD_ROW_FLOATS;  // floats per interleaved per-gaussian gradient row
 __device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {  // 16-byte aligned
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+__device__ __forceinline__ void red_add_v2(float* p, float a, float b) {  // 8-byte aligned
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
 // Warp-granular stage recycling.  Every warp consumes every batch at its own pace: it waits on the stage's
@@ -291,6 +338,7 @@ struct FwdState {
     F2 nA;        // -alpha_accum (a pixel outside the image starts saturated and never contributes)
     F2 wl;        // alpha_weight of the last contributing splat
     F2 C0, C1, C2;
+    F2 D;               // depth/alpha mode: sum of w * z (unused otherwise)
     int last0, last1;   // tile index + 1 of the last contributing splat (0: none)
     uint32_t badbits;   // sticky: top two bits set <=> some numerator left the exact-division range
     bool bad;           // sticky: some blend weight needs the double-precision expression
@@ -319,10 +367,12 @@ __device__ __forceinline__ void sts_u8(uint32_t addr, uint32_t v) {
 // position t0 + l of every group into a byte flag per record (flag_addr: this warp's [GROUPS][BATCH] bytes, zero on
 // entry); after the walk one ballot per 32 records turns the flags into the group's 128-bit record mask, stored to
 // gm_warp[group][word], and the flags are cleared again.
-template <bool CHECK, bool MARK>
+// DEPTH: also D += w * z, z from the stage's z array zs (same weight w as the colour blend).
+template <bool CHECK, bool MARK, bool DEPTH = false>
 __device__ __forceinline__ void fwd_walk(const float4* __restrict__ rec4, uint32_t list_addr, uint32_t dummy_addr,
                                          int my_cnt, int iters, int next_base, F2 fpx, float fpy, FwdState& st,
-                                         uint32_t* __restrict__ gm_warp, uint32_t flag_addr, int lane) {
+                                         uint32_t* __restrict__ gm_warp, uint32_t flag_addr, int lane,
+                                         const float* __restrict__ zs = nullptr) {
     const float neg_sat = -GSR_SAT_THRESH;
     int lj0 = -1, lj1 = -1;  // record (within this batch) of the last contribution
     for (int t0 = 0; t0 < iters; t0 += (MARK ? 32 : BATCH)) {
@@ -369,6 +419,7 @@ __device__ __forceinline__ void fwd_walk(const float4* __restrict__ rec4, uint32
         st.C0 = fma2(w, bc(q2.y), st.C0);
         st.C1 = fma2(w, bc(q2.z), st.C1);
         st.C2 = fma2(w, bc(q2.w), st.C2);
+        if (DEPTH) st.D = fma2(w, bc(zs[j]), st.D);
         lj0 = c0 ? j : lj0;
         lj1 = c1 ? j : lj1;
         if (MARK) {
@@ -414,18 +465,25 @@ struct ExactPixel {
     float A, wl, c0, c1, c2;
     int n;
 };
-template <bool GATHER>
-__device__ __noinline__ ExactPixel render_pixel_exact_warp(const RecSource src, int start, int total, float fpx,
-                                                           float fpy, int lane) {
+struct ExactPixelDepth {
+    ExactPixel p;
+    float d;  // sum of w * z, in the same order
+};
+template <bool GATHER, bool DEPTH>
+__device__ __forceinline__ ExactPixel exact_pixel(const RecSource& src, const DepthSource& ds, int start, int total,
+                                                  float fpx, float fpy, int lane, float& d) {
     ExactPixel o;
     o.A = o.wl = o.c0 = o.c1 = o.c2 = 0.0f;
     o.n = total;
+    d = 0.0f;
     bool stop = false;
     for (int base = 0; base < total && !stop; base += 32) {
         const int i = base + lane;
-        float alpha = 0.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f;
+        float alpha = 0.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f, zi = 0.0f;
         if (i < total) {
-            const size_t row = GATHER ? (size_t)source_id(src, start + i) : (size_t)(start + i);
+            const size_t row = DEPTH    ? (size_t)source_id_z(src, ds, start + i, zi)
+                               : GATHER ? (size_t)source_id(src, start + i)
+                                        : (size_t)(start + i);
             const float4* q = reinterpret_cast<const float4*>(src.base + row * REC);
             const float4 q0 = __ldg(q), q1 = __ldg(q + 1), q2 = __ldg(q + 2);
             const float du = __fsub_rn(fpx, q0.x), dv = __fsub_rn(fpy, q0.y);
@@ -455,23 +513,42 @@ __device__ __noinline__ ExactPixel render_pixel_exact_warp(const RecSource src, 
             o.c0 = __fmaf_rn(w, __shfl_sync(0xffffffffu, cr, k), o.c0);
             o.c1 = __fmaf_rn(w, __shfl_sync(0xffffffffu, cg, k), o.c1);
             o.c2 = __fmaf_rn(w, __shfl_sync(0xffffffffu, cb, k), o.c2);
+            if (DEPTH) d = __fmaf_rn(w, __shfl_sync(0xffffffffu, zi, k), d);
         }
     }
+    return o;
+}
+template <bool GATHER>
+__device__ __noinline__ ExactPixel render_pixel_exact_warp(const RecSource src, int start, int total, float fpx,
+                                                           float fpy, int lane) {
+    float d;
+    return exact_pixel<GATHER, false>(src, DepthSource{}, start, total, fpx, fpy, lane, d);
+}
+__device__ __noinline__ ExactPixelDepth render_pixel_exact_warp_depth(const RecSource src, const DepthSource ds,
+                                                                      int start, int total, float fpx, float fpy,
+                                                                      int lane) {
+    ExactPixelDepth o;
+    o.p = exact_pixel<true, true>(src, ds, start, total, fpx, fpy, lane, o.d);
     return o;
 }
 
 // MARK: also record, per (batch, warp, lane group), which staged records contributed (contribution masks for
 // the backward; `masks` must be zero-filled by the caller: a warp that skips a batch leaves its masks untouched)
-template <bool MARK, bool GATHER>
-__global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
-    k_render_fwd(const RecSource rs, const int32_t* __restrict__ ranges,
-                 const float* __restrict__ background, int W, int H, int32_t* __restrict__ n_out,
-                 float* __restrict__ w_out, float* __restrict__ image, uint32_t* __restrict__ masks) {
+// DEPTH (gather mode only): also the per-pixel depth D = sum w * z and alpha A (depth / alpha [H,W])
+template <bool MARK, bool GATHER, bool DEPTH>
+__device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* __restrict__ ranges,
+                                           const float* __restrict__ background, int W, int H,
+                                           int32_t* __restrict__ n_out, float* __restrict__ w_out,
+                                           float* __restrict__ image, uint32_t* __restrict__ masks,
+                                           const DepthSource& ds, float* __restrict__ depth,
+                                           float* __restrict__ alpha) {
+    static_assert(GATHER || !DEPTH, "depth/alpha maps are rendered by the gather kernels only");
     __shared__ __align__(128) float s_rec[STAGES][BATCH * REC];
     __shared__ __align__(8) uint64_t s_full[STAGES];
     __shared__ int s_cnt[STAGES];
     __shared__ __align__(16) uint8_t s_list[CTA_WARPS][LIST_BYTES];
     __shared__ __align__(16) uint8_t s_flag[CTA_WARPS][MARK ? FLAG_BYTES : 16];  // MARK: per-record flags (fwd_walk)
+    __shared__ __align__(16) float s_z[STAGES][DEPTH ? BATCH : 1];              // DEPTH: z of the staged records
 
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
@@ -497,7 +574,8 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     if (tid == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&s_full[s], GATHER ? 32 : 1);  // gather: one arrival per lane of the refilling warp
+            // gather: one arrival per lane of the refilling warp (two with DEPTH, see gather_batch)
+            mbar_init(&s_full[s], GATHER ? (DEPTH ? 64 : 32) : 1);
             s_cnt[s] = 0;
         }
         fence_mbar_init();
@@ -509,7 +587,7 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
         const int s = b % STAGES;
         const int cnt = min(BATCH, total - b * BATCH);
         if (GATHER) {
-            gather_batch(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane);
+            gather_batch<DEPTH>(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane, &ds, &s_z[s][0]);
         } else {
             const uint32_t bytes = (uint32_t)cnt * REC * 4u;
             mbar_arrive_expect_tx(&s_full[s], bytes);
@@ -525,6 +603,7 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     st.nA = pk(valid0 ? -0.0f : -1.0f, valid1 ? -0.0f : -1.0f);
     st.wl = bc(0.0f);
     st.C0 = st.C1 = st.C2 = bc(0.0f);
+    st.D = bc(0.0f);
     st.last0 = st.last1 = 0;
     st.badbits = 0u;
     st.bad = false;
@@ -545,12 +624,14 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
             const bool small = (live0 && lo(st.nA) > -0.015625f) || (live1 && hi(st.nA) > -0.015625f);
             if (__any_sync(0xffffffffu, small)) {
                 if (lane == 0) STAT(0, iters);
-                fwd_walk<true, MARK>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
-                                     MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane);
+                fwd_walk<true, MARK, DEPTH>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
+                                            MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane,
+                                            &s_z[s][0]);
             } else {
                 if (lane == 0) STAT(1, iters);
-                fwd_walk<false, MARK>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
-                                      MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane);
+                fwd_walk<false, MARK, DEPTH>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
+                                             MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane,
+                                             &s_z[s][0]);
             }
             if (lane == 0) { STAT(5, cnts[0] + cnts[1]); STAT(6, 2 * cnt); }
         }
@@ -567,6 +648,7 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     // pixels flagged by the walk: recompute them exactly, one at a time, with the whole warp
     float A0 = -lo(st.nA), A1 = -hi(st.nA), wl0 = lo(st.wl), wl1 = hi(st.wl);
     float r0 = lo(st.C0), g0 = lo(st.C1), b0 = lo(st.C2), r1 = hi(st.C0), g1 = hi(st.C1), b1 = hi(st.C2);
+    float D0 = lo(st.D), D1 = hi(st.D);
     // num_splats: the splat after the one that saturated the pixel, else every splat of the tile
     int n0 = (A0 > GSR_SAT_THRESH && st.last0 < total) ? st.last0 : total;
     int n1 = (A1 > GSR_SAT_THRESH && st.last1 < total) ? st.last1 : total;
@@ -581,6 +663,16 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
         todo &= todo - 1;
         const int sx = __shfl_sync(0xffffffffu, px, src), sy = __shfl_sync(0xffffffffu, py, src);
         const bool two = __shfl_sync(0xffffffffu, valid1 ? 1 : 0, src) != 0;
+        if (DEPTH) {
+            const ExactPixelDepth e0 = render_pixel_exact_warp_depth(rs, ds, start, total, (float)sx, (float)sy, lane);
+            if (lane == src) { A0 = e0.p.A; wl0 = e0.p.wl; n0 = e0.p.n; r0 = e0.p.c0; g0 = e0.p.c1; b0 = e0.p.c2; D0 = e0.d; }
+            if (two) {
+                const ExactPixelDepth e1 =
+                    render_pixel_exact_warp_depth(rs, ds, start, total, (float)(sx + 1), (float)sy, lane);
+                if (lane == src) { A1 = e1.p.A; wl1 = e1.p.wl; n1 = e1.p.n; r1 = e1.p.c0; g1 = e1.p.c1; b1 = e1.p.c2; D1 = e1.d; }
+            }
+            continue;
+        }
         const ExactPixel e0 = render_pixel_exact_warp<GATHER>(rs, start, total, (float)sx, (float)sy, lane);
         if (lane == src) { A0 = e0.A; wl0 = e0.wl; n0 = e0.n; r0 = e0.c0; g0 = e0.c1; b0 = e0.c2; }
         if (two) {
@@ -590,6 +682,10 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     }
 
     const float bg0 = background[0], bg1 = background[1], bg2 = background[2];
+    if (DEPTH) {  // alpha: the accumulated weight before any background; depth: no background term
+        if (valid0) { depth[(size_t)py * W + px] = D0; alpha[(size_t)py * W + px] = A0; }
+        if (valid1) { depth[(size_t)py * W + px + 1] = D1; alpha[(size_t)py * W + px + 1] = A1; }
+    }
     auto finish = [&](bool valid, int x, float A, float wlx, int nx, float c0, float c1, float c2) {
         if (!valid) return;
         if (A < GSR_BG_THRESH) {  // src/render.cu:169-175, double arithmetic
@@ -607,6 +703,27 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     };
     finish(valid0, px, A0, wl0, n0, r0, g0, b0);
     finish(valid1, px + 1, A1, wl1, n1, r1, g1, b1);
+}
+
+template <bool MARK, bool GATHER>
+__global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
+    k_render_fwd(const RecSource rs, const int32_t* __restrict__ ranges,
+                 const float* __restrict__ background, int W, int H, int32_t* __restrict__ n_out,
+                 float* __restrict__ w_out, float* __restrict__ image, uint32_t* __restrict__ masks) {
+    render_fwd<MARK, GATHER, false>(rs, ranges, background, W, H, n_out, w_out, image, masks, DepthSource{}, nullptr,
+                                    nullptr);
+}
+
+#ifndef GSR_FWD_DEPTH_MINB
+#define GSR_FWD_DEPTH_MINB 8
+#endif
+template <bool MARK>
+__global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_DEPTH_MINB)
+    k_render_fwd_depth(const RecSource rs, const DepthSource ds, const int32_t* __restrict__ ranges,
+                       const float* __restrict__ background, int W, int H, int32_t* __restrict__ n_out,
+                       float* __restrict__ w_out, float* __restrict__ image, float* __restrict__ depth,
+                       float* __restrict__ alpha, uint32_t* __restrict__ masks) {
+    render_fwd<MARK, true, true>(rs, ranges, background, W, H, n_out, w_out, image, masks, ds, depth, alpha);
 }
 
 // (float)(1.0 / (1.0 - (double)alpha)) — src/render_backward.cu:183 — without fp64: 1 - alpha is split
@@ -749,20 +866,27 @@ __device__ __forceinline__ void mask_lists(const uint32_t* __restrict__ gm, int 
 
 // MASKS: the per-group splat lists come from the forward's contribution masks (exactly the records that
 // contributed to the group's pixels) instead of the conservative footprint test
-template <bool MASKS, bool GATHER>
-__global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
-    k_render_bwd(const RecSource rs, const int32_t* __restrict__ sorted_idx,
-                 const int32_t* __restrict__ ranges, const float* __restrict__ background, int W, int H,
-                 const int32_t* __restrict__ n_in, const float* __restrict__ w_in,
-                 const float* __restrict__ grad_image, float* __restrict__ g_rgb,
-                 float* __restrict__ g_opa, float* __restrict__ g_uv, float* __restrict__ g_conic,
-                 const uint32_t* __restrict__ masks) {
+// DEPTH (gather mode, interleaved rows only): upstream gradients on the depth and alpha maps join d_alpha through the
+// same weight and r as colour, with two more back-to-front accumulators (no background term), and one more moment,
+// alpha * weight * dD, is reduced and flushed into the row's slot 9 (camera-frame z)
+template <bool MASKS, bool GATHER, bool DEPTH>
+__device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* __restrict__ sorted_idx,
+                                           const int32_t* __restrict__ ranges, const float* __restrict__ background,
+                                           int W, int H, const int32_t* __restrict__ n_in,
+                                           const float* __restrict__ w_in, const float* __restrict__ grad_image,
+                                           float* __restrict__ g_rgb, float* __restrict__ g_opa,
+                                           float* __restrict__ g_uv, float* __restrict__ g_conic,
+                                           const uint32_t* __restrict__ masks, const DepthSource& ds,
+                                           const float* __restrict__ grad_depth, const float* __restrict__ grad_alpha) {
+    static_assert(GATHER || !DEPTH, "depth/alpha gradients are reduced by the gather kernels only");
+    constexpr int NG = DEPTH ? NGRAD + 1 : NGRAD;  // moments per (record, batch)
     __shared__ __align__(128) float s_rec[BSTAGES][(BATCH + 1) * REC];  // + an all-zero record (alpha 0) behind each stage
     __shared__ __align__(8) uint64_t s_full[BSTAGES];
     __shared__ int s_cnt[BSTAGES];
-    __shared__ float s_acc[BSTAGES][BATCH * NGRAD];  // one moment accumulator per staged batch
+    __shared__ float s_acc[BSTAGES][BATCH * NG];  // one moment accumulator per staged batch
     __shared__ __align__(16) uint8_t s_list[CTA_WARPS][LIST_BYTES];
     __shared__ int s_maxn;
+    __shared__ __align__(16) float s_z[BSTAGES][DEPTH ? BATCH + 1 : 1];  // DEPTH: z of the staged records (+ 0)
 
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
@@ -798,11 +922,17 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
     }
     F2 weight = pk(wt0, wt1);
     const F2 d0 = pk(da[0], db[0]), d1 = pk(da[1], db[1]), d2 = pk(da[2], db[2]);
+    F2 dD = bc(0.0f), dA = bc(0.0f);
+    if (DEPTH) {
+        const size_t pix = (size_t)py * W + px;
+        dD = pk(valid0 ? grad_depth[pix] : 0.0f, valid1 ? grad_depth[pix + 1] : 0.0f);
+        dA = pk(valid0 ? grad_alpha[pix] : 0.0f, valid1 ? grad_alpha[pix + 1] : 0.0f);
+    }
     if (tid == 0) {
         s_maxn = 0;
 #pragma unroll
         for (int s = 0; s < BSTAGES; ++s) {
-            mbar_init(&s_full[s], GATHER ? 32 : 1);
+            mbar_init(&s_full[s], GATHER ? (DEPTH ? 64 : 32) : 1);
             s_cnt[s] = 0;
         }
         fence_mbar_init();
@@ -817,8 +947,9 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
         m = max(m, __shfl_xor_sync(0xffffffffu, m, 1));
         if (lane == 0) atomicMax(&s_maxn, m);
     }
-    for (int k = tid; k < BSTAGES * BATCH * NGRAD; k += CTA_THREADS) (&s_acc[0][0])[k] = 0.0f;
+    for (int k = tid; k < BSTAGES * BATCH * NG; k += CTA_THREADS) (&s_acc[0][0])[k] = 0.0f;
     if (tid < BSTAGES * REC) s_rec[tid / REC][BATCH * REC + tid % REC] = 0.0f;
+    if (DEPTH && tid < BSTAGES) s_z[tid][BATCH] = 0.0f;
     __syncthreads();
     const int total = s_maxn;  // deepest splat any pixel of this tile consumed
     const int nb = (total + BATCH - 1) / BATCH;
@@ -830,7 +961,7 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
         const int b = nb - 1 - k, s = k % BSTAGES;
         const int cnt = min(BATCH, total - b * BATCH);
         if (GATHER) {
-            gather_batch(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane);
+            gather_batch<DEPTH>(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane, &ds, &s_z[s][0]);
         } else {
             const uint32_t bytes = (uint32_t)cnt * REC * 4u;
             mbar_arrive_expect_tx(&s_full[s], bytes);
@@ -844,6 +975,7 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
 
     const float bg0 = background[0], bg1 = background[1], bg2 = background[2];
     F2 na0 = bc(-0.0f), na1 = bc(-0.0f), na2 = bc(-0.0f);  // -color_accum
+    F2 nd = bc(-0.0f), nw = bc(-0.0f);                      // DEPTH: -acc_d, -acc_a
     bool bgi0 = false, bgi1 = false;
     const int gl = lane % GROUP_LANES;
     // after the butterfly: (16 lanes) even lanes own moments 0..7 and lane 1 the ninth; (8 lanes) every lane owns
@@ -964,11 +1096,22 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
             const F2 t0 = fma2(weight, bc(q2.y), mul2(r, na0));
             const F2 t1 = fma2(weight, bc(q2.z), mul2(r, na1));
             const F2 t2 = fma2(weight, bc(q2.w), mul2(r, na2));
-            const F2 galpha = fma2(d2, t2, fma2(d1, t1, fma2(d0, t0, bc(0.0f))));
+            F2 galpha = fma2(d2, t2, fma2(d1, t1, fma2(d0, t0, bc(0.0f))));
+            float zj = 0.0f;
+            if (DEPTH) {  // d_alpha += (z*weight - acc_d*r)*dD + (weight - acc_a*r)*dA
+                zj = s_z[s][j];
+                const F2 td = fma2(weight, bc(zj), mul2(r, nd));
+                const F2 ta = fma2(r, nw, weight);
+                galpha = fma2(dA, ta, fma2(dD, td, galpha));
+            }
             // acc_c += weight * (alpha * col_c), kept negated
             na0 = fma2(weight, mul2(alpha, bc(-q2.y)), na0);
             na1 = fma2(weight, mul2(alpha, bc(-q2.z)), na1);
             na2 = fma2(weight, mul2(alpha, bc(-q2.w)), na2);
+            if (DEPTH) {  // acc_d += weight * (alpha * z), acc_a += weight * alpha, kept negated
+                nd = fma2(weight, mul2(alpha, bc(-zj)), nd);
+                nw = fma2(weight, mul2(alpha, bc(-1.0f)), nw);
+            }
             // Only nine per-pixel MOMENTS are reduced; the uv / conic gradient formulas
             // (src/render_backward.cu:216-229) are linear in them and are finished once per
             // (gaussian, tile) pair after the reduction, in the flush below:
@@ -993,19 +1136,28 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
             g8[6] = lo(m6) + hi(m6);
             g8[7] = lo(m7) + hi(m7);
             float gc2 = lo(m8) + hi(m8);
+            float gz = 0.0f;  // DEPTH: S9 = alpha*weight*dD -> d_z
+            if (DEPTH) {
+                const F2 mz = mul2(dD, aw);
+                gz = lo(mz) + hi(mz);
+            }
             const bool group_any = MASKS ? act : ((bal & group_mask) != 0u);
             if (GROUPS == 2) {
                 butterfly8_half(g8, lane);
                 gc2 = half_warp_sum(gc2);
+                if (DEPTH) gz = half_warp_sum(gz);
                 const float mine = (gl == 1) ? gc2 : g8[0];
-                if (group_any & owner) atomicAdd(&acc[j * NGRAD + my_slot], mine);
+                if (group_any & owner) atomicAdd(&acc[j * NG + my_slot], mine);
+                if (DEPTH && group_any && gl == 0) atomicAdd(&acc[j * NG + NGRAD], gz);
             } else {
                 butterfly8_quarter(g8, lane);
                 gc2 = quarter_warp_sum(gc2);
+                if (DEPTH) gz = quarter_warp_sum(gz);
                 if (group_any) {
-                    float* cell = reinterpret_cast<float*>(__cvta_shared_to_generic(acc_cell + j * (NGRAD * 4)));
+                    float* cell = reinterpret_cast<float*>(__cvta_shared_to_generic(acc_cell + j * (NG * 4)));
                     atomicAdd(cell, g8[0]);
                     if (gl == 0) atomicAdd(cell + 8, gc2);
+                    if (DEPTH && gl == 1) atomicAdd(cell + 8, gz);  // lane 1's cell + 8 is moment 9
                 }
             }
         }
@@ -1032,16 +1184,16 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
             for (int i = 0; i < BATCH / 32; ++i) {
                 const int r = lane + 32 * i;
                 if (r >= cnt) break;
-                float S[NGRAD];
+                float S[NG];
                 bool any = false;
 #pragma unroll
-                for (int q = 0; q < NGRAD; ++q) {
-                    S[q] = acc[r * NGRAD + q];
+                for (int q = 0; q < NG; ++q) {
+                    S[q] = acc[r * NG + q];
                     any |= (S[q] != 0.0f);
                 }
                 if (any) {
 #pragma unroll
-                    for (int q = 0; q < NGRAD; ++q) acc[r * NGRAD + q] = 0.0f;
+                    for (int q = 0; q < NG; ++q) acc[r * NG + q] = 0.0f;
                     const float4 q1 = rec4[r * 3 + 1];
                     const float a = q1.x, bh = 0.5f * q1.y, c = q1.z, rdet = rec4[r * 3 + 2].x;
                     const int gid = gids[i];
@@ -1051,14 +1203,18 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
                     // common_frac summed over pixels (render_backward.cu:221-223)
                     const float cf = (a * S[8] - 2.0f * bh * S[7] + c * S[6]) * rdet * rdet;
                     const float gc0 = -c * cf + S[8] * rdet, gc1 = bh * cf - S[7] * rdet, gc2 = -a * cf + S[6] * rdet;
-                    if (g_opa == nullptr) {
+                    if (DEPTH || g_opa == nullptr) {
                         // interleaved gradient rows [gaussian][12] = rgb3 opa | uv2 conic0 conic1 | conic2 pad3: the
                         // nine sums of a pair land in two adjacent 32-byte sectors through two 16-byte vector
-                        // reductions + one scalar (planar arrays: nine scalar reductions into four arrays)
+                        // reductions + one scalar (planar arrays: nine scalar reductions into four arrays).
+                        // DEPTH: conic2 z pad2, the last two through one 8-byte vector reduction
                         float* row = g_rgb + (size_t)gid * GRAD_ROW;
                         red_add_v4(row, GSR_SH0 * S[0], GSR_SH0 * S[1], GSR_SH0 * S[2], S[3]);
                         red_add_v4(row + 4, gu, gv, gc0, gc1);
-                        atomicAdd(row + 8, gc2);
+                        if (DEPTH)
+                            red_add_v2(row + 8, gc2, S[NG - 1]);
+                        else
+                            atomicAdd(row + 8, gc2);
                     } else {
                         atomicAdd(g_rgb + (size_t)gid * 3 + 0, GSR_SH0 * S[0]);
                         atomicAdd(g_rgb + (size_t)gid * 3 + 1, GSR_SH0 * S[1]);
@@ -1085,6 +1241,35 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
             }
         }
     }
+}
+
+template <bool MASKS, bool GATHER>
+__global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
+    k_render_bwd(const RecSource rs, const int32_t* __restrict__ sorted_idx,
+                 const int32_t* __restrict__ ranges, const float* __restrict__ background, int W, int H,
+                 const int32_t* __restrict__ n_in, const float* __restrict__ w_in,
+                 const float* __restrict__ grad_image, float* __restrict__ g_rgb,
+                 float* __restrict__ g_opa, float* __restrict__ g_uv, float* __restrict__ g_conic,
+                 const uint32_t* __restrict__ masks) {
+    render_bwd<MASKS, GATHER, false>(rs, sorted_idx, ranges, background, W, H, n_in, w_in, grad_image, g_rgb, g_opa,
+                                     g_uv, g_conic, masks, DepthSource{}, nullptr, nullptr);
+}
+
+#ifndef GSR_BWD_DEPTH_MINB
+// the two more per-pixel upstream gradients and accumulators do not fit the default build's 64 registers: at 72 (7 CTAs)
+// the masked walk reloads a spilled register every iteration, at 80 (6 CTAs) once per batch; at 5 CTAs (88-89
+// registers) neither variant keeps anything in local memory
+#define GSR_BWD_DEPTH_MINB 5
+#endif
+template <bool MASKS>
+__global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_DEPTH_MINB)
+    k_render_bwd_depth(const RecSource rs, const DepthSource ds, const int32_t* __restrict__ ranges,
+                       const float* __restrict__ background, int W, int H, const int32_t* __restrict__ n_in,
+                       const float* __restrict__ w_in, const float* __restrict__ grad_image,
+                       const float* __restrict__ grad_depth, const float* __restrict__ grad_alpha,
+                       float* __restrict__ grad_rows, const uint32_t* __restrict__ masks) {
+    render_bwd<MASKS, true, true>(rs, nullptr, ranges, background, W, H, n_in, w_in, grad_image, grad_rows, nullptr,
+                                  nullptr, nullptr, masks, ds, grad_depth, grad_alpha);
 }
 
 }  // namespace gsr
@@ -1179,6 +1364,65 @@ int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* ke
     return launch_backward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits), nullptr, ranges,
                                  background, H, W, n_in, w_in, grad_image, g_rgb, g_opa, g_uv, g_conic,
                                  contribution_masks, stream);
+}
+
+// the sort-key depth field of the pair list (or the per-gaussian depth keys, sorted id array): see DepthSource
+static bool make_depth_source(const uint64_t* keys_sorted, int id_bits, const uint32_t* depth_key,
+                              uint32_t depth_base, int depth_bits, DepthSource& ds) {
+    if (depth_bits < 1 || depth_bits > 32) return false;
+    if (depth_base == 0u && depth_bits != 32) return false;  // depth_key()'s transform uses all 32 bits
+    if (keys_sorted == nullptr && depth_key == nullptr) return false;
+    if (keys_sorted != nullptr && (id_bits <= 0 || id_bits + depth_bits > 64)) return false;
+    ds.zkey = depth_key;
+    ds.depth_base = depth_base;
+    ds.depth_mask = depth_bits == 32 ? ~0u : ((1u << depth_bits) - 1u);
+    ds.id_bits = keys_sorted != nullptr ? id_bits : 0;
+    return true;
+}
+
+int gsr_render_forward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                                    const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                                    int depth_bits, const int32_t* ranges, const float* background, int H, int W,
+                                    int32_t* n_out, float* w_out, float* image, float* depth, float* alpha,
+                                    uint32_t* contribution_masks, void* stream) {
+    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;
+    if (H <= 0 || W <= 0 || depth == nullptr || alpha == nullptr) return GSR_ERR_BAD_ARG;
+    DepthSource ds;
+    if (!make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds)) return GSR_ERR_BAD_ARG;
+    const RecSource src = make_source(gaussian_records, keys_sorted, ids_sorted, id_bits);
+    const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
+    if (contribution_masks != nullptr)
+        k_render_fwd_depth<true><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_out,
+                                                                          w_out, image, depth, alpha,
+                                                                          contribution_masks);
+    else
+        k_render_fwd_depth<false><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_out,
+                                                                           w_out, image, depth, alpha, nullptr);
+    return (int)cudaGetLastError();
+}
+
+int gsr_render_backward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                                     const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                                     int depth_bits, const int32_t* ranges, const float* background, int H, int W,
+                                     const int32_t* n_in, const float* w_in, const float* grad_image,
+                                     const float* grad_depth, const float* grad_alpha, float* grad_rows,
+                                     const uint32_t* contribution_masks, void* stream) {
+    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;
+    if (H <= 0 || W <= 0 || grad_image == nullptr || grad_depth == nullptr || grad_alpha == nullptr) return GSR_ERR_BAD_ARG;
+    if (grad_rows == nullptr || (reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0) return GSR_ERR_BAD_ARG;
+    DepthSource ds;
+    if (!make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds)) return GSR_ERR_BAD_ARG;
+    const RecSource src = make_source(gaussian_records, keys_sorted, ids_sorted, id_bits);
+    const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
+    if (contribution_masks != nullptr)
+        k_render_bwd_depth<true><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_in,
+                                                                          w_in, grad_image, grad_depth, grad_alpha,
+                                                                          grad_rows, contribution_masks);
+    else
+        k_render_bwd_depth<false><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_in,
+                                                                           w_in, grad_image, grad_depth, grad_alpha,
+                                                                           grad_rows, nullptr);
+    return (int)cudaGetLastError();
 }
 
 const char* gsr_version(void) { return "gsr_b200 0.1 sm_90a"; }

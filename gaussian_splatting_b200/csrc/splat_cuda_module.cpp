@@ -645,10 +645,73 @@ torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, torch::
     return slab;
 }
 
+// Depth/alpha mode of the two calls above (gather mode only).  Forward: + depth [H,W,1], alpha [H,W,1]; zkey: the
+// per-gaussian depth keys of the forward (read when the pair list is a sorted id array).
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+fused_render_forward_depth(torch::Tensor records, torch::Tensor ranges, torch::Tensor background, int64_t H, int64_t W,
+                           int64_t P, bool record_masks, c10::optional<torch::Tensor> keys_sorted,
+                           c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, torch::Tensor zkey,
+                           int64_t depth_base, int64_t depth_bits) {
+    CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
+    TORCH_CHECK(background.numel() == 3, "Background RGB must have 3 elements");
+    c10::cuda::CUDAGuard guard(records.device());
+    auto opt = records.options();
+    torch::Tensor image = torch::empty({H, W, 3}, opt);
+    torch::Tensor n = torch::empty({H, W}, opt.dtype(torch::kInt32));
+    torch::Tensor w = torch::empty({H, W}, opt);
+    torch::Tensor depth = torch::empty({H, W, 1}, opt);
+    torch::Tensor alpha = torch::empty({H, W, 1}, opt);
+    torch::Tensor masks = record_masks
+                              ? torch::zeros({(int64_t)gsr_contribution_mask_words(P, (int)H, (int)W)}, opt.dtype(torch::kInt32))
+                              : torch::empty({0}, opt.dtype(torch::kInt32));
+    const bool by_key = keys_sorted.has_value() && keys_sorted->numel() > 0;
+    const bool by_id = !by_key && ids_sorted.has_value() && ids_sorted->numel() > 0;
+    TORCH_CHECK(by_key || by_id || P == 0, "gather mode needs the sorted pair list");
+    // an empty view (P == 0) still runs the kernel, which then reads no pair: any well-formed source will do
+    const int32_t dummy_id = 0;
+    check_rc(gsr_render_forward_gather_depth(
+                 F32PTR(records), by_key ? (const uint64_t*)keys_sorted->data_ptr<int64_t>() : nullptr, (int)id_bits,
+                 by_id ? ids_sorted->data_ptr<int>() : (by_key ? nullptr : &dummy_id),
+                 (const uint32_t*)zkey.data_ptr<int>(), (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(),
+                 F32PTR(background), (int)H, (int)W, n.data_ptr<int>(), F32PTR(w), F32PTR(image), F32PTR(depth),
+                 F32PTR(alpha), record_masks ? (uint32_t*)masks.data_ptr<int>() : nullptr, cur_stream()),
+             "gsr_render_forward_gather_depth");
+    return std::make_tuple(image, n, w, masks, depth, alpha);
+}
+
+// interleaved rows [N,12]: rgb3 opacity | uv2 conic0 conic1 | conic2 z pad2
+torch::Tensor fused_render_backward_depth(torch::Tensor grad_image, torch::Tensor grad_depth, torch::Tensor grad_alpha,
+                                          int64_t N, torch::Tensor records, torch::Tensor ids_sorted,
+                                          torch::Tensor ranges, torch::Tensor background, torch::Tensor n,
+                                          torch::Tensor w, torch::Tensor masks,
+                                          c10::optional<torch::Tensor> keys_sorted, int64_t id_bits,
+                                          torch::Tensor zkey, int64_t depth_base, int64_t depth_bits) {
+    CHECK_VALID_INPUT(grad_image); CHECK_FLOAT_TENSOR(grad_image);
+    CHECK_VALID_INPUT(grad_depth); CHECK_FLOAT_TENSOR(grad_depth);
+    CHECK_VALID_INPUT(grad_alpha); CHECK_FLOAT_TENSOR(grad_alpha);
+    const int H = n.size(0), W = n.size(1);
+    TORCH_CHECK(grad_image.numel() == (int64_t)H * W * 3, "grad_image must be HxWx3");
+    TORCH_CHECK(grad_depth.numel() == (int64_t)H * W && grad_alpha.numel() == (int64_t)H * W,
+                "grad_depth and grad_alpha must hold H*W values");
+    c10::cuda::CUDAGuard guard(grad_image.device());
+    torch::Tensor slab = torch::zeros({N * (int64_t)GSR_GRAD_ROW_FLOATS}, grad_image.options());
+    const bool by_key = keys_sorted.has_value() && keys_sorted->numel() > 0;
+    const int32_t dummy_id = 0;
+    check_rc(gsr_render_backward_gather_depth(
+                 F32PTR(records), by_key ? (const uint64_t*)keys_sorted->data_ptr<int64_t>() : nullptr, (int)id_bits,
+                 by_key ? nullptr : (ids_sorted.numel() > 0 ? ids_sorted.data_ptr<int>() : &dummy_id),
+                 (const uint32_t*)zkey.data_ptr<int>(), (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(),
+                 F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w), F32PTR(grad_image), F32PTR(grad_depth),
+                 F32PTR(grad_alpha), slab.data_ptr<float>(),
+                 masks.numel() > 0 ? (const uint32_t*)masks.data_ptr<int>() : nullptr, cur_stream()),
+             "gsr_render_backward_gather_depth");
+    return slab;
+}
+
 // grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab [9N] (rows by gaussian).
 // grad_uv_compact [M,2] (optional): gradient on the compact uv, added to — or, with use_slab_uv false, replacing —
-// the slab's uv section.
-std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::Tensor xyz,
+// the slab's uv section.  depth: the slab is the rows of fused_render_backward_depth (slot 9 = gradient on z).
+static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, torch::Tensor slab, torch::Tensor xyz,
                                                      torch::Tensor quaternion, torch::Tensor scale,
                                                      torch::Tensor opacity_logit,
                                                      c10::optional<torch::Tensor> sh_rest,
@@ -662,6 +725,7 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
     const int64_t N = xyz.size(0);
     const bool rows = slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS && N > 0;  // interleaved [N,12] (else planar [9N])
     TORCH_CHECK(rows || slab.numel() == N * 9, "gradient slab must hold 9 (planar) or 12 (rows) floats per gaussian");
+    TORCH_CHECK(!depth || rows || N == 0, "the depth/alpha backward needs the interleaved gradient rows");
     c10::cuda::CUDAGuard guard(xyz.device());
     auto opt = xyz.options();
     const float* g_rgb = slab.data_ptr<float>();
@@ -705,6 +769,16 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
                   o_o = section(3, {N}), o_dc = section(4, {N, 3});
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
+    if (depth) {
+        check_rc(gsr_preprocess_backward_depth((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
+                                               F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
+                                               camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
+                                               visible.data_ptr<uint8_t>(), N > 0 ? slab.data_ptr<float>() : nullptr,
+                                               use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q),
+                                               F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr,
+                                               cur_stream()),
+                 "gsr_preprocess_backward_depth");
+    } else
     check_rc(gsr_preprocess_backward((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
                                      F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
                                      camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
@@ -719,6 +793,22 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
     out.push_back(flat);  // last: the allocation all the others are views of
     return out;
 }
+
+#define GSR_PREPROCESS_BWD_ARGS                                                                                   \
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale,                         \
+        torch::Tensor opacity_logit, c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,          \
+        torch::Tensor K, c10::optional<torch::Tensor> camera_centre, torch::Tensor visible,                      \
+        c10::optional<torch::Tensor> out_flat, c10::optional<torch::Tensor> grad_uv_compact,                     \
+        c10::optional<torch::Tensor> scan, bool use_slab_uv
+std::vector<torch::Tensor> fused_preprocess_backward(GSR_PREPROCESS_BWD_ARGS) {
+    return preprocess_backward_impl(false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
+                                    camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
+}
+std::vector<torch::Tensor> fused_preprocess_backward_depth(GSR_PREPROCESS_BWD_ARGS) {
+    return preprocess_backward_impl(true, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
+                                    camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
+}
+#undef GSR_PREPROCESS_BWD_ARGS
 
 // sizes of the flat parameter / gradient layout: exclusive end of each section, in elements
 std::vector<int64_t> flat_section_ends(int64_t N, int64_t n_sh_rest) {
@@ -968,6 +1058,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("fused_render_forward", &fused_render_forward, "tile renderer forward on a record stream");
     m.def("fused_render_backward", &fused_render_backward, "tile renderer backward -> per-gaussian gradient slab");
     m.def("fused_preprocess_backward", &fused_preprocess_backward, "fused per-gaussian backward");
+    m.def("fused_render_forward_depth", &fused_render_forward_depth,
+          "tile renderer forward (gather mode) with depth and alpha maps");
+    m.def("fused_render_backward_depth", &fused_render_backward_depth,
+          "tile renderer backward (gather mode) with depth and alpha upstream gradients -> rows incl. z");
+    m.def("fused_preprocess_backward_depth", &fused_preprocess_backward_depth,
+          "fused per-gaussian backward from rows carrying the camera-frame z gradient");
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");

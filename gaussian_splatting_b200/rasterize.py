@@ -244,7 +244,8 @@ class _ViewState:
 
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges", "stream_rec", "gather",
                  "records", "keys_sorted", "id_bits", "slab_width",
-                 "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed")
+                 "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
+                 "depth_alpha", "zkey", "depth_base", "depth_bits", "depth", "alpha")
 
     @property
     def ids_sorted(self):
@@ -265,6 +266,8 @@ class _ViewState:
         self.background = None  # set by rasterize() before the projection node runs (it pre-launches the renderer)
         self.image = None
         self.speculation_overflowed = False
+        self.depth_alpha = False  # render_depth_alpha: the tile kernels also produce depth / alpha [H,W,1]
+        self.depth = self.alpha = None
 
 
 class _stage:
@@ -329,15 +332,21 @@ class _ProjectGaussians(torch.autograd.Function):
                                    "the int32 pair index of the native path (P must be < 2^31)")
             return M_, P_
 
-        gather = USE_RECORD_GATHER
+        # depth / alpha maps are rendered by the gather kernels only (they read z off the sorted pair keys)
+        gather = USE_RECORD_GATHER or state.depth_alpha
 
         def bin_and_render(M_, P_, speculative):
             with _stage(state, "bin_sort_gather"):
                 binned = ext.fused_bin(records, zkey, visible, scan, M_, P_, H, W, mh, depth_bits, speculative, gather,
                                        tile_mask if USE_TILE_MASKS else None, tile_win if USE_TILE_MASKS else None)
             with _stage(state, "render_fwd"):
-                rendered = ext.fused_render_forward(records if gather else binned[2], binned[1], background, H, W, P_,
-                                                    record_masks, binned[5], binned[0], binned[6], gather)
+                if state.depth_alpha:
+                    rendered = ext.fused_render_forward_depth(records, binned[1], background, H, W, P_, record_masks,
+                                                              binned[5], binned[0], binned[6], zkey, depth_base,
+                                                              depth_bits)
+                else:
+                    rendered = ext.fused_render_forward(records if gather else binned[2], binned[1], background, H, W,
+                                                        P_, record_masks, binned[5], binned[0], binned[6], gather)
             return binned, rendered
 
         # The host needs M and P (the shape of the returned uv; the size of the pair buffers).  Reading them right
@@ -378,7 +387,10 @@ class _ProjectGaussians(torch.autograd.Function):
         _note_pairs(key, P)
         ids_sorted, ranges, stream_rec, vis_idx, uv, keys_sorted, id_bits = binned
         state.gather, state.records, state.keys_sorted, state.id_bits = gather, records, keys_sorted, int(id_bits)
-        state.image, state.n_per_pixel, state.w_per_pixel, state.masks = rendered
+        state.image, state.n_per_pixel, state.w_per_pixel, state.masks = rendered[:4]
+        if state.depth_alpha:
+            state.depth, state.alpha = rendered[4:]
+            state.zkey, state.depth_base, state.depth_bits = zkey, depth_base, depth_bits
         state.N, state.M, state.P, state.H, state.W = xyz.shape[0], M, P, H, W
         state.visible = visible
         state.vis_idx = state.vis_idx32 = vis_idx                # int32 [M]: visible gaussians, ascending
@@ -409,10 +421,10 @@ class _ProjectGaussians(torch.autograd.Function):
         if grad_uv is not None and st.M > 0:
             guv = grad_uv.contiguous()
         with _stage(st, "preprocess_bwd"):
-            grads = native().fused_preprocess_backward(slab, xyz, quaternion, scale, opacity_flat, sh,
-                                                       camera_T_world, K, centre, st.visible, st.grad_out,
-                                                       guv, st.scan if guv is not None else None,
-                                                       not st.uv_grad_emitted)
+            # depth/alpha mode: the rows also carry the render backward's gradient on camera-frame z (slot 9)
+            fn = native().fused_preprocess_backward_depth if st.depth_alpha else native().fused_preprocess_backward
+            grads = fn(slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible,
+                       st.grad_out, guv, st.scan if guv is not None else None, not st.uv_grad_emitted)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
@@ -436,25 +448,60 @@ class _CompositeTiles(torch.autograd.Function):
                                                   st.records if st.gather else st.stream_rec, st._ids_sorted,
                                                   st.ranges, st.background, st.n_per_pixel, st.w_per_pixel, st.masks,
                                                   st.keys_sorted, st.id_bits, st.gather)
-        # The render pass's gradient on the compact uv is a gather of the slab's uv section (28 us at 3M).  It
-        # reaches the per-gaussian backward through the slab anyway, so it is only materialised when it can be
-        # OBSERVED: the caller retained uv's gradient (the reference trainer does, splat_py/trainer.py:360) or
-        # hooked the tensor.
-        uv_t = st.uv_ref() if st.uv_ref is not None else None
-        watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
-        st.uv_grad_emitted = bool(watched)
-        if not watched:
-            return None, slab, None, None
-        N = st.N
-        if st.slab_width == 12:   # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3
-            grad_uv = slab.view(N, 12).index_select(0, st.vis_idx)[:, 4:6].contiguous()
-        else:                     # planar: rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3]
-            grad_uv = slab[4 * N:6 * N].view(N, 2).index_select(0, st.vis_idx)
-        return grad_uv, slab, None, None
+        return _render_grads(st, slab)
+
+
+class _CompositeTilesDepth(torch.autograd.Function):
+    """_CompositeTiles with the depth and alpha maps the renderer produced alongside the image."""
+
+    @staticmethod
+    def forward(ctx, uv, carrier, background_rgb, state):
+        outs = (state.image, state.depth, state.alpha)
+        state.image = state.depth = state.alpha = None
+        ctx.state = state
+        return outs
+
+    @staticmethod
+    def backward(ctx, grad_image, grad_depth, grad_alpha):
+        st = ctx.state
+        with _stage(st, "render_bwd"):
+            slab = native().fused_render_backward_depth(grad_image.contiguous(), grad_depth.contiguous(),
+                                                        grad_alpha.contiguous(), st.N, st.records, st._ids_sorted,
+                                                        st.ranges, st.background, st.n_per_pixel, st.w_per_pixel,
+                                                        st.masks, st.keys_sorted, st.id_bits, st.zkey, st.depth_base,
+                                                        st.depth_bits)
+        return _render_grads(st, slab)
+
+
+def _render_grads(st, slab):
+    """Gradients of a composite node for (uv, carrier, background, state) from the render backward's slab."""
+    # The render pass's gradient on the compact uv is a gather of the slab's uv section (28 us at 3M).  It
+    # reaches the per-gaussian backward through the slab anyway, so it is only materialised when it can be
+    # OBSERVED: the caller retained uv's gradient (the reference trainer does, splat_py/trainer.py:360) or
+    # hooked the tensor.
+    uv_t = st.uv_ref() if st.uv_ref is not None else None
+    watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
+    st.uv_grad_emitted = bool(watched)
+    if not watched:
+        return None, slab, None, None
+    N = st.N
+    if st.slab_width == 12:   # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3 (depth mode: z pad2)
+        grad_uv = slab.view(N, 12).index_select(0, st.vis_idx)[:, 4:6].contiguous()
+    else:                     # planar: rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3]
+        grad_uv = slab[4 * N:6 * N].view(N, 2).index_select(0, st.vis_idx)
+    return grad_uv, slab, None, None
 
 
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
-              use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None):
+              use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
+              render_depth_alpha=False):
+    """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
+    returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
+    accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
+    colour, z_i the camera-frame z, with no background term (expected depth: depth / alpha.clamp_min(eps)).  fp32
+    and precomputed SH colours only; always on the fused gather kernels."""
+    if render_depth_alpha and gaussians.sh is not None and not use_sh_precompute:
+        raise ValueError("render_depth_alpha needs use_sh_precompute=True (per-pixel SH colours are not supported)")
     if gaussians.sh is not None and not use_sh_precompute:
         return rasterize_unfused(gaussians, camera_T_world, camera, near_thresh, far_thresh,
                                  cull_mask_padding, mh_dist, use_sh_precompute, background_rgb)
@@ -462,6 +509,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
         raise TypeError("the fused rasterizer is fp32; use rasterize_unfused for float64 inputs")
     state = _ViewState(profile)
     state.grad_out = grad_out
+    state.depth_alpha = bool(render_depth_alpha)
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))
@@ -471,8 +519,13 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
         None if gaussians.sh is None else gaussians.sh.contiguous(),
         camera_T_world.contiguous(), camera.K.contiguous(), state, cfg)
     state.uv_ref = weakref.ref(uv)
-    image = _CompositeTiles.apply(uv, carrier, state.background, state)
     culling_mask = state.visible == 0
+    if state.depth_alpha:
+        image, depth, alpha = _CompositeTilesDepth.apply(uv, carrier, state.background, state)
+        if return_state:
+            return image, culling_mask, uv, depth, alpha, state
+        return image, culling_mask, uv, depth, alpha
+    image = _CompositeTiles.apply(uv, carrier, state.background, state)
     if return_state:
         return image, culling_mask, uv, state
     return image, culling_mask, uv

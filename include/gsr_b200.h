@@ -176,6 +176,30 @@ int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* ke
                                const float* grad_image, float* grad_rgb, float* grad_opacity, float* grad_uv,
                                float* grad_conic, float* grad_rows, const uint32_t* contribution_masks, void* stream);
 
+/* Depth and alpha maps from the same walk (gather kernels only, precomputed colours).  Per pixel, over the splats the
+ * colour blend composites (same weights w_i, same saturation early-out):
+ *   alpha [H,W] = the accumulated sum of w_i before any background (0 where nothing contributes),
+ *   depth [H,W] = D, D <- fma(w_i, z_i, D) front to back, z_i the camera-frame z of gaussian i; no background term
+ *                 (un-normalised: expected depth is depth / alpha).
+ * z_i is decoded from the depth field of the sorted pair keys — bits(z) - depth_base, or depth_key()'s
+ * order-preserving transform when depth_base == 0 (then depth_bits must be 32) — and, with ids_sorted instead of
+ * keys_sorted, from the per-gaussian depth keys depth_key [N] (gsr_preprocess_forward's output).
+ * The backward takes upstream gradients on all three maps (all three non-NULL; zeros where a map has none) and
+ * accumulates interleaved rows rgb3 opacity | uv2 conic0 conic1 | conic2 z pad2 into grad_rows [N,12] (16-byte
+ * aligned, zero-filled), z being the gradient on the camera-frame z; gsr_preprocess_backward_depth consumes them.
+ * Argument errors return GSR_ERR_BAD_ARG. */
+int gsr_render_forward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                                    const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                                    int depth_bits, const int32_t* tile_ranges, const float* background_rgb, int H,
+                                    int W, int32_t* num_splats_per_pixel, float* final_weight_per_pixel, float* image,
+                                    float* depth, float* alpha, uint32_t* contribution_masks, void* stream);
+int gsr_render_backward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                                     const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                                     int depth_bits, const int32_t* tile_ranges, const float* background_rgb, int H,
+                                     int W, const int32_t* num_splats_per_pixel, const float* final_weight_per_pixel,
+                                     const float* grad_image, const float* grad_depth, const float* grad_alpha,
+                                     float* grad_rows, const uint32_t* contribution_masks, void* stream);
+
 /* General renderers: any dtype, any n_sh in {1,4,9,16} (per-pixel SH via view_dir_by_pixel
  * [H,W,3]); same semantics as the reference's template instantiations
  * (fp64: no +0.25 dilation, exp(), no 1/255 skip — src/render.cu:117-148). */
@@ -305,6 +329,14 @@ int gsr_preprocess_backward(int N, int n_sh_rest, const float* xyz, const float*
                             const float* grad_rows, int use_rows_uv,
                             const float* grad_uv_compact, const uint64_t* scan, float* g_xyz, float* g_quaternion,
                             float* g_scale, float* g_opacity_logit, float* g_rgb_dc, float* g_sh_rest, void* stream);
+/* The same from the rows of gsr_render_backward_gather_depth (grad_rows required, 16-byte aligned): row slot 9, the
+ * gradient on the camera-frame z, joins grad_xyz as camera_T_world[2, :3] * g_z.  No gradient goes to the pose. */
+int gsr_preprocess_backward_depth(int N, int n_sh_rest, const float* xyz, const float* quaternion, const float* scale,
+                                  const float* opacity_logit, const float* camera_T_world, const float* K,
+                                  const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                                  int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
+                                  float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                                  float* g_sh_rest, void* stream);
 
 /* ---- optimizer step on the flat parameter buffer (SURVEY.md 8(f) rank 2) ----------------------------
  * Replaces torch.optim.Adam.step() as configured by splat_py/optimizer_manager.py:13-44 (one parameter group
