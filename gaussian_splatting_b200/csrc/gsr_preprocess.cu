@@ -140,18 +140,21 @@ __device__ __forceinline__ void coop_copy(float* __restrict__ dst, const float* 
     for (int k = threadIdx.x; k < n_floats; k += PRE_THREADS) dst[k] = src[k];
 }
 
-template <int N_SH, bool HAS_SH>
-__global__ void __launch_bounds__(PRE_THREADS, 7)
-    k_preprocess_fwd(int N, const float* __restrict__ xyz, const float* __restrict__ xyz_cam, int cam_first,
-                     const float* __restrict__ quat,
-                     const float* __restrict__ scale, const float* __restrict__ opa_logit,
-                     const float* __restrict__ rgb_dc, const float* __restrict__ sh_rest,
-                     const float* __restrict__ Tdev, const float* __restrict__ Kdev,
-                     const float* __restrict__ camdev, float width, float height, float near_t, float far_t,
-                     float pad, float mh, int ntx, int nty, uint32_t depth_base,
-                     float* __restrict__ records, uint32_t* __restrict__ zkey,
-                     uint8_t* __restrict__ visible, uint64_t* __restrict__ packed, uint64_t* __restrict__ tile_mask,
-                     uint32_t* __restrict__ tile_win, int use_tma) {
+#define GSR_PRE_FWD_PARAMS                                                                                         \
+    int N, const float* __restrict__ xyz, const float* __restrict__ xyz_cam, int cam_first,                        \
+        const float* __restrict__ quat, const float* __restrict__ scale, const float* __restrict__ opa_logit,      \
+        const float* __restrict__ rgb_dc, const float* __restrict__ sh_rest, const float* __restrict__ Tdev,       \
+        const float* __restrict__ Kdev, const float* __restrict__ camdev, float width, float height, float near_t, \
+        float far_t, float pad, float mh, int ntx, int nty, uint32_t depth_base, float* __restrict__ records,      \
+        uint32_t* __restrict__ zkey, uint8_t* __restrict__ visible, uint64_t* __restrict__ packed,                 \
+        uint64_t* __restrict__ tile_mask, uint32_t* __restrict__ tile_win, int use_tma
+#define GSR_PRE_FWD_FORWARD                                                                                        \
+    N, xyz, xyz_cam, cam_first, quat, scale, opa_logit, rgb_dc, sh_rest, Tdev, Kdev, camdev, width, height, near_t, \
+        far_t, pad, mh, ntx, nty, depth_base, records, zkey, visible, packed, tile_mask, tile_win, use_tma
+// ANTIALIAS: the record's opacity is sigmoid(o) * aa_rho(conic) (gsr_record.cuh); the culling bound tau' is formed
+// from that compensated opacity
+template <int N_SH, bool HAS_SH, bool ANTIALIAS>
+__device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS) {
     constexpr int NR3 = HAS_SH ? 3 * (N_SH - 1) : 1;
     __shared__ ViewConsts vc;
     __shared__ __align__(128) float s_sh[PRE_THREADS * NR3];       // SH coefficients of the CTA's gaussians
@@ -215,7 +218,8 @@ __global__ void __launch_bounds__(PRE_THREADS, 7)
             W[6] = vc.T[8]; W[7] = vc.T[9]; W[8] = vc.T[10];
             conic_from<float>(S9, J, W, conic, nullptr);
 
-            const float opa = sigmoid_torch(opl);
+            float opa = sigmoid_torch(opl);
+            if (ANTIALIAS) opa = __fmul_rn(opa, aa_rho(conic[0], conic[1], conic[2]));
             float dc[3] = {dc0, dc1, dc2};
             float col[3];
             if (HAS_SH) {
@@ -278,14 +282,32 @@ __global__ void __launch_bounds__(PRE_THREADS, 7)
     if (HAS_SH && tma && tid == 0) mbar_wait(&s_bar, 0);  // never exit with the SH load still in flight
 }
 
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, 7) k_preprocess_fwd(GSR_PRE_FWD_PARAMS) {
+    preprocess_fwd<N_SH, HAS_SH, false>(GSR_PRE_FWD_FORWARD);
+}
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, 7) k_preprocess_fwd_aa(GSR_PRE_FWD_PARAMS) {
+    preprocess_fwd<N_SH, HAS_SH, true>(GSR_PRE_FWD_FORWARD);
+}
+#undef GSR_PRE_FWD_PARAMS
+#undef GSR_PRE_FWD_FORWARD
+
 // Fused VJP.  g_rgb/g_opa/g_uv/g_conic are the per-Gaussian sums produced by the render backward
 // (indexed by original gaussian).  Order of the chain: SURVEY.md Appendix A "Per-Gaussian backward".
 #ifndef GSR_PRE_BWD_MINB
 #define GSR_PRE_BWD_MINB 6
 #endif
+// the anti-aliased backward re-forms the conic for rho's gradient: at 6 CTAs per SM (80 registers) that spills, at 5
+// it does not
+#ifndef GSR_PRE_BWD_AA_MINB
+#define GSR_PRE_BWD_AA_MINB 5
+#endif
 // DEPTH: the interleaved rows carry the render backward's camera-frame z gradient in slot 9 (conic2 z pad2); it joins
-// the z component of the camera-frame position gradient before grad_xyz = W^T grad_xyz_cam
-template <int N_SH, bool HAS_SH, bool DEPTH>
+// the z component of the camera-frame position gradient before grad_xyz = W^T grad_xyz_cam.
+// ANTIALIAS: the rows' opacity slot is the gradient on the compensated opacity sigmoid(o) * rho of k_preprocess_fwd_aa;
+// it is carried back to sigmoid(o) and, through rho, to the conic.
+template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS>
 __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ xyz, const float* __restrict__ quat,
                      const float* __restrict__ scale, const float* __restrict__ opa_logit,
                      const float* __restrict__ Tdev, const float* __restrict__ Kdev,
@@ -367,6 +389,25 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
         W[3] = vc.T[4]; W[4] = vc.T[5]; W[5] = vc.T[6];
         W[6] = vc.T[8]; W[7] = vc.T[9]; W[8] = vc.T[10];
 
+        float rho = 1.0f;
+        if (ANTIALIAS) {
+            // The row's opacity slot is g' = dL/d(sigmoid(o) * rho).  With A = c0 + 1/4, C = c2 + 1/4, bh = c1 / 2,
+            // det = A C - bh^2 and rho^2 = det0 / det, the cancellation-free forms of the conic derivatives are
+            //   drho/dc0 = (c2 C + bh^2) / (8 rho det^2),  drho/dc2 = (c0 A + bh^2) / (8 rho det^2),
+            //   drho/dc1 = -bh (A + C - 1/4) / (8 rho det^2)
+            // (c2 - rho^2 C = (c2 C + bh^2) / (4 det), 1 - rho^2 = (A + C - 1/4) / (4 det)).  Where rho == 0 the
+            // gradient is infinite but the splat never contributed (g' == 0): no gradient goes through rho there.
+            float cn[3];
+            conic_from<float>(S9, J, W, cn, nullptr);
+            rho = aa_rho(cn[0], cn[1], cn[2]);
+            const float A = cn[0] + 0.25f, C = cn[2] + 0.25f, bh = 0.5f * cn[1];
+            const float rd = 1.0f / (A * C - bh * bh);
+            const float k = (0.125f * gov * sigmoid_torch(opl)) * rd / rho * rd;
+            const float kr = rho > 0.0f ? k : 0.0f;
+            gcv[0] += kr * (cn[2] * C + bh * bh);
+            gcv[1] -= kr * bh * (A + C - 0.25f);
+            gcv[2] += kr * (cn[0] * A + bh * bh);
+        }
         const float gc[3] = {gcv[0], gcv[1], gcv[2]};
         float gS[9], gJ[6];
         conic_bwd<float>(S9, J, W, gc, gS, gJ);
@@ -380,6 +421,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
 #pragma unroll
         for (int k = 0; k < 3; ++k) gx[k] = W[0 + k] * gp[0] + W[3 + k] * gp[1] + W[6 + k] * gp[2];
         const float sg = sigmoid_torch(opl);
+        if (ANTIALIAS) gov *= rho;       // gradient on sigmoid(o)
         go = gov * ((1.0f - sg) * sg);  // torch sigmoid_backward: grad * (1 - y) * y
 
         const float gr[3] = {grv[0], grv[1], grv[2]};
@@ -444,11 +486,19 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
         g_uv_compact, scan, o_xyz, o_quat, o_scale, o_opa, o_dc, o_sh, use_tma
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB) k_preprocess_bwd(GSR_PRE_BWD_PARAMS) {
-    preprocess_bwd<N_SH, HAS_SH, false>(GSR_PRE_BWD_FORWARD);
+    preprocess_bwd<N_SH, HAS_SH, false, false>(GSR_PRE_BWD_FORWARD);
 }
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB) k_preprocess_bwd_depth(GSR_PRE_BWD_PARAMS) {
-    preprocess_bwd<N_SH, HAS_SH, true>(GSR_PRE_BWD_FORWARD);
+    preprocess_bwd<N_SH, HAS_SH, true, false>(GSR_PRE_BWD_FORWARD);
+}
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_AA_MINB) k_preprocess_bwd_aa(GSR_PRE_BWD_PARAMS) {
+    preprocess_bwd<N_SH, HAS_SH, false, true>(GSR_PRE_BWD_FORWARD);
+}
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_AA_MINB) k_preprocess_bwd_depth_aa(GSR_PRE_BWD_PARAMS) {
+    preprocess_bwd<N_SH, HAS_SH, true, true>(GSR_PRE_BWD_FORWARD);
 }
 #undef GSR_PRE_BWD_PARAMS
 #undef GSR_PRE_BWD_FORWARD
@@ -475,15 +525,18 @@ size_t gsr_preprocess_temp_bytes(int N) {
     return align256(b) + align256(sizeof(uint64_t) * (size_t)(N > 0 ? N : 1));
 }
 
-int gsr_preprocess_forward(int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
-                           int cam_first, const float* quaternion,
-                           const float* scale, const float* opacity_logit, const float* rgb_dc,
-                           const float* sh_rest, const float* camera_T_world, const float* K,
-                           const float* camera_centre, int H, int W, float near_thresh, float far_thresh,
-                           float cull_mask_padding, float mh_dist, uint32_t depth_base, float* records,
-                           uint32_t* depth_key,
-                           uint8_t* visible, uint64_t* scan, uint64_t* tile_mask, uint32_t* tile_win, void* temp,
-                           size_t temp_bytes, void* stream) {
+#define GSR_PRE_FWD_API_PARAMS                                                                                     \
+    int N, int n_sh_rest, const float *xyz, const float *xyz_camera_frame, int cam_first, const float *quaternion, \
+        const float *scale, const float *opacity_logit, const float *rgb_dc, const float *sh_rest,                 \
+        const float *camera_T_world, const float *K, const float *camera_centre, int H, int W, float near_thresh,  \
+        float far_thresh, float cull_mask_padding, float mh_dist, uint32_t depth_base, float *records,             \
+        uint32_t *depth_key, uint8_t *visible, uint64_t *scan, uint64_t *tile_mask, uint32_t *tile_win,            \
+        void *temp, size_t temp_bytes, void *stream
+#define GSR_PRE_FWD_API_FORWARD                                                                                      \
+    N, n_sh_rest, xyz, xyz_camera_frame, cam_first, quaternion, scale, opacity_logit, rgb_dc, sh_rest,               \
+        camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,     \
+        records, depth_key, visible, scan, tile_mask, tile_win, temp, temp_bytes, stream
+static int preprocess_forward(bool antialiased, GSR_PRE_FWD_API_PARAMS) {
     cudaStream_t st = (cudaStream_t)stream;
     if (N <= 0) return GSR_OK;
     if (temp_bytes < gsr_preprocess_temp_bytes(N)) return GSR_ERR_BAD_ARG;
@@ -499,12 +552,22 @@ int gsr_preprocess_forward(int N, int n_sh_rest, const float* xyz, const float* 
         camera_centre, (float)W, (float)H,                                                                 \
         near_thresh, far_thresh, cull_mask_padding, mh_dist, ntx, nty, depth_base, records, depth_key, visible, \
         packed, tile_mask, tile_win, use_tma
-    switch (n_sh_rest) {
-        case 0: k_preprocess_fwd<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        case 3: k_preprocess_fwd<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        case 8: k_preprocess_fwd<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        case 15: k_preprocess_fwd<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-        default: return GSR_ERR_UNSUPPORTED;
+    if (antialiased) {
+        switch (n_sh_rest) {
+            case 0: k_preprocess_fwd_aa<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 3: k_preprocess_fwd_aa<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 8: k_preprocess_fwd_aa<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 15: k_preprocess_fwd_aa<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            default: return GSR_ERR_UNSUPPORTED;
+        }
+    } else {
+        switch (n_sh_rest) {
+            case 0: k_preprocess_fwd<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 3: k_preprocess_fwd<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 8: k_preprocess_fwd<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            case 15: k_preprocess_fwd<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
+            default: return GSR_ERR_UNSUPPORTED;
+        }
     }
 #undef GSR_PRE_ARGS
     cudaError_t e = cub::DeviceScan::InclusiveSum(temp, scan_bytes, packed, scan, N, st);
@@ -512,7 +575,15 @@ int gsr_preprocess_forward(int N, int n_sh_rest, const float* xyz, const float* 
     return (int)cudaGetLastError();
 }
 
-static int preprocess_backward(bool depth, int N, int n_sh_rest, const float* xyz, const float* quaternion,
+int gsr_preprocess_forward(GSR_PRE_FWD_API_PARAMS) { return preprocess_forward(false, GSR_PRE_FWD_API_FORWARD); }
+
+int gsr_preprocess_forward_antialiased(GSR_PRE_FWD_API_PARAMS) {
+    return preprocess_forward(true, GSR_PRE_FWD_API_FORWARD);
+}
+#undef GSR_PRE_FWD_API_PARAMS
+#undef GSR_PRE_FWD_API_FORWARD
+
+static int preprocess_backward(bool depth, bool antialiased, int N, int n_sh_rest, const float* xyz, const float* quaternion,
                             const float* scale, const float* opacity_logit, const float* camera_T_world,
                             const float* K, const float* camera_centre, const uint8_t* visible,
                             const float* grad_rgb,
@@ -533,23 +604,24 @@ static int preprocess_backward(bool depth, int N, int n_sh_rest, const float* xy
     N, xyz, quaternion, scale, opacity_logit, camera_T_world, K, camera_centre, visible, grad_rgb,         \
         grad_opacity, grad_uv,                                                                             \
         grad_conic, grad_rows, use_rows_uv, grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, use_tma
-    if (depth) {
-        switch (n_sh_rest) {
-            case 0: k_preprocess_bwd_depth<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            case 3: k_preprocess_bwd_depth<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            case 8: k_preprocess_bwd_depth<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            case 15: k_preprocess_bwd_depth<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            default: return GSR_ERR_UNSUPPORTED;
-        }
-    } else {
-        switch (n_sh_rest) {
-            case 0: k_preprocess_bwd<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            case 3: k_preprocess_bwd<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            case 8: k_preprocess_bwd<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            case 15: k_preprocess_bwd<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
-            default: return GSR_ERR_UNSUPPORTED;
-        }
+#define GSR_PRE_BWD_SWITCH(kernel)                                                      \
+    switch (n_sh_rest) {                                                                \
+        case 0: kernel<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;          \
+        case 3: kernel<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;           \
+        case 8: kernel<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;           \
+        case 15: kernel<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;         \
+        default: return GSR_ERR_UNSUPPORTED;                                            \
     }
+    if (antialiased && depth) {
+        GSR_PRE_BWD_SWITCH(k_preprocess_bwd_depth_aa)
+    } else if (antialiased) {
+        GSR_PRE_BWD_SWITCH(k_preprocess_bwd_aa)
+    } else if (depth) {
+        GSR_PRE_BWD_SWITCH(k_preprocess_bwd_depth)
+    } else {
+        GSR_PRE_BWD_SWITCH(k_preprocess_bwd)
+    }
+#undef GSR_PRE_BWD_SWITCH
 #undef GSR_PRE_ARGS
     return (int)cudaGetLastError();
 }
@@ -561,7 +633,7 @@ int gsr_preprocess_backward(int N, int n_sh_rest, const float* xyz, const float*
                             const float* grad_rows, int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
                             float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
                             float* g_sh_rest, void* stream) {
-    return preprocess_backward(false, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
+    return preprocess_backward(false, false, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
                                camera_centre, visible, grad_rgb, grad_opacity, grad_uv, grad_conic, grad_rows,
                                use_rows_uv, grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit,
                                g_rgb_dc, g_sh_rest, stream);
@@ -574,8 +646,22 @@ int gsr_preprocess_backward_depth(int N, int n_sh_rest, const float* xyz, const 
                                   float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
                                   float* g_sh_rest, void* stream) {
     if (N > 0 && (grad_rows == nullptr || (reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0)) return GSR_ERR_BAD_ARG;
-    return preprocess_backward(true, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
+    return preprocess_backward(true, false, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
                                camera_centre, visible, nullptr, nullptr, nullptr, nullptr, grad_rows, use_rows_uv,
+                               grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc,
+                               g_sh_rest, stream);
+}
+
+int gsr_preprocess_backward_antialiased(int N, int n_sh_rest, const float* xyz, const float* quaternion,
+                                        const float* scale, const float* opacity_logit, const float* camera_T_world,
+                                        const float* K, const float* camera_centre, const uint8_t* visible,
+                                        const float* grad_rows, int depth, int use_rows_uv,
+                                        const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
+                                        float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                                        float* g_sh_rest, void* stream) {
+    if (N > 0 && (grad_rows == nullptr || (reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0)) return GSR_ERR_BAD_ARG;
+    return preprocess_backward(depth != 0, true, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world,
+                               K, camera_centre, visible, nullptr, nullptr, nullptr, nullptr, grad_rows, use_rows_uv,
                                grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc,
                                g_sh_rest, stream);
 }

@@ -46,6 +46,23 @@ __device__ __forceinline__ bool footprint_hits(const FootprintBounds& f, float d
     return (dx2 + dy2 <= f.r2) && (dx2 <= f.hx2) && (dy2 <= f.hy2);
 }
 
+// Anti-aliased mode: the opacity factor rho = sqrt(max(det0, 0) / det) that gives the dilated splat the mass of the
+// undilated one (det0 = det of the undilated 2-D covariance, det = det of the dilated one, as make_record forms it).
+// Pinned operation order; tests/antialiased_oracle.c reproduces it bit for bit:
+//   a = c0 + 1/4;  c = c2 + 1/4;  bh = c1 * 1/2;  bb = bh * bh
+//   det  = fma(a, c, -bb);  det0 = fma(c0, c2, -bb)
+//   rho  = sqrt_rn(div_rn(fmax(det0, 0), det))
+// rho == 0 where det0 <= 0 in fp32 (needles seen end-on, underflowing scales): the splat then never contributes.
+__device__ __forceinline__ float aa_rho(float c0, float c1, float c2) {
+    const float a = __fadd_rn(c0, 0.25f);
+    const float c = __fadd_rn(c2, 0.25f);
+    const float bh = __fmul_rn(c1, 0.5f);
+    const float bb = __fmul_rn(bh, bh);
+    const float det = __fmaf_rn(a, c, -bb);
+    const float det0 = __fmaf_rn(c0, c2, -bb);
+    return __fsqrt_rn(__fdiv_rn(fmaxf(det0, 0.0f), det));
+}
+
 __device__ __forceinline__ void make_record(float u, float v, float c0, float c1, float c2, float opa,
                                             float r, float g, float b, float* __restrict__ rec) {
     // a, b, c, det: src/render.cu:117-127 (fp32 branch: +0.25 dilation), rounding order of the reference build

@@ -415,7 +415,7 @@ fused_preprocess_forward_impl(
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles) {
+    bool with_tiles, bool antialiased = false) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc); CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -463,7 +463,8 @@ fused_preprocess_forward_impl(
     torch::Tensor tile_win = torch::empty({with_tiles ? N : 0}, opt.dtype(torch::kInt32));
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
-    check_rc(gsr_preprocess_forward(N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion), F32PTR(scale),
+    check_rc((antialiased ? gsr_preprocess_forward_antialiased : gsr_preprocess_forward)(
+                 N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion), F32PTR(scale),
                                     F32PTR(opacity_logit), F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world),
                                     F32PTR(K), centre_ptr, (int)H, (int)W, (float)near_thresh, (float)far_thresh,
                                     (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base, F32PTR(records),
@@ -472,7 +473,7 @@ fused_preprocess_forward_impl(
                                     with_tiles && N > 0 ? (uint64_t*)tile_mask.data_ptr<int64_t>() : nullptr,
                                     with_tiles && N > 0 ? (uint32_t*)tile_win.data_ptr<int>() : nullptr, temp.data_ptr(), tb,
                                     cur_stream()),
-             "gsr_preprocess_forward");
+             antialiased ? "gsr_preprocess_forward_antialiased" : "gsr_preprocess_forward");
     return std::make_tuple(records, zkey, visible, scan, tile_mask, tile_win);
 }
 
@@ -496,6 +497,18 @@ fused_preprocess_forward_tiles(
     return fused_preprocess_forward_impl(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
                                          camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh,
                                          cull_mask_padding, mh_dist, depth_base, true);
+}
+
+// fused_preprocess_forward_tiles with the anti-aliased opacity compensation (gsr_preprocess_forward_antialiased)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+fused_preprocess_forward_tiles_antialiased(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base) {
+    return fused_preprocess_forward_impl(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
+                                         camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh,
+                                         cull_mask_padding, mh_dist, depth_base, true, true);
 }
 
 // (M, P known) -> sorted gaussian ids [P] i32, tile ranges [n_tiles+1] i32, sorted record stream [P,12],
@@ -711,7 +724,8 @@ torch::Tensor fused_render_backward_depth(torch::Tensor grad_image, torch::Tenso
 // grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab [9N] (rows by gaussian).
 // grad_uv_compact [M,2] (optional): gradient on the compact uv, added to — or, with use_slab_uv false, replacing —
 // the slab's uv section.  depth: the slab is the rows of fused_render_backward_depth (slot 9 = gradient on z).
-static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, torch::Tensor slab, torch::Tensor xyz,
+// antialiased: the rows' opacity slot is the gradient on the compensated opacity (gsr_preprocess_backward_antialiased).
+static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, bool antialiased, torch::Tensor slab, torch::Tensor xyz,
                                                      torch::Tensor quaternion, torch::Tensor scale,
                                                      torch::Tensor opacity_logit,
                                                      c10::optional<torch::Tensor> sh_rest,
@@ -726,6 +740,7 @@ static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, torch::Te
     const bool rows = slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS && N > 0;  // interleaved [N,12] (else planar [9N])
     TORCH_CHECK(rows || slab.numel() == N * 9, "gradient slab must hold 9 (planar) or 12 (rows) floats per gaussian");
     TORCH_CHECK(!depth || rows || N == 0, "the depth/alpha backward needs the interleaved gradient rows");
+    TORCH_CHECK(!antialiased || rows || N == 0, "the anti-aliased backward needs the interleaved gradient rows");
     c10::cuda::CUDAGuard guard(xyz.device());
     auto opt = xyz.options();
     const float* g_rgb = slab.data_ptr<float>();
@@ -769,7 +784,16 @@ static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, torch::Te
                   o_o = section(3, {N}), o_dc = section(4, {N, 3});
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
-    if (depth) {
+    if (antialiased) {
+        check_rc(gsr_preprocess_backward_antialiased(
+                     (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit),
+                     F32PTR(camera_T_world), F32PTR(K),
+                     camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
+                     visible.data_ptr<uint8_t>(), N > 0 ? slab.data_ptr<float>() : nullptr, depth ? 1 : 0,
+                     use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s),
+                     F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr, cur_stream()),
+                 "gsr_preprocess_backward_antialiased");
+    } else if (depth) {
         check_rc(gsr_preprocess_backward_depth((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
                                                F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
                                                camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
@@ -801,12 +825,17 @@ static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, torch::Te
         c10::optional<torch::Tensor> out_flat, c10::optional<torch::Tensor> grad_uv_compact,                     \
         c10::optional<torch::Tensor> scan, bool use_slab_uv
 std::vector<torch::Tensor> fused_preprocess_backward(GSR_PREPROCESS_BWD_ARGS) {
-    return preprocess_backward_impl(false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
+    return preprocess_backward_impl(false, false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
                                     camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
 }
 std::vector<torch::Tensor> fused_preprocess_backward_depth(GSR_PREPROCESS_BWD_ARGS) {
-    return preprocess_backward_impl(true, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
+    return preprocess_backward_impl(true, false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
                                     camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
+}
+// depth: the rows of fused_render_backward_depth
+std::vector<torch::Tensor> fused_preprocess_backward_antialiased(GSR_PREPROCESS_BWD_ARGS, bool depth) {
+    return preprocess_backward_impl(depth, true, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world,
+                                    K, camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
 }
 #undef GSR_PREPROCESS_BWD_ARGS
 
@@ -1064,6 +1093,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "tile renderer backward (gather mode) with depth and alpha upstream gradients -> rows incl. z");
     m.def("fused_preprocess_backward_depth", &fused_preprocess_backward_depth,
           "fused per-gaussian backward from rows carrying the camera-frame z gradient");
+    m.def("fused_preprocess_forward_tiles_antialiased", &fused_preprocess_forward_tiles_antialiased,
+          "fused per-gaussian stage with the anti-aliased opacity compensation");
+    m.def("fused_preprocess_backward_antialiased", &fused_preprocess_backward_antialiased,
+          "fused per-gaussian backward of the anti-aliased stage (rows; depth: rows carrying the z gradient)");
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");

@@ -245,7 +245,7 @@ class _ViewState:
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges", "stream_rec", "gather",
                  "records", "keys_sorted", "id_bits", "slab_width",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
-                 "depth_alpha", "zkey", "depth_base", "depth_bits", "depth", "alpha")
+                 "depth_alpha", "zkey", "depth_base", "depth_bits", "depth", "alpha", "antialiased")
 
     @property
     def ids_sorted(self):
@@ -268,6 +268,7 @@ class _ViewState:
         self.speculation_overflowed = False
         self.depth_alpha = False  # render_depth_alpha: the tile kernels also produce depth / alpha [H,W,1]
         self.depth = self.alpha = None
+        self.antialiased = False  # opacity compensation for the 0.25 px^2 dilation (rasterize(antialiased=True))
 
 
 class _stage:
@@ -317,7 +318,10 @@ class _ProjectGaussians(torch.autograd.Function):
                 centre = torch.linalg.inv_ex(camera_T_world)[0][:3, 3].contiguous()
         with _stage(state, "preprocess_fwd"):
             # tile_mask / tile_win: the tiles each gaussian hits, tested once here and only expanded by the pair emission
-            records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward_tiles(
+            # antialiased: the records carry sigmoid(opacity) * rho (include/gsr_b200.h)
+            preprocess = (ext.fused_preprocess_forward_tiles_antialiased if state.antialiased
+                          else ext.fused_preprocess_forward_tiles)
+            records, zkey, visible, scan, tile_mask, tile_win = preprocess(
                 xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
                 pad, mh, depth_base)
         record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])  # a backward pass can follow
@@ -332,8 +336,9 @@ class _ProjectGaussians(torch.autograd.Function):
                                    "the int32 pair index of the native path (P must be < 2^31)")
             return M_, P_
 
-        # depth / alpha maps are rendered by the gather kernels only (they read z off the sorted pair keys)
-        gather = USE_RECORD_GATHER or state.depth_alpha
+        # depth / alpha maps are rendered by the gather kernels only (they read z off the sorted pair keys); the
+        # anti-aliased backward reads the interleaved gradient rows only the gather kernels write
+        gather = USE_RECORD_GATHER or state.depth_alpha or state.antialiased
 
         def bin_and_render(M_, P_, speculative):
             with _stage(state, "bin_sort_gather"):
@@ -422,9 +427,13 @@ class _ProjectGaussians(torch.autograd.Function):
             guv = grad_uv.contiguous()
         with _stage(st, "preprocess_bwd"):
             # depth/alpha mode: the rows also carry the render backward's gradient on camera-frame z (slot 9)
-            fn = native().fused_preprocess_backward_depth if st.depth_alpha else native().fused_preprocess_backward
-            grads = fn(slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible,
-                       st.grad_out, guv, st.scan if guv is not None else None, not st.uv_grad_emitted)
+            args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible,
+                    st.grad_out, guv, st.scan if guv is not None else None, not st.uv_grad_emitted)
+            if st.antialiased:   # the rows' opacity slot is the gradient on sigmoid(opacity) * rho
+                grads = native().fused_preprocess_backward_antialiased(*args, st.depth_alpha)
+            else:
+                fn = native().fused_preprocess_backward_depth if st.depth_alpha else native().fused_preprocess_backward
+                grads = fn(*args)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
@@ -494,12 +503,21 @@ def _render_grads(st, slab):
 
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
-              render_depth_alpha=False):
+              render_depth_alpha=False, antialiased=False):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
     colour, z_i the camera-frame z, with no background term (expected depth: depth / alpha.clamp_min(eps)).  fp32
-    and precomputed SH colours only; always on the fused gather kernels."""
+    and precomputed SH colours only; always on the fused gather kernels.
+
+    antialiased=True: every splat's opacity is multiplied by rho = sqrt(max(det S, 0) / det(S + 0.25 I)), S its 2-D
+    covariance, so that the 0.25 px^2 dilation the renderer applies no longer adds mass to splats smaller than a pixel
+    (the "antialiased" mode of Mip-Splatting's 2-D filter).  Gradients flow through rho to the covariance.  Return
+    values are unchanged; combines with render_depth_alpha.  fp32 and precomputed SH colours only."""
+    if antialiased and gaussians.xyz.dtype != torch.float32:
+        raise TypeError("antialiased needs fp32 inputs (the fp64 renderer applies no dilation to compensate)")
+    if antialiased and gaussians.sh is not None and not use_sh_precompute:
+        raise ValueError("antialiased needs use_sh_precompute=True (per-pixel SH colours are not supported)")
     if render_depth_alpha and gaussians.sh is not None and not use_sh_precompute:
         raise ValueError("render_depth_alpha needs use_sh_precompute=True (per-pixel SH colours are not supported)")
     if gaussians.sh is not None and not use_sh_precompute:
@@ -510,6 +528,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     state = _ViewState(profile)
     state.grad_out = grad_out
     state.depth_alpha = bool(render_depth_alpha)
+    state.antialiased = bool(antialiased)
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))

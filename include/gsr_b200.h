@@ -268,6 +268,20 @@ int gsr_preprocess_forward(int N, int n_sh_rest, const float* xyz, const float* 
                            uint32_t* depth_key,
                            uint8_t* visible, uint64_t* scan, uint64_t* tile_mask, uint32_t* tile_win, void* temp,
                            size_t temp_bytes, void* stream);
+/* Anti-aliased mode (Mip-Splatting's 2-D filter, "antialiased" rasterize mode): the same outputs, except that each
+ * record's opacity is sigmoid(opacity_logit) * rho with
+ *   rho = sqrt(max(det0, 0) / det),  det0 = det of the 2-D covariance, det = det of the covariance + 0.25 I
+ * (the +0.25 px^2 dilation the tile renderers apply), so the dilated splat carries the mass of the undilated one.
+ * The culling bound is formed from the compensated opacity.  rho == 0 where det0 <= 0 in fp32: the splat then never
+ * contributes.  Operation order: gsr_record.cuh aa_rho. */
+int gsr_preprocess_forward_antialiased(int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
+                                       int cam_first, const float* quaternion, const float* scale,
+                                       const float* opacity_logit, const float* rgb_dc, const float* sh_rest,
+                                       const float* camera_T_world, const float* K, const float* camera_centre, int H,
+                                       int W, float near_thresh, float far_thresh, float cull_mask_padding,
+                                       float mh_dist, uint32_t depth_base, float* records, uint32_t* depth_key,
+                                       uint8_t* visible, uint64_t* scan, uint64_t* tile_mask, uint32_t* tile_win,
+                                       void* temp, size_t temp_bytes, void* stream);
 
 /* emits the (tile, depth) keys and original-gaussian ids of all P pairs, the compact list of
  * visible gaussian ids vis_idx int32 [M] and the compacted uv [M,2] the reference returns */
@@ -337,6 +351,18 @@ int gsr_preprocess_backward_depth(int N, int n_sh_rest, const float* xyz, const 
                                   int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
                                   float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
                                   float* g_sh_rest, void* stream);
+/* Backward of gsr_preprocess_forward_antialiased from interleaved rows (grad_rows required, 16-byte aligned; depth != 0:
+ * the rows of gsr_render_backward_gather_depth, slot 9 carrying the z gradient, as in gsr_preprocess_backward_depth).
+ * The rows' opacity slot g is the gradient on the compensated opacity sigmoid(o) * rho: sigmoid(o) receives g * rho
+ * and the 2-D covariance g * sigmoid(o) * grad(rho).  Where rho == 0 no gradient goes through rho (its gradient is
+ * infinite there, and g is 0 because the splat never contributed). */
+int gsr_preprocess_backward_antialiased(int N, int n_sh_rest, const float* xyz, const float* quaternion,
+                                        const float* scale, const float* opacity_logit, const float* camera_T_world,
+                                        const float* K, const float* camera_centre, const uint8_t* visible,
+                                        const float* grad_rows, int depth, int use_rows_uv,
+                                        const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
+                                        float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                                        float* g_sh_rest, void* stream);
 
 /* ---- optimizer step on the flat parameter buffer (SURVEY.md 8(f) rank 2) ----------------------------
  * Replaces torch.optim.Adam.step() as configured by splat_py/optimizer_manager.py:13-44 (one parameter group

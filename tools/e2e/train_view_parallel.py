@@ -53,6 +53,9 @@ def main():
                     help="shim: L1 + the SSIM stand-in through permuted NCHW views, like run_trainer.py's reference arm; "
                          "fused: gaussian_splatting_b200.loss.photometric_loss in the step and its ssim() in evaluate() "
                          "(one forward and one backward kernel)")
+    ap.add_argument("--antialiased", action="store_true",
+                    help="rasterize(antialiased=True): opacity compensation for the 0.25 px^2 dilation, in training and "
+                         "evaluation")
     a = ap.parse_args()
 
     real_stdout = os.fdopen(os.dup(1), "w")
@@ -165,7 +168,7 @@ def main():
                 im = images[int(t)]
                 pred, _, _ = rasterize(g, im.camera_T_world, cams[im.camera_id], config.near_thresh, config.far_thresh,
                                        config.cull_mask_padding, config.mh_dist, config.use_sh_precompute,
-                                       torch.zeros(3, device=dev))
+                                       torch.zeros(3, device=dev), antialiased=a.antialiased)
                 l2 = torch.nn.functional.mse_loss(pred.clip(0, 1), im.image)
                 psnrs.append(-10 * torch.log10(l2).item())
                 if a.loss == "fused":
@@ -204,7 +207,7 @@ def main():
         image, mask, uv, state = rasterize(g, im.camera_T_world, cams[im.camera_id], config.near_thresh,
                                            config.far_thresh, config.cull_mask_padding, config.mh_dist,
                                            config.use_sh_precompute, background, return_state=True,
-                                           grad_out=grads_sym)
+                                           grad_out=grads_sym, antialiased=a.antialiased)
         uv.retain_grad()
         if timed:
             ev[1].record()
@@ -275,6 +278,7 @@ def main():
                           if world > 1 else "FlatAdam (gsr_adam_step)"),
             "loss": ("fused: photometric_loss (gsr_photometric_loss_forward / _backward), ssim() in evaluation"
                      if a.loss == "fused" else "shim: l1_loss + SSIM stand-in (tools/e2e/shims) through NCHW views"),
+            "antialiased": a.antialiased,
             "device": torch.cuda.get_device_name(local),
         }
         real_stdout.write("E2E " + json.dumps(line) + "\n")
