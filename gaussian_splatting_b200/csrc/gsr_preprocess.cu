@@ -507,6 +507,8 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 
 static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
+constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED;
+
 }  // namespace gsr
 
 using namespace gsr;
@@ -525,19 +527,15 @@ size_t gsr_preprocess_temp_bytes(int N) {
     return align256(b) + align256(sizeof(uint64_t) * (size_t)(N > 0 ? N : 1));
 }
 
-#define GSR_PRE_FWD_API_PARAMS                                                                                     \
-    int N, int n_sh_rest, const float *xyz, const float *xyz_camera_frame, int cam_first, const float *quaternion, \
-        const float *scale, const float *opacity_logit, const float *rgb_dc, const float *sh_rest,                 \
-        const float *camera_T_world, const float *K, const float *camera_centre, int H, int W, float near_thresh,  \
-        float far_thresh, float cull_mask_padding, float mh_dist, uint32_t depth_base, float *records,             \
-        uint32_t *depth_key, uint8_t *visible, uint64_t *scan, uint64_t *tile_mask, uint32_t *tile_win,            \
-        void *temp, size_t temp_bytes, void *stream
-#define GSR_PRE_FWD_API_FORWARD                                                                                      \
-    N, n_sh_rest, xyz, xyz_camera_frame, cam_first, quaternion, scale, opacity_logit, rgb_dc, sh_rest,               \
-        camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,     \
-        records, depth_key, visible, scan, tile_mask, tile_win, temp, temp_bytes, stream
-static int preprocess_forward(bool antialiased, GSR_PRE_FWD_API_PARAMS) {
+int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
+                           int cam_first, const float* quaternion, const float* scale, const float* opacity_logit,
+                           const float* rgb_dc, const float* sh_rest, const float* camera_T_world, const float* K,
+                           const float* camera_centre, int H, int W, float near_thresh, float far_thresh,
+                           float cull_mask_padding, float mh_dist, uint32_t depth_base, float* records,
+                           uint32_t* depth_key, uint8_t* visible, uint64_t* scan, uint64_t* tile_mask,
+                           uint32_t* tile_win, void* temp, size_t temp_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
+    if ((mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
     if (N <= 0) return GSR_OK;
     if (temp_bytes < gsr_preprocess_temp_bytes(N)) return GSR_ERR_BAD_ARG;
     if ((tile_mask == nullptr) != (tile_win == nullptr)) return GSR_ERR_BAD_ARG;
@@ -552,7 +550,7 @@ static int preprocess_forward(bool antialiased, GSR_PRE_FWD_API_PARAMS) {
         camera_centre, (float)W, (float)H,                                                                 \
         near_thresh, far_thresh, cull_mask_padding, mh_dist, ntx, nty, depth_base, records, depth_key, visible, \
         packed, tile_mask, tile_win, use_tma
-    if (antialiased) {
+    if (mode & GSR_MODE_ANTIALIASED) {
         switch (n_sh_rest) {
             case 0: k_preprocess_fwd_aa<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
             case 3: k_preprocess_fwd_aa<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
@@ -575,24 +573,18 @@ static int preprocess_forward(bool antialiased, GSR_PRE_FWD_API_PARAMS) {
     return (int)cudaGetLastError();
 }
 
-int gsr_preprocess_forward(GSR_PRE_FWD_API_PARAMS) { return preprocess_forward(false, GSR_PRE_FWD_API_FORWARD); }
-
-int gsr_preprocess_forward_antialiased(GSR_PRE_FWD_API_PARAMS) {
-    return preprocess_forward(true, GSR_PRE_FWD_API_FORWARD);
-}
-#undef GSR_PRE_FWD_API_PARAMS
-#undef GSR_PRE_FWD_API_FORWARD
-
-static int preprocess_backward(bool depth, bool antialiased, int N, int n_sh_rest, const float* xyz, const float* quaternion,
+int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
                             const float* scale, const float* opacity_logit, const float* camera_T_world,
-                            const float* K, const float* camera_centre, const uint8_t* visible,
-                            const float* grad_rgb,
+                            const float* K, const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
                             const float* grad_opacity, const float* grad_uv, const float* grad_conic,
-                            const float* grad_rows, int use_rows_uv,
-                            const float* grad_uv_compact, const uint64_t* scan, float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit,
-                            float* g_rgb_dc, float* g_sh_rest, void* stream) {
+                            const float* grad_rows, int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
+                            float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                            float* g_sh_rest, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
+    if ((mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
     if (N <= 0) return GSR_OK;
+    // the depth/alpha and anti-aliased kernels read the render backward's sums from the interleaved rows only
+    if (mode != 0 && (grad_rows == nullptr || !aligned16(grad_rows))) return GSR_ERR_BAD_ARG;
     if (grad_uv_compact != nullptr && scan == nullptr) return GSR_ERR_BAD_ARG;
     const dim3 grid((N + PRE_THREADS - 1) / PRE_THREADS), block(PRE_THREADS);
     const int use_tma = (aligned16(g_xyz) && aligned16(g_quaternion) && aligned16(g_scale) &&
@@ -612,6 +604,7 @@ static int preprocess_backward(bool depth, bool antialiased, int N, int n_sh_res
         case 15: kernel<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;         \
         default: return GSR_ERR_UNSUPPORTED;                                            \
     }
+    const bool depth = (mode & GSR_MODE_DEPTH_ALPHA) != 0, antialiased = (mode & GSR_MODE_ANTIALIASED) != 0;
     if (antialiased && depth) {
         GSR_PRE_BWD_SWITCH(k_preprocess_bwd_depth_aa)
     } else if (antialiased) {
@@ -624,46 +617,6 @@ static int preprocess_backward(bool depth, bool antialiased, int N, int n_sh_res
 #undef GSR_PRE_BWD_SWITCH
 #undef GSR_PRE_ARGS
     return (int)cudaGetLastError();
-}
-
-int gsr_preprocess_backward(int N, int n_sh_rest, const float* xyz, const float* quaternion, const float* scale,
-                            const float* opacity_logit, const float* camera_T_world, const float* K,
-                            const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
-                            const float* grad_opacity, const float* grad_uv, const float* grad_conic,
-                            const float* grad_rows, int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
-                            float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
-                            float* g_sh_rest, void* stream) {
-    return preprocess_backward(false, false, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
-                               camera_centre, visible, grad_rgb, grad_opacity, grad_uv, grad_conic, grad_rows,
-                               use_rows_uv, grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit,
-                               g_rgb_dc, g_sh_rest, stream);
-}
-
-int gsr_preprocess_backward_depth(int N, int n_sh_rest, const float* xyz, const float* quaternion, const float* scale,
-                                  const float* opacity_logit, const float* camera_T_world, const float* K,
-                                  const float* camera_centre, const uint8_t* visible, const float* grad_rows,
-                                  int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
-                                  float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
-                                  float* g_sh_rest, void* stream) {
-    if (N > 0 && (grad_rows == nullptr || (reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0)) return GSR_ERR_BAD_ARG;
-    return preprocess_backward(true, false, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world, K,
-                               camera_centre, visible, nullptr, nullptr, nullptr, nullptr, grad_rows, use_rows_uv,
-                               grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc,
-                               g_sh_rest, stream);
-}
-
-int gsr_preprocess_backward_antialiased(int N, int n_sh_rest, const float* xyz, const float* quaternion,
-                                        const float* scale, const float* opacity_logit, const float* camera_T_world,
-                                        const float* K, const float* camera_centre, const uint8_t* visible,
-                                        const float* grad_rows, int depth, int use_rows_uv,
-                                        const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
-                                        float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
-                                        float* g_sh_rest, void* stream) {
-    if (N > 0 && (grad_rows == nullptr || (reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0)) return GSR_ERR_BAD_ARG;
-    return preprocess_backward(depth != 0, true, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, camera_T_world,
-                               K, camera_centre, visible, nullptr, nullptr, nullptr, nullptr, grad_rows, use_rows_uv,
-                               grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc,
-                               g_sh_rest, stream);
 }
 
 }  // extern "C"

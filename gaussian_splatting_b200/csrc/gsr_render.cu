@@ -1285,87 +1285,6 @@ static RecSource make_source(const float* base, const uint64_t* keys, const int3
     return src;
 }
 
-template <bool GATHER>
-static int launch_forward(const RecSource& src, const int32_t* ranges, const float* background, int H, int W,
-                          int32_t* n_out, float* w_out, float* image, uint32_t* masks, void* stream) {
-    if (H <= 0 || W <= 0) return GSR_ERR_BAD_ARG;
-    const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
-    if (masks != nullptr)
-        k_render_fwd<true, GATHER><<<grid, block, 0, (cudaStream_t)stream>>>(src, ranges, background, W, H, n_out, w_out,
-                                                                             image, masks);
-    else
-        k_render_fwd<false, GATHER><<<grid, block, 0, (cudaStream_t)stream>>>(src, ranges, background, W, H, n_out,
-                                                                              w_out, image, nullptr);
-    return (int)cudaGetLastError();
-}
-
-template <bool GATHER>
-static int launch_backward(const RecSource& src, const int32_t* sorted_idx, const int32_t* ranges,
-                           const float* background, int H, int W, const int32_t* n_in, const float* w_in,
-                           const float* grad_image, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
-                           const uint32_t* masks, void* stream) {
-    if (H <= 0 || W <= 0) return GSR_ERR_BAD_ARG;
-    const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
-    if (masks != nullptr)
-        k_render_bwd<true, GATHER><<<grid, block, 0, (cudaStream_t)stream>>>(src, sorted_idx, ranges, background, W, H,
-                                                                             n_in, w_in, grad_image, g_rgb, g_opa, g_uv,
-                                                                             g_conic, masks);
-    else
-        k_render_bwd<false, GATHER><<<grid, block, 0, (cudaStream_t)stream>>>(src, sorted_idx, ranges, background, W, H,
-                                                                              n_in, w_in, grad_image, g_rgb, g_opa, g_uv,
-                                                                              g_conic, nullptr);
-    return (int)cudaGetLastError();
-}
-
-extern "C" {
-
-size_t gsr_contribution_mask_words(int64_t P, int H, int W) {
-    if (P < 0 || H <= 0 || W <= 0) return 0;
-    const int64_t n_tiles = (int64_t)((W + TILE - 1) / TILE) * ((H + TILE - 1) / TILE);
-    return (size_t)(P / BATCH + n_tiles + 1) * MASK_WORDS_PER_SLOT;
-}
-
-int gsr_render_forward(const float* records, const int32_t* ranges, const float* background, int H, int W,
-                       int32_t* n_out, float* w_out, float* image, uint32_t* contribution_masks, void* stream) {
-    return launch_forward<false>(make_source(records, nullptr, nullptr, 0), ranges, background, H, W, n_out, w_out,
-                                 image, contribution_masks, stream);
-}
-
-int gsr_render_backward(const float* records, const int32_t* sorted_idx, const int32_t* ranges,
-                        const float* background, int H, int W, const int32_t* n_in, const float* w_in,
-                        const float* grad_image, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
-                        const uint32_t* contribution_masks, void* stream) {
-    return launch_backward<false>(make_source(records, nullptr, nullptr, 0), sorted_idx, ranges, background, H, W, n_in,
-                                  w_in, grad_image, g_rgb, g_opa, g_uv, g_conic, contribution_masks, stream);
-}
-
-int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                              const int32_t* ids_sorted, const int32_t* ranges, const float* background, int H, int W,
-                              int32_t* n_out, float* w_out, float* image, uint32_t* contribution_masks,
-                              void* stream) {
-    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;  // exactly one id source
-    return launch_forward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits), ranges, background, H,
-                                W, n_out, w_out, image, contribution_masks, stream);
-}
-
-int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                               const int32_t* ids_sorted, const int32_t* ranges, const float* background, int H,
-                               int W, const int32_t* n_in, const float* w_in, const float* grad_image, float* g_rgb,
-                               float* g_opa, float* g_uv, float* g_conic, float* grad_rows,
-                               const uint32_t* contribution_masks, void* stream) {
-    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;
-    if (grad_rows != nullptr) {  // interleaved rows: the kernel sees them as g_rgb with the other three NULL
-        if ((reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0) return GSR_ERR_BAD_ARG;
-        g_rgb = grad_rows;
-        g_opa = g_uv = g_conic = nullptr;
-    } else if (g_rgb == nullptr || g_opa == nullptr || g_uv == nullptr || g_conic == nullptr) {
-        return GSR_ERR_BAD_ARG;
-    }
-    return launch_backward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits), nullptr, ranges,
-                                 background, H, W, n_in, w_in, grad_image, g_rgb, g_opa, g_uv, g_conic,
-                                 contribution_masks, stream);
-}
-
 // the sort-key depth field of the pair list (or the per-gaussian depth keys, sorted id array): see DepthSource
 static bool make_depth_source(const uint64_t* keys_sorted, int id_bits, const uint32_t* depth_key,
                               uint32_t depth_base, int depth_bits, DepthSource& ds) {
@@ -1380,49 +1299,119 @@ static bool make_depth_source(const uint64_t* keys_sorted, int id_bits, const ui
     return true;
 }
 
-int gsr_render_forward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                                    const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
-                                    int depth_bits, const int32_t* ranges, const float* background, int H, int W,
-                                    int32_t* n_out, float* w_out, float* image, float* depth, float* alpha,
-                                    uint32_t* contribution_masks, void* stream) {
-    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;
-    if (H <= 0 || W <= 0 || depth == nullptr || alpha == nullptr) return GSR_ERR_BAD_ARG;
-    DepthSource ds;
-    if (!make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds)) return GSR_ERR_BAD_ARG;
-    const RecSource src = make_source(gaussian_records, keys_sorted, ids_sorted, id_bits);
+// ds != nullptr: the depth/alpha kernels (gather mode only)
+template <bool GATHER>
+static int launch_forward(const RecSource& src, const DepthSource* ds, const int32_t* ranges, const float* background,
+                          int H, int W, int32_t* n_out, float* w_out, float* image, float* depth, float* alpha,
+                          uint32_t* masks, void* stream) {
+    if (H <= 0 || W <= 0) return GSR_ERR_BAD_ARG;
     const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
-    if (contribution_masks != nullptr)
-        k_render_fwd_depth<true><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_out,
-                                                                          w_out, image, depth, alpha,
-                                                                          contribution_masks);
-    else
-        k_render_fwd_depth<false><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_out,
-                                                                           w_out, image, depth, alpha, nullptr);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (ds != nullptr) {
+        if (masks != nullptr)
+            k_render_fwd_depth<true><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_out, w_out, image,
+                                                             depth, alpha, masks);
+        else
+            k_render_fwd_depth<false><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_out, w_out, image,
+                                                              depth, alpha, nullptr);
+    } else if (masks != nullptr) {
+        k_render_fwd<true, GATHER><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image, masks);
+    } else {
+        k_render_fwd<false, GATHER><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image,
+                                                            nullptr);
+    }
     return (int)cudaGetLastError();
 }
 
-int gsr_render_backward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                                     const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
-                                     int depth_bits, const int32_t* ranges, const float* background, int H, int W,
-                                     const int32_t* n_in, const float* w_in, const float* grad_image,
-                                     const float* grad_depth, const float* grad_alpha, float* grad_rows,
-                                     const uint32_t* contribution_masks, void* stream) {
-    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;
-    if (H <= 0 || W <= 0 || grad_image == nullptr || grad_depth == nullptr || grad_alpha == nullptr) return GSR_ERR_BAD_ARG;
-    if (grad_rows == nullptr || (reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0) return GSR_ERR_BAD_ARG;
-    DepthSource ds;
-    if (!make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds)) return GSR_ERR_BAD_ARG;
-    const RecSource src = make_source(gaussian_records, keys_sorted, ids_sorted, id_bits);
+// ds != nullptr: the depth/alpha kernels (gather mode only; the gradients go to interleaved rows, passed as g_rgb)
+template <bool GATHER>
+static int launch_backward(const RecSource& src, const DepthSource* ds, const int32_t* sorted_idx,
+                           const int32_t* ranges, const float* background, int H, int W, const int32_t* n_in,
+                           const float* w_in, const float* grad_image, const float* grad_depth,
+                           const float* grad_alpha, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
+                           const uint32_t* masks, void* stream) {
+    if (H <= 0 || W <= 0) return GSR_ERR_BAD_ARG;
     const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
-    if (contribution_masks != nullptr)
-        k_render_bwd_depth<true><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_in,
-                                                                          w_in, grad_image, grad_depth, grad_alpha,
-                                                                          grad_rows, contribution_masks);
-    else
-        k_render_bwd_depth<false><<<grid, block, 0, (cudaStream_t)stream>>>(src, ds, ranges, background, W, H, n_in,
-                                                                           w_in, grad_image, grad_depth, grad_alpha,
-                                                                           grad_rows, nullptr);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (ds != nullptr) {
+        if (masks != nullptr)
+            k_render_bwd_depth<true><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_in, w_in,
+                                                             grad_image, grad_depth, grad_alpha, g_rgb, masks);
+        else
+            k_render_bwd_depth<false><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_in, w_in,
+                                                              grad_image, grad_depth, grad_alpha, g_rgb, nullptr);
+    } else if (masks != nullptr) {
+        k_render_bwd<true, GATHER><<<grid, block, 0, st>>>(src, sorted_idx, ranges, background, W, H, n_in, w_in,
+                                                           grad_image, g_rgb, g_opa, g_uv, g_conic, masks);
+    } else {
+        k_render_bwd<false, GATHER><<<grid, block, 0, st>>>(src, sorted_idx, ranges, background, W, H, n_in, w_in,
+                                                            grad_image, g_rgb, g_opa, g_uv, g_conic, nullptr);
+    }
     return (int)cudaGetLastError();
+}
+
+extern "C" {
+
+size_t gsr_contribution_mask_words(int64_t P, int H, int W) {
+    if (P < 0 || H <= 0 || W <= 0) return 0;
+    const int64_t n_tiles = (int64_t)((W + TILE - 1) / TILE) * ((H + TILE - 1) / TILE);
+    return (size_t)(P / BATCH + n_tiles + 1) * MASK_WORDS_PER_SLOT;
+}
+
+int gsr_render_forward(const float* records, const int32_t* ranges, const float* background, int H, int W,
+                       int32_t* n_out, float* w_out, float* image, uint32_t* contribution_masks, void* stream) {
+    return launch_forward<false>(make_source(records, nullptr, nullptr, 0), nullptr, ranges, background, H, W, n_out,
+                                 w_out, image, nullptr, nullptr, contribution_masks, stream);
+}
+
+int gsr_render_backward(const float* records, const int32_t* sorted_idx, const int32_t* ranges,
+                        const float* background, int H, int W, const int32_t* n_in, const float* w_in,
+                        const float* grad_image, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
+                        const uint32_t* contribution_masks, void* stream) {
+    return launch_backward<false>(make_source(records, nullptr, nullptr, 0), nullptr, sorted_idx, ranges, background,
+                                  H, W, n_in, w_in, grad_image, nullptr, nullptr, g_rgb, g_opa, g_uv, g_conic,
+                                  contribution_masks, stream);
+}
+
+int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                              const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base, int depth_bits,
+                              const int32_t* ranges, const float* background, int H, int W, int32_t* n_out,
+                              float* w_out, float* image, float* depth, float* alpha, uint32_t* contribution_masks,
+                              void* stream) {
+    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;  // exactly one id source
+    if ((depth == nullptr) != (alpha == nullptr)) return GSR_ERR_BAD_ARG;
+    DepthSource ds;
+    if (depth != nullptr && !make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds))
+        return GSR_ERR_BAD_ARG;
+    return launch_forward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
+                                depth != nullptr ? &ds : nullptr, ranges, background, H, W, n_out, w_out, image, depth,
+                                alpha, contribution_masks, stream);
+}
+
+int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                               const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                               int depth_bits, const int32_t* ranges, const float* background, int H, int W,
+                               const int32_t* n_in, const float* w_in, const float* grad_image,
+                               const float* grad_depth, const float* grad_alpha, float* g_rgb, float* g_opa,
+                               float* g_uv, float* g_conic, float* grad_rows, const uint32_t* contribution_masks,
+                               void* stream) {
+    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;
+    if (grad_image == nullptr || (grad_depth == nullptr) != (grad_alpha == nullptr)) return GSR_ERR_BAD_ARG;
+    DepthSource ds;
+    if (grad_depth != nullptr &&
+        (grad_rows == nullptr || !make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds)))
+        return GSR_ERR_BAD_ARG;
+    if (grad_rows != nullptr) {  // interleaved rows: the kernel sees them as g_rgb with the other three NULL
+        if ((reinterpret_cast<uintptr_t>(grad_rows) & 15u) != 0) return GSR_ERR_BAD_ARG;
+        g_rgb = grad_rows;
+        g_opa = g_uv = g_conic = nullptr;
+    } else if (g_rgb == nullptr || g_opa == nullptr || g_uv == nullptr || g_conic == nullptr) {
+        return GSR_ERR_BAD_ARG;
+    }
+    return launch_backward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
+                                 grad_depth != nullptr ? &ds : nullptr, nullptr, ranges, background, H, W, n_in, w_in,
+                                 grad_image, grad_depth, grad_alpha, g_rgb, g_opa, g_uv, g_conic, contribution_masks,
+                                 stream);
 }
 
 const char* gsr_version(void) { return "gsr_b200 0.1 sm_90a"; }

@@ -407,15 +407,14 @@ void render_depth_cuda(torch::Tensor xyz_camera_frame, torch::Tensor uvs, torch:
 // ---------------------------------------------------------------------------------------------
 #define F32PTR(t) ((t).data_ptr<float>())
 
-// returns (records[N,12], depth_key[N] i32-viewed u32, visible[N] u8, scan[N] i64-viewed u64)
-// returns (records, depth_key, visible, scan, tile_mask, tile_win); the last two are empty unless with_tiles
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-fused_preprocess_forward_impl(
+// returns [records [N,12], depth_key [N] i32-viewed u32, visible [N] u8, scan [N] i64-viewed u64] and, with_tiles,
+// also [tile_mask [N] i64-viewed u64, tile_win [N] i32-viewed u32].  mode: GSR_MODE_* bits
+std::vector<torch::Tensor> fused_preprocess_forward(
     torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, bool antialiased = false) {
+    bool with_tiles, int64_t mode) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc); CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -463,9 +462,8 @@ fused_preprocess_forward_impl(
     torch::Tensor tile_win = torch::empty({with_tiles ? N : 0}, opt.dtype(torch::kInt32));
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
-    check_rc((antialiased ? gsr_preprocess_forward_antialiased : gsr_preprocess_forward)(
-                 N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion), F32PTR(scale),
-                                    F32PTR(opacity_logit), F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world),
+    check_rc(gsr_preprocess_forward((int)mode, N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion),
+                                    F32PTR(scale), F32PTR(opacity_logit), F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world),
                                     F32PTR(K), centre_ptr, (int)H, (int)W, (float)near_thresh, (float)far_thresh,
                                     (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base, F32PTR(records),
                                     (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),
@@ -473,42 +471,9 @@ fused_preprocess_forward_impl(
                                     with_tiles && N > 0 ? (uint64_t*)tile_mask.data_ptr<int64_t>() : nullptr,
                                     with_tiles && N > 0 ? (uint32_t*)tile_win.data_ptr<int>() : nullptr, temp.data_ptr(), tb,
                                     cur_stream()),
-             antialiased ? "gsr_preprocess_forward_antialiased" : "gsr_preprocess_forward");
-    return std::make_tuple(records, zkey, visible, scan, tile_mask, tile_win);
-}
-
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> fused_preprocess_forward(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base) {
-    auto r = fused_preprocess_forward_impl(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
-                                           camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh,
-                                           cull_mask_padding, mh_dist, depth_base, false);
-    return std::make_tuple(std::get<0>(r), std::get<1>(r), std::get<2>(r), std::get<3>(r));
-}
-
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-fused_preprocess_forward_tiles(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base) {
-    return fused_preprocess_forward_impl(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
-                                         camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh,
-                                         cull_mask_padding, mh_dist, depth_base, true);
-}
-
-// fused_preprocess_forward_tiles with the anti-aliased opacity compensation (gsr_preprocess_forward_antialiased)
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-fused_preprocess_forward_tiles_antialiased(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base) {
-    return fused_preprocess_forward_impl(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
-                                         camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh,
-                                         cull_mask_padding, mh_dist, depth_base, true, true);
+             "gsr_preprocess_forward");
+    if (!with_tiles) return {records, zkey, visible, scan};
+    return {records, zkey, visible, scan, tile_mask, tile_win};
 }
 
 // (M, P known) -> sorted gaussian ids [P] i32, tile ranges [n_tiles+1] i32, sorted record stream [P,12],
@@ -586,54 +551,93 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
                            uv, keys_sorted, (int64_t)id_bits);
 }
 
-// image [H,W,3], n [H,W] i32, wlast [H,W], contribution masks (i32 words; empty when record_masks is false)
-// records: the record stream [P,12] — or, when keys_sorted / ids_sorted name the sorted pair list (gather mode), the
-// per-gaussian record array [N,12]
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor> fused_render_forward(
-    torch::Tensor stream_rec, torch::Tensor ranges, torch::Tensor background, int64_t H, int64_t W, int64_t P,
-    bool record_masks, c10::optional<torch::Tensor> keys_sorted, c10::optional<torch::Tensor> ids_sorted,
-    int64_t id_bits, bool gather) {
+// The sorted pair list the gather kernels read record ids through: the keys when the id rides in them, else the sorted
+// id array.  An empty view (P == 0) may have neither (the key/value fallback narrows its id array to nothing); the
+// kernels still run, to write the background, and read no pair: any well-formed source will do.
+struct PairSource {
+    const uint64_t* keys;
+    const int32_t* ids;
+};
+PairSource pair_source(const c10::optional<torch::Tensor>& keys_sorted, const c10::optional<torch::Tensor>& ids_sorted,
+                       int64_t P) {
+    static const int32_t no_pair = 0;
+    if (keys_sorted.has_value() && keys_sorted->numel() > 0)
+        return {(const uint64_t*)keys_sorted->data_ptr<int64_t>(), nullptr};
+    if (ids_sorted.has_value() && ids_sorted->numel() > 0) return {nullptr, ids_sorted->data_ptr<int>()};
+    TORCH_CHECK(P == 0, "gather mode needs the sorted pair list");
+    return {nullptr, &no_pair};
+}
+
+// returns (image [H,W,3], n [H,W] i32, wlast [H,W], contribution masks (i32 words; empty when record_masks is false),
+// depth [H,W,1], alpha [H,W,1]); depth and alpha are None unless depth_key (the per-gaussian depth keys of the forward,
+// read when the pair list is a sorted id array) asks for the depth/alpha kernels.
+// records: the record stream [P,12] — or, in gather mode, the per-gaussian record array [N,12] read through the sorted
+// pair list keys_sorted / ids_sorted
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
+fused_render_forward(torch::Tensor records, torch::Tensor ranges, torch::Tensor background, int64_t H, int64_t W,
+                     int64_t P, bool record_masks, c10::optional<torch::Tensor> keys_sorted,
+                     c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, bool gather,
+                     c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits) {
     CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
     TORCH_CHECK(background.numel() == 3, "Background RGB must have 3 elements");
-    c10::cuda::CUDAGuard guard(stream_rec.device());
-    auto opt = stream_rec.options();
+    TORCH_CHECK(gather || !depth_key.has_value(), "depth and alpha maps come from the gather kernels only");
+    c10::cuda::CUDAGuard guard(records.device());
+    auto opt = records.options();
     torch::Tensor image = torch::empty({H, W, 3}, opt);
     torch::Tensor n = torch::empty({H, W}, opt.dtype(torch::kInt32));
     torch::Tensor w = torch::empty({H, W}, opt);
+    torch::Tensor depth, alpha;
+    if (depth_key.has_value()) {
+        depth = torch::empty({H, W, 1}, opt);
+        alpha = torch::empty({H, W, 1}, opt);
+    }
     torch::Tensor masks = record_masks
                               ? torch::zeros({(int64_t)gsr_contribution_mask_words(P, (int)H, (int)W)}, opt.dtype(torch::kInt32))
                               : torch::empty({0}, opt.dtype(torch::kInt32));
     uint32_t* mptr = record_masks ? (uint32_t*)masks.data_ptr<int>() : nullptr;
     if (gather) {
-        const bool by_key = keys_sorted.has_value() && keys_sorted->numel() > 0;
-        TORCH_CHECK(by_key || (ids_sorted.has_value() && ids_sorted->numel() > 0) || P == 0, "gather mode needs the sorted pair list");
-        check_rc(gsr_render_forward_gather(F32PTR(stream_rec),
-                                           by_key ? (const uint64_t*)keys_sorted->data_ptr<int64_t>() : nullptr, (int)id_bits,
-                                           (!by_key && ids_sorted.has_value() && ids_sorted->numel() > 0) ? ids_sorted->data_ptr<int>() : nullptr,
-                                           ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W, n.data_ptr<int>(),
-                                           F32PTR(w), F32PTR(image), mptr, cur_stream()),
+        const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+        check_rc(gsr_render_forward_gather(
+                     F32PTR(records), ps.keys, (int)id_bits, ps.ids,
+                     depth_key.has_value() ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr,
+                     (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
+                     n.data_ptr<int>(), F32PTR(w), F32PTR(image), depth.defined() ? F32PTR(depth) : nullptr,
+                     alpha.defined() ? F32PTR(alpha) : nullptr, mptr, cur_stream()),
                  "gsr_render_forward_gather");
     } else {
-        check_rc(gsr_render_forward(F32PTR(stream_rec), ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
+        check_rc(gsr_render_forward(F32PTR(records), ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
                                     n.data_ptr<int>(), F32PTR(w), F32PTR(image), mptr, cur_stream()),
                  "gsr_render_forward");
     }
-    return std::make_tuple(image, n, w, masks);
+    return std::make_tuple(image, n, w, masks, depth, alpha);
 }
 
-// per-gaussian gradient slab, flat [9N]: rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3], rows indexed by
-// gaussian; zero-filled, then accumulated into by the render backward
-torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, torch::Tensor stream_rec,
+// per-gaussian gradient slab, rows indexed by gaussian; zero-filled, then accumulated into by the render backward.
+// Gather mode: interleaved rows [N,12] rgb3 opacity | uv2 conic0 conic1 | conic2 pad3 (vector reductions); with
+// grad_depth / grad_alpha [H,W,1] (the upstream gradients on the depth/alpha maps, with the forward's depth keys)
+// conic2 z pad2, z the gradient on the camera-frame z.  Record-stream mode: planar [9N] rgb [N,3] | opacity [N] |
+// uv [N,2] | conic [N,3].
+torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, int64_t P, torch::Tensor records,
                                     torch::Tensor ids_sorted, torch::Tensor ranges, torch::Tensor background,
                                     torch::Tensor n, torch::Tensor w, torch::Tensor masks,
-                                    c10::optional<torch::Tensor> keys_sorted, int64_t id_bits, bool gather) {
+                                    c10::optional<torch::Tensor> keys_sorted, int64_t id_bits, bool gather,
+                                    c10::optional<torch::Tensor> grad_depth, c10::optional<torch::Tensor> grad_alpha,
+                                    c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits) {
     CHECK_VALID_INPUT(grad_image); CHECK_FLOAT_TENSOR(grad_image);
     const int H = n.size(0), W = n.size(1);
     TORCH_CHECK(grad_image.dim() == 3 && grad_image.size(0) == H && grad_image.size(1) == W &&
                     grad_image.size(2) == 3,
                 "grad_image must be HxWx3");
+    const bool depth = grad_depth.has_value();
+    if (depth) {
+        TORCH_CHECK(gather && grad_alpha.has_value() && depth_key.has_value(),
+                    "the depth/alpha backward needs gather mode, grad_alpha and depth_key");
+        CHECK_VALID_INPUT((*grad_depth)); CHECK_FLOAT_TENSOR((*grad_depth));
+        CHECK_VALID_INPUT((*grad_alpha)); CHECK_FLOAT_TENSOR((*grad_alpha));
+        TORCH_CHECK(grad_depth->numel() == (int64_t)H * W && grad_alpha->numel() == (int64_t)H * W,
+                    "grad_depth and grad_alpha must hold H*W values");
+    }
     c10::cuda::CUDAGuard guard(grad_image.device());
-    // gather mode: interleaved rows [N,12] (vector reductions); stream mode: planar [9N]
     torch::Tensor slab = torch::zeros({N * (gather ? (int64_t)GSR_GRAD_ROW_FLOATS : 9)}, grad_image.options());
     float* g_rgb = slab.data_ptr<float>();
     float* g_opa = g_rgb + (size_t)N * 3;
@@ -641,16 +645,17 @@ torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, torch::
     float* g_conic = g_uv + (size_t)N * 2;
     const uint32_t* mptr = masks.numel() > 0 ? (const uint32_t*)masks.data_ptr<int>() : nullptr;
     if (gather) {
-        const bool by_key = keys_sorted.has_value() && keys_sorted->numel() > 0;
-        check_rc(gsr_render_backward_gather(F32PTR(stream_rec),
-                                            by_key ? (const uint64_t*)keys_sorted->data_ptr<int64_t>() : nullptr, (int)id_bits,
-                                            (!by_key && ids_sorted.numel() > 0) ? ids_sorted.data_ptr<int>() : nullptr,
-                                            ranges.data_ptr<int>(), F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w),
-                                            F32PTR(grad_image), nullptr, nullptr, nullptr, nullptr, g_rgb, mptr,
-                                            cur_stream()),
+        const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+        check_rc(gsr_render_backward_gather(
+                     F32PTR(records), ps.keys, (int)id_bits, ps.ids,
+                     depth ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr, (uint32_t)depth_base,
+                     (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w),
+                     F32PTR(grad_image), depth ? F32PTR((*grad_depth)) : nullptr,
+                     depth ? F32PTR((*grad_alpha)) : nullptr, nullptr, nullptr, nullptr, nullptr, g_rgb, mptr,
+                     cur_stream()),
                  "gsr_render_backward_gather");
     } else {
-        check_rc(gsr_render_backward(F32PTR(stream_rec), ids_sorted.data_ptr<int>(), ranges.data_ptr<int>(),
+        check_rc(gsr_render_backward(F32PTR(records), ids_sorted.data_ptr<int>(), ranges.data_ptr<int>(),
                                      F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w), F32PTR(grad_image),
                                      g_rgb, g_opa, g_uv, g_conic, mptr, cur_stream()),
                  "gsr_render_backward");
@@ -658,89 +663,24 @@ torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, torch::
     return slab;
 }
 
-// Depth/alpha mode of the two calls above (gather mode only).  Forward: + depth [H,W,1], alpha [H,W,1]; zkey: the
-// per-gaussian depth keys of the forward (read when the pair list is a sorted id array).
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
-fused_render_forward_depth(torch::Tensor records, torch::Tensor ranges, torch::Tensor background, int64_t H, int64_t W,
-                           int64_t P, bool record_masks, c10::optional<torch::Tensor> keys_sorted,
-                           c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, torch::Tensor zkey,
-                           int64_t depth_base, int64_t depth_bits) {
-    CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
-    TORCH_CHECK(background.numel() == 3, "Background RGB must have 3 elements");
-    c10::cuda::CUDAGuard guard(records.device());
-    auto opt = records.options();
-    torch::Tensor image = torch::empty({H, W, 3}, opt);
-    torch::Tensor n = torch::empty({H, W}, opt.dtype(torch::kInt32));
-    torch::Tensor w = torch::empty({H, W}, opt);
-    torch::Tensor depth = torch::empty({H, W, 1}, opt);
-    torch::Tensor alpha = torch::empty({H, W, 1}, opt);
-    torch::Tensor masks = record_masks
-                              ? torch::zeros({(int64_t)gsr_contribution_mask_words(P, (int)H, (int)W)}, opt.dtype(torch::kInt32))
-                              : torch::empty({0}, opt.dtype(torch::kInt32));
-    const bool by_key = keys_sorted.has_value() && keys_sorted->numel() > 0;
-    const bool by_id = !by_key && ids_sorted.has_value() && ids_sorted->numel() > 0;
-    TORCH_CHECK(by_key || by_id || P == 0, "gather mode needs the sorted pair list");
-    // an empty view (P == 0) still runs the kernel, which then reads no pair: any well-formed source will do
-    const int32_t dummy_id = 0;
-    check_rc(gsr_render_forward_gather_depth(
-                 F32PTR(records), by_key ? (const uint64_t*)keys_sorted->data_ptr<int64_t>() : nullptr, (int)id_bits,
-                 by_id ? ids_sorted->data_ptr<int>() : (by_key ? nullptr : &dummy_id),
-                 (const uint32_t*)zkey.data_ptr<int>(), (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(),
-                 F32PTR(background), (int)H, (int)W, n.data_ptr<int>(), F32PTR(w), F32PTR(image), F32PTR(depth),
-                 F32PTR(alpha), record_masks ? (uint32_t*)masks.data_ptr<int>() : nullptr, cur_stream()),
-             "gsr_render_forward_gather_depth");
-    return std::make_tuple(image, n, w, masks, depth, alpha);
-}
-
-// interleaved rows [N,12]: rgb3 opacity | uv2 conic0 conic1 | conic2 z pad2
-torch::Tensor fused_render_backward_depth(torch::Tensor grad_image, torch::Tensor grad_depth, torch::Tensor grad_alpha,
-                                          int64_t N, torch::Tensor records, torch::Tensor ids_sorted,
-                                          torch::Tensor ranges, torch::Tensor background, torch::Tensor n,
-                                          torch::Tensor w, torch::Tensor masks,
-                                          c10::optional<torch::Tensor> keys_sorted, int64_t id_bits,
-                                          torch::Tensor zkey, int64_t depth_base, int64_t depth_bits) {
-    CHECK_VALID_INPUT(grad_image); CHECK_FLOAT_TENSOR(grad_image);
-    CHECK_VALID_INPUT(grad_depth); CHECK_FLOAT_TENSOR(grad_depth);
-    CHECK_VALID_INPUT(grad_alpha); CHECK_FLOAT_TENSOR(grad_alpha);
-    const int H = n.size(0), W = n.size(1);
-    TORCH_CHECK(grad_image.numel() == (int64_t)H * W * 3, "grad_image must be HxWx3");
-    TORCH_CHECK(grad_depth.numel() == (int64_t)H * W && grad_alpha.numel() == (int64_t)H * W,
-                "grad_depth and grad_alpha must hold H*W values");
-    c10::cuda::CUDAGuard guard(grad_image.device());
-    torch::Tensor slab = torch::zeros({N * (int64_t)GSR_GRAD_ROW_FLOATS}, grad_image.options());
-    const bool by_key = keys_sorted.has_value() && keys_sorted->numel() > 0;
-    const int32_t dummy_id = 0;
-    check_rc(gsr_render_backward_gather_depth(
-                 F32PTR(records), by_key ? (const uint64_t*)keys_sorted->data_ptr<int64_t>() : nullptr, (int)id_bits,
-                 by_key ? nullptr : (ids_sorted.numel() > 0 ? ids_sorted.data_ptr<int>() : &dummy_id),
-                 (const uint32_t*)zkey.data_ptr<int>(), (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(),
-                 F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w), F32PTR(grad_image), F32PTR(grad_depth),
-                 F32PTR(grad_alpha), slab.data_ptr<float>(),
-                 masks.numel() > 0 ? (const uint32_t*)masks.data_ptr<int>() : nullptr, cur_stream()),
-             "gsr_render_backward_gather_depth");
-    return slab;
-}
-
-// grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab [9N] (rows by gaussian).
-// grad_uv_compact [M,2] (optional): gradient on the compact uv, added to — or, with use_slab_uv false, replacing —
-// the slab's uv section.  depth: the slab is the rows of fused_render_backward_depth (slot 9 = gradient on z).
-// antialiased: the rows' opacity slot is the gradient on the compensated opacity (gsr_preprocess_backward_antialiased).
-static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, bool antialiased, torch::Tensor slab, torch::Tensor xyz,
-                                                     torch::Tensor quaternion, torch::Tensor scale,
-                                                     torch::Tensor opacity_logit,
+// grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab of fused_render_backward: planar
+// [9N] or interleaved rows [N,12] (rows by gaussian).  grad_uv_compact [M,2] (optional): gradient on the compact uv,
+// added to — or, with use_slab_uv false, replacing — the slab's uv section.  mode: the GSR_MODE_* bits of the forward
+// (gsr_preprocess_backward): GSR_MODE_DEPTH_ALPHA reads the z gradient of the depth/alpha rows, GSR_MODE_ANTIALIASED
+// takes the rows' opacity slot as the gradient on the compensated opacity.
+std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
+                                                     torch::Tensor scale, torch::Tensor opacity_logit,
                                                      c10::optional<torch::Tensor> sh_rest,
                                                      torch::Tensor camera_T_world, torch::Tensor K,
                                                      c10::optional<torch::Tensor> camera_centre,
-                                                     torch::Tensor visible,
-                                                     c10::optional<torch::Tensor> out_flat,
+                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
                                                      c10::optional<torch::Tensor> grad_uv_compact,
-                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv) {
+                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
+                                                     int64_t mode) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     const int64_t N = xyz.size(0);
     const bool rows = slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS && N > 0;  // interleaved [N,12] (else planar [9N])
     TORCH_CHECK(rows || slab.numel() == N * 9, "gradient slab must hold 9 (planar) or 12 (rows) floats per gaussian");
-    TORCH_CHECK(!depth || rows || N == 0, "the depth/alpha backward needs the interleaved gradient rows");
-    TORCH_CHECK(!antialiased || rows || N == 0, "the anti-aliased backward needs the interleaved gradient rows");
     c10::cuda::CUDAGuard guard(xyz.device());
     auto opt = xyz.options();
     const float* g_rgb = slab.data_ptr<float>();
@@ -784,26 +724,7 @@ static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, bool anti
                   o_o = section(3, {N}), o_dc = section(4, {N, 3});
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
-    if (antialiased) {
-        check_rc(gsr_preprocess_backward_antialiased(
-                     (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit),
-                     F32PTR(camera_T_world), F32PTR(K),
-                     camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
-                     visible.data_ptr<uint8_t>(), N > 0 ? slab.data_ptr<float>() : nullptr, depth ? 1 : 0,
-                     use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s),
-                     F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr, cur_stream()),
-                 "gsr_preprocess_backward_antialiased");
-    } else if (depth) {
-        check_rc(gsr_preprocess_backward_depth((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
-                                               F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
-                                               camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
-                                               visible.data_ptr<uint8_t>(), N > 0 ? slab.data_ptr<float>() : nullptr,
-                                               use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q),
-                                               F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr,
-                                               cur_stream()),
-                 "gsr_preprocess_backward_depth");
-    } else
-    check_rc(gsr_preprocess_backward((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
+    check_rc(gsr_preprocess_backward((int)mode, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
                                      F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
                                      camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
                                      visible.data_ptr<uint8_t>(), g_rgb, g_opa, g_uv, g_conic,
@@ -817,27 +738,6 @@ static std::vector<torch::Tensor> preprocess_backward_impl(bool depth, bool anti
     out.push_back(flat);  // last: the allocation all the others are views of
     return out;
 }
-
-#define GSR_PREPROCESS_BWD_ARGS                                                                                   \
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale,                         \
-        torch::Tensor opacity_logit, c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,          \
-        torch::Tensor K, c10::optional<torch::Tensor> camera_centre, torch::Tensor visible,                      \
-        c10::optional<torch::Tensor> out_flat, c10::optional<torch::Tensor> grad_uv_compact,                     \
-        c10::optional<torch::Tensor> scan, bool use_slab_uv
-std::vector<torch::Tensor> fused_preprocess_backward(GSR_PREPROCESS_BWD_ARGS) {
-    return preprocess_backward_impl(false, false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
-                                    camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
-}
-std::vector<torch::Tensor> fused_preprocess_backward_depth(GSR_PREPROCESS_BWD_ARGS) {
-    return preprocess_backward_impl(true, false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
-                                    camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
-}
-// depth: the rows of fused_render_backward_depth
-std::vector<torch::Tensor> fused_preprocess_backward_antialiased(GSR_PREPROCESS_BWD_ARGS, bool depth) {
-    return preprocess_backward_impl(depth, true, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world,
-                                    K, camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv);
-}
-#undef GSR_PREPROCESS_BWD_ARGS
 
 // sizes of the flat parameter / gradient layout: exclusive end of each section, in elements
 std::vector<int64_t> flat_section_ends(int64_t N, int64_t n_sh_rest) {
@@ -1080,23 +980,21 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "precompute rgb from sh per gaussian backward");
     m.def("render_depth_cuda", &render_depth_cuda, "Render depth CUDA");
     // fused path
-    m.def("fused_preprocess_forward", &fused_preprocess_forward, "fused per-gaussian stage");
-    m.def("fused_preprocess_forward_tiles", &fused_preprocess_forward_tiles,
-          "fused per-gaussian stage, also returning every gaussian's tile-hit mask and window");
+    m.def("fused_preprocess_forward", &fused_preprocess_forward,
+          "fused per-gaussian stage (with_tiles: also every gaussian's tile-hit mask and window; mode: MODE_* bits)",
+          py::arg("xyz"), py::arg("xyz_camera_frame"), py::arg("quaternion"), py::arg("scale"),
+          py::arg("opacity_logit"), py::arg("rgb_dc"), py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"),
+          py::arg("camera_centre"), py::arg("H"), py::arg("W"), py::arg("near_thresh"), py::arg("far_thresh"),
+          py::arg("cull_mask_padding"), py::arg("mh_dist"), py::arg("depth_base"), py::arg("with_tiles") = false,
+          py::arg("mode") = 0);
     m.def("fused_bin", &fused_bin, "pair emission + radix sort + tile ranges + record stream");
-    m.def("fused_render_forward", &fused_render_forward, "tile renderer forward on a record stream");
-    m.def("fused_render_backward", &fused_render_backward, "tile renderer backward -> per-gaussian gradient slab");
-    m.def("fused_preprocess_backward", &fused_preprocess_backward, "fused per-gaussian backward");
-    m.def("fused_render_forward_depth", &fused_render_forward_depth,
-          "tile renderer forward (gather mode) with depth and alpha maps");
-    m.def("fused_render_backward_depth", &fused_render_backward_depth,
-          "tile renderer backward (gather mode) with depth and alpha upstream gradients -> rows incl. z");
-    m.def("fused_preprocess_backward_depth", &fused_preprocess_backward_depth,
-          "fused per-gaussian backward from rows carrying the camera-frame z gradient");
-    m.def("fused_preprocess_forward_tiles_antialiased", &fused_preprocess_forward_tiles_antialiased,
-          "fused per-gaussian stage with the anti-aliased opacity compensation");
-    m.def("fused_preprocess_backward_antialiased", &fused_preprocess_backward_antialiased,
-          "fused per-gaussian backward of the anti-aliased stage (rows; depth: rows carrying the z gradient)");
+    m.def("fused_render_forward", &fused_render_forward,
+          "tile renderer forward (with depth_key: also the depth and alpha maps)");
+    m.def("fused_render_backward", &fused_render_backward,
+          "tile renderer backward -> per-gaussian gradient slab (with grad_depth / grad_alpha: rows incl. z)");
+    m.def("fused_preprocess_backward", &fused_preprocess_backward, "fused per-gaussian backward (mode: MODE_* bits)");
+    m.attr("MODE_DEPTH_ALPHA") = GSR_MODE_DEPTH_ALPHA;
+    m.attr("MODE_ANTIALIASED") = GSR_MODE_ANTIALIASED;
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");

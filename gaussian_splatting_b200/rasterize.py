@@ -245,7 +245,7 @@ class _ViewState:
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges", "stream_rec", "gather",
                  "records", "keys_sorted", "id_bits", "slab_width",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
-                 "depth_alpha", "zkey", "depth_base", "depth_bits", "depth", "alpha", "antialiased")
+                 "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha")
 
     @property
     def ids_sorted(self):
@@ -266,9 +266,10 @@ class _ViewState:
         self.background = None  # set by rasterize() before the projection node runs (it pre-launches the renderer)
         self.image = None
         self.speculation_overflowed = False
-        self.depth_alpha = False  # render_depth_alpha: the tile kernels also produce depth / alpha [H,W,1]
+        # MODE_* bits of the native fused path: MODE_DEPTH_ALPHA (render_depth_alpha: the tile kernels also produce
+        # depth / alpha [H,W,1]), MODE_ANTIALIASED (opacity compensation for the 0.25 px^2 dilation)
+        self.mode = 0
         self.depth = self.alpha = None
-        self.antialiased = False  # opacity compensation for the 0.25 px^2 dilation (rasterize(antialiased=True))
 
 
 class _stage:
@@ -318,12 +319,9 @@ class _ProjectGaussians(torch.autograd.Function):
                 centre = torch.linalg.inv_ex(camera_T_world)[0][:3, 3].contiguous()
         with _stage(state, "preprocess_fwd"):
             # tile_mask / tile_win: the tiles each gaussian hits, tested once here and only expanded by the pair emission
-            # antialiased: the records carry sigmoid(opacity) * rho (include/gsr_b200.h)
-            preprocess = (ext.fused_preprocess_forward_tiles_antialiased if state.antialiased
-                          else ext.fused_preprocess_forward_tiles)
-            records, zkey, visible, scan, tile_mask, tile_win = preprocess(
+            records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(
                 xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
-                pad, mh, depth_base)
+                pad, mh, depth_base, True, state.mode)
         record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])  # a backward pass can follow
         background = state.background
 
@@ -338,20 +336,17 @@ class _ProjectGaussians(torch.autograd.Function):
 
         # depth / alpha maps are rendered by the gather kernels only (they read z off the sorted pair keys); the
         # anti-aliased backward reads the interleaved gradient rows only the gather kernels write
-        gather = USE_RECORD_GATHER or state.depth_alpha or state.antialiased
+        gather = USE_RECORD_GATHER or state.mode != 0
+        depth_keys = zkey if state.mode & ext.MODE_DEPTH_ALPHA else None
 
         def bin_and_render(M_, P_, speculative):
             with _stage(state, "bin_sort_gather"):
                 binned = ext.fused_bin(records, zkey, visible, scan, M_, P_, H, W, mh, depth_bits, speculative, gather,
                                        tile_mask if USE_TILE_MASKS else None, tile_win if USE_TILE_MASKS else None)
             with _stage(state, "render_fwd"):
-                if state.depth_alpha:
-                    rendered = ext.fused_render_forward_depth(records, binned[1], background, H, W, P_, record_masks,
-                                                              binned[5], binned[0], binned[6], zkey, depth_base,
-                                                              depth_bits)
-                else:
-                    rendered = ext.fused_render_forward(records if gather else binned[2], binned[1], background, H, W,
-                                                        P_, record_masks, binned[5], binned[0], binned[6], gather)
+                rendered = ext.fused_render_forward(records if gather else binned[2], binned[1], background, H, W, P_,
+                                                    record_masks, binned[5], binned[0], binned[6], gather, depth_keys,
+                                                    depth_base, depth_bits)
             return binned, rendered
 
         # The host needs M and P (the shape of the returned uv; the size of the pair buffers).  Reading them right
@@ -392,10 +387,8 @@ class _ProjectGaussians(torch.autograd.Function):
         _note_pairs(key, P)
         ids_sorted, ranges, stream_rec, vis_idx, uv, keys_sorted, id_bits = binned
         state.gather, state.records, state.keys_sorted, state.id_bits = gather, records, keys_sorted, int(id_bits)
-        state.image, state.n_per_pixel, state.w_per_pixel, state.masks = rendered[:4]
-        if state.depth_alpha:
-            state.depth, state.alpha = rendered[4:]
-            state.zkey, state.depth_base, state.depth_bits = zkey, depth_base, depth_bits
+        state.image, state.n_per_pixel, state.w_per_pixel, state.masks, state.depth, state.alpha = rendered
+        state.zkey, state.depth_base, state.depth_bits = depth_keys, depth_base, depth_bits
         state.N, state.M, state.P, state.H, state.W = xyz.shape[0], M, P, H, W
         state.visible = visible
         state.vis_idx = state.vis_idx32 = vis_idx                # int32 [M]: visible gaussians, ascending
@@ -426,14 +419,10 @@ class _ProjectGaussians(torch.autograd.Function):
         if grad_uv is not None and st.M > 0:
             guv = grad_uv.contiguous()
         with _stage(st, "preprocess_bwd"):
-            # depth/alpha mode: the rows also carry the render backward's gradient on camera-frame z (slot 9)
-            args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible,
-                    st.grad_out, guv, st.scan if guv is not None else None, not st.uv_grad_emitted)
-            if st.antialiased:   # the rows' opacity slot is the gradient on sigmoid(opacity) * rho
-                grads = native().fused_preprocess_backward_antialiased(*args, st.depth_alpha)
-            else:
-                fn = native().fused_preprocess_backward_depth if st.depth_alpha else native().fused_preprocess_backward
-                grads = fn(*args)
+            grads = native().fused_preprocess_backward(slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K,
+                                                       centre, st.visible, st.grad_out, guv,
+                                                       st.scan if guv is not None else None, not st.uv_grad_emitted,
+                                                       st.mode)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
@@ -441,64 +430,41 @@ class _ProjectGaussians(torch.autograd.Function):
 
 
 class _CompositeTiles(torch.autograd.Function):
+    """uv, carrier -> image, or (image, depth, alpha) with the depth/alpha maps."""
+
     @staticmethod
     def forward(ctx, uv, carrier, background_rgb, state):
         # the tile renderer was already enqueued by the projection node (right behind the binning, before the host
-        # learned the pair count): this node only ties the image to uv and to the gradient carrier
-        image, state.image = state.image, None
-        ctx.state = state
-        return image
-
-    @staticmethod
-    def backward(ctx, grad_image):
-        st = ctx.state
-        with _stage(st, "render_bwd"):
-            slab = native().fused_render_backward(grad_image.contiguous(), st.N,
-                                                  st.records if st.gather else st.stream_rec, st._ids_sorted,
-                                                  st.ranges, st.background, st.n_per_pixel, st.w_per_pixel, st.masks,
-                                                  st.keys_sorted, st.id_bits, st.gather)
-        return _render_grads(st, slab)
-
-
-class _CompositeTilesDepth(torch.autograd.Function):
-    """_CompositeTiles with the depth and alpha maps the renderer produced alongside the image."""
-
-    @staticmethod
-    def forward(ctx, uv, carrier, background_rgb, state):
-        outs = (state.image, state.depth, state.alpha)
+        # learned the pair count): this node only ties its outputs to uv and to the gradient carrier
+        outs = state.image if state.depth is None else (state.image, state.depth, state.alpha)
         state.image = state.depth = state.alpha = None
         ctx.state = state
         return outs
 
     @staticmethod
-    def backward(ctx, grad_image, grad_depth, grad_alpha):
+    def backward(ctx, grad_image, grad_depth=None, grad_alpha=None):
         st = ctx.state
         with _stage(st, "render_bwd"):
-            slab = native().fused_render_backward_depth(grad_image.contiguous(), grad_depth.contiguous(),
-                                                        grad_alpha.contiguous(), st.N, st.records, st._ids_sorted,
-                                                        st.ranges, st.background, st.n_per_pixel, st.w_per_pixel,
-                                                        st.masks, st.keys_sorted, st.id_bits, st.zkey, st.depth_base,
-                                                        st.depth_bits)
-        return _render_grads(st, slab)
-
-
-def _render_grads(st, slab):
-    """Gradients of a composite node for (uv, carrier, background, state) from the render backward's slab."""
-    # The render pass's gradient on the compact uv is a gather of the slab's uv section (28 us at 3M).  It
-    # reaches the per-gaussian backward through the slab anyway, so it is only materialised when it can be
-    # OBSERVED: the caller retained uv's gradient (the reference trainer does, splat_py/trainer.py:360) or
-    # hooked the tensor.
-    uv_t = st.uv_ref() if st.uv_ref is not None else None
-    watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
-    st.uv_grad_emitted = bool(watched)
-    if not watched:
-        return None, slab, None, None
-    N = st.N
-    if st.slab_width == 12:   # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3 (depth mode: z pad2)
-        grad_uv = slab.view(N, 12).index_select(0, st.vis_idx)[:, 4:6].contiguous()
-    else:                     # planar: rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3]
-        grad_uv = slab[4 * N:6 * N].view(N, 2).index_select(0, st.vis_idx)
-    return grad_uv, slab, None, None
+            slab = native().fused_render_backward(
+                grad_image.contiguous(), st.N, st.P, st.records if st.gather else st.stream_rec, st._ids_sorted,
+                st.ranges, st.background, st.n_per_pixel, st.w_per_pixel, st.masks, st.keys_sorted, st.id_bits,
+                st.gather, None if grad_depth is None else grad_depth.contiguous(),
+                None if grad_alpha is None else grad_alpha.contiguous(), st.zkey, st.depth_base, st.depth_bits)
+        # The render pass's gradient on the compact uv is a gather of the slab's uv section (28 us at 3M).  It
+        # reaches the per-gaussian backward through the slab anyway, so it is only materialised when it can be
+        # OBSERVED: the caller retained uv's gradient (the reference trainer does, splat_py/trainer.py:360) or
+        # hooked the tensor.
+        uv_t = st.uv_ref() if st.uv_ref is not None else None
+        watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
+        st.uv_grad_emitted = bool(watched)
+        if not watched:
+            return None, slab, None, None
+        N = st.N
+        if st.slab_width == 12:   # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3 (depth mode: z pad2)
+            grad_uv = slab.view(N, 12).index_select(0, st.vis_idx)[:, 4:6].contiguous()
+        else:                     # planar: rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3]
+            grad_uv = slab[4 * N:6 * N].view(N, 2).index_select(0, st.vis_idx)
+        return grad_uv, slab, None, None
 
 
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
@@ -525,10 +491,10 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
                                  cull_mask_padding, mh_dist, use_sh_precompute, background_rgb)
     if gaussians.xyz.dtype != torch.float32:
         raise TypeError("the fused rasterizer is fp32; use rasterize_unfused for float64 inputs")
+    ext = native()
     state = _ViewState(profile)
     state.grad_out = grad_out
-    state.depth_alpha = bool(render_depth_alpha)
-    state.antialiased = bool(antialiased)
+    state.mode = (ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))
@@ -539,15 +505,10 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
         camera_T_world.contiguous(), camera.K.contiguous(), state, cfg)
     state.uv_ref = weakref.ref(uv)
     culling_mask = state.visible == 0
-    if state.depth_alpha:
-        image, depth, alpha = _CompositeTilesDepth.apply(uv, carrier, state.background, state)
-        if return_state:
-            return image, culling_mask, uv, depth, alpha, state
-        return image, culling_mask, uv, depth, alpha
-    image = _CompositeTiles.apply(uv, carrier, state.background, state)
-    if return_state:
-        return image, culling_mask, uv, state
-    return image, culling_mask, uv
+    outs = _CompositeTiles.apply(uv, carrier, state.background, state)
+    image, maps = (outs[0], outs[1:]) if render_depth_alpha else (outs, ())
+    result = (image, culling_mask, uv, *maps)
+    return (*result, state) if return_state else result
 
 
 def project_and_bin(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist):

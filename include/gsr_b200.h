@@ -38,6 +38,12 @@ extern "C" {
 /* floats per packed splat record consumed by the tile renderers (48 bytes) */
 #define GSR_REC_FLOATS 12
 
+/* Modes of the fused per-Gaussian stage (`mode` of gsr_preprocess_forward / gsr_preprocess_backward), a bit mask.
+ * The tile renderers take no mode word: gsr_render_*_gather run in depth/alpha mode when they are given the depth
+ * and alpha maps (forward) or their upstream gradients (backward). */
+#define GSR_MODE_DEPTH_ALPHA 1 /* gradient rows carry the render backward's camera-frame z gradient */
+#define GSR_MODE_ANTIALIASED 2 /* opacity compensation for the renderer's 0.25 px^2 dilation */
+
 /* library identification: returns e.g. "gsr_b200 0.1 sm_90a" */
 const char* gsr_version(void);
 
@@ -160,45 +166,39 @@ int gsr_render_backward(const float* records, const int32_t* sorted_gaussian_idx
  * — keys_sorted (gaussian id in the low id_bits of every key, gsr_sort_keys' output) or ids_sorted (gsr_sort_pairs'
  * id output); exactly one of the two is non-NULL.  3 x 16-byte cp.async per record, issued by the warp that recycles
  * a pipeline stage, completion on the stage's mbarrier; gsr_gather_records* and the [P,12] stream are not needed.
- * Gradient rows are indexed by gaussian id. */
-int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                              const int32_t* ids_sorted, const int32_t* tile_ranges, const float* background_rgb, int H,
-                              int W, int32_t* num_splats_per_pixel, float* final_weight_per_pixel, float* image,
-                              uint32_t* contribution_masks, void* stream);
-/* Gradient destination: the four planar arrays (grad_rows NULL), or grad_rows [N, GSR_GRAD_ROW_FLOATS] (16-byte
- * aligned, zero-filled; then the four planar pointers are ignored): one interleaved row per gaussian,
- * rgb3 opacity | uv2 conic0 conic1 | conic2 pad3, accumulated with 16-byte vector reductions — the nine sums of a pair
- * touch two adjacent 32-byte sectors instead of four arrays.  gsr_preprocess_backward reads either form. */
-#define GSR_GRAD_ROW_FLOATS 12
-int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                               const int32_t* ids_sorted, const int32_t* tile_ranges, const float* background_rgb, int H,
-                               int W, const int32_t* num_splats_per_pixel, const float* final_weight_per_pixel,
-                               const float* grad_image, float* grad_rgb, float* grad_opacity, float* grad_uv,
-                               float* grad_conic, float* grad_rows, const uint32_t* contribution_masks, void* stream);
-
-/* Depth and alpha maps from the same walk (gather kernels only, precomputed colours).  Per pixel, over the splats the
- * colour blend composites (same weights w_i, same saturation early-out):
+ * Gradient rows are indexed by gaussian id.
+ *
+ * Depth and alpha maps from the same walk (precomputed colours), when depth and alpha are non-NULL (both or neither;
+ * NULL: colour only, and depth_key / depth_base / depth_bits are not read).  Per pixel, over the splats the colour
+ * blend composites (same weights w_i, same saturation early-out):
  *   alpha [H,W] = the accumulated sum of w_i before any background (0 where nothing contributes),
  *   depth [H,W] = D, D <- fma(w_i, z_i, D) front to back, z_i the camera-frame z of gaussian i; no background term
  *                 (un-normalised: expected depth is depth / alpha).
  * z_i is decoded from the depth field of the sorted pair keys — bits(z) - depth_base, or depth_key()'s
  * order-preserving transform when depth_base == 0 (then depth_bits must be 32) — and, with ids_sorted instead of
  * keys_sorted, from the per-gaussian depth keys depth_key [N] (gsr_preprocess_forward's output).
- * The backward takes upstream gradients on all three maps (all three non-NULL; zeros where a map has none) and
- * accumulates interleaved rows rgb3 opacity | uv2 conic0 conic1 | conic2 z pad2 into grad_rows [N,12] (16-byte
- * aligned, zero-filled), z being the gradient on the camera-frame z; gsr_preprocess_backward_depth consumes them.
  * Argument errors return GSR_ERR_BAD_ARG. */
-int gsr_render_forward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                                    const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
-                                    int depth_bits, const int32_t* tile_ranges, const float* background_rgb, int H,
-                                    int W, int32_t* num_splats_per_pixel, float* final_weight_per_pixel, float* image,
-                                    float* depth, float* alpha, uint32_t* contribution_masks, void* stream);
-int gsr_render_backward_gather_depth(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
-                                     const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
-                                     int depth_bits, const int32_t* tile_ranges, const float* background_rgb, int H,
-                                     int W, const int32_t* num_splats_per_pixel, const float* final_weight_per_pixel,
-                                     const float* grad_image, const float* grad_depth, const float* grad_alpha,
-                                     float* grad_rows, const uint32_t* contribution_masks, void* stream);
+int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                              const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base, int depth_bits,
+                              const int32_t* tile_ranges, const float* background_rgb, int H, int W,
+                              int32_t* num_splats_per_pixel, float* final_weight_per_pixel, float* image, float* depth,
+                              float* alpha, uint32_t* contribution_masks, void* stream);
+/* Gradient destination: the four planar arrays (grad_rows NULL), or grad_rows [N, GSR_GRAD_ROW_FLOATS] (16-byte
+ * aligned, zero-filled; then the four planar pointers are ignored): one interleaved row per gaussian,
+ * rgb3 opacity | uv2 conic0 conic1 | conic2 pad3, accumulated with 16-byte vector reductions — the nine sums of a pair
+ * touch two adjacent 32-byte sectors instead of four arrays.  gsr_preprocess_backward reads either form.
+ * Depth/alpha mode: grad_depth and grad_alpha [H,W] non-NULL (both or neither; zeros where a map has no gradient),
+ * the depth descriptor as in the forward, grad_rows required; the rows are then rgb3 opacity | uv2 conic0 conic1 |
+ * conic2 z pad2, z being the gradient on the camera-frame z, which gsr_preprocess_backward consumes with
+ * GSR_MODE_DEPTH_ALPHA. */
+#define GSR_GRAD_ROW_FLOATS 12
+int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                               const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                               int depth_bits, const int32_t* tile_ranges, const float* background_rgb, int H, int W,
+                               const int32_t* num_splats_per_pixel, const float* final_weight_per_pixel,
+                               const float* grad_image, const float* grad_depth, const float* grad_alpha,
+                               float* grad_rgb, float* grad_opacity, float* grad_uv, float* grad_conic,
+                               float* grad_rows, const uint32_t* contribution_masks, void* stream);
 
 /* General renderers: any dtype, any n_sh in {1,4,9,16} (per-pixel SH via view_dir_by_pixel
  * [H,W,3]); same semantics as the reference's template instantiations
@@ -258,8 +258,14 @@ size_t gsr_preprocess_temp_bytes(int N);
  *                           window has at most 64 tiles, the tiles hit as a bit mask over the window (bit =
  *                           (tx - x0) * height + (ty - y0)) and the window as x0 | y0 << 8 | width << 16 |
  *                           height << 24; tile_win = 0xffffffff for larger windows.  gsr_emit_keys / gsr_emit_pairs
- *                           expand the mask instead of repeating the OBB tests. */
-int gsr_preprocess_forward(int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
+ *                           expand the mask instead of repeating the OBB tests.
+ * mode: GSR_MODE_* bits; only GSR_MODE_ANTIALIASED changes this stage (Mip-Splatting's 2-D filter, "antialiased"
+ *   rasterize mode): each record's opacity is then sigmoid(opacity_logit) * rho with
+ *     rho = sqrt(max(det0, 0) / det),  det0 = det of the 2-D covariance, det = det of the covariance + 0.25 I
+ *   (the +0.25 px^2 dilation the tile renderers apply), so the dilated splat carries the mass of the undilated one.
+ *   The culling bound is formed from the compensated opacity.  rho == 0 where det0 <= 0 in fp32: the splat then never
+ *   contributes.  Operation order: gsr_record.cuh aa_rho. */
+int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
                            int cam_first, const float* quaternion,
                            const float* scale, const float* opacity_logit, const float* rgb_dc,
                            const float* sh_rest, const float* camera_T_world, const float* K,
@@ -268,20 +274,6 @@ int gsr_preprocess_forward(int N, int n_sh_rest, const float* xyz, const float* 
                            uint32_t* depth_key,
                            uint8_t* visible, uint64_t* scan, uint64_t* tile_mask, uint32_t* tile_win, void* temp,
                            size_t temp_bytes, void* stream);
-/* Anti-aliased mode (Mip-Splatting's 2-D filter, "antialiased" rasterize mode): the same outputs, except that each
- * record's opacity is sigmoid(opacity_logit) * rho with
- *   rho = sqrt(max(det0, 0) / det),  det0 = det of the 2-D covariance, det = det of the covariance + 0.25 I
- * (the +0.25 px^2 dilation the tile renderers apply), so the dilated splat carries the mass of the undilated one.
- * The culling bound is formed from the compensated opacity.  rho == 0 where det0 <= 0 in fp32: the splat then never
- * contributes.  Operation order: gsr_record.cuh aa_rho. */
-int gsr_preprocess_forward_antialiased(int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
-                                       int cam_first, const float* quaternion, const float* scale,
-                                       const float* opacity_logit, const float* rgb_dc, const float* sh_rest,
-                                       const float* camera_T_world, const float* K, const float* camera_centre, int H,
-                                       int W, float near_thresh, float far_thresh, float cull_mask_padding,
-                                       float mh_dist, uint32_t depth_base, float* records, uint32_t* depth_key,
-                                       uint8_t* visible, uint64_t* scan, uint64_t* tile_mask, uint32_t* tile_win,
-                                       void* temp, size_t temp_bytes, void* stream);
 
 /* emits the (tile, depth) keys and original-gaussian ids of all P pairs, the compact list of
  * visible gaussian ids vis_idx int32 [M] and the compacted uv [M,2] the reference returns */
@@ -335,34 +327,20 @@ int gsr_gather_records_keys(int P, int id_bits, const uint64_t* keys_sorted, con
  * inclusive scan of gsr_preprocess_forward) — what a caller added upstream of uv, or the total autograd hands over.
  * grad_rows != NULL: the interleaved rows of gsr_render_backward_gather instead of the four planar arrays
  * (grad_uv == NULL then still means "skip the render backward's uv sums").
+ * mode: the GSR_MODE_* bits of the forward and the render backward; either bit requires grad_rows (16-byte aligned).
+ *   GSR_MODE_DEPTH_ALPHA: the rows of the depth/alpha render backward: row slot 9, the gradient on the camera-frame z,
+ *   joins grad_xyz as camera_T_world[2, :3] * g_z.  No gradient goes to the pose.
+ *   GSR_MODE_ANTIALIASED: the rows' opacity slot g is the gradient on the compensated opacity sigmoid(o) * rho:
+ *   sigmoid(o) receives g * rho and the 2-D covariance g * sigmoid(o) * grad(rho).  Where rho == 0 no gradient goes
+ *   through rho (its gradient is infinite there, and g is 0 because the splat never contributed).
  * Writes dense parameter gradients for all N gaussians (zeros for culled ones). */
-int gsr_preprocess_backward(int N, int n_sh_rest, const float* xyz, const float* quaternion,
+int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
                             const float* scale, const float* opacity_logit, const float* camera_T_world,
                             const float* K, const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
                             const float* grad_opacity, const float* grad_uv, const float* grad_conic,
                             const float* grad_rows, int use_rows_uv,
                             const float* grad_uv_compact, const uint64_t* scan, float* g_xyz, float* g_quaternion,
                             float* g_scale, float* g_opacity_logit, float* g_rgb_dc, float* g_sh_rest, void* stream);
-/* The same from the rows of gsr_render_backward_gather_depth (grad_rows required, 16-byte aligned): row slot 9, the
- * gradient on the camera-frame z, joins grad_xyz as camera_T_world[2, :3] * g_z.  No gradient goes to the pose. */
-int gsr_preprocess_backward_depth(int N, int n_sh_rest, const float* xyz, const float* quaternion, const float* scale,
-                                  const float* opacity_logit, const float* camera_T_world, const float* K,
-                                  const float* camera_centre, const uint8_t* visible, const float* grad_rows,
-                                  int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
-                                  float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
-                                  float* g_sh_rest, void* stream);
-/* Backward of gsr_preprocess_forward_antialiased from interleaved rows (grad_rows required, 16-byte aligned; depth != 0:
- * the rows of gsr_render_backward_gather_depth, slot 9 carrying the z gradient, as in gsr_preprocess_backward_depth).
- * The rows' opacity slot g is the gradient on the compensated opacity sigmoid(o) * rho: sigmoid(o) receives g * rho
- * and the 2-D covariance g * sigmoid(o) * grad(rho).  Where rho == 0 no gradient goes through rho (its gradient is
- * infinite there, and g is 0 because the splat never contributed). */
-int gsr_preprocess_backward_antialiased(int N, int n_sh_rest, const float* xyz, const float* quaternion,
-                                        const float* scale, const float* opacity_logit, const float* camera_T_world,
-                                        const float* K, const float* camera_centre, const uint8_t* visible,
-                                        const float* grad_rows, int depth, int use_rows_uv,
-                                        const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
-                                        float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
-                                        float* g_sh_rest, void* stream);
 
 /* ---- optimizer step on the flat parameter buffer (SURVEY.md 8(f) rank 2) ----------------------------
  * Replaces torch.optim.Adam.step() as configured by splat_py/optimizer_manager.py:13-44 (one parameter group

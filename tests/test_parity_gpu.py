@@ -639,6 +639,41 @@ def test_everything_culled_gives_background():
     assert float(r["g_xyz"].abs().max()) == 0.0
 
 
+@pytest.mark.parametrize("depth_alpha", [False, True])
+def test_everything_culled_on_the_key_value_fallback(depth_alpha):
+    """An empty view (P = 0 pairs) when the gaussian id does not fit the sort key: 4k and far = inf (full 32-bit
+    depth keys) leave 17 id bits, too few for 200 000 gaussians, so the sort carries a separate id array, which the
+    empty view narrows to nothing.  It renders the background and gives zero gradients both as the first view of its
+    size (the pair count is read before binning) and in steady state (pair buffers sized from the previous view)."""
+    from gaussian_splatting_b200 import rasterize as R
+
+    n = 200_000
+    sc = scenes.np_scene(n, "4k", sh_degree=0, seed=0)
+    sc["xyz"] = sc["xyz"].copy()
+    sc["xyz"][:, 2] = -5.0  # behind the camera
+    G = to_t(synth.make_upstream_grad("4k").numpy())
+    cam = Camera(sc["W"], sc["H"], to_t(sc["K"]))
+    bg = torch.full((3,), 0.5, device=dev())
+    key = (dev().index if dev().index is not None else torch.cuda.current_device(), n, sc["H"], sc["W"])
+    R._PAIR_HISTORY.pop(key, None)
+    for view in ("first view", "steady state"):
+        g = gaussians_from(sc)
+        out = rasterize(g, to_t(sc["T"]), cam, 0.3, float("inf"), 100, 3.0, True, bg, render_depth_alpha=depth_alpha)
+        image, mask, uv = out[:3]
+        uv.retain_grad()
+        loss = (image * G).sum()
+        if depth_alpha:
+            depth, alpha = out[3:]
+            assert not bool(depth.any()) and not bool(alpha.any()), view
+            loss = loss + depth.sum() + alpha.sum()
+        loss.backward()
+        assert bool(mask.all()) and uv.shape == (0, 2), view
+        assert torch.equal(image, torch.full_like(image, 0.5)), view
+        assert float(g.xyz.grad.abs().max()) == 0.0, view
+    assert R._PAIR_HISTORY[key] == [0, 0]
+    R._PAIR_HISTORY.pop(key, None)
+
+
 def test_empty_scene():
     sc = scenes.np_scene(64, "tiny", sh_degree=0, seed=0)
     sc = {k: (v[:0] if isinstance(v, np.ndarray) and v.shape[:1] == (64,) else v) for k, v in sc.items()}
