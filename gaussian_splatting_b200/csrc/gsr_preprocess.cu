@@ -507,7 +507,8 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 
 static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
-constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED;
+// GSR_MODE_ABSGRAD only changes the render backward (row slots 10-11, which the per-gaussian backward does not read)
+constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD;
 
 }  // namespace gsr
 
@@ -583,7 +584,8 @@ int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, co
     cudaStream_t st = (cudaStream_t)stream;
     if ((mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
     if (N <= 0) return GSR_OK;
-    // the depth/alpha and anti-aliased kernels read the render backward's sums from the interleaved rows only
+    // the depth/alpha and anti-aliased kernels read the render backward's sums from the interleaved rows only (and so
+    // does every absgrad backward: its render stage writes rows)
     if (mode != 0 && (grad_rows == nullptr || !aligned16(grad_rows))) return GSR_ERR_BAD_ARG;
     if (grad_uv_compact != nullptr && scan == nullptr) return GSR_ERR_BAD_ARG;
     const dim3 grid((N + PRE_THREADS - 1) / PRE_THREADS), block(PRE_THREADS);

@@ -804,6 +804,26 @@ __device__ __forceinline__ float quarter_warp_sum(float v) {
     v += __shfl_xor_sync(0xffffffffu, v, 1);
     return v;
 }
+// Sum 4 per-lane values across each QUARTER-warp with 4 shuffles: lane L ends with, in v[0], the total of value index
+// 2*bit1(L) + bit0(L) (lanes 4..7 of a quarter hold the same totals as lanes 0..3)
+__device__ __forceinline__ void butterfly4_quarter_low(float* v, int lane) {
+    {
+        const bool up = lane & 1;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const float send = up ? v[2 * i] : v[2 * i + 1];
+            const float keep = up ? v[2 * i + 1] : v[2 * i];
+            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
+        }
+    }
+    {
+        const bool up = lane & 2;
+        const float send = up ? v[0] : v[1];
+        const float keep = up ? v[1] : v[0];
+        v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+    }
+    v[0] += __shfl_xor_sync(0xffffffffu, v[0], 4);
+}
 
 __device__ __forceinline__ float half_warp_sum(float v) {
     v += __shfl_xor_sync(0xffffffffu, v, 8);
@@ -869,7 +889,10 @@ __device__ __forceinline__ void mask_lists(const uint32_t* __restrict__ gm, int 
 // DEPTH (gather mode, interleaved rows only): upstream gradients on the depth and alpha maps join d_alpha through the
 // same weight and r as colour, with two more back-to-front accumulators (no background term), and one more moment,
 // alpha * weight * dD, is reduced and flushed into the row's slot 9 (camera-frame z)
-template <bool MASKS, bool GATHER, bool DEPTH>
+// ABSGRAD (gather mode, interleaved rows only): two more moments, sum |2c*hu - (b+b)*hv| and sum |2a*hv - (b+b)*hu| with
+// the absolute value taken per pixel, before any sum; times |rdet| they are sum_p |d_u| and sum_p |d_v| (AbsGS), flushed
+// into the row's slots 10 and 11.  Moments 8..11 are then gc2, z (DEPTH, else 0), |u|, |v|
+template <bool MASKS, bool GATHER, bool DEPTH, bool ABSGRAD = false>
 __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* __restrict__ sorted_idx,
                                            const int32_t* __restrict__ ranges, const float* __restrict__ background,
                                            int W, int H, const int32_t* __restrict__ n_in,
@@ -879,7 +902,8 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
                                            const uint32_t* __restrict__ masks, const DepthSource& ds,
                                            const float* __restrict__ grad_depth, const float* __restrict__ grad_alpha) {
     static_assert(GATHER || !DEPTH, "depth/alpha gradients are reduced by the gather kernels only");
-    constexpr int NG = DEPTH ? NGRAD + 1 : NGRAD;  // moments per (record, batch)
+    static_assert(GATHER || !ABSGRAD, "absolute uv gradients are reduced by the gather kernels only");
+    constexpr int NG = ABSGRAD ? NGRAD + 3 : DEPTH ? NGRAD + 1 : NGRAD;  // moments per (record, batch)
     __shared__ __align__(128) float s_rec[BSTAGES][(BATCH + 1) * REC];  // + an all-zero record (alpha 0) behind each stage
     __shared__ __align__(8) uint64_t s_full[BSTAGES];
     __shared__ int s_cnt[BSTAGES];
@@ -1141,6 +1165,14 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
                 const F2 mz = mul2(dD, aw);
                 gz = lo(mz) + hi(mz);
             }
+            // ABSGRAD: S10, S11 = |2c*hu - (b+b)*hv|, |2a*hv - (b+b)*hu| per pixel (d_u = -rdet * eu, d_v = -rdet * ev)
+            float gau = 0.0f, gav = 0.0f;
+            if (ABSGRAD) {
+                const F2 eu = fma2(bc(q1.z + q1.z), hu, mul2(bc(-q1.y), hv));
+                const F2 ev = fma2(bc(q1.x + q1.x), hv, mul2(bc(-q1.y), hu));
+                gau = fabsf(lo(eu)) + fabsf(hi(eu));
+                gav = fabsf(lo(ev)) + fabsf(hi(ev));
+            }
             const bool group_any = MASKS ? act : ((bal & group_mask) != 0u);
             if (GROUPS == 2) {
                 butterfly8_half(g8, lane);
@@ -1149,6 +1181,23 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
                 const float mine = (gl == 1) ? gc2 : g8[0];
                 if (group_any & owner) atomicAdd(&acc[j * NG + my_slot], mine);
                 if (DEPTH && group_any && gl == 0) atomicAdd(&acc[j * NG + NGRAD], gz);
+                if (ABSGRAD) {
+                    gau = half_warp_sum(gau);
+                    gav = half_warp_sum(gav);
+                    if (group_any && gl == 2) atomicAdd(&acc[j * NG + NGRAD + 1], gau);
+                    if (group_any && gl == 3) atomicAdd(&acc[j * NG + NGRAD + 2], gav);
+                }
+            } else if (ABSGRAD) {
+                // moments 8..11 reduced together: lane gl < 4 of the group ends with moment 8 + gl and adds it with
+                // the same atomic instruction as the others' share of moments 0..7
+                butterfly8_quarter(g8, lane);
+                float t4[4] = {gc2, gz, gau, gav};
+                butterfly4_quarter_low(t4, lane);
+                if (group_any) {
+                    float* cell = reinterpret_cast<float*>(__cvta_shared_to_generic(acc_cell + j * (NG * 4)));
+                    atomicAdd(cell, g8[0]);
+                    if (gl < 4) atomicAdd(cell + 8, t4[0]);
+                }
             } else {
                 butterfly8_quarter(g8, lane);
                 gc2 = quarter_warp_sum(gc2);
@@ -1203,15 +1252,19 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
                     // common_frac summed over pixels (render_backward.cu:221-223)
                     const float cf = (a * S[8] - 2.0f * bh * S[7] + c * S[6]) * rdet * rdet;
                     const float gc0 = -c * cf + S[8] * rdet, gc1 = bh * cf - S[7] * rdet, gc2 = -a * cf + S[6] * rdet;
-                    if (DEPTH || g_opa == nullptr) {
+                    if (DEPTH || ABSGRAD || g_opa == nullptr) {
                         // interleaved gradient rows [gaussian][12] = rgb3 opa | uv2 conic0 conic1 | conic2 pad3: the
                         // nine sums of a pair land in two adjacent 32-byte sectors through two 16-byte vector
                         // reductions + one scalar (planar arrays: nine scalar reductions into four arrays).
-                        // DEPTH: conic2 z pad2, the last two through one 8-byte vector reduction
+                        // DEPTH: conic2 z pad2, the last two through one 8-byte vector reduction.
+                        // ABSGRAD: conic2 z|0 |u| |v|, the whole tail through a third 16-byte vector reduction
                         float* row = g_rgb + (size_t)gid * GRAD_ROW;
                         red_add_v4(row, GSR_SH0 * S[0], GSR_SH0 * S[1], GSR_SH0 * S[2], S[3]);
                         red_add_v4(row + 4, gu, gv, gc0, gc1);
-                        if (DEPTH)
+                        if (ABSGRAD)
+                            red_add_v4(row + 8, gc2, DEPTH ? S[NGRAD] : 0.0f, fabsf(rdet) * S[NGRAD + 1],
+                                       fabsf(rdet) * S[NGRAD + 2]);
+                        else if (DEPTH)
                             red_add_v2(row + 8, gc2, S[NG - 1]);
                         else
                             atomicAdd(row + 8, gc2);
@@ -1272,6 +1325,33 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_DEPTH_MINB)
                                   nullptr, nullptr, masks, ds, grad_depth, grad_alpha);
 }
 
+// Absolute uv gradients (GSR_MODE_ABSGRAD), colour only or with depth/alpha (DEPTH).  The two more moments are
+// transient per step (no per-pixel state persists), so the masked colour-only kernel keeps the default 8 CTAs per SM
+// with no local memory, and the depth ones the depth kernel's 5; s_acc grows to 12 floats per record (27.8 KB of shared
+// memory: 8 CTAs still fit).  The colour-only kernel without masks also carries the candidate-list build: at 8 CTAs it
+// spills (32-byte frame, reloaded in the walk), at 7 (72 registers) still 8 bytes; at 6 (78 registers) nothing
+#ifndef GSR_BWD_ABS_MINB
+#define GSR_BWD_ABS_MINB 8
+#endif
+#ifndef GSR_BWD_ABS_NOMASK_MINB
+#define GSR_BWD_ABS_NOMASK_MINB 6
+#endif
+#ifndef GSR_BWD_DEPTH_ABS_MINB
+#define GSR_BWD_DEPTH_ABS_MINB 5
+#endif
+template <bool MASKS, bool DEPTH>
+__global__ void __launch_bounds__(CTA_THREADS, DEPTH   ? GSR_BWD_DEPTH_ABS_MINB
+                                               : MASKS ? GSR_BWD_ABS_MINB
+                                                       : GSR_BWD_ABS_NOMASK_MINB)
+    k_render_bwd_abs(const RecSource rs, const DepthSource ds, const int32_t* __restrict__ ranges,
+                     const float* __restrict__ background, int W, int H, const int32_t* __restrict__ n_in,
+                     const float* __restrict__ w_in, const float* __restrict__ grad_image,
+                     const float* __restrict__ grad_depth, const float* __restrict__ grad_alpha,
+                     float* __restrict__ grad_rows, const uint32_t* __restrict__ masks) {
+    render_bwd<MASKS, true, DEPTH, true>(rs, nullptr, ranges, background, W, H, n_in, w_in, grad_image, grad_rows,
+                                         nullptr, nullptr, nullptr, masks, ds, grad_depth, grad_alpha);
+}
+
 }  // namespace gsr
 
 using namespace gsr;
@@ -1323,9 +1403,10 @@ static int launch_forward(const RecSource& src, const DepthSource* ds, const int
     return (int)cudaGetLastError();
 }
 
-// ds != nullptr: the depth/alpha kernels (gather mode only; the gradients go to interleaved rows, passed as g_rgb)
+// ds != nullptr: the depth/alpha kernels; absgrad: the absolute-uv-gradient kernels (both gather mode only; the
+// gradients go to interleaved rows, passed as g_rgb)
 template <bool GATHER>
-static int launch_backward(const RecSource& src, const DepthSource* ds, const int32_t* sorted_idx,
+static int launch_backward(const RecSource& src, const DepthSource* ds, bool absgrad, const int32_t* sorted_idx,
                            const int32_t* ranges, const float* background, int H, int W, const int32_t* n_in,
                            const float* w_in, const float* grad_image, const float* grad_depth,
                            const float* grad_alpha, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
@@ -1333,7 +1414,21 @@ static int launch_backward(const RecSource& src, const DepthSource* ds, const in
     if (H <= 0 || W <= 0) return GSR_ERR_BAD_ARG;
     const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
     cudaStream_t st = (cudaStream_t)stream;
-    if (ds != nullptr) {
+    if (absgrad) {
+        const DepthSource d = ds != nullptr ? *ds : DepthSource{};
+        if (ds != nullptr && masks != nullptr)
+            k_render_bwd_abs<true, true><<<grid, block, 0, st>>>(src, d, ranges, background, W, H, n_in, w_in,
+                                                                 grad_image, grad_depth, grad_alpha, g_rgb, masks);
+        else if (ds != nullptr)
+            k_render_bwd_abs<false, true><<<grid, block, 0, st>>>(src, d, ranges, background, W, H, n_in, w_in,
+                                                                  grad_image, grad_depth, grad_alpha, g_rgb, nullptr);
+        else if (masks != nullptr)
+            k_render_bwd_abs<true, false><<<grid, block, 0, st>>>(src, d, ranges, background, W, H, n_in, w_in,
+                                                                  grad_image, nullptr, nullptr, g_rgb, masks);
+        else
+            k_render_bwd_abs<false, false><<<grid, block, 0, st>>>(src, d, ranges, background, W, H, n_in, w_in,
+                                                                   grad_image, nullptr, nullptr, g_rgb, nullptr);
+    } else if (ds != nullptr) {
         if (masks != nullptr)
             k_render_bwd_depth<true><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_in, w_in,
                                                              grad_image, grad_depth, grad_alpha, g_rgb, masks);
@@ -1368,7 +1463,8 @@ int gsr_render_backward(const float* records, const int32_t* sorted_idx, const i
                         const float* background, int H, int W, const int32_t* n_in, const float* w_in,
                         const float* grad_image, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
                         const uint32_t* contribution_masks, void* stream) {
-    return launch_backward<false>(make_source(records, nullptr, nullptr, 0), nullptr, sorted_idx, ranges, background,
+    return launch_backward<false>(make_source(records, nullptr, nullptr, 0), nullptr, false, sorted_idx, ranges,
+                                  background,
                                   H, W, n_in, w_in, grad_image, nullptr, nullptr, g_rgb, g_opa, g_uv, g_conic,
                                   contribution_masks, stream);
 }
@@ -1388,13 +1484,17 @@ int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* key
                                 alpha, contribution_masks, stream);
 }
 
-int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+int gsr_render_backward_gather(int mode, const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
                                const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
                                int depth_bits, const int32_t* ranges, const float* background, int H, int W,
                                const int32_t* n_in, const float* w_in, const float* grad_image,
                                const float* grad_depth, const float* grad_alpha, float* g_rgb, float* g_opa,
                                float* g_uv, float* g_conic, float* grad_rows, const uint32_t* contribution_masks,
                                void* stream) {
+    // the other stages' bits are accepted and ignored: depth/alpha is selected by the maps' gradients
+    if ((mode & ~(GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD)) != 0) return GSR_ERR_BAD_ARG;
+    const bool absgrad = (mode & GSR_MODE_ABSGRAD) != 0;
+    if (absgrad && grad_rows == nullptr) return GSR_ERR_BAD_ARG;  // slots 10-11 exist only in the interleaved rows
     if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;
     if (grad_image == nullptr || (grad_depth == nullptr) != (grad_alpha == nullptr)) return GSR_ERR_BAD_ARG;
     DepthSource ds;
@@ -1409,7 +1509,8 @@ int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* ke
         return GSR_ERR_BAD_ARG;
     }
     return launch_backward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
-                                 grad_depth != nullptr ? &ds : nullptr, nullptr, ranges, background, H, W, n_in, w_in,
+                                 grad_depth != nullptr ? &ds : nullptr, absgrad, nullptr, ranges, background, H, W,
+                                 n_in, w_in,
                                  grad_image, grad_depth, grad_alpha, g_rgb, g_opa, g_uv, g_conic, contribution_masks,
                                  stream);
 }

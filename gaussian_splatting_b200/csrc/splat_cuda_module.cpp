@@ -615,14 +615,17 @@ fused_render_forward(torch::Tensor records, torch::Tensor ranges, torch::Tensor 
 // per-gaussian gradient slab, rows indexed by gaussian; zero-filled, then accumulated into by the render backward.
 // Gather mode: interleaved rows [N,12] rgb3 opacity | uv2 conic0 conic1 | conic2 pad3 (vector reductions); with
 // grad_depth / grad_alpha [H,W,1] (the upstream gradients on the depth/alpha maps, with the forward's depth keys)
-// conic2 z pad2, z the gradient on the camera-frame z.  Record-stream mode: planar [9N] rgb [N,3] | opacity [N] |
-// uv [N,2] | conic [N,3].
+// conic2 z pad2, z the gradient on the camera-frame z.  mode: GSR_MODE_* bits, passed to gsr_render_backward_gather
+// (GSR_MODE_ABSGRAD: conic2 z|0 |u| |v|, the per-pixel absolute uv gradients summed).  Record-stream mode: planar [9N]
+// rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3].
 torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, int64_t P, torch::Tensor records,
                                     torch::Tensor ids_sorted, torch::Tensor ranges, torch::Tensor background,
                                     torch::Tensor n, torch::Tensor w, torch::Tensor masks,
                                     c10::optional<torch::Tensor> keys_sorted, int64_t id_bits, bool gather,
                                     c10::optional<torch::Tensor> grad_depth, c10::optional<torch::Tensor> grad_alpha,
-                                    c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits) {
+                                    c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits,
+                                    int64_t mode) {
+    TORCH_CHECK(gather || (mode & GSR_MODE_ABSGRAD) == 0, "absolute uv gradients come from the gather kernels only");
     CHECK_VALID_INPUT(grad_image); CHECK_FLOAT_TENSOR(grad_image);
     const int H = n.size(0), W = n.size(1);
     TORCH_CHECK(grad_image.dim() == 3 && grad_image.size(0) == H && grad_image.size(1) == W &&
@@ -647,7 +650,7 @@ torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, int64_t
     if (gather) {
         const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
         check_rc(gsr_render_backward_gather(
-                     F32PTR(records), ps.keys, (int)id_bits, ps.ids,
+                     (int)mode, F32PTR(records), ps.keys, (int)id_bits, ps.ids,
                      depth ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr, (uint32_t)depth_base,
                      (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w),
                      F32PTR(grad_image), depth ? F32PTR((*grad_depth)) : nullptr,
@@ -991,10 +994,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("fused_render_forward", &fused_render_forward,
           "tile renderer forward (with depth_key: also the depth and alpha maps)");
     m.def("fused_render_backward", &fused_render_backward,
-          "tile renderer backward -> per-gaussian gradient slab (with grad_depth / grad_alpha: rows incl. z)");
+          "tile renderer backward -> per-gaussian gradient slab (with grad_depth / grad_alpha: rows incl. z; "
+          "mode: MODE_* bits, MODE_ABSGRAD: rows incl. the absolute uv gradients)",
+          py::arg("grad_image"), py::arg("N"), py::arg("P"), py::arg("records"), py::arg("ids_sorted"),
+          py::arg("ranges"), py::arg("background"), py::arg("n"), py::arg("w"), py::arg("masks"),
+          py::arg("keys_sorted"), py::arg("id_bits"), py::arg("gather"), py::arg("grad_depth"), py::arg("grad_alpha"),
+          py::arg("depth_key"), py::arg("depth_base"), py::arg("depth_bits"), py::arg("mode") = 0);
     m.def("fused_preprocess_backward", &fused_preprocess_backward, "fused per-gaussian backward (mode: MODE_* bits)");
     m.attr("MODE_DEPTH_ALPHA") = GSR_MODE_DEPTH_ALPHA;
     m.attr("MODE_ANTIALIASED") = GSR_MODE_ANTIALIASED;
+    m.attr("MODE_ABSGRAD") = GSR_MODE_ABSGRAD;
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");

@@ -25,12 +25,28 @@ class DensificationStats:
         self.xyz_grad_accum = torch.zeros(n_gaussians, 3, dtype=dtype, device=device)
         self.grad_accum_count = torch.zeros(n_gaussians, dtype=torch.int32, device=device)
 
-    def accumulate(self, state, uv: torch.Tensor, xyz: torch.Tensor, K: torch.Tensor) -> None:
+    def accumulate(self, state, uv: torch.Tensor, xyz: torch.Tensor, K: torch.Tensor, absgrad: bool = False) -> None:
         """state: the `_ViewState` rasterize(..., return_state=True) returned; uv: the compact uv it returned (with
         `.grad` retained); xyz: the position parameter (with `.grad`); K: the camera's 3x3 intrinsic matrix.
-        Like the reference, scales `uv.grad` by the focal lengths in place."""
-        assert uv.grad is not None, "call uv.retain_grad() before backward()"
-        native().densify_accumulate(state.vis_idx32, uv.grad, xyz.grad.contiguous(), K.contiguous(),
+        Like the reference, scales `uv.grad` by the focal lengths in place.
+
+        absgrad=True (the view rendered with rasterize(..., absgrad=True)): accumulates `uv.absgrad`, the per-pixel
+        absolute screen-space gradients summed (AbsGS), instead of |uv.grad|, scaled in place the same way; uv.grad
+        need not be retained.  Consequences for `plan_adaptive_density_control`, which reads the accumulator as
+        before:
+          * the default percentile selection (use_fractional_densification) works as is; a fixed uv_grad_threshold is
+            on a different scale (absgrad >= |uv.grad|, often several times larger) and must be retuned;
+          * the "zero gradient" delete rule deletes fewer splats: a splat whose per-pixel pulls cancelled exactly has
+            a zero uv.grad but a non-zero absgrad, and is kept."""
+        if absgrad:
+            g = state.uv_absgrad  # the tensor uv.absgrad also refers to
+            if g is None:
+                raise RuntimeError("accumulate(absgrad=True) needs a view rendered with rasterize(..., absgrad=True) "
+                                   "and its backward")
+        else:
+            assert uv.grad is not None, "call uv.retain_grad() before backward()"
+            g = uv.grad
+        native().densify_accumulate(state.vis_idx32, g, xyz.grad.contiguous(), K.contiguous(),
                                     self.uv_grad_accum, self.xyz_grad_accum, self.grad_accum_count)
 
 

@@ -245,7 +245,7 @@ class _ViewState:
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges", "stream_rec", "gather",
                  "records", "keys_sorted", "id_bits", "slab_width",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
-                 "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha")
+                 "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad")
 
     @property
     def ids_sorted(self):
@@ -267,9 +267,11 @@ class _ViewState:
         self.image = None
         self.speculation_overflowed = False
         # MODE_* bits of the native fused path: MODE_DEPTH_ALPHA (render_depth_alpha: the tile kernels also produce
-        # depth / alpha [H,W,1]), MODE_ANTIALIASED (opacity compensation for the 0.25 px^2 dilation)
+        # depth / alpha [H,W,1]), MODE_ANTIALIASED (opacity compensation for the 0.25 px^2 dilation), MODE_ABSGRAD
+        # (the render backward also sums |d loss_p / d uv| per pixel)
         self.mode = 0
         self.depth = self.alpha = None
+        self.uv_absgrad = None  # MODE_ABSGRAD: [M,2], set by every render backward
 
 
 class _stage:
@@ -449,12 +451,20 @@ class _CompositeTiles(torch.autograd.Function):
                 grad_image.contiguous(), st.N, st.P, st.records if st.gather else st.stream_rec, st._ids_sorted,
                 st.ranges, st.background, st.n_per_pixel, st.w_per_pixel, st.masks, st.keys_sorted, st.id_bits,
                 st.gather, None if grad_depth is None else grad_depth.contiguous(),
-                None if grad_alpha is None else grad_alpha.contiguous(), st.zkey, st.depth_base, st.depth_bits)
+                None if grad_alpha is None else grad_alpha.contiguous(), st.zkey, st.depth_base, st.depth_bits,
+                st.mode)
+        uv_t = st.uv_ref() if st.uv_ref is not None else None
+        if st.mode & native().MODE_ABSGRAD:
+            # sum over pixels of |d loss_p / d uv| (rows' slots 10-11), in the compact order of uv; replaced, not
+            # accumulated, by every backward.  Also set as uv.absgrad (gsplat's convention) while uv is alive.  The two
+            # columns are selected before the rows: gathering whole 48-byte rows first costs 1.5 ms at 3M (H100)
+            st.uv_absgrad = slab.view(st.N, 12)[:, 10:12].index_select(0, st.vis_idx)
+            if uv_t is not None:
+                uv_t.absgrad = st.uv_absgrad
         # The render pass's gradient on the compact uv is a gather of the slab's uv section (28 us at 3M).  It
         # reaches the per-gaussian backward through the slab anyway, so it is only materialised when it can be
         # OBSERVED: the caller retained uv's gradient (the reference trainer does, splat_py/trainer.py:360) or
         # hooked the tensor.
-        uv_t = st.uv_ref() if st.uv_ref is not None else None
         watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
         st.uv_grad_emitted = bool(watched)
         if not watched:
@@ -469,7 +479,7 @@ class _CompositeTiles(torch.autograd.Function):
 
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
-              render_depth_alpha=False, antialiased=False):
+              render_depth_alpha=False, antialiased=False, absgrad=False):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
@@ -479,7 +489,20 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     antialiased=True: every splat's opacity is multiplied by rho = sqrt(max(det S, 0) / det(S + 0.25 I)), S its 2-D
     covariance, so that the 0.25 px^2 dilation the renderer applies no longer adds mass to splats smaller than a pixel
     (the "antialiased" mode of Mip-Splatting's 2-D filter).  Gradients flow through rho to the covariance.  Return
-    values are unchanged; combines with render_depth_alpha.  fp32 and precomputed SH colours only."""
+    values are unchanged; combines with render_depth_alpha.  fp32 and precomputed SH colours only.
+
+    absgrad=True: the render backward also sums, per visible gaussian, the ABSOLUTE value of every pixel's gradient on
+    its projected mean, sum_p |d <G_p, out_p> / d uv| (AbsGS; gsplat's absgrad), where uv.grad sums the signed values
+    and lets opposite pulls of the pixels under a large splat cancel.  After each backward it is uv.absgrad [M,2] (set
+    on the returned uv while that tensor is alive; no retain_grad() needed) and state.uv_absgrad, replaced, not
+    accumulated.  Pixels in units, like uv.grad; only the render stage's part (not a gradient the caller adds on uv);
+    G_p includes the depth / alpha maps' upstream gradients with render_depth_alpha.  For densification:
+    DensificationStats.accumulate(..., absgrad=True).  Return values, uv.grad and all gradients are unchanged;
+    combines with render_depth_alpha and antialiased.  fp32 and precomputed SH colours only."""
+    if absgrad and gaussians.xyz.dtype != torch.float32:
+        raise TypeError("absgrad needs fp32 inputs (the fused rasterizer's render backward forms it)")
+    if absgrad and gaussians.sh is not None and not use_sh_precompute:
+        raise ValueError("absgrad needs use_sh_precompute=True (per-pixel SH colours are not supported)")
     if antialiased and gaussians.xyz.dtype != torch.float32:
         raise TypeError("antialiased needs fp32 inputs (the fp64 renderer applies no dilation to compensate)")
     if antialiased and gaussians.sh is not None and not use_sh_precompute:
@@ -494,7 +517,8 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     ext = native()
     state = _ViewState(profile)
     state.grad_out = grad_out
-    state.mode = (ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
+    state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
+                  | (ext.MODE_ABSGRAD if absgrad else 0))
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))

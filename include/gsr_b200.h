@@ -38,11 +38,13 @@ extern "C" {
 /* floats per packed splat record consumed by the tile renderers (48 bytes) */
 #define GSR_REC_FLOATS 12
 
-/* Modes of the fused per-Gaussian stage (`mode` of gsr_preprocess_forward / gsr_preprocess_backward), a bit mask.
- * The tile renderers take no mode word: gsr_render_*_gather run in depth/alpha mode when they are given the depth
- * and alpha maps (forward) or their upstream gradients (backward). */
+/* Modes of the fused rasterizer, a bit mask: the `mode` of gsr_preprocess_forward / gsr_preprocess_backward and of
+ * gsr_render_backward_gather, so a caller passes one mode word to every stage; each stage ignores the bits that do not
+ * concern it.  The tile renderers run in depth/alpha mode when they are given the depth and alpha maps (forward) or
+ * their upstream gradients (backward). */
 #define GSR_MODE_DEPTH_ALPHA 1 /* gradient rows carry the render backward's camera-frame z gradient */
 #define GSR_MODE_ANTIALIASED 2 /* opacity compensation for the renderer's 0.25 px^2 dilation */
+#define GSR_MODE_ABSGRAD 4     /* gradient rows also carry sum over pixels of |d loss_p / d uv| (AbsGS) */
 
 /* library identification: returns e.g. "gsr_b200 0.1 sm_90a" */
 const char* gsr_version(void);
@@ -190,9 +192,16 @@ int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* key
  * Depth/alpha mode: grad_depth and grad_alpha [H,W] non-NULL (both or neither; zeros where a map has no gradient),
  * the depth descriptor as in the forward, grad_rows required; the rows are then rgb3 opacity | uv2 conic0 conic1 |
  * conic2 z pad2, z being the gradient on the camera-frame z, which gsr_preprocess_backward consumes with
- * GSR_MODE_DEPTH_ALPHA. */
+ * GSR_MODE_DEPTH_ALPHA.
+ * mode: GSR_MODE_* bits; only GSR_MODE_ABSGRAD changes this stage (other known bits are ignored, unknown ones are
+ * GSR_ERR_BAD_ARG).  It requires grad_rows; the rows' last four floats are then conic2 z|0 |u| |v|, flushed as one
+ * more 16-byte vector reduction, with
+ *   |u| = sum over pixels p of |d <G_p, out_p> / d u|,  |v| likewise,
+ * G_p the upstream gradients at pixel p (image, and depth / alpha when given): the absolute value is taken per pixel
+ * before summing, so pulls in opposite directions do not cancel (AbsGS).  Units are pixels, like grad_uv.
+ * gsr_preprocess_backward does not read slots 10-11. */
 #define GSR_GRAD_ROW_FLOATS 12
-int gsr_render_backward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+int gsr_render_backward_gather(int mode, const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
                                const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
                                int depth_bits, const int32_t* tile_ranges, const float* background_rgb, int H, int W,
                                const int32_t* num_splats_per_pixel, const float* final_weight_per_pixel,
@@ -327,7 +336,8 @@ int gsr_gather_records_keys(int P, int id_bits, const uint64_t* keys_sorted, con
  * inclusive scan of gsr_preprocess_forward) — what a caller added upstream of uv, or the total autograd hands over.
  * grad_rows != NULL: the interleaved rows of gsr_render_backward_gather instead of the four planar arrays
  * (grad_uv == NULL then still means "skip the render backward's uv sums").
- * mode: the GSR_MODE_* bits of the forward and the render backward; either bit requires grad_rows (16-byte aligned).
+ * mode: the GSR_MODE_* bits of the forward and the render backward; any bit requires grad_rows (16-byte aligned).
+ *   GSR_MODE_ABSGRAD changes nothing here (the rows' slots 10-11 are not read).
  *   GSR_MODE_DEPTH_ALPHA: the rows of the depth/alpha render backward: row slot 9, the gradient on the camera-frame z,
  *   joins grad_xyz as camera_T_world[2, :3] * g_z.  No gradient goes to the pose.
  *   GSR_MODE_ANTIALIASED: the rows' opacity slot g is the gradient on the compensated opacity sigmoid(o) * rho:

@@ -56,6 +56,9 @@ def main():
     ap.add_argument("--antialiased", action="store_true",
                     help="rasterize(antialiased=True): opacity compensation for the 0.25 px^2 dilation, in training and "
                          "evaluation")
+    ap.add_argument("--absgrad", action="store_true",
+                    help="rasterize(absgrad=True) in training, and densification statistics accumulated from uv.absgrad "
+                         "(per-pixel absolute screen-space gradients, AbsGS) instead of |uv.grad|")
     a = ap.parse_args()
 
     real_stdout = os.fdopen(os.dup(1), "w")
@@ -207,8 +210,9 @@ def main():
         image, mask, uv, state = rasterize(g, im.camera_T_world, cams[im.camera_id], config.near_thresh,
                                            config.far_thresh, config.cull_mask_padding, config.mh_dist,
                                            config.use_sh_precompute, background, return_state=True,
-                                           grad_out=grads_sym, antialiased=a.antialiased)
-        uv.retain_grad()
+                                           grad_out=grads_sym, antialiased=a.antialiased, absgrad=a.absgrad)
+        if not a.absgrad:
+            uv.retain_grad()
         if timed:
             ev[1].record()
         if a.loss == "fused":
@@ -222,7 +226,7 @@ def main():
             ev[2].record()
         # per-view statistics BEFORE the collective: they are this rank's own view (trainer.py:376-385); the xyz
         # gradient they use is this view's, so they are taken from the still un-averaged buffer
-        stats.accumulate(state, uv, g.xyz, cams[im.camera_id].K)
+        stats.accumulate(state, uv, g.xyz, cams[im.camera_id].K, absgrad=a.absgrad)
         if sharded:
             opt.step()  # barrier, reduce-scatter + Adam + all-gather in one kernel over peer memory, barrier
         else:
@@ -278,7 +282,7 @@ def main():
                           if world > 1 else "FlatAdam (gsr_adam_step)"),
             "loss": ("fused: photometric_loss (gsr_photometric_loss_forward / _backward), ssim() in evaluation"
                      if a.loss == "fused" else "shim: l1_loss + SSIM stand-in (tools/e2e/shims) through NCHW views"),
-            "antialiased": a.antialiased,
+            "antialiased": a.antialiased, "absgrad": a.absgrad,
             "device": torch.cuda.get_device_name(local),
         }
         real_stdout.write("E2E " + json.dumps(line) + "\n")
