@@ -241,7 +241,9 @@ __global__ void __launch_bounds__(TILE_PIXELS)
         const float mh = (c * du * du - (b + b) * du * dv + a * dv * dv) / det;
         float alpha = 0.0f;
         if (mh > 0.0f) alpha = opacity[g] * __expf(-0.5f * mh);
-        A += alpha * (1.0f - A);
+        // the reference forms the weight in double (its `1.0` literal) and rounds it once; an fp32 FMA differs
+        const float w = (float)((1.0 - (double)A) * (double)alpha);
+        A += w;
         if (A > alpha_threshold) {
             const float x = xyz_cam[g * 3 + 0], y = xyz_cam[g * 3 + 1], z = xyz_cam[g * 3 + 2];
             out = sqrtf(x * x + y * y + z * z);  // range, not z (src/depth.cu:102-105)
