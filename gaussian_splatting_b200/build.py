@@ -128,6 +128,15 @@ def build_ext(force: bool = False) -> Path:
     return out
 
 
+def build_render_variant(out_dir, flags) -> Path:
+    """The tile renderers alone (gsr_render.cu: the gsr_render_* entry points of the C ABI) compiled with extra -D
+    flags into out_dir/libgsr_render_variant.so, for A/B checks of compile-time alternatives (not used by the
+    package; out_dir should lie outside the tree)."""
+    out = Path(out_dir) / "libgsr_render_variant.so"
+    _run([_nvcc(), *NVCC_FLAGS, *flags, "-shared", "-cudart", "shared", str(CSRC / "gsr_render.cu"), "-o", str(out)])
+    return out
+
+
 def build(force: bool = False, verbose: bool = False):
     lib = build_lib(force=force, verbose=verbose)
     ext = build_ext(force=force)

@@ -8,9 +8,9 @@ namespace gsr {
 // Culling bound stored in the record: tau' such that a pixel at offset d from the mean with
 // d^T Sigma^-1 d > tau' provably has alpha = opacity * exp(-mh/2) below the reference's 1/255 skip
 // threshold (alpha < t  <=  mh > 2 ln(opacity / t)).  tau' is the exact bound inflated by 6% plus a
-// condition-number term, and the footprint tests add 1 px^2 of slack, so that neither the fp32 rounding of
-// mh in the kernels nor the few-ulp error of ex2.approx can make a culled pixel pass the reference's test;
-// culling is therefore invisible in the results (checked bitwise against the reference).
+// condition-number term, so that neither the fp32 rounding of mh in the kernels nor the few-ulp error of
+// ex2.approx can make a culled pixel pass the reference's test (row_cull adds only margins for its own fp32
+// evaluation); culling is therefore invisible in the results (checked bitwise against the reference).
 // Returns -1 when the splat can never reach the threshold, +inf when nothing can be proven.
 __device__ __forceinline__ float cull_tau(float a, float bh, float c, float det, float opa) {
     if (!(opa > 0.0039137f)) return -1.0f;  // 0.998 / 255: opacity * g <= opacity can never reach 1/255
@@ -44,6 +44,85 @@ __device__ __forceinline__ FootprintBounds footprint_bounds(float tau, float a, 
 __device__ __forceinline__ bool footprint_hits(const FootprintBounds& f, float dx, float dy) {
     const float dx2 = dx * dx, dy2 = dy * dy;
     return (dx2 + dy2 <= f.r2) && (dx2 <= f.hx2) && (dy2 <= f.hy2);
+}
+
+__device__ __forceinline__ float sqrt_approx(float x) {  // MUFU, a few ulps; 0 for x <= 2^-126
+    float y;
+    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+__device__ __forceinline__ float rcp_approx(float x) {
+    float y;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
+
+// Exact culling of a row band of pixel blocks.  The blocks share the rows y0 .. y0+3 (the slab dv in [lo, hi],
+// dv = y - v) and differ only in their columns.  Per record this computes the x-interval of the ellipse
+// E = {d^T Sigma^-1 d <= tau'} intersected with the slab; a block of columns x0 .. x0+w is then hit iff
+// xlo <= x0 - u <= xhi (row_block_hits: one subtraction and two compares per block).
+//
+// At fixed dv, E spans du in (bh dv -+ sqrt(det (tau' c - dv^2))) / c.  The right end R(dv) is concave with its
+// maximum sqrt(tau' a) at dv* = bh sqrt(tau'/a) (the ellipse's rightmost point), the left end L(dv) = -R(-dv)
+// convex with its minimum at -dv*.  So over the slab: max R = sqrt(tau' a) if dv* lies in the slab, else R at
+// the slab end nearer dv*; likewise min L.
+//
+// Conservative by construction, in exact arithmetic and in fp32:
+//   * tau' keeps its margin (cull_tau): pixels outside E cannot reach the 1/255 skip threshold.
+//   * The interval is evaluated for tau'(1 + 2^-18): the rounding of tau' c and of dv^2 (2^-24 relative each) can
+//     then never make tau' c - dv^2 smaller than its exact value, even where it cancels to 0 at the ellipse's top
+//     and bottom (where the square root would amplify a rounding error into 2^-12 of the width).
+//   * The slab ends carry a rounding error of 2^-24 |lo|, dv* one of a few ulps; e = 2^-18 (|lo| + |hi| + |dv*|)
+//     exceeds both.  dv* counts as inside when it is within 2e of the slab; otherwise the end is moved by e
+//     TOWARDS dv*, where R (L) is monotone, so the evaluated end is never below (above) the exact one.
+//   * The interval is widened by m = 2^-18 sqrt(tau' a) + 2^-12 px: every term of R and L is at most
+//     sqrt(tau' a) in size, so the few-ulp errors of the MUFU square roots and reciprocals, the products and
+//     x0 - u stay below the relative part; the absolute part covers coordinates' ulps and flushed denormals.
+//   * The result is never looser than the previous circle-and-box test (footprint_bounds): the row test is that
+//     test's y box intersected with the exact y extent tau'(1 + 2^-18) c, the interval is clipped to that test's
+//     x box sqrt(tau' a + 1) shrunk by 2^-19 (its rounding and the square root's), and the few-ulp margins above
+//     stay inside the bounding circle's 1.0001 lambda_max + 1 px^2.  Where the 1 px^2 of the box falls below
+//     those 2^-19 (sqrt(tau' a) > 512 px) the clip can cut pixels with d^T Sigma^-1 d > tau'(1 - 2^-18), which
+//     tau''s 6 % margin covers.
+//   * Sentinels need no branch: tau' < 0 fails the row test (its y extent is negative); tau' = +inf (and any
+//     overflow) turns the ends into +-inf or NaN, and fminf / fmaxf against the box (then infinite) list the
+//     block.
+// tests/cull_oracle.c restates this in C; its test checks every culled block against the kernel's per-pixel alpha.
+struct RowCull {
+    float xlo, xhi;  // x0 - u of a block of columns x0 .. x0+w must lie in [xlo, xhi]
+    bool rows;       // the record's ellipse reaches rows y0 .. y0+3 at all
+};
+__device__ __forceinline__ RowCull row_cull(float v, float tau, float a, float b2, float c, float det, float y0,
+                                            float w) {
+    constexpr float GROW = 1.0f + 0x1p-18f, EREL = 0x1p-18f, MABS = 0x1p-12f, BOX_SHRINK = 1.0f - 0x1p-19f;
+    RowCull r;
+    const float bh = 0.5f * b2;
+    const float lo = y0 - v, hi = (y0 + 3.0f) - v;
+    const float dy = fmaxf(fmaxf(lo, -hi), 0.0f);
+    const float te = tau * GROW;
+    const float tc = te * c;
+    r.rows = dy * dy <= fminf(tc, fmaf(tau, c, 1.0f));
+    const float X = sqrt_approx(te * a);
+    const float ds = bh * X * rcp_approx(a);
+    const float e = (fabsf(lo) + fabsf(hi) + fabsf(ds)) * EREL;
+    const float lo1 = lo - e, hi1 = hi + e, lo2 = lo1 - e, hi2 = hi1 + e;
+    const float slo = sqrt_approx(det * fmaxf(fmaf(-lo1, lo1, tc), 0.0f));
+    const float shi = sqrt_approx(det * fmaxf(fmaf(-hi1, hi1, tc), 0.0f));
+    const float rc = rcp_approx(c);
+    const bool rup = ds > hi2, lup = -ds > hi2;
+    float R = fmaf(bh, rup ? hi1 : lo1, rup ? shi : slo) * rc;
+    float L = fmaf(bh, lup ? hi1 : lo1, -(lup ? shi : slo)) * rc;
+    R = (ds >= lo2 && !rup) ? X : R;
+    L = (-ds >= lo2 && !lup) ? -X : L;
+    const float m = fmaf(X, EREL, MABS);
+    const float B = sqrt_approx(fmaf(tau, a, 1.0f)) * BOX_SHRINK;
+    r.xhi = fminf(R + m, B);
+    r.xlo = fmaxf(L - m, -B) - w;
+    return r;
+}
+// NaN-safe: an interval end that is NaN lists the block
+__device__ __forceinline__ bool row_block_hits(const RowCull& r, float dx0) {
+    return r.rows & !(dx0 > r.xhi) & !(dx0 < r.xlo);
 }
 
 // Anti-aliased mode: the opacity factor rho = sqrt(max(det0, 0) / det) that gives the dilated splat the mass of the

@@ -265,7 +265,12 @@ __device__ __forceinline__ bool stage_checkout(int* cnt, int lane) {
 
 // Compact, per lane group, the indices of the staged records whose footprint can touch that group's pixel
 // block (ascending record order).  list: [GROUPS][BATCH] bytes of this warp.  cnt[g] = list lengths
-// (warp-uniform).  Lane l tests records l, l+32, ... against all blocks.
+// (warp-uniform).  Lane l tests records l, l+32, ... against all blocks: the exact ellipse-vs-block test
+// (row_cull, gsr_record.cuh), or with -DGSR_CULL_BOX=1 the looser bounding circle AND box it refines (kept to
+// check that both give the same bits, tests/test_fwd_culling_gpu.py).
+#ifndef GSR_CULL_BOX
+#define GSR_CULL_BOX 0
+#endif
 template <bool WANT_UNSAFE = false>
 __device__ __forceinline__ bool build_lists(const float4* __restrict__ rec4, int cnt, int lane, float wx0,
                                             float wy0, uint8_t* __restrict__ list, int (&cnts)[GROUPS]) {
@@ -282,14 +287,22 @@ __device__ __forceinline__ bool build_lists(const float4* __restrict__ rec4, int
         if (j < cnt) {
             const float4 q0 = rec4[j * 3];
             const float4 q1 = rec4[j * 3 + 1];
+#if GSR_CULL_BOX
             const float dy = fmaxf(fmaxf(wy0 - q0.y, q0.y - (wy0 + 3.0f)), 0.0f);
             const FootprintBounds fb = footprint_bounds(q0.z, q1.x, q1.y, q1.z);
+#else
+            const RowCull rc = row_cull(q0.y, q0.z, q1.x, q1.y, q1.z, q1.w, wy0, (float)(GROUP_W - 1));
+#endif
             bool any = false;
 #pragma unroll
             for (int g = 0; g < GROUPS; ++g) {
                 const float x0 = wx0 + (float)(g * GROUP_W);
+#if GSR_CULL_BOX
                 const float dx = fmaxf(fmaxf(x0 - q0.x, q0.x - (x0 + (float)(GROUP_W - 1))), 0.0f);
                 hit[g] = footprint_hits(fb, dx, dy);
+#else
+                hit[g] = row_block_hits(rc, x0 - q0.x);
+#endif
                 any |= hit[g];
             }
             // the hoisted-reciprocal division is exact only for |det| in [1e-18, 1e18]
@@ -634,6 +647,9 @@ __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* _
                                              &s_z[s][0]);
             }
             if (lane == 0) { STAT(5, cnts[0] + cnts[1]); STAT(6, 2 * cnt); }
+#ifdef GSR_STATS
+            if (lane == 0) { int sum = 0; for (int g = 0; g < GROUPS; ++g) sum += cnts[g]; STAT(4, sum); STAT(7, 1); }
+#endif
         }
         if (stage_checkout(&s_cnt[s], lane) && b + STAGES < nb) {  // warp-uniform: this warp left the stage last
             if (GATHER) {
@@ -1031,6 +1047,7 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
         asm volatile("" : "+r"(base_idx));  // likewise held in a register (ptxas re-derived it from k and nb per step)
 #ifdef GSR_STATS
         if (lane == 0) { STAT(8, iters); STAT(10, cnts[0] + cnts[1]); STAT(13, 1); STAT(14, cnt); }
+        if (lane == 0) { int sum = 0; for (int g = 0; g < GROUPS; ++g) sum += cnts[g]; STAT(15, sum); }
 #endif
 
         // BG: handle the background term of a pixel's FIRST contribution (src/render_backward.cu:172-181).
