@@ -25,6 +25,7 @@ LIB = PKG / "libgsr_b200.so"
 CU_SOURCES = [
     "gsr_pergaussian.cu",
     "gsr_preprocess.cu",
+    "gsr_filter3d.cu",
     "gsr_binning.cu",
     "gsr_render.cu",
     "gsr_render_generic.cu",

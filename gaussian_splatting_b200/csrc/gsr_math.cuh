@@ -106,14 +106,10 @@ __device__ __forceinline__ void quat_to_rot(T qw, T qx, T qy, T qz, T* __restric
     R[8] = A::fma(y2, -qy, omx);
 }
 
+// Sigma_world = R diag(v) R^T from the rotation and the per-axis variances v_k
 template <typename T>
-__device__ __forceinline__ void sigma_world(T qw, T qx, T qy, T qz, T s0, T s1, T s2,
-                                            T* __restrict__ S /*6*/) {
+__device__ __forceinline__ void sigma_from_rv(const T* __restrict__ R, T v0, T v1, T v2, T* __restrict__ S /*6*/) {
     using A = Ar<T>;
-    T R[9];
-    quat_to_rot<T>(qw, qx, qy, qz, R);
-    const T e0 = A::exp(s0), e1 = A::exp(s1), e2 = A::exp(s2);
-    const T v0 = A::mul(e0, e0), v1 = A::mul(e1, e1), v2 = A::mul(e2, e2);
     // S_ab = fma(v2, Ra2*Rb2, fma(v0, Ra0*Rb0, v1*(Ra1*Rb1)))
 #define GSR_SAB(a, b)                                                                        \
     A::fma(v2, A::mul(R[3 * a + 2], R[3 * b + 2]),                                           \
@@ -125,6 +121,24 @@ __device__ __forceinline__ void sigma_world(T qw, T qx, T qy, T qz, T s0, T s1, 
     S[4] = GSR_SAB(1, 2);
     S[5] = GSR_SAB(2, 2);
 #undef GSR_SAB
+}
+
+template <typename T>
+__device__ __forceinline__ void sigma_world(T qw, T qx, T qy, T qz, T s0, T s1, T s2,
+                                            T* __restrict__ S /*6*/) {
+    using A = Ar<T>;
+    T R[9];
+    quat_to_rot<T>(qw, qx, qy, qz, R);
+    const T e0 = A::exp(s0), e1 = A::exp(s1), e2 = A::exp(s2);
+    sigma_from_rv<T>(R, A::mul(e0, e0), A::mul(e1, e1), A::mul(e2, e2), S);
+}
+
+// Sigma_world from given per-axis variances (the 3-D filter's exp(s)^2 + f^2, gsr_record.cuh f3d_filter)
+template <typename T>
+__device__ __forceinline__ void sigma_world_var(T qw, T qx, T qy, T qz, T v0, T v1, T v2, T* __restrict__ S /*6*/) {
+    T R[9];
+    quat_to_rot<T>(qw, qx, qy, qz, R);
+    sigma_from_rv<T>(R, v0, v1, v2, S);
 }
 
 // ---------------------------------------------------------------------------

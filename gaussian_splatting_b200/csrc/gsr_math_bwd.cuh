@@ -83,12 +83,12 @@ __device__ __forceinline__ void conic_bwd(const T* __restrict__ S /*9*/, const T
         for (int c = 0; c < 2; ++c) gJ[c * 3 + r] = gJt[r * 2 + c];
 }
 
-// VJP of Sigma_world wrt (quaternion, log-scale).  Reference: src/projection_backward.cu:185-314.
+// VJP of Sigma_world = R diag(e)^2 R^T wrt the quaternion and, through de[k] = d e_k / d s_k, the log-scale s.
+// Reference: src/projection_backward.cu:185-314.
 template <typename T>
-__device__ __forceinline__ void sigma_world_bwd(T qw, T qx, T qy, T qz, T s0, T s1, T s2,
-                                                const T* __restrict__ G /*9*/, T* __restrict__ gq /*4 wxyz*/,
-                                                T* __restrict__ gs /*3*/) {
-    const T e[3] = {Ar<T>::exp(s0), Ar<T>::exp(s1), Ar<T>::exp(s2)};
+__device__ __forceinline__ void sigma_world_bwd_e(T qw, T qx, T qy, T qz, const T* __restrict__ e /*3*/,
+                                                  const T* __restrict__ de /*3*/, const T* __restrict__ G /*9*/,
+                                                  T* __restrict__ gq /*4 wxyz*/, T* __restrict__ gs /*3*/) {
     const T nq = Ar<T>::sqrt(qw * qw + qx * qx + qy * qy + qz * qz);
     const T w = qw / nq, x = qx / nq, y = qy / nq, z = qz / nq;
     T R[9];
@@ -122,7 +122,7 @@ __device__ __forceinline__ void sigma_world_bwd(T qw, T qx, T qy, T qz, T s0, T 
     mm<T, 3, 3, 3>(Rt, gRS, gSa);
     mm<T, 3, 3, 3>(gSR, R, gSb);
 #pragma unroll
-    for (int k = 0; k < 3; ++k) gs[k] = (gSa[k * 4] + gSb[k * 4]) * e[k];
+    for (int k = 0; k < 3; ++k) gs[k] = (gSa[k * 4] + gSb[k * 4]) * de[k];
 
     T gn[4];
     gn[0] = -T(2) * z * gR[1] + T(2) * y * gR[2] + T(2) * z * gR[3] - T(2) * x * gR[5] -
@@ -139,6 +139,32 @@ __device__ __forceinline__ void sigma_world_bwd(T qw, T qx, T qy, T qz, T s0, T 
     const T dot = q[0] * gn[0] + q[1] * gn[1] + q[2] * gn[2] + q[3] * gn[3];
 #pragma unroll
     for (int i = 0; i < 4; ++i) gq[i] = gn[i] / nq - q[i] * dot / n3;
+}
+
+template <typename T>
+__device__ __forceinline__ void sigma_world_bwd(T qw, T qx, T qy, T qz, T s0, T s1, T s2,
+                                                const T* __restrict__ G /*9*/, T* __restrict__ gq /*4 wxyz*/,
+                                                T* __restrict__ gs /*3*/) {
+    const T e[3] = {Ar<T>::exp(s0), Ar<T>::exp(s1), Ar<T>::exp(s2)};
+    sigma_world_bwd_e<T>(qw, qx, qy, qz, e, e, G, gq, gs);
+}
+
+// 3-D filter (Mip-Splatting): Sigma = R diag(v + F) R^T with v_k = e_k^2.  The quaternion gradient is the plain one at
+// e'_k = sqrt(v_k + F); the scale chain is d/ds_k (v_k + F) = 2 v_k, i.e. the plain one with de'_k = v_k / e'_k.
+// F == 0 selects e' = de' = e, the unfiltered VJP.
+template <typename T>
+__device__ __forceinline__ void sigma_world_bwd_f3d(T qw, T qx, T qy, T qz, const T* __restrict__ e /*3*/,
+                                                    const T* __restrict__ v /*3*/, const T* __restrict__ vp /*3*/,
+                                                    T F, const T* __restrict__ G /*9*/, T* __restrict__ gq /*4*/,
+                                                    T* __restrict__ gs /*3*/) {
+    T ep[3], dep[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const T r = Ar<T>::sqrt(vp[k]);
+        ep[k] = F == T(0) ? e[k] : r;
+        dep[k] = F == T(0) ? e[k] : v[k] / r;
+    }
+    sigma_world_bwd_e<T>(qw, qx, qy, qz, ep, dep, G, gq, gs);
 }
 
 }  // namespace gsr

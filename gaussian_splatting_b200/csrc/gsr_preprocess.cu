@@ -153,8 +153,10 @@ __device__ __forceinline__ void coop_copy(float* __restrict__ dst, const float* 
         far_t, pad, mh, ntx, nty, depth_base, records, zkey, visible, packed, tile_mask, tile_win, use_tma
 // ANTIALIAS: the record's opacity is sigmoid(o) * aa_rho(conic) (gsr_record.cuh); the culling bound tau' is formed
 // from that compensated opacity
-template <int N_SH, bool HAS_SH, bool ANTIALIAS>
-__device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS) {
+// FILTER3D: Mip-Splatting's 3-D filter, f = filter3d[i]: Sigma_world is formed from the variances exp(s)^2 + f^2 and
+// the opacity is multiplied by coef before rho (gsr_record.cuh f3d_filter)
+template <int N_SH, bool HAS_SH, bool ANTIALIAS, bool FILTER3D>
+__device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* __restrict__ filter3d) {
     constexpr int NR3 = HAS_SH ? 3 * (N_SH - 1) : 1;
     __shared__ ViewConsts vc;
     __shared__ __align__(128) float s_sh[PRE_THREADS * NR3];       // SH coefficients of the CTA's gaussians
@@ -209,8 +211,18 @@ __device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS) {
         visible[i] = vis ? 1 : 0;
         uint64_t pk = 0ull;
         if (vis) {
-            float S6[6], S9[9], J[6], W[9], conic[3];
-            sigma_world<float>(q0, q1, q2, q3, sc0, sc1, sc2, S6);
+            float S6[6], S9[9], J[6], W[9], conic[3], coef = 1.0f;
+            if (FILTER3D) {
+                const float f = filter3d[i];
+                const float F = __fmul_rn(f, f);
+                const float e0 = expf(sc0), e1 = expf(sc1), e2 = expf(sc2);
+                const float v[3] = {__fmul_rn(e0, e0), __fmul_rn(e1, e1), __fmul_rn(e2, e2)};
+                float vp[3], t[3];
+                coef = f3d_filter(v, F, vp, t);
+                sigma_world_var<float>(q0, q1, q2, q3, vp[0], vp[1], vp[2], S6);
+            } else {
+                sigma_world<float>(q0, q1, q2, q3, sc0, sc1, sc2, S6);
+            }
             sym6_to_full(S6, S9);
             proj_jacobian<float>(px, py, pz, vc.K[0], vc.K[4], J);
             W[0] = vc.T[0]; W[1] = vc.T[1]; W[2] = vc.T[2];
@@ -219,6 +231,7 @@ __device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS) {
             conic_from<float>(S9, J, W, conic, nullptr);
 
             float opa = sigmoid_torch(opl);
+            if (FILTER3D) opa = __fmul_rn(opa, coef);
             if (ANTIALIAS) opa = __fmul_rn(opa, aa_rho(conic[0], conic[1], conic[2]));
             float dc[3] = {dc0, dc1, dc2};
             float col[3];
@@ -284,11 +297,24 @@ __device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS) {
 
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, 7) k_preprocess_fwd(GSR_PRE_FWD_PARAMS) {
-    preprocess_fwd<N_SH, HAS_SH, false>(GSR_PRE_FWD_FORWARD);
+    preprocess_fwd<N_SH, HAS_SH, false, false>(GSR_PRE_FWD_FORWARD, nullptr);
 }
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, 7) k_preprocess_fwd_aa(GSR_PRE_FWD_PARAMS) {
-    preprocess_fwd<N_SH, HAS_SH, true>(GSR_PRE_FWD_FORWARD);
+    preprocess_fwd<N_SH, HAS_SH, true, false>(GSR_PRE_FWD_FORWARD, nullptr);
+}
+#ifndef GSR_PRE_FWD_F3D_MINB
+#define GSR_PRE_FWD_F3D_MINB 7
+#endif
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_FWD_F3D_MINB)
+    k_preprocess_fwd_f3d(GSR_PRE_FWD_PARAMS, const float* __restrict__ filter3d) {
+    preprocess_fwd<N_SH, HAS_SH, false, true>(GSR_PRE_FWD_FORWARD, filter3d);
+}
+template <int N_SH, bool HAS_SH>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_FWD_F3D_MINB)
+    k_preprocess_fwd_aa_f3d(GSR_PRE_FWD_PARAMS, const float* __restrict__ filter3d) {
+    preprocess_fwd<N_SH, HAS_SH, true, true>(GSR_PRE_FWD_FORWARD, filter3d);
 }
 #undef GSR_PRE_FWD_PARAMS
 #undef GSR_PRE_FWD_FORWARD
@@ -307,7 +333,10 @@ __global__ void __launch_bounds__(PRE_THREADS, 7) k_preprocess_fwd_aa(GSR_PRE_FW
 // the z component of the camera-frame position gradient before grad_xyz = W^T grad_xyz_cam.
 // ANTIALIAS: the rows' opacity slot is the gradient on the compensated opacity sigmoid(o) * rho of k_preprocess_fwd_aa;
 // it is carried back to sigmoid(o) and, through rho, to the conic.
-template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS>
+// FILTER3D: Sigma_world of the 3-D filtered variances (k_preprocess_fwd_f3d); the opacity slot (after rho) is the
+// gradient on sigmoid(o) * coef, carried back to sigmoid(o) and, through coef, to the log-scales.  No gradient goes
+// to the filter.
+template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS, bool FILTER3D>
 __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ xyz, const float* __restrict__ quat,
                      const float* __restrict__ scale, const float* __restrict__ opa_logit,
                      const float* __restrict__ Tdev, const float* __restrict__ Kdev,
@@ -318,7 +347,8 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
                      const float* __restrict__ g_uv_compact,
                      const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
                      float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa,
-                     float* __restrict__ o_dc, float* __restrict__ o_sh, int use_tma) {
+                     float* __restrict__ o_dc, float* __restrict__ o_sh, int use_tma,
+                     const float* __restrict__ filter3d) {
     constexpr int NR = N_SH - 1;
     constexpr int NR3 = HAS_SH ? 3 * NR : 1;
     // all outputs of the CTA's 128 gaussians are staged in shared memory and leave as six bulk stores
@@ -342,8 +372,9 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
     // every thread fetches its gaussian's inputs before the view constants are fetched (cooperatively): the
     // memory latencies overlap instead of queueing up behind one thread's 28 loads
     float x = 0.f, y = 0.f, z = 0.f, qw = 1.f, qx = 0.f, qy = 0.f, qz = 0.f, s0 = 0.f, s1 = 0.f, s2 = 0.f, opl = 0.f,
-          gcv[3] = {0.f, 0.f, 0.f}, guv[2] = {0.f, 0.f}, gov = 0.f, grv[3] = {0.f, 0.f, 0.f}, gzc = 0.f;
+          gcv[3] = {0.f, 0.f, 0.f}, guv[2] = {0.f, 0.f}, gov = 0.f, grv[3] = {0.f, 0.f, 0.f}, gzc = 0.f, f = 0.f;
     if (vis) {
+        if (FILTER3D) f = filter3d[i];
         x = xyz[i * 3 + 0]; y = xyz[i * 3 + 1]; z = xyz[i * 3 + 2];
         qw = quat[i * 4 + 0]; qx = quat[i * 4 + 1]; qy = quat[i * 4 + 2]; qz = quat[i * 4 + 3];
         s0 = scale[i * 3 + 0]; s1 = scale[i * 3 + 1]; s2 = scale[i * 3 + 2];
@@ -382,7 +413,18 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
         float px, py, pz;
         transform_point<float>(vc.T, x, y, z, px, py, pz);
         float S6[6], S9[9], J[6], W[9];
-        sigma_world<float>(qw, qx, qy, qz, s0, s1, s2, S6);
+        // 3-D filter: the forward's variances and opacity factor, re-formed (gsr_record.cuh f3d_filter)
+        float e[3], v[3], vp[3], t[3], F = 0.f, coef = 1.f;
+        if (FILTER3D) {
+            F = __fmul_rn(f, f);
+            e[0] = expf(s0); e[1] = expf(s1); e[2] = expf(s2);
+#pragma unroll
+            for (int k = 0; k < 3; ++k) v[k] = __fmul_rn(e[k], e[k]);
+            coef = f3d_filter(v, F, vp, t);
+            sigma_world_var<float>(qw, qx, qy, qz, vp[0], vp[1], vp[2], S6);
+        } else {
+            sigma_world<float>(qw, qx, qy, qz, s0, s1, s2, S6);
+        }
         sym6_to_full(S6, S9);
         proj_jacobian<float>(px, py, pz, vc.K[0], vc.K[4], J);
         W[0] = vc.T[0]; W[1] = vc.T[1]; W[2] = vc.T[2];
@@ -402,7 +444,8 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
             rho = aa_rho(cn[0], cn[1], cn[2]);
             const float A = cn[0] + 0.25f, C = cn[2] + 0.25f, bh = 0.5f * cn[1];
             const float rd = 1.0f / (A * C - bh * bh);
-            const float k = (0.125f * gov * sigmoid_torch(opl)) * rd / rho * rd;
+            const float k =
+                (0.125f * gov * (FILTER3D ? __fmul_rn(sigmoid_torch(opl), coef) : sigmoid_torch(opl))) * rd / rho * rd;
             const float kr = rho > 0.0f ? k : 0.0f;
             gcv[0] += kr * (cn[2] * C + bh * bh);
             gcv[1] -= kr * bh * (A + C - 0.25f);
@@ -411,7 +454,11 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
         const float gc[3] = {gcv[0], gcv[1], gcv[2]};
         float gS[9], gJ[6];
         conic_bwd<float>(S9, J, W, gc, gS, gJ);
-        sigma_world_bwd<float>(qw, qx, qy, qz, s0, s1, s2, gS, gq, gs);
+        if (FILTER3D) {
+            sigma_world_bwd_f3d<float>(qw, qx, qy, qz, e, v, vp, F, gS, gq, gs);
+        } else {
+            sigma_world_bwd<float>(qw, qx, qy, qz, s0, s1, s2, gS, gq, gs);
+        }
         float gp_j[3], gp_uv[3] = {0.f, 0.f, 0.f};
         proj_jacobian_bwd<float>(px, py, pz, vc.K[0], vc.K[4], gJ, gp_j);
         project_uv_bwd<float>(px, py, pz, vc.K[0], vc.K[4], guv[0], guv[1], gp_uv);
@@ -421,7 +468,15 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
 #pragma unroll
         for (int k = 0; k < 3; ++k) gx[k] = W[0 + k] * gp[0] + W[3 + k] * gp[1] + W[6 + k] * gp[2];
         const float sg = sigmoid_torch(opl);
-        if (ANTIALIAS) gov *= rho;       // gradient on sigmoid(o)
+        if (ANTIALIAS) gov *= rho;       // gradient on sigmoid(o) (3-D filter: on sigmoid(o) * coef)
+        if (FILTER3D) {
+            // d coef / d s_k = coef (1 - t_k), 1 - t_k = F / v'_k (no cancellation); 0 where F == 0.  Where coef == 0
+            // the splat never contributed: gov == 0 and every term here is an exact, finite 0.
+            const float gc = gov * sg * coef;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) gs[k] += gc * (F == 0.0f ? 0.0f : F / vp[k]);
+            gov *= coef;
+        }
         go = gov * ((1.0f - sg) * sg);  // torch sigmoid_backward: grad * (1 - y) * y
 
         const float gr[3] = {grv[0], grv[1], grv[2]};
@@ -486,20 +541,34 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
         g_uv_compact, scan, o_xyz, o_quat, o_scale, o_opa, o_dc, o_sh, use_tma
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB) k_preprocess_bwd(GSR_PRE_BWD_PARAMS) {
-    preprocess_bwd<N_SH, HAS_SH, false, false>(GSR_PRE_BWD_FORWARD);
+    preprocess_bwd<N_SH, HAS_SH, false, false, false>(GSR_PRE_BWD_FORWARD, nullptr);
 }
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB) k_preprocess_bwd_depth(GSR_PRE_BWD_PARAMS) {
-    preprocess_bwd<N_SH, HAS_SH, true, false>(GSR_PRE_BWD_FORWARD);
+    preprocess_bwd<N_SH, HAS_SH, true, false, false>(GSR_PRE_BWD_FORWARD, nullptr);
 }
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_AA_MINB) k_preprocess_bwd_aa(GSR_PRE_BWD_PARAMS) {
-    preprocess_bwd<N_SH, HAS_SH, false, true>(GSR_PRE_BWD_FORWARD);
+    preprocess_bwd<N_SH, HAS_SH, false, true, false>(GSR_PRE_BWD_FORWARD, nullptr);
 }
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_AA_MINB) k_preprocess_bwd_depth_aa(GSR_PRE_BWD_PARAMS) {
-    preprocess_bwd<N_SH, HAS_SH, true, true>(GSR_PRE_BWD_FORWARD);
+    preprocess_bwd<N_SH, HAS_SH, true, true, false>(GSR_PRE_BWD_FORWARD, nullptr);
 }
+#ifndef GSR_PRE_BWD_F3D_MINB
+#define GSR_PRE_BWD_F3D_MINB 5
+#endif
+#define GSR_PRE_BWD_F3D_KERNEL(name, depth, aa)                                                                    \
+    template <int N_SH, bool HAS_SH>                                                                             \
+    __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_F3D_MINB)                                         \
+        name(GSR_PRE_BWD_PARAMS, const float* __restrict__ filter3d) {                                           \
+        preprocess_bwd<N_SH, HAS_SH, depth, aa, true>(GSR_PRE_BWD_FORWARD, filter3d);                            \
+    }
+GSR_PRE_BWD_F3D_KERNEL(k_preprocess_bwd_f3d, false, false)
+GSR_PRE_BWD_F3D_KERNEL(k_preprocess_bwd_depth_f3d, true, false)
+GSR_PRE_BWD_F3D_KERNEL(k_preprocess_bwd_aa_f3d, false, true)
+GSR_PRE_BWD_F3D_KERNEL(k_preprocess_bwd_depth_aa_f3d, true, true)
+#undef GSR_PRE_BWD_F3D_KERNEL
 #undef GSR_PRE_BWD_PARAMS
 #undef GSR_PRE_BWD_FORWARD
 
@@ -508,7 +577,7 @@ static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t
 static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // GSR_MODE_ABSGRAD only changes the render backward (row slots 10-11, which the per-gaussian backward does not read)
-constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD;
+constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD | GSR_MODE_FILTER3D;
 
 }  // namespace gsr
 
@@ -530,13 +599,15 @@ size_t gsr_preprocess_temp_bytes(int N) {
 
 int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
                            int cam_first, const float* quaternion, const float* scale, const float* opacity_logit,
-                           const float* rgb_dc, const float* sh_rest, const float* camera_T_world, const float* K,
+                           const float* filter3d, const float* rgb_dc, const float* sh_rest,
+                           const float* camera_T_world, const float* K,
                            const float* camera_centre, int H, int W, float near_thresh, float far_thresh,
                            float cull_mask_padding, float mh_dist, uint32_t depth_base, float* records,
                            uint32_t* depth_key, uint8_t* visible, uint64_t* scan, uint64_t* tile_mask,
                            uint32_t* tile_win, void* temp, size_t temp_bytes, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if ((mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
+    if (((mode & GSR_MODE_FILTER3D) != 0) != (filter3d != nullptr)) return GSR_ERR_BAD_ARG;
     if (N <= 0) return GSR_OK;
     if (temp_bytes < gsr_preprocess_temp_bytes(N)) return GSR_ERR_BAD_ARG;
     if ((tile_mask == nullptr) != (tile_win == nullptr)) return GSR_ERR_BAD_ARG;
@@ -551,7 +622,19 @@ int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, con
         camera_centre, (float)W, (float)H,                                                                 \
         near_thresh, far_thresh, cull_mask_padding, mh_dist, ntx, nty, depth_base, records, depth_key, visible, \
         packed, tile_mask, tile_win, use_tma
-    if (mode & GSR_MODE_ANTIALIASED) {
+#define GSR_PRE_FWD_F3D_SWITCH(kernel)                                                                  \
+    switch (n_sh_rest) {                                                                                \
+        case 0: kernel<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;                \
+        case 3: kernel<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;                 \
+        case 8: kernel<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;                 \
+        case 15: kernel<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;               \
+        default: return GSR_ERR_UNSUPPORTED;                                                            \
+    }
+    if ((mode & GSR_MODE_FILTER3D) && (mode & GSR_MODE_ANTIALIASED)) {
+        GSR_PRE_FWD_F3D_SWITCH(k_preprocess_fwd_aa_f3d)
+    } else if (mode & GSR_MODE_FILTER3D) {
+        GSR_PRE_FWD_F3D_SWITCH(k_preprocess_fwd_f3d)
+    } else if (mode & GSR_MODE_ANTIALIASED) {
         switch (n_sh_rest) {
             case 0: k_preprocess_fwd_aa<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
             case 3: k_preprocess_fwd_aa<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;
@@ -568,6 +651,7 @@ int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, con
             default: return GSR_ERR_UNSUPPORTED;
         }
     }
+#undef GSR_PRE_FWD_F3D_SWITCH
 #undef GSR_PRE_ARGS
     cudaError_t e = cub::DeviceScan::InclusiveSum(temp, scan_bytes, packed, scan, N, st);
     if (e != cudaSuccess) return (int)e;
@@ -575,7 +659,8 @@ int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, con
 }
 
 int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
-                            const float* scale, const float* opacity_logit, const float* camera_T_world,
+                            const float* scale, const float* opacity_logit, const float* filter3d,
+                            const float* camera_T_world,
                             const float* K, const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
                             const float* grad_opacity, const float* grad_uv, const float* grad_conic,
                             const float* grad_rows, int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
@@ -583,6 +668,7 @@ int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, co
                             float* g_sh_rest, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if ((mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
+    if (((mode & GSR_MODE_FILTER3D) != 0) != (filter3d != nullptr)) return GSR_ERR_BAD_ARG;
     if (N <= 0) return GSR_OK;
     // the depth/alpha and anti-aliased kernels read the render backward's sums from the interleaved rows only (and so
     // does every absgrad backward: its render stage writes rows)
@@ -607,7 +693,26 @@ int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, co
         default: return GSR_ERR_UNSUPPORTED;                                            \
     }
     const bool depth = (mode & GSR_MODE_DEPTH_ALPHA) != 0, antialiased = (mode & GSR_MODE_ANTIALIASED) != 0;
-    if (antialiased && depth) {
+    if (mode & GSR_MODE_FILTER3D) {
+#define GSR_PRE_BWD_F3D_SWITCH(kernel)                                                      \
+    switch (n_sh_rest) {                                                                    \
+        case 0: kernel<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;    \
+        case 3: kernel<4, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;     \
+        case 8: kernel<9, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;     \
+        case 15: kernel<16, true><<<grid, block, 0, st>>>(GSR_PRE_ARGS, filter3d); break;   \
+        default: return GSR_ERR_UNSUPPORTED;                                                \
+    }
+        if (antialiased && depth) {
+            GSR_PRE_BWD_F3D_SWITCH(k_preprocess_bwd_depth_aa_f3d)
+        } else if (antialiased) {
+            GSR_PRE_BWD_F3D_SWITCH(k_preprocess_bwd_aa_f3d)
+        } else if (depth) {
+            GSR_PRE_BWD_F3D_SWITCH(k_preprocess_bwd_depth_f3d)
+        } else {
+            GSR_PRE_BWD_F3D_SWITCH(k_preprocess_bwd_f3d)
+        }
+#undef GSR_PRE_BWD_F3D_SWITCH
+    } else if (antialiased && depth) {
         GSR_PRE_BWD_SWITCH(k_preprocess_bwd_depth_aa)
     } else if (antialiased) {
         GSR_PRE_BWD_SWITCH(k_preprocess_bwd_aa)

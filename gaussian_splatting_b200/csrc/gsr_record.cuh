@@ -142,6 +142,23 @@ __device__ __forceinline__ float aa_rho(float c0, float c1, float c2) {
     return __fsqrt_rn(__fdiv_rn(fmaxf(det0, 0.0f), det));
 }
 
+// 3-D smoothing filter (Mip-Splatting): Sigma_world = R diag(v + F) R^T with v_k = exp(s_k)^2 and F = f^2, f the
+// filter's standard deviation in world units, and the opacity factor coef = sqrt(det Sigma / det(Sigma + F I)) that
+// keeps the filtered gaussian's 3-D mass.  Per axis, so that tiny scales do not underflow a product of variances.
+// Pinned operation order; tests/filter3d_oracle.c reproduces it bit for bit:
+//   v'_k = v_k + F;  t_k = F == 0 ? 1 : v_k / v'_k  (IEEE division);  coef = sqrt_rn((t_0 * t_1) * t_2)
+// F == 0 gives v' = v and coef = 1 exactly: the unfiltered record.  coef == 0 where the t_k product underflows (a scale
+// far below the filter): the splat then never contributes.
+__device__ __forceinline__ float f3d_filter(const float* __restrict__ v, float F, float* __restrict__ vp,
+                                            float* __restrict__ t) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        vp[k] = __fadd_rn(v[k], F);
+        t[k] = F == 0.0f ? 1.0f : __fdiv_rn(v[k], vp[k]);
+    }
+    return __fsqrt_rn(__fmul_rn(__fmul_rn(t[0], t[1]), t[2]));
+}
+
 __device__ __forceinline__ void make_record(float u, float v, float c0, float c1, float c2, float opa,
                                             float r, float g, float b, float* __restrict__ rec) {
     // a, b, c, det: src/render.cu:117-127 (fp32 branch: +0.25 dilation), rounding order of the reference build

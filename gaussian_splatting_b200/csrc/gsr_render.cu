@@ -1509,7 +1509,8 @@ int gsr_render_backward_gather(int mode, const float* gaussian_records, const ui
                                float* g_uv, float* g_conic, float* grad_rows, const uint32_t* contribution_masks,
                                void* stream) {
     // the other stages' bits are accepted and ignored: depth/alpha is selected by the maps' gradients
-    if ((mode & ~(GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD)) != 0) return GSR_ERR_BAD_ARG;
+    if ((mode & ~(GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD | GSR_MODE_FILTER3D)) != 0)
+        return GSR_ERR_BAD_ARG;
     const bool absgrad = (mode & GSR_MODE_ABSGRAD) != 0;
     if (absgrad && grad_rows == nullptr) return GSR_ERR_BAD_ARG;  // slots 10-11 exist only in the interleaved rows
     if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;

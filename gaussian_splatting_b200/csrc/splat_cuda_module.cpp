@@ -407,6 +407,15 @@ void render_depth_cuda(torch::Tensor xyz_camera_frame, torch::Tensor uvs, torch:
 // ---------------------------------------------------------------------------------------------
 #define F32PTR(t) ((t).data_ptr<float>())
 
+// the 3-D filter [N] or [N,1] of the fused per-gaussian stages (GSR_MODE_FILTER3D), or NULL
+static const float* filter3d_ptr(const c10::optional<torch::Tensor>& filter3d, int64_t N) {
+    if (!filter3d.has_value()) return nullptr;
+    const torch::Tensor& f = *filter3d;
+    CHECK_VALID_INPUT(f); CHECK_FLOAT_TENSOR(f);
+    TORCH_CHECK(f.numel() == N && (f.dim() == 1 || (f.dim() == 2 && f.size(1) == 1)), "filter3d must have shape [N] or [N,1]");
+    return f.data_ptr<float>();
+}
+
 // returns [records [N,12], depth_key [N] i32-viewed u32, visible [N] u8, scan [N] i64-viewed u64] and, with_tiles,
 // also [tile_mask [N] i64-viewed u64, tile_win [N] i32-viewed u32].  mode: GSR_MODE_* bits
 std::vector<torch::Tensor> fused_preprocess_forward(
@@ -414,7 +423,7 @@ std::vector<torch::Tensor> fused_preprocess_forward(
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, int64_t mode) {
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc); CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -462,8 +471,9 @@ std::vector<torch::Tensor> fused_preprocess_forward(
     torch::Tensor tile_win = torch::empty({with_tiles ? N : 0}, opt.dtype(torch::kInt32));
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
+    const float* f3d = filter3d_ptr(filter3d, N);
     check_rc(gsr_preprocess_forward((int)mode, N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion),
-                                    F32PTR(scale), F32PTR(opacity_logit), F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world),
+                                    F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world),
                                     F32PTR(K), centre_ptr, (int)H, (int)W, (float)near_thresh, (float)far_thresh,
                                     (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base, F32PTR(records),
                                     (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),
@@ -670,7 +680,7 @@ torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, int64_t
 // [9N] or interleaved rows [N,12] (rows by gaussian).  grad_uv_compact [M,2] (optional): gradient on the compact uv,
 // added to — or, with use_slab_uv false, replacing — the slab's uv section.  mode: the GSR_MODE_* bits of the forward
 // (gsr_preprocess_backward): GSR_MODE_DEPTH_ALPHA reads the z gradient of the depth/alpha rows, GSR_MODE_ANTIALIASED
-// takes the rows' opacity slot as the gradient on the compensated opacity.
+// takes the rows' opacity slot as the gradient on the compensated opacity, GSR_MODE_FILTER3D needs the forward's filter3d.
 std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
                                                      torch::Tensor scale, torch::Tensor opacity_logit,
                                                      c10::optional<torch::Tensor> sh_rest,
@@ -679,7 +689,7 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
                                                      torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
                                                      c10::optional<torch::Tensor> grad_uv_compact,
                                                      c10::optional<torch::Tensor> scan, bool use_slab_uv,
-                                                     int64_t mode) {
+                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     const int64_t N = xyz.size(0);
     const bool rows = slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS && N > 0;  // interleaved [N,12] (else planar [9N])
@@ -727,8 +737,9 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
                   o_o = section(3, {N}), o_dc = section(4, {N, 3});
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
+    const float* f3d = filter3d_ptr(filter3d, N);
     check_rc(gsr_preprocess_backward((int)mode, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
-                                     F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
+                                     F32PTR(opacity_logit), f3d, F32PTR(camera_T_world), F32PTR(K),
                                      camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
                                      visible.data_ptr<uint8_t>(), g_rgb, g_opa, g_uv, g_conic,
                                      rows ? slab.data_ptr<float>() : nullptr, use_slab_uv ? 1 : 0, g_uv_compact,
@@ -739,6 +750,29 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
     out.push_back(flat);  // last: the allocation all the others are views of
+    return out;
+}
+
+// Mip-Splatting's 3-D filter size per gaussian (gsr_filter3d): xyz [N,3], camera_T_world [C,4,4], K [C,3,3],
+// width / height int32 [C], all on xyz's device -> filter3d [N]
+torch::Tensor filter3d(torch::Tensor xyz, torch::Tensor camera_T_world, torch::Tensor K, torch::Tensor width,
+                       torch::Tensor height, double near, double margin, double variance) {
+    CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K); CHECK_VALID_INPUT(width);
+    CHECK_VALID_INPUT(height);
+    CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(camera_T_world); CHECK_FLOAT_TENSOR(K);
+    CHECK_INT_TENSOR(width); CHECK_INT_TENSOR(height);
+    TORCH_CHECK(xyz.dim() == 2 && xyz.size(1) == 3, "xyz must have shape Nx3");
+    const int64_t C = camera_T_world.size(0);
+    TORCH_CHECK(camera_T_world.dim() == 3 && camera_T_world.size(1) == 4 && camera_T_world.size(2) == 4,
+                "camera_T_world must have shape Cx4x4");
+    TORCH_CHECK(K.dim() == 3 && K.size(0) == C && K.size(1) == 3 && K.size(2) == 3, "K must have shape Cx3x3");
+    TORCH_CHECK(width.numel() == C && height.numel() == C, "width and height must hold C values");
+    c10::cuda::CUDAGuard guard(xyz.device());
+    torch::Tensor out = torch::empty({xyz.size(0)}, xyz.options());
+    check_rc(gsr_filter3d((int)xyz.size(0), F32PTR(xyz), (int)C, F32PTR(camera_T_world), F32PTR(K),
+                          width.data_ptr<int>(), height.data_ptr<int>(), (float)near, (float)margin, (float)variance,
+                          F32PTR(out), cur_stream()),
+             "gsr_filter3d");
     return out;
 }
 
@@ -989,7 +1023,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("opacity_logit"), py::arg("rgb_dc"), py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"),
           py::arg("camera_centre"), py::arg("H"), py::arg("W"), py::arg("near_thresh"), py::arg("far_thresh"),
           py::arg("cull_mask_padding"), py::arg("mh_dist"), py::arg("depth_base"), py::arg("with_tiles") = false,
-          py::arg("mode") = 0);
+          py::arg("mode") = 0, py::arg("filter3d") = py::none());
     m.def("fused_bin", &fused_bin, "pair emission + radix sort + tile ranges + record stream");
     m.def("fused_render_forward", &fused_render_forward,
           "tile renderer forward (with depth_key: also the depth and alpha maps)");
@@ -1000,10 +1034,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("ranges"), py::arg("background"), py::arg("n"), py::arg("w"), py::arg("masks"),
           py::arg("keys_sorted"), py::arg("id_bits"), py::arg("gather"), py::arg("grad_depth"), py::arg("grad_alpha"),
           py::arg("depth_key"), py::arg("depth_base"), py::arg("depth_bits"), py::arg("mode") = 0);
-    m.def("fused_preprocess_backward", &fused_preprocess_backward, "fused per-gaussian backward (mode: MODE_* bits)");
+    m.def("fused_preprocess_backward", &fused_preprocess_backward,
+          "fused per-gaussian backward (mode: MODE_* bits; filter3d: the forward's, with MODE_FILTER3D)",
+          py::arg("slab"), py::arg("xyz"), py::arg("quaternion"), py::arg("scale"), py::arg("opacity_logit"),
+          py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"), py::arg("camera_centre"), py::arg("visible"),
+          py::arg("out_flat"), py::arg("grad_uv_compact"), py::arg("scan"), py::arg("use_slab_uv"), py::arg("mode"),
+          py::arg("filter3d") = py::none());
+    m.def("filter3d", &filter3d, "Mip-Splatting's 3-D filter size per gaussian from the training cameras (gsr_filter3d)",
+          py::arg("xyz"), py::arg("camera_T_world"), py::arg("K"), py::arg("width"), py::arg("height"),
+          py::arg("near"), py::arg("margin"), py::arg("variance"));
     m.attr("MODE_DEPTH_ALPHA") = GSR_MODE_DEPTH_ALPHA;
     m.attr("MODE_ANTIALIASED") = GSR_MODE_ANTIALIASED;
     m.attr("MODE_ABSGRAD") = GSR_MODE_ABSGRAD;
+    m.attr("MODE_FILTER3D") = GSR_MODE_FILTER3D;
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");

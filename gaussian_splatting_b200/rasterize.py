@@ -245,7 +245,7 @@ class _ViewState:
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges", "stream_rec", "gather",
                  "records", "keys_sorted", "id_bits", "slab_width",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
-                 "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad")
+                 "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad", "filter3d")
 
     @property
     def ids_sorted(self):
@@ -268,8 +268,10 @@ class _ViewState:
         self.speculation_overflowed = False
         # MODE_* bits of the native fused path: MODE_DEPTH_ALPHA (render_depth_alpha: the tile kernels also produce
         # depth / alpha [H,W,1]), MODE_ANTIALIASED (opacity compensation for the 0.25 px^2 dilation), MODE_ABSGRAD
-        # (the render backward also sums |d loss_p / d uv| per pixel)
+        # (the render backward also sums |d loss_p / d uv| per pixel), MODE_FILTER3D (Mip-Splatting's 3-D filter in the
+        # per-gaussian stages: filter3d [N], a constant)
         self.mode = 0
+        self.filter3d = None
         self.depth = self.alpha = None
         self.uv_absgrad = None  # MODE_ABSGRAD: [M,2], set by every render backward
 
@@ -323,7 +325,7 @@ class _ProjectGaussians(torch.autograd.Function):
             # tile_mask / tile_win: the tiles each gaussian hits, tested once here and only expanded by the pair emission
             records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(
                 xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
-                pad, mh, depth_base, True, state.mode)
+                pad, mh, depth_base, True, state.mode, state.filter3d)
         record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])  # a backward pass can follow
         background = state.background
 
@@ -424,7 +426,7 @@ class _ProjectGaussians(torch.autograd.Function):
             grads = native().fused_preprocess_backward(slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K,
                                                        centre, st.visible, st.grad_out, guv,
                                                        st.scan if guv is not None else None, not st.uv_grad_emitted,
-                                                       st.mode)
+                                                       st.mode, st.filter3d)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
@@ -479,7 +481,7 @@ class _CompositeTiles(torch.autograd.Function):
 
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
-              render_depth_alpha=False, antialiased=False, absgrad=False):
+              render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
@@ -498,7 +500,30 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     accumulated.  Pixels in units, like uv.grad; only the render stage's part (not a gradient the caller adds on uv);
     G_p includes the depth / alpha maps' upstream gradients with render_depth_alpha.  For densification:
     DensificationStats.accumulate(..., absgrad=True).  Return values, uv.grad and all gradients are unchanged;
-    combines with render_depth_alpha and antialiased.  fp32 and precomputed SH colours only."""
+    combines with render_depth_alpha and antialiased.  fp32 and precomputed SH colours only.
+
+    filter3d: Mip-Splatting's 3-D smoothing filter, an fp32 CUDA tensor [N] or [N,1] of standard deviations f in world
+    units (gaussian_splatting_b200.filter3d.compute_filter3d, from the training cameras).  Every gaussian is rendered
+    with the world covariance R diag(exp(2 scale) + f^2) R^T and the opacity sigmoid(o) * coef, coef =
+    sqrt(prod_k exp(2 scale_k) / (exp(2 scale_k) + f^2)), which keeps its 3-D mass (DESIGN.md 3.13); f is only used
+    squared, and f = 0 renders exactly as without the filter.  The filter is a constant: it gets no gradient, and the
+    parameter gradients (state.grad_flat as usual) are those of the raw parameters.  Return values and uv.grad keep
+    their meaning; combines with antialiased (coef comes before rho), render_depth_alpha, absgrad, return_state and
+    grad_out.  After densification changes N the filter must be recomputed: a filter of another length raises
+    ValueError.  fp32 and precomputed SH colours only; the values are not checked (no host synchronisation)."""
+    if filter3d is not None:
+        if gaussians.xyz.dtype != torch.float32:
+            raise TypeError("filter3d needs fp32 inputs (the fused rasterizer's per-gaussian stages apply it)")
+        if gaussians.sh is not None and not use_sh_precompute:
+            raise ValueError("filter3d needs use_sh_precompute=True (per-pixel SH colours are not supported)")
+        if filter3d.requires_grad:
+            raise ValueError("filter3d is a constant of the scene (no gradient flows to it): pass filter3d.detach()")
+        if filter3d.dtype != torch.float32:
+            raise TypeError(f"filter3d must be float32, got {filter3d.dtype}")
+        n = gaussians.xyz.shape[0]
+        if not (tuple(filter3d.shape) in ((n,), (n, 1))):
+            raise ValueError(f"filter3d has shape {tuple(filter3d.shape)} but there are {n} gaussians: recompute it "
+                             "(compute_filter3d) after densification changes the gaussians")
     if absgrad and gaussians.xyz.dtype != torch.float32:
         raise TypeError("absgrad needs fp32 inputs (the fused rasterizer's render backward forms it)")
     if absgrad and gaussians.sh is not None and not use_sh_precompute:
@@ -518,7 +543,8 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     state = _ViewState(profile)
     state.grad_out = grad_out
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
-                  | (ext.MODE_ABSGRAD if absgrad else 0))
+                  | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
+    state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))

@@ -45,6 +45,7 @@ extern "C" {
 #define GSR_MODE_DEPTH_ALPHA 1 /* gradient rows carry the render backward's camera-frame z gradient */
 #define GSR_MODE_ANTIALIASED 2 /* opacity compensation for the renderer's 0.25 px^2 dilation */
 #define GSR_MODE_ABSGRAD 4     /* gradient rows also carry sum over pixels of |d loss_p / d uv| (AbsGS) */
+#define GSR_MODE_FILTER3D 8    /* Mip-Splatting's 3-D smoothing filter in the per-gaussian stages (gsr_filter3d) */
 
 /* library identification: returns e.g. "gsr_b200 0.1 sm_90a" */
 const char* gsr_version(void);
@@ -273,10 +274,16 @@ size_t gsr_preprocess_temp_bytes(int N);
  *     rho = sqrt(max(det0, 0) / det),  det0 = det of the 2-D covariance, det = det of the covariance + 0.25 I
  *   (the +0.25 px^2 dilation the tile renderers apply), so the dilated splat carries the mass of the undilated one.
  *   The culling bound is formed from the compensated opacity.  rho == 0 where det0 <= 0 in fp32: the splat then never
- *   contributes.  Operation order: gsr_record.cuh aa_rho. */
+ *   contributes.  Operation order: gsr_record.cuh aa_rho.
+ * GSR_MODE_FILTER3D (Mip-Splatting's 3-D smoothing filter): filter3d [N] is required with the bit and must be NULL
+ *   without it (else GSR_ERR_BAD_ARG).  f = filter3d[i] is a standard deviation in world units, used only squared:
+ *   Sigma_world is formed from the variances v_k + f^2 (v_k = exp(scale_k)^2) and the opacity is multiplied by
+ *   coef = sqrt(prod_k v_k / (v_k + f^2)), before rho when GSR_MODE_ANTIALIASED is set too; the culling bound is formed
+ *   from the final opacity.  f == 0 gives the unfiltered record bit for bit.  Operation order: gsr_record.cuh
+ *   f3d_filter.  The render stages ignore the bit. */
 int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
                            int cam_first, const float* quaternion,
-                           const float* scale, const float* opacity_logit, const float* rgb_dc,
+                           const float* scale, const float* opacity_logit, const float* filter3d, const float* rgb_dc,
                            const float* sh_rest, const float* camera_T_world, const float* K,
                            const float* camera_centre, int H, int W, float near_thresh, float far_thresh,
                            float cull_mask_padding, float mh_dist, uint32_t depth_base, float* records,
@@ -343,14 +350,32 @@ int gsr_gather_records_keys(int P, int id_bits, const uint64_t* keys_sorted, con
  *   GSR_MODE_ANTIALIASED: the rows' opacity slot g is the gradient on the compensated opacity sigmoid(o) * rho:
  *   sigmoid(o) receives g * rho and the 2-D covariance g * sigmoid(o) * grad(rho).  Where rho == 0 no gradient goes
  *   through rho (its gradient is infinite there, and g is 0 because the splat never contributed).
+ *   GSR_MODE_FILTER3D: filter3d [N] as in gsr_preprocess_forward (required iff the bit is set).  The rows' opacity
+ *   slot (times rho with GSR_MODE_ANTIALIASED) is the gradient g on sigmoid(o) * coef: sigmoid(o) receives g * coef and
+ *   scale_k additionally g * sigmoid(o) * coef * f^2 / (v_k + f^2).  No gradient goes to filter3d.
  * Writes dense parameter gradients for all N gaussians (zeros for culled ones). */
 int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
-                            const float* scale, const float* opacity_logit, const float* camera_T_world,
+                            const float* scale, const float* opacity_logit, const float* filter3d,
+                            const float* camera_T_world,
                             const float* K, const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
                             const float* grad_opacity, const float* grad_uv, const float* grad_conic,
                             const float* grad_rows, int use_rows_uv,
                             const float* grad_uv_compact, const uint64_t* scan, float* g_xyz, float* g_quaternion,
                             float* g_scale, float* g_opacity_logit, float* g_rgb_dc, float* g_sh_rest, void* stream);
+
+/* Mip-Splatting's 3-D filter size per gaussian, from C cameras: camera_T_world [C,4,4], K [C,3,3], width / height
+ * int32 [C] (all on the device) and xyz [N,3] -> filter3d [N] (standard deviations in world units).
+ * Camera c sees gaussian i when, with p = T_c x and (u, v) formed as gsr_preprocess_forward forms them (fp32,
+ * csrc/gsr_math.cuh transform_point / project_uv):
+ *   p_z > near,  -(m W_c) <= u <= (1 + m) W_c,  -(m H_c) <= v <= (1 + m) H_c    (m = margin; products rounded to fp32)
+ * and then samples it at r_c = p_z / max(fx_c, fy_c) world units per pixel (IEEE division).  r_i = min over the
+ * cameras that see i; filter3d[i] = sqrtf(variance) * r_i, sqrtf(variance) rounded to float once.  Gaussians no camera
+ * sees get the largest r_i of the seen ones; when none is seen at all, every filter3d[i] is 0.  Deterministic.
+ * Intrinsics are expected to have positive focal lengths (not checked: no host synchronisation).
+ * GSR_ERR_BAD_ARG for C < 1, near < 0, negative (or NaN) margin or variance, or (N > 0) NULL pointers.  N == 0 returns
+ * GSR_OK. */
+int gsr_filter3d(int N, const float* xyz, int C, const float* camera_T_world, const float* K, const int* width,
+                 const int* height, float near, float margin, float variance, float* filter3d, void* stream);
 
 /* ---- optimizer step on the flat parameter buffer (SURVEY.md 8(f) rank 2) ----------------------------
  * Replaces torch.optim.Adam.step() as configured by splat_py/optimizer_manager.py:13-44 (one parameter group

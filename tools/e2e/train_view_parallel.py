@@ -59,6 +59,10 @@ def main():
     ap.add_argument("--absgrad", action="store_true",
                     help="rasterize(absgrad=True) in training, and densification statistics accumulated from uv.absgrad "
                          "(per-pixel absolute screen-space gradients, AbsGS) instead of |uv.grad|")
+    ap.add_argument("--filter3d", action="store_true",
+                    help="Mip-Splatting's 3-D smoothing filter in training and evaluation: computed from the training "
+                         "cameras before the first step, after every densification pass and every 100 steps after "
+                         "densification ends (not in the last 100); every rank computes the same filter")
     a = ap.parse_args()
 
     real_stdout = os.fdopen(os.dup(1), "w")
@@ -76,6 +80,7 @@ def main():
 
     import gaussian_splatting_b200 as gsb
     from gaussian_splatting_b200.densify import AdaptiveDensityControl, DensificationStats
+    from gaussian_splatting_b200.filter3d import compute_filter3d
     from gaussian_splatting_b200.flat_adam import REFERENCE_LR_MULTIPLIERS as mult, FlatAdam
     from gaussian_splatting_b200.loss import photometric_loss, ssim as fused_ssim
     from gaussian_splatting_b200.rasterize import rasterize
@@ -163,6 +168,18 @@ def main():
     test_split = np.arange(0, n_img, config.test_split_ratio)
     train_split = torch.tensor(sorted(set(range(n_img)) - set(test_split.tolist())), dtype=torch.int, device=dev)
     train_prob = torch.ones(len(train_split), dtype=torch.float32, device=dev) / len(train_split)
+    train_ims = [images[int(k)] for k in train_split.tolist()]
+    train_cams = dict(camera_T_worlds=torch.stack([im.camera_T_world for im in train_ims]),
+                      Ks=torch.stack([cams[im.camera_id].K for im in train_ims]),
+                      widths=[int(cams[im.camera_id].width) for im in train_ims],
+                      heights=[int(cams[im.camera_id].height) for im in train_ims])
+
+    def refresh_filter():
+        """Mip-Splatting's 3-D filter from the training cameras (the same on every rank: replicas are identical and
+        the kernel is deterministic); None without --filter3d."""
+        return compute_filter3d(g.xyz, **train_cams) if a.filter3d else None
+
+    filt = refresh_filter()
 
     def evaluate():
         psnrs, ssims = [], []
@@ -171,7 +188,7 @@ def main():
                 im = images[int(t)]
                 pred, _, _ = rasterize(g, im.camera_T_world, cams[im.camera_id], config.near_thresh, config.far_thresh,
                                        config.cull_mask_padding, config.mh_dist, config.use_sh_precompute,
-                                       torch.zeros(3, device=dev), antialiased=a.antialiased)
+                                       torch.zeros(3, device=dev), antialiased=a.antialiased, filter3d=filt)
                 l2 = torch.nn.functional.mse_loss(pred.clip(0, 1), im.image)
                 psnrs.append(-10 * torch.log10(l2).item())
                 if a.loss == "fused":
@@ -210,7 +227,8 @@ def main():
         image, mask, uv, state = rasterize(g, im.camera_T_world, cams[im.camera_id], config.near_thresh,
                                            config.far_thresh, config.cull_mask_padding, config.mh_dist,
                                            config.use_sh_precompute, background, return_state=True,
-                                           grad_out=grads_sym, antialiased=a.antialiased, absgrad=a.absgrad)
+                                           grad_out=grads_sym, antialiased=a.antialiased, absgrad=a.absgrad,
+                                           filter3d=filt)
         if not a.absgrad:
             uv.retain_grad()
         if timed:
@@ -245,6 +263,9 @@ def main():
             torch.cuda.synchronize()
             t_adc += time.time() - t_a
             adc_log.append(dict(iter=i, **{k: info.get(k) for k in ("deleted", "cloned", "split", "n_out")}))
+            filt = refresh_filter()
+        elif a.filter3d and i >= config.adaptive_control_end and i % 100 == 0 and i < config.num_iters - 100:
+            filt = refresh_filter()
         if config.reset_opacity_start < i < config.reset_opacity_end and i % config.reset_opacity_interval == 0:
             relayout(adc.reset_opacity)
         if i > 0 and i % config.add_sh_band_interval == 0:
@@ -282,7 +303,7 @@ def main():
                           if world > 1 else "FlatAdam (gsr_adam_step)"),
             "loss": ("fused: photometric_loss (gsr_photometric_loss_forward / _backward), ssim() in evaluation"
                      if a.loss == "fused" else "shim: l1_loss + SSIM stand-in (tools/e2e/shims) through NCHW views"),
-            "antialiased": a.antialiased, "absgrad": a.absgrad,
+            "antialiased": a.antialiased, "absgrad": a.absgrad, "filter3d": a.filter3d,
             "device": torch.cuda.get_device_name(local),
         }
         real_stdout.write("E2E " + json.dumps(line) + "\n")
