@@ -1,5 +1,5 @@
-// gsr_binning.cu — (gaussian, tile) pair generation, depth sort, tile ranges and the
-// packed per-pair record stream the tile renderers consume.
+// gsr_binning.cu — (gaussian, tile) pair generation, depth sort and tile ranges, and the
+// per-gaussian record packing of the reference-surface renderers.
 //
 // Replaces the reference's src/tile_culling.cu:124-340: instead of an fp64 key
 // z + (max_z+1)*tile sorted by torch::sort plus an index_select, each pair gets
@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(BIN_THREADS)
     const int i = blockIdx.x * BIN_THREADS + threadIdx.x;
     if (cap > 0) {
         // Speculatively sized buffers (the host has not read P yet): positions [P, cap) get the all-ones key, which
-        // sorts behind every real pair (tile field >= n_tiles) and is ignored by the range / gather kernels
+        // sorts behind every real pair (tile field >= n_tiles) and is ignored by the range kernel
         const int64_t P = (int64_t)(scan[N - 1] & 0xffffffffu);
         for (int64_t p = P + (int64_t)blockIdx.x * BIN_THREADS + threadIdx.x; p < cap;
              p += (int64_t)gridDim.x * BIN_THREADS) {
@@ -177,46 +177,15 @@ __global__ void __launch_bounds__(BIN_THREADS) k_ids_to_i32(int P, const uint32_
     if (p < P) out[p] = (int32_t)in[p];
 }
 
-// one 48-byte record per pair, three 16-byte lanes per record: thread -> (pair, lane)
 __global__ void __launch_bounds__(BIN_THREADS)
-    k_gather_records(int P, const uint32_t* __restrict__ ids, const float4* __restrict__ rec,
-                     float4* __restrict__ out, const uint64_t* __restrict__ scan, int32_t* __restrict__ rank_out) {
-    const int64_t t = (int64_t)blockIdx.x * BIN_THREADS + threadIdx.x;
-    if (t >= (int64_t)P * 3) return;
-    const int p = (int)(t / 3), lane = (int)(t % 3);
-    const uint32_t id = ids[p];
-    if (lane == 0 && rank_out != nullptr) rank_out[p] = (int32_t)(scan[id] >> 32) - 1;
-    out[t] = __ldg(rec + (size_t)id * 3 + lane);
-}
-
-// same, ids taken from the low id_bits of the sorted keys; also writes, for the backward's flush, the row of the
-// per-gaussian gradient arrays each pair accumulates into: the gaussian id, or — when the packed scan of the
-// per-gaussian stage is given — its RANK among the visible gaussians (compact gradient arrays of M rows)
-__global__ void __launch_bounds__(BIN_THREADS)
-    k_gather_records_keys(int P, const uint64_t* __restrict__ keys, uint64_t id_mask,
-                          const float4* __restrict__ rec, float4* __restrict__ out,
-                          int32_t* __restrict__ ids_out, const uint64_t* __restrict__ scan) {
-    const int64_t t = (int64_t)blockIdx.x * BIN_THREADS + threadIdx.x;
-    if (t >= (int64_t)P * 3) return;
-    const int p = (int)(t / 3), lane = (int)(t % 3);
-    const uint64_t key = keys[p];
-    if (key == ~0ull) return;  // padding of a speculatively sized buffer
-    const uint32_t id = (uint32_t)(key & id_mask);
-    if (lane == 0) ids_out[p] = (scan != nullptr) ? (int32_t)(scan[id] >> 32) - 1 : (int32_t)id;
-    out[t] = __ldg(rec + (size_t)id * 3 + lane);
-}
-
-__global__ void __launch_bounds__(BIN_THREADS)
-    k_pack_records(int P, const int32_t* __restrict__ idx, const float* __restrict__ uvs,
-                   const float* __restrict__ opacity, const float* __restrict__ rgb,
-                   const float* __restrict__ conic, float* __restrict__ out) {
-    const int p = blockIdx.x * BIN_THREADS + threadIdx.x;
-    if (p >= P) return;
-    const int g = idx[p];
+    k_pack_records(int N, const float* __restrict__ uvs, const float* __restrict__ opacity,
+                   const float* __restrict__ rgb, const float* __restrict__ conic, float* __restrict__ out) {
+    const int g = blockIdx.x * BIN_THREADS + threadIdx.x;
+    if (g >= N) return;
     float rec[REC];
     make_record(uvs[g * 2], uvs[g * 2 + 1], conic[g * 3], conic[g * 3 + 1], conic[g * 3 + 2], opacity[g],
                 rgb[g * 3], rgb[g * 3 + 1], rgb[g * 3 + 2], rec);
-    float4* o = reinterpret_cast<float4*>(out + (size_t)p * REC);
+    float4* o = reinterpret_cast<float4*>(out + (size_t)g * REC);
     o[0] = make_float4(rec[0], rec[1], rec[2], rec[3]);
     o[1] = make_float4(rec[4], rec[5], rec[6], rec[7]);
     o[2] = make_float4(rec[8], rec[9], rec[10], rec[11]);
@@ -365,29 +334,11 @@ int gsr_sort_keys(int P, int n_tiles, int depth_bits, int id_bits, const uint64_
     return (int)e;
 }
 
-int gsr_gather_records_keys(int P, int id_bits, const uint64_t* keys_sorted, const float* records, float* out,
-                            int32_t* ids_sorted, const uint64_t* scan, void* stream) {
+int gsr_pack_gaussian_records(int N, const float* uvs, const float* opacity, const float* rgb, const float* conic,
+                              float* records, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    if (P <= 0) return GSR_OK;
-    k_gather_records_keys<<<BGRID((int64_t)P * 3)>>>(P, keys_sorted, (((uint64_t)1) << id_bits) - 1,
-                                                     (const float4*)records, (float4*)out, ids_sorted, scan);
-    return (int)cudaGetLastError();
-}
-
-int gsr_gather_records(int P, const uint32_t* ids_sorted, const float* records, float* out, const uint64_t* scan,
-                       int32_t* ranks_sorted, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (P <= 0) return GSR_OK;
-    if ((scan == nullptr) != (ranks_sorted == nullptr)) return GSR_ERR_BAD_ARG;
-    k_gather_records<<<BGRID((int64_t)P * 3)>>>(P, ids_sorted, (const float4*)records, (float4*)out, scan, ranks_sorted);
-    return (int)cudaGetLastError();
-}
-
-int gsr_pack_records(int P, const int32_t* idx, const float* uvs, const float* opacity, const float* rgb,
-                     const float* conic, float* records, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (P <= 0) return GSR_OK;
-    k_pack_records<<<BGRID(P)>>>(P, idx, uvs, opacity, rgb, conic, records);
+    if (N <= 0) return GSR_OK;
+    k_pack_records<<<BGRID(N)>>>(N, uvs, opacity, rgb, conic, records);
     return (int)cudaGetLastError();
 }
 

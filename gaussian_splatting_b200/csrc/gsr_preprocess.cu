@@ -319,8 +319,8 @@ __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_FWD_F3D_MINB)
 #undef GSR_PRE_FWD_PARAMS
 #undef GSR_PRE_FWD_FORWARD
 
-// Fused VJP.  g_rgb/g_opa/g_uv/g_conic are the per-Gaussian sums produced by the render backward
-// (indexed by original gaussian).  Order of the chain: SURVEY.md Appendix A "Per-Gaussian backward".
+// Fused VJP.  g_rows are the per-Gaussian sums produced by the render backward, one interleaved row per original
+// gaussian.  Order of the chain: SURVEY.md Appendix A "Per-Gaussian backward".
 #ifndef GSR_PRE_BWD_MINB
 #define GSR_PRE_BWD_MINB 6
 #endif
@@ -341,9 +341,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
                      const float* __restrict__ scale, const float* __restrict__ opa_logit,
                      const float* __restrict__ Tdev, const float* __restrict__ Kdev,
                      const float* __restrict__ camdev, const uint8_t* __restrict__ visible,
-                     const float* __restrict__ g_rgb,
-                     const float* __restrict__ g_opa, const float* __restrict__ g_uv,
-                     const float* __restrict__ g_conic, const float* __restrict__ g_rows, int rows_uv,
+                     const float* __restrict__ g_rows, int rows_uv,
                      const float* __restrict__ g_uv_compact,
                      const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
                      float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa,
@@ -379,27 +377,21 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
         qw = quat[i * 4 + 0]; qx = quat[i * 4 + 1]; qy = quat[i * 4 + 2]; qz = quat[i * 4 + 3];
         s0 = scale[i * 3 + 0]; s1 = scale[i * 3 + 1]; s2 = scale[i * 3 + 2];
         opl = opa_logit[i];
-        if (g_rows != nullptr) {  // interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3
-            const float4* row = reinterpret_cast<const float4*>(g_rows + (size_t)i * GSR_GRAD_ROW_FLOATS);
-            const float4 r0 = row[0], r1 = row[1];
-            grv[0] = r0.x; grv[1] = r0.y; grv[2] = r0.z; gov = r0.w;
-            if (rows_uv) { guv[0] = r1.x; guv[1] = r1.y; }
-            gcv[0] = r1.z; gcv[1] = r1.w;
-            if (DEPTH) {
-                const float2 r2 = *reinterpret_cast<const float2*>(g_rows + (size_t)i * GSR_GRAD_ROW_FLOATS + 8);
-                gcv[2] = r2.x;
-                gzc = r2.y;
-            } else {
-                gcv[2] = g_rows[(size_t)i * GSR_GRAD_ROW_FLOATS + 8];
-            }
-        } else {
-        gcv[0] = g_conic[i * 3 + 0]; gcv[1] = g_conic[i * 3 + 1]; gcv[2] = g_conic[i * 3 + 2];
-        // gradient on the projected mean = the render backward's sum (g_uv, by gaussian; may be absent) + whatever
+        // interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3
+        const float4* row = reinterpret_cast<const float4*>(g_rows + (size_t)i * GSR_GRAD_ROW_FLOATS);
+        const float4 r0 = row[0], r1 = row[1];
+        grv[0] = r0.x; grv[1] = r0.y; grv[2] = r0.z; gov = r0.w;
+        // gradient on the projected mean = the render backward's sum (the row's uv, unless rows_uv is 0) + whatever
         // arrives on the COMPACT uv rasterize returned (g_uv_compact [M,2]; row = rank among the visible gaussians,
         // read off the forward's packed inclusive scan)
-        if (g_uv != nullptr) { guv[0] = g_uv[i * 2 + 0]; guv[1] = g_uv[i * 2 + 1]; }
-        gov = g_opa[i];
-        grv[0] = g_rgb[i * 3 + 0]; grv[1] = g_rgb[i * 3 + 1]; grv[2] = g_rgb[i * 3 + 2];
+        if (rows_uv) { guv[0] = r1.x; guv[1] = r1.y; }
+        gcv[0] = r1.z; gcv[1] = r1.w;
+        if (DEPTH) {
+            const float2 r2 = *reinterpret_cast<const float2*>(g_rows + (size_t)i * GSR_GRAD_ROW_FLOATS + 8);
+            gcv[2] = r2.x;
+            gzc = r2.y;
+        } else {
+            gcv[2] = g_rows[(size_t)i * GSR_GRAD_ROW_FLOATS + 8];
         }
         if (g_uv_compact != nullptr) {
             const size_t r = (size_t)(scan[i] >> 32) - 1;
@@ -530,15 +522,14 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
 #define GSR_PRE_BWD_PARAMS                                                                                          \
     int N, const float* __restrict__ xyz, const float* __restrict__ quat, const float* __restrict__ scale,          \
         const float* __restrict__ opa_logit, const float* __restrict__ Tdev, const float* __restrict__ Kdev,        \
-        const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rgb,     \
-        const float* __restrict__ g_opa, const float* __restrict__ g_uv, const float* __restrict__ g_conic,         \
-        const float* __restrict__ g_rows, int rows_uv, const float* __restrict__ g_uv_compact,                      \
+        const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rows,    \
+        int rows_uv, const float* __restrict__ g_uv_compact,                                                         \
         const uint64_t* __restrict__ scan, float* __restrict__ o_xyz, float* __restrict__ o_quat,                   \
         float* __restrict__ o_scale, float* __restrict__ o_opa, float* __restrict__ o_dc, float* __restrict__ o_sh, \
         int use_tma
 #define GSR_PRE_BWD_FORWARD                                                                                      \
-    N, xyz, quat, scale, opa_logit, Tdev, Kdev, camdev, visible, g_rgb, g_opa, g_uv, g_conic, g_rows, rows_uv, \
-        g_uv_compact, scan, o_xyz, o_quat, o_scale, o_opa, o_dc, o_sh, use_tma
+    N, xyz, quat, scale, opa_logit, Tdev, Kdev, camdev, visible, g_rows, rows_uv, g_uv_compact, scan, o_xyz, o_quat, \
+        o_scale, o_opa, o_dc, o_sh, use_tma
 template <int N_SH, bool HAS_SH>
 __global__ void __launch_bounds__(PRE_THREADS, GSR_PRE_BWD_MINB) k_preprocess_bwd(GSR_PRE_BWD_PARAMS) {
     preprocess_bwd<N_SH, HAS_SH, false, false, false>(GSR_PRE_BWD_FORWARD, nullptr);
@@ -661,8 +652,7 @@ int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, con
 int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
                             const float* scale, const float* opacity_logit, const float* filter3d,
                             const float* camera_T_world,
-                            const float* K, const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
-                            const float* grad_opacity, const float* grad_uv, const float* grad_conic,
+                            const float* K, const float* camera_centre, const uint8_t* visible,
                             const float* grad_rows, int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
                             float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
                             float* g_sh_rest, void* stream) {
@@ -670,9 +660,7 @@ int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, co
     if ((mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
     if (((mode & GSR_MODE_FILTER3D) != 0) != (filter3d != nullptr)) return GSR_ERR_BAD_ARG;
     if (N <= 0) return GSR_OK;
-    // the depth/alpha and anti-aliased kernels read the render backward's sums from the interleaved rows only (and so
-    // does every absgrad backward: its render stage writes rows)
-    if (mode != 0 && (grad_rows == nullptr || !aligned16(grad_rows))) return GSR_ERR_BAD_ARG;
+    if (grad_rows == nullptr || !aligned16(grad_rows)) return GSR_ERR_BAD_ARG;
     if (grad_uv_compact != nullptr && scan == nullptr) return GSR_ERR_BAD_ARG;
     const dim3 grid((N + PRE_THREADS - 1) / PRE_THREADS), block(PRE_THREADS);
     const int use_tma = (aligned16(g_xyz) && aligned16(g_quaternion) && aligned16(g_scale) &&
@@ -681,9 +669,8 @@ int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, co
                             ? 1
                             : 0;
 #define GSR_PRE_ARGS                                                                                   \
-    N, xyz, quaternion, scale, opacity_logit, camera_T_world, K, camera_centre, visible, grad_rgb,         \
-        grad_opacity, grad_uv,                                                                             \
-        grad_conic, grad_rows, use_rows_uv, grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, use_tma
+    N, xyz, quaternion, scale, opacity_logit, camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, \
+        grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, use_tma
 #define GSR_PRE_BWD_SWITCH(kernel)                                                      \
     switch (n_sh_rest) {                                                                \
         case 0: kernel<1, false><<<grid, block, 0, st>>>(GSR_PRE_ARGS); break;          \

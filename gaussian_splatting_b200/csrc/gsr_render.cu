@@ -8,11 +8,11 @@
 // order (read off the reference's SASS, DESIGN.md "Rounding contract").
 //
 // Structure (what is different from the reference):
-//   * input is a depth-sorted, tile-contiguous stream of 48-byte records; batches of BATCH records are
-//     staged into a shared-memory ring by 1-D TMA bulk copies (cp.async.bulk + mbarrier) instead of 256
-//     threads gathering 4-byte fields through an index array.  Stages are recycled at WARP granularity
-//     (stage_checkout): the last warp to leave a stage re-arms it and issues the next copy, there is no
-//     CTA-wide barrier in either batch loop;
+//   * input is the per-gaussian array of 48-byte records, read in depth order through the sorted pair list;
+//     batches of BATCH records are staged into a shared-memory ring by 16-byte cp.async copies completing on
+//     an mbarrier, instead of 256 threads gathering 4-byte fields through an index array.  Stages are recycled
+//     at WARP granularity (stage_checkout): the last warp to leave a stage re-arms it and fetches the next
+//     batch, there is no CTA-wide barrier in either batch loop;
 //   * a CTA is 128 threads; a lane carries TWO horizontally adjacent pixels and evaluates them as pairs of
 //     scalar IEEE operations (gsr_f32x2.cuh; du is a pixel pair, dv and all per-splat constants are shared by
 //     both halves), so the per-splat work of a lane is paid once for two pixels;
@@ -97,7 +97,7 @@ constexpr int LIST_DUMMY = GROUPS * BATCH;
 // Contribution masks (forward -> backward): for every (tile, batch, warp, lane group) one BATCH-bit mask whose bit j
 // is set when staged record j of the batch contributed to at least one pixel of the group's block.  The backward
 // walks exactly the set bits, in ascending record order.  Slot of batch b of a tile whose
-// records start at stream position `start`: start / BATCH + tile + b (unique: a tile has at most total / BATCH + 1
+// records start at pair position `start`: start / BATCH + tile + b (unique: a tile has at most total / BATCH + 1
 // batches), i.e. at most P / BATCH + n_tiles + 1 slots of MASK_WORDS_PER_SLOT 32-bit words.
 constexpr int MASK_WORDS = BATCH / 32;
 constexpr int MASK_WORDS_PER_SLOT = CTA_WARPS * GROUPS * MASK_WORDS;
@@ -147,15 +147,14 @@ __device__ __forceinline__ bool div_fast_ok(float num) {
     return (__float_as_uint(num) - 0x1e000000u) < 0x40000000u;
 }
 
-// Where a tile's records come from.  stream != nullptr: the depth-sorted, tile-contiguous record stream (one bulk
-// copy per batch, issued by one thread).  Otherwise GATHER: the per-gaussian record array + the sorted pair keys
-// (gaussian id in their low bits, or a sorted id array): the warp that recycles a stage fetches the batch's 128
-// records itself, 3 x 16-byte cp.async per record, completion tracked by the stage's mbarrier
-// (cp.async.mbarrier.arrive.noinc, one arrival per lane).  No stream is ever written or read: the tile kernels are
-// issue-bound, the scattered 48-byte reads hide behind the walk.
+// Where a tile's records come from: the per-gaussian record array + the sorted pair keys (gaussian id in their low
+// bits, or a sorted id array).  The warp that recycles a stage fetches the batch's 128 records itself, 3 x 16-byte
+// cp.async per record, completion tracked by the stage's mbarrier (cp.async.mbarrier.arrive.noinc, one arrival per
+// lane).  No tile-ordered copy of the records is ever written: the tile kernels are issue-bound, the scattered
+// 48-byte reads hide behind the walk.
 struct RecSource {
-    const float* base;        // stream [P,12] (bulk mode) or per-gaussian records [N,12] (gather mode)
-    const uint64_t* keys;     // gather mode: sorted keys, id = key & id_mask ...
+    const float* base;        // per-gaussian records [N,12]
+    const uint64_t* keys;     // sorted keys, id = key & id_mask ...
     const int32_t* ids;       // ... or sorted gaussian ids when the id does not ride in the key
     uint64_t id_mask;
 };
@@ -245,10 +244,10 @@ __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {  // 8-b
 
 // Warp-granular stage recycling.  Every warp consumes every batch at its own pace: it waits on the stage's
 // "full" mbarrier, works, and then checks out of the stage through a counter; the LAST warp to check out
-// re-arms the barrier and issues the bulk copy of the batch STAGES further on.  Nobody ever waits for a
-// slower warp except through the data itself, so the per-batch imbalance between the four row bands of a
-// tile averages out over the tile instead of being paid at a CTA barrier per batch.
-// Returns true (warp-uniform) for the warp that was last.  The caller then runs `refill` on lane 0.
+// fetches the batch STAGES further on.  Nobody ever waits for a slower warp except through the data itself,
+// so the per-batch imbalance between the four row bands of a tile averages out over the tile instead of being
+// paid at a CTA barrier per batch.
+// Returns true (warp-uniform) for the warp that was last.  The caller then fetches the next batch with that warp.
 __device__ __forceinline__ bool stage_checkout(int* cnt, int lane) {
     __syncwarp();  // every lane of this warp is past its reads of the stage
     int last = 0;
@@ -482,7 +481,7 @@ struct ExactPixelDepth {
     ExactPixel p;
     float d;  // sum of w * z, in the same order
 };
-template <bool GATHER, bool DEPTH>
+template <bool DEPTH>
 __device__ __forceinline__ ExactPixel exact_pixel(const RecSource& src, const DepthSource& ds, int start, int total,
                                                   float fpx, float fpy, int lane, float& d) {
     ExactPixel o;
@@ -494,9 +493,7 @@ __device__ __forceinline__ ExactPixel exact_pixel(const RecSource& src, const De
         const int i = base + lane;
         float alpha = 0.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f, zi = 0.0f;
         if (i < total) {
-            const size_t row = DEPTH    ? (size_t)source_id_z(src, ds, start + i, zi)
-                               : GATHER ? (size_t)source_id(src, start + i)
-                                        : (size_t)(start + i);
+            const size_t row = DEPTH ? (size_t)source_id_z(src, ds, start + i, zi) : (size_t)source_id(src, start + i);
             const float4* q = reinterpret_cast<const float4*>(src.base + row * REC);
             const float4 q0 = __ldg(q), q1 = __ldg(q + 1), q2 = __ldg(q + 2);
             const float du = __fsub_rn(fpx, q0.x), dv = __fsub_rn(fpy, q0.y);
@@ -531,31 +528,29 @@ __device__ __forceinline__ ExactPixel exact_pixel(const RecSource& src, const De
     }
     return o;
 }
-template <bool GATHER>
 __device__ __noinline__ ExactPixel render_pixel_exact_warp(const RecSource src, int start, int total, float fpx,
                                                            float fpy, int lane) {
     float d;
-    return exact_pixel<GATHER, false>(src, DepthSource{}, start, total, fpx, fpy, lane, d);
+    return exact_pixel<false>(src, DepthSource{}, start, total, fpx, fpy, lane, d);
 }
 __device__ __noinline__ ExactPixelDepth render_pixel_exact_warp_depth(const RecSource src, const DepthSource ds,
                                                                       int start, int total, float fpx, float fpy,
                                                                       int lane) {
     ExactPixelDepth o;
-    o.p = exact_pixel<true, true>(src, ds, start, total, fpx, fpy, lane, o.d);
+    o.p = exact_pixel<true>(src, ds, start, total, fpx, fpy, lane, o.d);
     return o;
 }
 
 // MARK: also record, per (batch, warp, lane group), which staged records contributed (contribution masks for
 // the backward; `masks` must be zero-filled by the caller: a warp that skips a batch leaves its masks untouched)
-// DEPTH (gather mode only): also the per-pixel depth D = sum w * z and alpha A (depth / alpha [H,W])
-template <bool MARK, bool GATHER, bool DEPTH>
+// DEPTH: also the per-pixel depth D = sum w * z and alpha A (depth / alpha [H,W])
+template <bool MARK, bool DEPTH>
 __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* __restrict__ ranges,
                                            const float* __restrict__ background, int W, int H,
                                            int32_t* __restrict__ n_out, float* __restrict__ w_out,
                                            float* __restrict__ image, uint32_t* __restrict__ masks,
                                            const DepthSource& ds, float* __restrict__ depth,
                                            float* __restrict__ alpha) {
-    static_assert(GATHER || !DEPTH, "depth/alpha maps are rendered by the gather kernels only");
     __shared__ __align__(128) float s_rec[STAGES][BATCH * REC];
     __shared__ __align__(8) uint64_t s_full[STAGES];
     __shared__ int s_cnt[STAGES];
@@ -587,27 +582,20 @@ __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* _
     if (tid == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; ++s) {
-            // gather: one arrival per lane of the refilling warp (two with DEPTH, see gather_batch)
-            mbar_init(&s_full[s], GATHER ? (DEPTH ? 64 : 32) : 1);
+            // one arrival per lane of the refilling warp (two with DEPTH, see gather_batch)
+            mbar_init(&s_full[s], DEPTH ? 64 : 32);
             s_cnt[s] = 0;
         }
         fence_mbar_init();
     }
     __syncthreads();
-    // bulk mode: ONE thread arms the stage's barrier and starts the bulk copy of batch b;
-    // gather mode: the WHOLE calling warp fetches the batch's records (gather_batch)
+    // the WHOLE calling warp fetches the records of batch b (gather_batch)
     auto load_batch = [&](int b) {
         const int s = b % STAGES;
         const int cnt = min(BATCH, total - b * BATCH);
-        if (GATHER) {
-            gather_batch<DEPTH>(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane, &ds, &s_z[s][0]);
-        } else {
-            const uint32_t bytes = (uint32_t)cnt * REC * 4u;
-            mbar_arrive_expect_tx(&s_full[s], bytes);
-            tma_load_1d(&s_rec[s][0], rs.base + (size_t)(start + b * BATCH) * REC, bytes, &s_full[s]);
-        }
+        gather_batch<DEPTH>(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane, &ds, &s_z[s][0]);
     };
-    if (GATHER ? (warp == 0) : (tid == 0)) {
+    if (warp == 0) {
         const int pre = nb < STAGES ? nb : STAGES;
         for (int b = 0; b < pre; ++b) load_batch(b);
     }
@@ -651,14 +639,8 @@ __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* _
             if (lane == 0) { int sum = 0; for (int g = 0; g < GROUPS; ++g) sum += cnts[g]; STAT(4, sum); STAT(7, 1); }
 #endif
         }
-        if (stage_checkout(&s_cnt[s], lane) && b + STAGES < nb) {  // warp-uniform: this warp left the stage last
-            if (GATHER) {
-                load_batch(b + STAGES);
-            } else if (lane == 0) {
-                fence_proxy_async_smem();  // generic-proxy reads of the stage before the async-proxy overwrite
-                load_batch(b + STAGES);
-            }
-        }
+        if (stage_checkout(&s_cnt[s], lane) && b + STAGES < nb)  // warp-uniform: this warp left the stage last
+            load_batch(b + STAGES);
     }
 
     // pixels flagged by the walk: recompute them exactly, one at a time, with the whole warp
@@ -689,10 +671,10 @@ __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* _
             }
             continue;
         }
-        const ExactPixel e0 = render_pixel_exact_warp<GATHER>(rs, start, total, (float)sx, (float)sy, lane);
+        const ExactPixel e0 = render_pixel_exact_warp(rs, start, total, (float)sx, (float)sy, lane);
         if (lane == src) { A0 = e0.A; wl0 = e0.wl; n0 = e0.n; r0 = e0.c0; g0 = e0.c1; b0 = e0.c2; }
         if (two) {
-            const ExactPixel e1 = render_pixel_exact_warp<GATHER>(rs, start, total, (float)(sx + 1), (float)sy, lane);
+            const ExactPixel e1 = render_pixel_exact_warp(rs, start, total, (float)(sx + 1), (float)sy, lane);
             if (lane == src) { A1 = e1.A; wl1 = e1.wl; n1 = e1.n; r1 = e1.c0; g1 = e1.c1; b1 = e1.c2; }
         }
     }
@@ -721,13 +703,12 @@ __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* _
     finish(valid1, px + 1, A1, wl1, n1, r1, g1, b1);
 }
 
-template <bool MARK, bool GATHER>
+template <bool MARK>
 __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_MINB)
     k_render_fwd(const RecSource rs, const int32_t* __restrict__ ranges,
                  const float* __restrict__ background, int W, int H, int32_t* __restrict__ n_out,
                  float* __restrict__ w_out, float* __restrict__ image, uint32_t* __restrict__ masks) {
-    render_fwd<MARK, GATHER, false>(rs, ranges, background, W, H, n_out, w_out, image, masks, DepthSource{}, nullptr,
-                                    nullptr);
+    render_fwd<MARK, false>(rs, ranges, background, W, H, n_out, w_out, image, masks, DepthSource{}, nullptr, nullptr);
 }
 
 #ifndef GSR_FWD_DEPTH_MINB
@@ -739,7 +720,7 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_DEPTH_MINB)
                        const float* __restrict__ background, int W, int H, int32_t* __restrict__ n_out,
                        float* __restrict__ w_out, float* __restrict__ image, float* __restrict__ depth,
                        float* __restrict__ alpha, uint32_t* __restrict__ masks) {
-    render_fwd<MARK, true, true>(rs, ranges, background, W, H, n_out, w_out, image, masks, ds, depth, alpha);
+    render_fwd<MARK, true>(rs, ranges, background, W, H, n_out, w_out, image, masks, ds, depth, alpha);
 }
 
 // (float)(1.0 / (1.0 - (double)alpha)) — src/render_backward.cu:183 — without fp64: 1 - alpha is split
@@ -902,14 +883,14 @@ __device__ __forceinline__ void mask_lists(const uint32_t* __restrict__ gm, int 
 
 // MASKS: the per-group splat lists come from the forward's contribution masks (exactly the records that
 // contributed to the group's pixels) instead of the conservative footprint test
-// DEPTH (gather mode, interleaved rows only): upstream gradients on the depth and alpha maps join d_alpha through the
+// DEPTH (interleaved rows only): upstream gradients on the depth and alpha maps join d_alpha through the
 // same weight and r as colour, with two more back-to-front accumulators (no background term), and one more moment,
 // alpha * weight * dD, is reduced and flushed into the row's slot 9 (camera-frame z)
-// ABSGRAD (gather mode, interleaved rows only): two more moments, sum |2c*hu - (b+b)*hv| and sum |2a*hv - (b+b)*hu| with
+// ABSGRAD (interleaved rows only): two more moments, sum |2c*hu - (b+b)*hv| and sum |2a*hv - (b+b)*hu| with
 // the absolute value taken per pixel, before any sum; times |rdet| they are sum_p |d_u| and sum_p |d_v| (AbsGS), flushed
 // into the row's slots 10 and 11.  Moments 8..11 are then gc2, z (DEPTH, else 0), |u|, |v|
-template <bool MASKS, bool GATHER, bool DEPTH, bool ABSGRAD = false>
-__device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* __restrict__ sorted_idx,
+template <bool MASKS, bool DEPTH, bool ABSGRAD = false>
+__device__ __forceinline__ void render_bwd(const RecSource& rs,
                                            const int32_t* __restrict__ ranges, const float* __restrict__ background,
                                            int W, int H, const int32_t* __restrict__ n_in,
                                            const float* __restrict__ w_in, const float* __restrict__ grad_image,
@@ -917,8 +898,6 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
                                            float* __restrict__ g_uv, float* __restrict__ g_conic,
                                            const uint32_t* __restrict__ masks, const DepthSource& ds,
                                            const float* __restrict__ grad_depth, const float* __restrict__ grad_alpha) {
-    static_assert(GATHER || !DEPTH, "depth/alpha gradients are reduced by the gather kernels only");
-    static_assert(GATHER || !ABSGRAD, "absolute uv gradients are reduced by the gather kernels only");
     constexpr int NG = ABSGRAD ? NGRAD + 3 : DEPTH ? NGRAD + 1 : NGRAD;  // moments per (record, batch)
     __shared__ __align__(128) float s_rec[BSTAGES][(BATCH + 1) * REC];  // + an all-zero record (alpha 0) behind each stage
     __shared__ __align__(8) uint64_t s_full[BSTAGES];
@@ -972,7 +951,7 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
         s_maxn = 0;
 #pragma unroll
         for (int s = 0; s < BSTAGES; ++s) {
-            mbar_init(&s_full[s], GATHER ? (DEPTH ? 64 : 32) : 1);
+            mbar_init(&s_full[s], DEPTH ? 64 : 32);
             s_cnt[s] = 0;
         }
         fence_mbar_init();
@@ -995,20 +974,13 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
     const int nb = (total + BATCH - 1) / BATCH;
     if (nb == 0) return;
 
-    // batches are walked last -> first; pipeline slot k holds batch nb-1-k
-    // bulk mode: one thread; gather mode: the whole calling warp (see k_render_fwd)
+    // batches are walked last -> first; pipeline slot k holds batch nb-1-k, fetched by the whole calling warp
     auto load_slot = [&](int k) {
         const int b = nb - 1 - k, s = k % BSTAGES;
         const int cnt = min(BATCH, total - b * BATCH);
-        if (GATHER) {
-            gather_batch<DEPTH>(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane, &ds, &s_z[s][0]);
-        } else {
-            const uint32_t bytes = (uint32_t)cnt * REC * 4u;
-            mbar_arrive_expect_tx(&s_full[s], bytes);
-            tma_load_1d(&s_rec[s][0], rs.base + (size_t)(start + b * BATCH) * REC, bytes, &s_full[s]);
-        }
+        gather_batch<DEPTH>(rs, start + b * BATCH, cnt, &s_rec[s][0], &s_full[s], lane, &ds, &s_z[s][0]);
     };
-    if (GATHER ? (warp == 0) : (tid == 0)) {
+    if (warp == 0) {
         const int pre = nb < BSTAGES ? nb : BSTAGES;
         for (int k = 0; k < pre; ++k) load_slot(k);
     }
@@ -1242,9 +1214,7 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
 #pragma unroll
             for (int i = 0; i < BATCH / 32; ++i) {
                 const int r = lane + 32 * i;
-                gids[i] = (r >= cnt) ? 0
-                          : GATHER ? (int)source_id(rs, start + b * BATCH + r)
-                                   : __ldg(sorted_idx + start + b * BATCH + r);
+                gids[i] = (r >= cnt) ? 0 : (int)source_id(rs, start + b * BATCH + r);
             }
 #pragma unroll
             for (int i = 0; i < BATCH / 32; ++i) {
@@ -1300,29 +1270,23 @@ __device__ __forceinline__ void render_bwd(const RecSource& rs, const int32_t* _
             }
             __syncwarp();
             if (k + BSTAGES < nb) {
-                if (GATHER) {
-                    __threadfence_block();  // every lane: its share of the cleared accumulator before its arrival
-                    load_slot(k + BSTAGES);
-                } else if (lane == 0) {
-                    __threadfence_block();     // cleared accumulator before the barrier is re-armed
-                    fence_proxy_async_smem();  // generic-proxy reads of the stage before the async-proxy overwrite
-                    load_slot(k + BSTAGES);
-                }
+                __threadfence_block();  // every lane: its share of the cleared accumulator before its arrival
+                load_slot(k + BSTAGES);
             }
         }
     }
 }
 
-template <bool MASKS, bool GATHER>
+template <bool MASKS>
 __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_MINB)
-    k_render_bwd(const RecSource rs, const int32_t* __restrict__ sorted_idx,
+    k_render_bwd(const RecSource rs,
                  const int32_t* __restrict__ ranges, const float* __restrict__ background, int W, int H,
                  const int32_t* __restrict__ n_in, const float* __restrict__ w_in,
                  const float* __restrict__ grad_image, float* __restrict__ g_rgb,
                  float* __restrict__ g_opa, float* __restrict__ g_uv, float* __restrict__ g_conic,
                  const uint32_t* __restrict__ masks) {
-    render_bwd<MASKS, GATHER, false>(rs, sorted_idx, ranges, background, W, H, n_in, w_in, grad_image, g_rgb, g_opa,
-                                     g_uv, g_conic, masks, DepthSource{}, nullptr, nullptr);
+    render_bwd<MASKS, false>(rs, ranges, background, W, H, n_in, w_in, grad_image, g_rgb, g_opa, g_uv, g_conic, masks,
+                             DepthSource{}, nullptr, nullptr);
 }
 
 #ifndef GSR_BWD_DEPTH_MINB
@@ -1338,8 +1302,8 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_BWD_DEPTH_MINB)
                        const float* __restrict__ w_in, const float* __restrict__ grad_image,
                        const float* __restrict__ grad_depth, const float* __restrict__ grad_alpha,
                        float* __restrict__ grad_rows, const uint32_t* __restrict__ masks) {
-    render_bwd<MASKS, true, true>(rs, nullptr, ranges, background, W, H, n_in, w_in, grad_image, grad_rows, nullptr,
-                                  nullptr, nullptr, masks, ds, grad_depth, grad_alpha);
+    render_bwd<MASKS, true>(rs, ranges, background, W, H, n_in, w_in, grad_image, grad_rows, nullptr, nullptr, nullptr,
+                            masks, ds, grad_depth, grad_alpha);
 }
 
 // Absolute uv gradients (GSR_MODE_ABSGRAD), colour only or with depth/alpha (DEPTH).  The two more moments are
@@ -1365,8 +1329,8 @@ __global__ void __launch_bounds__(CTA_THREADS, DEPTH   ? GSR_BWD_DEPTH_ABS_MINB
                      const float* __restrict__ w_in, const float* __restrict__ grad_image,
                      const float* __restrict__ grad_depth, const float* __restrict__ grad_alpha,
                      float* __restrict__ grad_rows, const uint32_t* __restrict__ masks) {
-    render_bwd<MASKS, true, DEPTH, true>(rs, nullptr, ranges, background, W, H, n_in, w_in, grad_image, grad_rows,
-                                         nullptr, nullptr, nullptr, masks, ds, grad_depth, grad_alpha);
+    render_bwd<MASKS, DEPTH, true>(rs, ranges, background, W, H, n_in, w_in, grad_image, grad_rows, nullptr, nullptr,
+                                   nullptr, masks, ds, grad_depth, grad_alpha);
 }
 
 }  // namespace gsr
@@ -1396,8 +1360,7 @@ static bool make_depth_source(const uint64_t* keys_sorted, int id_bits, const ui
     return true;
 }
 
-// ds != nullptr: the depth/alpha kernels (gather mode only)
-template <bool GATHER>
+// ds != nullptr: the depth/alpha kernels
 static int launch_forward(const RecSource& src, const DepthSource* ds, const int32_t* ranges, const float* background,
                           int H, int W, int32_t* n_out, float* w_out, float* image, float* depth, float* alpha,
                           uint32_t* masks, void* stream) {
@@ -1412,19 +1375,16 @@ static int launch_forward(const RecSource& src, const DepthSource* ds, const int
             k_render_fwd_depth<false><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_out, w_out, image,
                                                               depth, alpha, nullptr);
     } else if (masks != nullptr) {
-        k_render_fwd<true, GATHER><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image, masks);
+        k_render_fwd<true><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image, masks);
     } else {
-        k_render_fwd<false, GATHER><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image,
-                                                            nullptr);
+        k_render_fwd<false><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image, nullptr);
     }
     return (int)cudaGetLastError();
 }
 
-// ds != nullptr: the depth/alpha kernels; absgrad: the absolute-uv-gradient kernels (both gather mode only; the
-// gradients go to interleaved rows, passed as g_rgb)
-template <bool GATHER>
-static int launch_backward(const RecSource& src, const DepthSource* ds, bool absgrad, const int32_t* sorted_idx,
-                           const int32_t* ranges, const float* background, int H, int W, const int32_t* n_in,
+// ds != nullptr: the depth/alpha kernels; absgrad: the absolute-uv-gradient kernels (both write interleaved rows,
+// passed as g_rgb)
+static int launch_backward(const RecSource& src, const DepthSource* ds, bool absgrad, const int32_t* ranges, const float* background, int H, int W, const int32_t* n_in,
                            const float* w_in, const float* grad_image, const float* grad_depth,
                            const float* grad_alpha, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
                            const uint32_t* masks, void* stream) {
@@ -1453,11 +1413,11 @@ static int launch_backward(const RecSource& src, const DepthSource* ds, bool abs
             k_render_bwd_depth<false><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_in, w_in,
                                                               grad_image, grad_depth, grad_alpha, g_rgb, nullptr);
     } else if (masks != nullptr) {
-        k_render_bwd<true, GATHER><<<grid, block, 0, st>>>(src, sorted_idx, ranges, background, W, H, n_in, w_in,
-                                                           grad_image, g_rgb, g_opa, g_uv, g_conic, masks);
+        k_render_bwd<true><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_in, w_in, grad_image, g_rgb, g_opa,
+                                                   g_uv, g_conic, masks);
     } else {
-        k_render_bwd<false, GATHER><<<grid, block, 0, st>>>(src, sorted_idx, ranges, background, W, H, n_in, w_in,
-                                                            grad_image, g_rgb, g_opa, g_uv, g_conic, nullptr);
+        k_render_bwd<false><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_in, w_in, grad_image, g_rgb, g_opa,
+                                                    g_uv, g_conic, nullptr);
     }
     return (int)cudaGetLastError();
 }
@@ -1470,22 +1430,6 @@ size_t gsr_contribution_mask_words(int64_t P, int H, int W) {
     return (size_t)(P / BATCH + n_tiles + 1) * MASK_WORDS_PER_SLOT;
 }
 
-int gsr_render_forward(const float* records, const int32_t* ranges, const float* background, int H, int W,
-                       int32_t* n_out, float* w_out, float* image, uint32_t* contribution_masks, void* stream) {
-    return launch_forward<false>(make_source(records, nullptr, nullptr, 0), nullptr, ranges, background, H, W, n_out,
-                                 w_out, image, nullptr, nullptr, contribution_masks, stream);
-}
-
-int gsr_render_backward(const float* records, const int32_t* sorted_idx, const int32_t* ranges,
-                        const float* background, int H, int W, const int32_t* n_in, const float* w_in,
-                        const float* grad_image, float* g_rgb, float* g_opa, float* g_uv, float* g_conic,
-                        const uint32_t* contribution_masks, void* stream) {
-    return launch_backward<false>(make_source(records, nullptr, nullptr, 0), nullptr, false, sorted_idx, ranges,
-                                  background,
-                                  H, W, n_in, w_in, grad_image, nullptr, nullptr, g_rgb, g_opa, g_uv, g_conic,
-                                  contribution_masks, stream);
-}
-
 int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
                               const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base, int depth_bits,
                               const int32_t* ranges, const float* background, int H, int W, int32_t* n_out,
@@ -1496,9 +1440,9 @@ int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* key
     DepthSource ds;
     if (depth != nullptr && !make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds))
         return GSR_ERR_BAD_ARG;
-    return launch_forward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
-                                depth != nullptr ? &ds : nullptr, ranges, background, H, W, n_out, w_out, image, depth,
-                                alpha, contribution_masks, stream);
+    return launch_forward(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
+                          depth != nullptr ? &ds : nullptr, ranges, background, H, W, n_out, w_out, image, depth, alpha,
+                          contribution_masks, stream);
 }
 
 int gsr_render_backward_gather(int mode, const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
@@ -1526,11 +1470,9 @@ int gsr_render_backward_gather(int mode, const float* gaussian_records, const ui
     } else if (g_rgb == nullptr || g_opa == nullptr || g_uv == nullptr || g_conic == nullptr) {
         return GSR_ERR_BAD_ARG;
     }
-    return launch_backward<true>(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
-                                 grad_depth != nullptr ? &ds : nullptr, absgrad, nullptr, ranges, background, H, W,
-                                 n_in, w_in,
-                                 grad_image, grad_depth, grad_alpha, g_rgb, g_opa, g_uv, g_conic, contribution_masks,
-                                 stream);
+    return launch_backward(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
+                           grad_depth != nullptr ? &ds : nullptr, absgrad, ranges, background, H, W, n_in, w_in,
+                           grad_image, grad_depth, grad_alpha, g_rgb, g_opa, g_uv, g_conic, contribution_masks, stream);
 }
 
 const char* gsr_version(void) { return "gsr_b200 0.1 sm_90a"; }

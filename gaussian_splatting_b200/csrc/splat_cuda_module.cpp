@@ -254,6 +254,33 @@ struct RenderShapes {
     int N, H, W, n_sh;
 };
 
+// The sorted pair list the tile renderers read record ids through: the keys when the id rides in them, else the
+// sorted id array.  An empty view (P == 0) may have neither (the key/value fallback narrows its id array to nothing);
+// the kernels still run, to write the background, and read no pair: any well-formed source will do.
+struct PairSource {
+    const uint64_t* keys;
+    const int32_t* ids;
+};
+PairSource pair_source(const c10::optional<torch::Tensor>& keys_sorted, const c10::optional<torch::Tensor>& ids_sorted,
+                       int64_t P) {
+    static const int32_t no_pair = 0;
+    if (keys_sorted.has_value() && keys_sorted->numel() > 0)
+        return {(const uint64_t*)keys_sorted->data_ptr<int64_t>(), nullptr};
+    if (ids_sorted.has_value() && ids_sorted->numel() > 0) return {nullptr, ids_sorted->data_ptr<int>()};
+    TORCH_CHECK(P == 0, "the tile renderers need the sorted pair list");
+    return {nullptr, &no_pair};
+}
+
+// fp32 per-gaussian arrays of the reference surface -> the renderers' per-gaussian records [N,12]
+torch::Tensor pack_records(const torch::Tensor& uvs, const torch::Tensor& opacity, const torch::Tensor& rgb,
+                           const torch::Tensor& conic, int N) {
+    torch::Tensor records = torch::empty({std::max(N, 1), GSR_REC_FLOATS}, uvs.options());
+    check_rc(gsr_pack_gaussian_records(N, uvs.data_ptr<float>(), opacity.data_ptr<float>(), rgb.data_ptr<float>(),
+                                       conic.data_ptr<float>(), records.data_ptr<float>(), cur_stream()),
+             "gsr_pack_gaussian_records");
+    return records;
+}
+
 RenderShapes check_render_inputs(const torch::Tensor& uvs, const torch::Tensor& opacity, const torch::Tensor& rgb,
                                  const torch::Tensor& conic, const torch::Tensor& view_dir_by_pixel,
                                  const torch::Tensor& ranges, const torch::Tensor& idx,
@@ -303,18 +330,16 @@ void render_tiles_cuda(torch::Tensor uvs, torch::Tensor opacity, torch::Tensor r
     const int dt = common_dtype(uvs, {&opacity, &rgb, &conic, &view_dir_by_pixel, &background_rgb,
                                       &final_weight_per_pixel, &rendered_image});
     c10::cuda::CUDAGuard guard(uvs.device());
-    const int P = gaussian_idx_by_splat_idx.numel();
     if (dt == GSR_F32 && s.n_sh == 1) {
-        torch::Tensor records = torch::empty({std::max(P, 1), GSR_REC_FLOATS}, uvs.options());
-        check_rc(gsr_pack_records(P, gaussian_idx_by_splat_idx.data_ptr<int>(), uvs.data_ptr<float>(),
-                                  opacity.data_ptr<float>(), rgb.data_ptr<float>(), conic.data_ptr<float>(),
-                                  records.data_ptr<float>(), cur_stream()),
-                 "gsr_pack_records");
-        check_rc(gsr_render_forward(records.data_ptr<float>(), splat_start_end_idx_by_tile_idx.data_ptr<int>(),
-                                    background_rgb.data_ptr<float>(), s.H, s.W,
-                                    num_splats_per_pixel.data_ptr<int>(), final_weight_per_pixel.data_ptr<float>(),
-                                    rendered_image.data_ptr<float>(), nullptr, cur_stream()),
-                 "gsr_render_forward");
+        const torch::Tensor records = pack_records(uvs, opacity, rgb, conic, s.N);
+        const PairSource ps = pair_source(c10::nullopt, gaussian_idx_by_splat_idx, gaussian_idx_by_splat_idx.numel());
+        check_rc(gsr_render_forward_gather(records.data_ptr<float>(), nullptr, 0, ps.ids, nullptr, 0, 0,
+                                           splat_start_end_idx_by_tile_idx.data_ptr<int>(),
+                                           background_rgb.data_ptr<float>(), s.H, s.W,
+                                           num_splats_per_pixel.data_ptr<int>(),
+                                           final_weight_per_pixel.data_ptr<float>(), rendered_image.data_ptr<float>(),
+                                           nullptr, nullptr, nullptr, cur_stream()),
+                 "gsr_render_forward_gather");
     } else {
         check_rc(gsr_render_forward_generic(
                      dt, s.N, s.n_sh, uvs.data_ptr(), opacity.data_ptr(), rgb.data_ptr(), conic.data_ptr(),
@@ -350,21 +375,19 @@ void render_tiles_backward_cuda(torch::Tensor uvs, torch::Tensor opacity, torch:
                                       &final_weight_per_pixel, &grad_image, &grad_rgb, &grad_opacity, &grad_uvs,
                                       &grad_conic});
     c10::cuda::CUDAGuard guard(uvs.device());
-    const int P = gaussian_idx_by_splat_idx.numel();
     if (dt == GSR_F32 && s.n_sh == 1) {
-        torch::Tensor records = torch::empty({std::max(P, 1), GSR_REC_FLOATS}, uvs.options());
-        check_rc(gsr_pack_records(P, gaussian_idx_by_splat_idx.data_ptr<int>(), uvs.data_ptr<float>(),
-                                  opacity.data_ptr<float>(), rgb.data_ptr<float>(), conic.data_ptr<float>(),
-                                  records.data_ptr<float>(), cur_stream()),
-                 "gsr_pack_records");
-        check_rc(gsr_render_backward(records.data_ptr<float>(), gaussian_idx_by_splat_idx.data_ptr<int>(),
-                                     splat_start_end_idx_by_tile_idx.data_ptr<int>(),
-                                     background_rgb.data_ptr<float>(), s.H, s.W,
-                                     num_splats_per_pixel.data_ptr<int>(), final_weight_per_pixel.data_ptr<float>(),
-                                     grad_image.data_ptr<float>(), grad_rgb.data_ptr<float>(),
-                                     grad_opacity.data_ptr<float>(), grad_uvs.data_ptr<float>(),
-                                     grad_conic.data_ptr<float>(), nullptr, cur_stream()),
-                 "gsr_render_backward");
+        const torch::Tensor records = pack_records(uvs, opacity, rgb, conic, s.N);
+        const PairSource ps = pair_source(c10::nullopt, gaussian_idx_by_splat_idx, gaussian_idx_by_splat_idx.numel());
+        // the caller's planar gradient arrays, accumulated into as the reference does
+        check_rc(gsr_render_backward_gather(0, records.data_ptr<float>(), nullptr, 0, ps.ids, nullptr, 0, 0,
+                                            splat_start_end_idx_by_tile_idx.data_ptr<int>(),
+                                            background_rgb.data_ptr<float>(), s.H, s.W,
+                                            num_splats_per_pixel.data_ptr<int>(),
+                                            final_weight_per_pixel.data_ptr<float>(), grad_image.data_ptr<float>(),
+                                            nullptr, nullptr, grad_rgb.data_ptr<float>(),
+                                            grad_opacity.data_ptr<float>(), grad_uvs.data_ptr<float>(),
+                                            grad_conic.data_ptr<float>(), nullptr, nullptr, cur_stream()),
+                 "gsr_render_backward_gather");
     } else {
         check_rc(gsr_render_backward_generic(
                      dt, s.N, s.n_sh, uvs.data_ptr(), opacity.data_ptr(), rgb.data_ptr(), conic.data_ptr(),
@@ -486,17 +509,17 @@ std::vector<torch::Tensor> fused_preprocess_forward(
     return {records, zkey, visible, scan, tile_mask, tile_win};
 }
 
-// (M, P known) -> sorted gaussian ids [P] i32, tile ranges [n_tiles+1] i32, sorted record stream [P,12],
+// (M, P known) -> the sorted pair list the tile renderers read records through, tile ranges [n_tiles+1] i32,
 //                 vis_idx [M] i32, uv [M,2]
 // speculative = true: M and P are CAPACITIES (the host has not read the real counts yet): buffers are sized by
 // them, the pair buffer is padded behind the real pairs (gsr_emit_*'s `capacity`), and every tensor is returned at
 // full capacity — the caller narrows them once it knows M and P, and redoes the call if P exceeded the capacity.
-// no_stream = true: the tile kernels will fetch records through the sorted pair list themselves
-// (gsr_render_*_gather): no record stream is produced; returns the sorted keys (and id_bits) instead.
-// returns (ids_sorted, ranges, stream_rec, vis_idx, uv, keys_sorted, id_bits)
-std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, int64_t> fused_bin(
+// The pair list is the sorted keys when the gaussian id rides in their low id_bits (ids_sorted is then empty), else
+// the sorted gaussian ids [P] i32 (keys_sorted is then empty and id_bits 0).
+// returns (ids_sorted, ranges, vis_idx, uv, keys_sorted, id_bits)
+std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, int64_t> fused_bin(
     torch::Tensor records, torch::Tensor zkey, torch::Tensor visible, torch::Tensor scan, int64_t M, int64_t P,
-    int64_t H, int64_t W, double mh_dist, int64_t depth_bits, bool speculative, bool no_stream,
+    int64_t H, int64_t W, double mh_dist, int64_t depth_bits, bool speculative,
     c10::optional<torch::Tensor> tile_mask, c10::optional<torch::Tensor> tile_win) {
     const bool tiles = tile_mask.has_value() && tile_win.has_value() && tile_mask->numel() == records.size(0) &&
                        tile_win->numel() == records.size(0) && records.size(0) > 0;
@@ -509,16 +532,14 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
     auto i32 = opt.dtype(torch::kInt32);
     const int64_t Pa = std::max<int64_t>(P, 1);
     torch::Tensor keys = torch::empty({2 * Pa}, opt.dtype(torch::kInt64));
-    const int id_bits_probe = gsr_packed_id_bits(N, n_tiles, (int)depth_bits);
-    // with the id in the key and no stream, nobody needs the separate id array
-    torch::Tensor ids_sorted = torch::empty({(no_stream && id_bits_probe > 0) ? 0 : Pa}, i32);
+    const int id_bits = gsr_packed_id_bits(N, n_tiles, (int)depth_bits);
+    // with the id in the key, nobody needs the separate id array
+    torch::Tensor ids_sorted = torch::empty({id_bits > 0 ? 0 : Pa}, i32);
     torch::Tensor vis_idx = torch::empty({M}, i32);
     torch::Tensor uv = torch::empty({M, 2}, opt);
     torch::Tensor ranges = torch::empty({n_tiles + 1}, i32);
-    torch::Tensor stream_rec = torch::empty({no_stream ? 0 : Pa, GSR_REC_FLOATS}, opt);
     uint64_t* keys_a = (uint64_t*)keys.data_ptr<int64_t>();
     uint64_t* keys_b = keys_a + Pa;
-    const int id_bits = gsr_packed_id_bits(N, n_tiles, (int)depth_bits);
     if (id_bits > 0) {  // (tile | depth | id) keys, keys-only radix sort
         check_rc(gsr_emit_keys(N, F32PTR(records), (const uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),
                                (const uint64_t*)scan.data_ptr<int64_t>(), ntx, nty, (float)mh_dist, (int)depth_bits,
@@ -533,10 +554,6 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
         check_rc(gsr_tile_ranges((int)P, n_tiles, (int)depth_bits + id_bits, keys_b, ranges.data_ptr<int>(),
                                  cur_stream()),
                  "gsr_tile_ranges");
-        if (!no_stream)
-            check_rc(gsr_gather_records_keys((int)P, id_bits, keys_b, F32PTR(records), F32PTR(stream_rec),
-                                             ids_sorted.data_ptr<int>(), nullptr, cur_stream()),
-                     "gsr_gather_records_keys");
     } else {
         torch::Tensor ids = torch::empty({Pa}, i32);
         check_rc(gsr_emit_pairs(N, F32PTR(records), (const uint32_t*)zkey.data_ptr<int>(),
@@ -551,46 +568,23 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
                  "gsr_sort_pairs");
         check_rc(gsr_tile_ranges((int)P, n_tiles, (int)depth_bits, keys_b, ranges.data_ptr<int>(), cur_stream()),
                  "gsr_tile_ranges");
-        if (!no_stream)
-            check_rc(gsr_gather_records((int)P, (const uint32_t*)ids_sorted.data_ptr<int>(), F32PTR(records),
-                                        F32PTR(stream_rec), nullptr, nullptr, cur_stream()),
-                     "gsr_gather_records");
     }
-    torch::Tensor keys_sorted = (no_stream && id_bits > 0) ? keys.narrow(0, Pa, Pa) : torch::empty({0}, opt.dtype(torch::kInt64));
-    return std::make_tuple(ids_sorted.numel() > 0 ? ids_sorted.narrow(0, 0, P) : ids_sorted, ranges, stream_rec, vis_idx,
-                           uv, keys_sorted, (int64_t)id_bits);
-}
-
-// The sorted pair list the gather kernels read record ids through: the keys when the id rides in them, else the sorted
-// id array.  An empty view (P == 0) may have neither (the key/value fallback narrows its id array to nothing); the
-// kernels still run, to write the background, and read no pair: any well-formed source will do.
-struct PairSource {
-    const uint64_t* keys;
-    const int32_t* ids;
-};
-PairSource pair_source(const c10::optional<torch::Tensor>& keys_sorted, const c10::optional<torch::Tensor>& ids_sorted,
-                       int64_t P) {
-    static const int32_t no_pair = 0;
-    if (keys_sorted.has_value() && keys_sorted->numel() > 0)
-        return {(const uint64_t*)keys_sorted->data_ptr<int64_t>(), nullptr};
-    if (ids_sorted.has_value() && ids_sorted->numel() > 0) return {nullptr, ids_sorted->data_ptr<int>()};
-    TORCH_CHECK(P == 0, "gather mode needs the sorted pair list");
-    return {nullptr, &no_pair};
+    torch::Tensor keys_sorted = id_bits > 0 ? keys.narrow(0, Pa, Pa) : torch::empty({0}, opt.dtype(torch::kInt64));
+    return std::make_tuple(ids_sorted.numel() > 0 ? ids_sorted.narrow(0, 0, P) : ids_sorted, ranges, vis_idx, uv,
+                           keys_sorted, (int64_t)id_bits);
 }
 
 // returns (image [H,W,3], n [H,W] i32, wlast [H,W], contribution masks (i32 words; empty when record_masks is false),
 // depth [H,W,1], alpha [H,W,1]); depth and alpha are None unless depth_key (the per-gaussian depth keys of the forward,
 // read when the pair list is a sorted id array) asks for the depth/alpha kernels.
-// records: the record stream [P,12] — or, in gather mode, the per-gaussian record array [N,12] read through the sorted
-// pair list keys_sorted / ids_sorted
+// records: the per-gaussian record array [N,12], read through the sorted pair list keys_sorted / ids_sorted
 std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor>
 fused_render_forward(torch::Tensor records, torch::Tensor ranges, torch::Tensor background, int64_t H, int64_t W,
                      int64_t P, bool record_masks, c10::optional<torch::Tensor> keys_sorted,
-                     c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, bool gather,
+                     c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
                      c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits) {
     CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
     TORCH_CHECK(background.numel() == 3, "Background RGB must have 3 elements");
-    TORCH_CHECK(gather || !depth_key.has_value(), "depth and alpha maps come from the gather kernels only");
     c10::cuda::CUDAGuard guard(records.device());
     auto opt = records.options();
     torch::Tensor image = torch::empty({H, W, 3}, opt);
@@ -605,37 +599,29 @@ fused_render_forward(torch::Tensor records, torch::Tensor ranges, torch::Tensor 
                               ? torch::zeros({(int64_t)gsr_contribution_mask_words(P, (int)H, (int)W)}, opt.dtype(torch::kInt32))
                               : torch::empty({0}, opt.dtype(torch::kInt32));
     uint32_t* mptr = record_masks ? (uint32_t*)masks.data_ptr<int>() : nullptr;
-    if (gather) {
-        const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
-        check_rc(gsr_render_forward_gather(
-                     F32PTR(records), ps.keys, (int)id_bits, ps.ids,
-                     depth_key.has_value() ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr,
-                     (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
-                     n.data_ptr<int>(), F32PTR(w), F32PTR(image), depth.defined() ? F32PTR(depth) : nullptr,
-                     alpha.defined() ? F32PTR(alpha) : nullptr, mptr, cur_stream()),
-                 "gsr_render_forward_gather");
-    } else {
-        check_rc(gsr_render_forward(F32PTR(records), ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
-                                    n.data_ptr<int>(), F32PTR(w), F32PTR(image), mptr, cur_stream()),
-                 "gsr_render_forward");
-    }
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    check_rc(gsr_render_forward_gather(
+                 F32PTR(records), ps.keys, (int)id_bits, ps.ids,
+                 depth_key.has_value() ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr,
+                 (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
+                 n.data_ptr<int>(), F32PTR(w), F32PTR(image), depth.defined() ? F32PTR(depth) : nullptr,
+                 alpha.defined() ? F32PTR(alpha) : nullptr, mptr, cur_stream()),
+             "gsr_render_forward_gather");
     return std::make_tuple(image, n, w, masks, depth, alpha);
 }
 
-// per-gaussian gradient slab, rows indexed by gaussian; zero-filled, then accumulated into by the render backward.
-// Gather mode: interleaved rows [N,12] rgb3 opacity | uv2 conic0 conic1 | conic2 pad3 (vector reductions); with
+// per-gaussian gradient slab, rows indexed by gaussian; zero-filled, then accumulated into by the render backward:
+// interleaved rows [N,12] rgb3 opacity | uv2 conic0 conic1 | conic2 pad3 (vector reductions); with
 // grad_depth / grad_alpha [H,W,1] (the upstream gradients on the depth/alpha maps, with the forward's depth keys)
 // conic2 z pad2, z the gradient on the camera-frame z.  mode: GSR_MODE_* bits, passed to gsr_render_backward_gather
-// (GSR_MODE_ABSGRAD: conic2 z|0 |u| |v|, the per-pixel absolute uv gradients summed).  Record-stream mode: planar [9N]
-// rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3].
+// (GSR_MODE_ABSGRAD: conic2 z|0 |u| |v|, the per-pixel absolute uv gradients summed).
 torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, int64_t P, torch::Tensor records,
                                     torch::Tensor ids_sorted, torch::Tensor ranges, torch::Tensor background,
                                     torch::Tensor n, torch::Tensor w, torch::Tensor masks,
-                                    c10::optional<torch::Tensor> keys_sorted, int64_t id_bits, bool gather,
+                                    c10::optional<torch::Tensor> keys_sorted, int64_t id_bits,
                                     c10::optional<torch::Tensor> grad_depth, c10::optional<torch::Tensor> grad_alpha,
                                     c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits,
                                     int64_t mode) {
-    TORCH_CHECK(gather || (mode & GSR_MODE_ABSGRAD) == 0, "absolute uv gradients come from the gather kernels only");
     CHECK_VALID_INPUT(grad_image); CHECK_FLOAT_TENSOR(grad_image);
     const int H = n.size(0), W = n.size(1);
     TORCH_CHECK(grad_image.dim() == 3 && grad_image.size(0) == H && grad_image.size(1) == W &&
@@ -643,41 +629,30 @@ torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, int64_t
                 "grad_image must be HxWx3");
     const bool depth = grad_depth.has_value();
     if (depth) {
-        TORCH_CHECK(gather && grad_alpha.has_value() && depth_key.has_value(),
-                    "the depth/alpha backward needs gather mode, grad_alpha and depth_key");
+        TORCH_CHECK(grad_alpha.has_value() && depth_key.has_value(),
+                    "the depth/alpha backward needs grad_alpha and depth_key");
         CHECK_VALID_INPUT((*grad_depth)); CHECK_FLOAT_TENSOR((*grad_depth));
         CHECK_VALID_INPUT((*grad_alpha)); CHECK_FLOAT_TENSOR((*grad_alpha));
         TORCH_CHECK(grad_depth->numel() == (int64_t)H * W && grad_alpha->numel() == (int64_t)H * W,
                     "grad_depth and grad_alpha must hold H*W values");
     }
     c10::cuda::CUDAGuard guard(grad_image.device());
-    torch::Tensor slab = torch::zeros({N * (gather ? (int64_t)GSR_GRAD_ROW_FLOATS : 9)}, grad_image.options());
-    float* g_rgb = slab.data_ptr<float>();
-    float* g_opa = g_rgb + (size_t)N * 3;
-    float* g_uv = g_opa + (size_t)N;
-    float* g_conic = g_uv + (size_t)N * 2;
+    torch::Tensor slab = torch::zeros({N * (int64_t)GSR_GRAD_ROW_FLOATS}, grad_image.options());
     const uint32_t* mptr = masks.numel() > 0 ? (const uint32_t*)masks.data_ptr<int>() : nullptr;
-    if (gather) {
-        const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
-        check_rc(gsr_render_backward_gather(
-                     (int)mode, F32PTR(records), ps.keys, (int)id_bits, ps.ids,
-                     depth ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr, (uint32_t)depth_base,
-                     (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w),
-                     F32PTR(grad_image), depth ? F32PTR((*grad_depth)) : nullptr,
-                     depth ? F32PTR((*grad_alpha)) : nullptr, nullptr, nullptr, nullptr, nullptr, g_rgb, mptr,
-                     cur_stream()),
-                 "gsr_render_backward_gather");
-    } else {
-        check_rc(gsr_render_backward(F32PTR(records), ids_sorted.data_ptr<int>(), ranges.data_ptr<int>(),
-                                     F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w), F32PTR(grad_image),
-                                     g_rgb, g_opa, g_uv, g_conic, mptr, cur_stream()),
-                 "gsr_render_backward");
-    }
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    check_rc(gsr_render_backward_gather(
+                 (int)mode, F32PTR(records), ps.keys, (int)id_bits, ps.ids,
+                 depth ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr, (uint32_t)depth_base,
+                 (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), H, W, n.data_ptr<int>(), F32PTR(w),
+                 F32PTR(grad_image), depth ? F32PTR((*grad_depth)) : nullptr,
+                 depth ? F32PTR((*grad_alpha)) : nullptr, nullptr, nullptr, nullptr, nullptr, F32PTR(slab), mptr,
+                 cur_stream()),
+             "gsr_render_backward_gather");
     return slab;
 }
 
-// grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab of fused_render_backward: planar
-// [9N] or interleaved rows [N,12] (rows by gaussian).  grad_uv_compact [M,2] (optional): gradient on the compact uv,
+// grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab of fused_render_backward:
+// interleaved rows [N,12] by gaussian.  grad_uv_compact [M,2] (optional): gradient on the compact uv,
 // added to — or, with use_slab_uv false, replacing — the slab's uv section.  mode: the GSR_MODE_* bits of the forward
 // (gsr_preprocess_backward): GSR_MODE_DEPTH_ALPHA reads the z gradient of the depth/alpha rows, GSR_MODE_ANTIALIASED
 // takes the rows' opacity slot as the gradient on the compensated opacity, GSR_MODE_FILTER3D needs the forward's filter3d.
@@ -692,14 +667,10 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
                                                      int64_t mode, c10::optional<torch::Tensor> filter3d) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     const int64_t N = xyz.size(0);
-    const bool rows = slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS && N > 0;  // interleaved [N,12] (else planar [9N])
-    TORCH_CHECK(rows || slab.numel() == N * 9, "gradient slab must hold 9 (planar) or 12 (rows) floats per gaussian");
+    TORCH_CHECK(slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ", GSR_GRAD_ROW_FLOATS,
+                " floats per gaussian");
     c10::cuda::CUDAGuard guard(xyz.device());
     auto opt = xyz.options();
-    const float* g_rgb = slab.data_ptr<float>();
-    const float* g_opa = g_rgb + (size_t)N * 3;
-    const float* g_uv = use_slab_uv ? g_opa + (size_t)N : nullptr;
-    const float* g_conic = g_opa + (size_t)N * 3;
     const int n_rest = sh_rest.has_value() ? (int)sh_rest->size(2) : 0;
     const float* g_uv_compact = nullptr;
     const uint64_t* scan_ptr = nullptr;
@@ -741,8 +712,7 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
     check_rc(gsr_preprocess_backward((int)mode, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
                                      F32PTR(opacity_logit), f3d, F32PTR(camera_T_world), F32PTR(K),
                                      camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
-                                     visible.data_ptr<uint8_t>(), g_rgb, g_opa, g_uv, g_conic,
-                                     rows ? slab.data_ptr<float>() : nullptr, use_slab_uv ? 1 : 0, g_uv_compact,
+                                     visible.data_ptr<uint8_t>(), slab.data_ptr<float>(), use_slab_uv ? 1 : 0, g_uv_compact,
                                      scan_ptr, F32PTR(o_xyz),
                                      F32PTR(o_q), F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc),
                                      n_rest ? F32PTR(g_sh) : nullptr, cur_stream()),
@@ -1024,7 +994,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("camera_centre"), py::arg("H"), py::arg("W"), py::arg("near_thresh"), py::arg("far_thresh"),
           py::arg("cull_mask_padding"), py::arg("mh_dist"), py::arg("depth_base"), py::arg("with_tiles") = false,
           py::arg("mode") = 0, py::arg("filter3d") = py::none());
-    m.def("fused_bin", &fused_bin, "pair emission + radix sort + tile ranges + record stream");
+    m.def("fused_bin", &fused_bin, "pair emission + radix sort + tile ranges");
     m.def("fused_render_forward", &fused_render_forward,
           "tile renderer forward (with depth_key: also the depth and alpha maps)");
     m.def("fused_render_backward", &fused_render_backward,
@@ -1032,7 +1002,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "mode: MODE_* bits, MODE_ABSGRAD: rows incl. the absolute uv gradients)",
           py::arg("grad_image"), py::arg("N"), py::arg("P"), py::arg("records"), py::arg("ids_sorted"),
           py::arg("ranges"), py::arg("background"), py::arg("n"), py::arg("w"), py::arg("masks"),
-          py::arg("keys_sorted"), py::arg("id_bits"), py::arg("gather"), py::arg("grad_depth"), py::arg("grad_alpha"),
+          py::arg("keys_sorted"), py::arg("id_bits"), py::arg("grad_depth"), py::arg("grad_alpha"),
           py::arg("depth_key"), py::arg("depth_base"), py::arg("depth_bits"), py::arg("mode") = 0);
     m.def("fused_preprocess_backward", &fused_preprocess_backward,
           "fused per-gaussian backward (mode: MODE_* bits; filter3d: the forward's, with MODE_FILTER3D)",

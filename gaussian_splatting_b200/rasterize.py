@@ -8,15 +8,14 @@ densification (splat_py/trainer.py:360,379-385).
 Implementation: two autograd nodes around the native fused kernels
 
     _ProjectGaussians   params -> uv [M,2], carrier          (gsr_preprocess_forward + binning)
-    _CompositeTiles     uv, carrier -> image                  (gsr_render_forward)
+    _CompositeTiles     uv, carrier -> image                  (gsr_render_forward_gather)
 
 (The tile renderer's forward kernel is enqueued by the projection node, right behind the binning and BEFORE the
 host reads the pair count; `_CompositeTiles` only ties its image into the graph.)
 
-``carrier`` is an uninitialised [12N] tensor ([9N] with the record stream) that only carries gradient: the
-render backward returns its per-Gaussian sums as the carrier's gradient — interleaved rows
-``rgb3 opacity | uv2 conic0 conic1 | conic2 pad3`` (planar rgb | opacity | uv | conic with the record stream) — and
-the per-Gaussian backward consumes them.  One host read per forward (the pair count, which sizes the pair
+``carrier`` is an uninitialised [12N] tensor that only carries gradient: the render backward returns its
+per-Gaussian sums as the carrier's gradient — interleaved rows ``rgb3 opacity | uv2 conic0 conic1 | conic2 pad3`` —
+and the per-Gaussian backward consumes them.  One host read per forward (the pair count, which sizes the pair
 buffers) and it is taken off the critical path: the buffers are sized from the previous views' counts and the
 count is only checked afterwards (DESIGN.md 3.5); the reference path has ~25 syncs.
 
@@ -55,10 +54,6 @@ IN_KERNEL_TRANSFORM = os.environ.get("GSR_TORCH_TRANSFORM", "0") != "1"
 # the forward records which (8x4 pixel block, splat) pairs contributed; the backward then visits exactly those
 # (GSR_NO_MASKS=1: the backward redoes the forward's conservative footprint test instead)
 USE_CONTRIBUTION_MASKS = os.environ.get("GSR_NO_MASKS", "0") != "1"
-# the tile kernels fetch their records through the sorted pair list themselves (cp.async gather, DESIGN.md 3.6); with
-# GSR_RECORD_STREAM=1 a separate kernel first writes the depth-sorted, tile-contiguous record stream they then read
-# with bulk copies (the round-1 arrangement)
-USE_RECORD_GATHER = os.environ.get("GSR_RECORD_STREAM", "0") != "1"
 # pair emission expands the tile-hit masks of the per-gaussian stage (GSR_RETEST_TILES=1: repeats the OBB tests)
 USE_TILE_MASKS = os.environ.get("GSR_RETEST_TILES", "0") != "1"
 IN_KERNEL_TRANSFORM_MIN_N = 16384
@@ -242,20 +237,26 @@ def _depth_key_params(near, far):
 class _ViewState:
     """Non-differentiable per-view buffers shared by the two autograd nodes."""
 
-    __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges", "stream_rec", "gather",
-                 "records", "keys_sorted", "id_bits", "slab_width",
+    __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges",
+                 "records", "keys_sorted", "id_bits",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
                  "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad", "filter3d")
 
     @property
     def ids_sorted(self):
         """int32 [P]: gaussian id of every sorted (gaussian, tile) pair (the reference's
-        `sorted_gaussian_idx_by_splat_idx`).  When the id rides in the sort key and the tile kernels gather through
-        the keys, nobody writes this array: it is extracted on demand."""
+        `sorted_gaussian_idx_by_splat_idx`).  When the id rides in the sort key the tile kernels read it from the
+        keys and nobody writes this array: it is extracted on demand."""
         if self._ids_sorted is not None and self._ids_sorted.numel() == 0 and self.P > 0 and self.keys_sorted is not None:
             mask = (1 << self.id_bits) - 1
             self._ids_sorted = (self.keys_sorted[:self.P] & mask).to(torch.int32)
         return self._ids_sorted
+
+    @property
+    def gather(self):
+        """Always True: the tile kernels read every record through the sorted pair list (there is no other record
+        source any more; kept readable for callers of return_state that check it)."""
+        return True
 
     def __init__(self, profile=None):
         self.profile = profile  # optional list: (stage name, start event, end event) per native call
@@ -338,19 +339,15 @@ class _ProjectGaussians(torch.autograd.Function):
                                    "the int32 pair index of the native path (P must be < 2^31)")
             return M_, P_
 
-        # depth / alpha maps are rendered by the gather kernels only (they read z off the sorted pair keys); the
-        # anti-aliased backward reads the interleaved gradient rows only the gather kernels write
-        gather = USE_RECORD_GATHER or state.mode != 0
         depth_keys = zkey if state.mode & ext.MODE_DEPTH_ALPHA else None
 
         def bin_and_render(M_, P_, speculative):
             with _stage(state, "bin_sort_gather"):
-                binned = ext.fused_bin(records, zkey, visible, scan, M_, P_, H, W, mh, depth_bits, speculative, gather,
+                binned = ext.fused_bin(records, zkey, visible, scan, M_, P_, H, W, mh, depth_bits, speculative,
                                        tile_mask if USE_TILE_MASKS else None, tile_win if USE_TILE_MASKS else None)
             with _stage(state, "render_fwd"):
-                rendered = ext.fused_render_forward(records if gather else binned[2], binned[1], background, H, W, P_,
-                                                    record_masks, binned[5], binned[0], binned[6], gather, depth_keys,
-                                                    depth_base, depth_bits)
+                rendered = ext.fused_render_forward(records, binned[1], background, H, W, P_, record_masks, binned[4],
+                                                    binned[0], binned[5], depth_keys, depth_base, depth_bits)
             return binned, rendered
 
         # The host needs M and P (the shape of the returned uv; the size of the pair buffers).  Reading them right
@@ -385,22 +382,21 @@ class _ProjectGaussians(torch.autograd.Function):
                 binned, rendered = bin_and_render(M, P, False)
                 state.speculation_overflowed = True
             else:
-                ids_c, ranges_c, stream_c, vis_c, uv_c, keys_c, idb = binned
-                binned = (ids_c.narrow(0, 0, P) if ids_c.numel() else ids_c, ranges_c, stream_c, vis_c.narrow(0, 0, M),
+                ids_c, ranges_c, vis_c, uv_c, keys_c, idb = binned
+                binned = (ids_c.narrow(0, 0, P) if ids_c.numel() else ids_c, ranges_c, vis_c.narrow(0, 0, M),
                           uv_c.narrow(0, 0, M), keys_c, idb)
         _note_pairs(key, P)
-        ids_sorted, ranges, stream_rec, vis_idx, uv, keys_sorted, id_bits = binned
-        state.gather, state.records, state.keys_sorted, state.id_bits = gather, records, keys_sorted, int(id_bits)
+        ids_sorted, ranges, vis_idx, uv, keys_sorted, id_bits = binned
+        state.records, state.keys_sorted, state.id_bits = records, keys_sorted, int(id_bits)
         state.image, state.n_per_pixel, state.w_per_pixel, state.masks, state.depth, state.alpha = rendered
         state.zkey, state.depth_base, state.depth_bits = depth_keys, depth_base, depth_bits
         state.N, state.M, state.P, state.H, state.W = xyz.shape[0], M, P, H, W
         state.visible = visible
         state.vis_idx = state.vis_idx32 = vis_idx                # int32 [M]: visible gaussians, ascending
-        state._ids_sorted, state.ranges, state.stream_rec = ids_sorted, ranges, stream_rec
+        state._ids_sorted, state.ranges = ids_sorted, ranges
         state.scan = scan
-        # gradient slab rows: 12 floats per gaussian (interleaved, gather mode) or 9 (planar, record-stream mode)
-        state.slab_width = 12 if gather else 9
-        carrier = torch.empty(state.slab_width * xyz.shape[0], dtype=xyz.dtype, device=xyz.device)
+        # gradient slab: one interleaved row of 12 floats per gaussian
+        carrier = torch.empty(12 * xyz.shape[0], dtype=xyz.dtype, device=xyz.device)
         ctx.state = state
         ctx.has_sh = sh is not None
         ctx.save_for_backward(xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre)
@@ -412,7 +408,7 @@ class _ProjectGaussians(torch.autograd.Function):
         st = ctx.state
         N = st.N
         if grad_carrier is None:
-            grad_carrier = torch.zeros(st.slab_width * N, dtype=xyz.dtype, device=xyz.device)
+            grad_carrier = torch.zeros(12 * N, dtype=xyz.dtype, device=xyz.device)
         slab = grad_carrier.contiguous()
         # Gradient on the projected means: the render backward's sums sit in the slab's uv section (by gaussian).
         # What autograd hands us for the COMPACT uv is either nothing / only what the caller added upstream of uv
@@ -450,9 +446,9 @@ class _CompositeTiles(torch.autograd.Function):
         st = ctx.state
         with _stage(st, "render_bwd"):
             slab = native().fused_render_backward(
-                grad_image.contiguous(), st.N, st.P, st.records if st.gather else st.stream_rec, st._ids_sorted,
-                st.ranges, st.background, st.n_per_pixel, st.w_per_pixel, st.masks, st.keys_sorted, st.id_bits,
-                st.gather, None if grad_depth is None else grad_depth.contiguous(),
+                grad_image.contiguous(), st.N, st.P, st.records, st._ids_sorted, st.ranges, st.background,
+                st.n_per_pixel, st.w_per_pixel, st.masks, st.keys_sorted, st.id_bits,
+                None if grad_depth is None else grad_depth.contiguous(),
                 None if grad_alpha is None else grad_alpha.contiguous(), st.zkey, st.depth_base, st.depth_bits,
                 st.mode)
         uv_t = st.uv_ref() if st.uv_ref is not None else None
@@ -471,11 +467,8 @@ class _CompositeTiles(torch.autograd.Function):
         st.uv_grad_emitted = bool(watched)
         if not watched:
             return None, slab, None, None
-        N = st.N
-        if st.slab_width == 12:   # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3 (depth mode: z pad2)
-            grad_uv = slab.view(N, 12).index_select(0, st.vis_idx)[:, 4:6].contiguous()
-        else:                     # planar: rgb [N,3] | opacity [N] | uv [N,2] | conic [N,3]
-            grad_uv = slab[4 * N:6 * N].view(N, 2).index_select(0, st.vis_idx)
+        # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3 (depth mode: z pad2)
+        grad_uv = slab.view(st.N, 12).index_select(0, st.vis_idx)[:, 4:6].contiguous()
         return grad_uv, slab, None, None
 
 
@@ -486,7 +479,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
     colour, z_i the camera-frame z, with no background term (expected depth: depth / alpha.clamp_min(eps)).  fp32
-    and precomputed SH colours only; always on the fused gather kernels.
+    and precomputed SH colours only.
 
     antialiased=True: every splat's opacity is multiplied by rho = sqrt(max(det S, 0) / det(S + 0.25 I)), S its 2-D
     covariance, so that the 0.25 px^2 dilation the renderer applies no longer adds mass to splats smaller than a pixel

@@ -129,15 +129,16 @@ int gsr_binning_emit_sort(int N, int P, const float* uvs, const float* xyz_camer
  * render_tiles_cuda / render_tiles_backward_cuda — src/bindings.cpp:3-33,
  * src/render.cu:191-422, src/render_backward.cu:287-595.
  *
- * The kernels consume a depth-sorted, tile-contiguous stream of 48-byte splat
- * records (GSR_REC_FLOATS floats per pair) that is staged into shared memory
- * by TMA bulk copies.  gsr_pack_records builds that stream from the
- * reference's per-Gaussian arrays.
+ * The kernels read one 48-byte splat record per Gaussian (GSR_REC_FLOATS
+ * floats) through the depth-sorted pair list of every tile.
+ * gsr_preprocess_forward writes these records; gsr_pack_gaussian_records builds them
+ * from the reference's per-Gaussian arrays.
  * ---------------------------------------------------------------------- */
-/* uvs [N,2], opacity [N] (post-sigmoid), rgb [N,3], conic [N,3], sorted idx [P] -> records [P,12] */
-int gsr_pack_records(int P, const int32_t* sorted_gaussian_idx, const float* uvs,
-                     const float* opacity, const float* rgb, const float* conic, float* records,
-                     void* stream);
+/* uvs [N,2], opacity [N] (post-sigmoid), rgb [N,3], conic [N,3] -> records [N,12], row i from Gaussian i.
+ * (Earlier releases exported gsr_pack_records, which packed one record per sorted pair; the new name makes a caller
+ * built against that argument list fail to resolve instead of passing its pointers into the wrong slots.) */
+int gsr_pack_gaussian_records(int N, const float* uvs, const float* opacity, const float* rgb, const float* conic,
+                              float* records, void* stream);
 
 /* Number of 32-bit words of the forward -> backward contribution masks for P (gaussian, tile) pairs on an H x W
  * image: per (tile, 128-record batch, warp, lane group) one 128-bit mask whose bit j is set when record j of the
@@ -145,31 +146,19 @@ int gsr_pack_records(int P, const int32_t* sorted_gaussian_idx, const float* uvs
  * same build. */
 size_t gsr_contribution_mask_words(int64_t P, int H, int W);
 
-/* records [P,12], tile_ranges [n_tiles+1], background [3] ->
+/* The tile renderers.  They fetch each batch's records themselves from the per-gaussian record array
+ * gaussian_records [N,12] through the sorted pair list — keys_sorted (gaussian id in the low id_bits of every key,
+ * gsr_sort_keys' output) or ids_sorted (gsr_sort_pairs' id output, or the reference's sorted_gaussian_idx); exactly
+ * one of the two is non-NULL.  3 x 16-byte cp.async per record, issued by the warp that recycles a pipeline stage,
+ * completion on the stage's mbarrier.  Gradients are indexed by gaussian id.
+ *
+ * Forward: tile_ranges [n_tiles+1], background [3] ->
  * image [H,W,3], num_splats_per_pixel int32 [H,W], final_weight_per_pixel [H,W].
  * contribution_masks: NULL, or gsr_contribution_mask_words(P, H, W) ZERO-FILLED words the kernel records the
- * contributing (pixel block, record) pairs in, for gsr_render_backward of the same view. */
-int gsr_render_forward(const float* records, const int32_t* tile_ranges, const float* background_rgb,
-                       int H, int W, int32_t* num_splats_per_pixel, float* final_weight_per_pixel,
-                       float* image, uint32_t* contribution_masks, void* stream);
-
-/* + grad_image [H,W,3]; accumulates into grad_rgb [N,3], grad_opacity [N], grad_uv [N,2],
- * grad_conic [N,3] at row sorted_gaussian_idx[p].
- * contribution_masks: NULL (the kernel finds the candidate records of every pixel block with its own
- * conservative footprint test, like the forward), or the masks the forward of this view recorded: the backward
- * then visits exactly the (pixel block, record) pairs that contributed. */
-int gsr_render_backward(const float* records, const int32_t* sorted_gaussian_idx,
-                        const int32_t* tile_ranges, const float* background_rgb, int H, int W,
-                        const int32_t* num_splats_per_pixel, const float* final_weight_per_pixel,
-                        const float* grad_image, float* grad_rgb, float* grad_opacity,
-                        float* grad_uv, float* grad_conic, const uint32_t* contribution_masks, void* stream);
-
-/* The same two kernels WITHOUT a record stream: the tile kernels fetch each batch's records themselves from the
- * per-gaussian record array gaussian_records [N,12] (gsr_preprocess_forward's output), through the sorted pair list
- * — keys_sorted (gaussian id in the low id_bits of every key, gsr_sort_keys' output) or ids_sorted (gsr_sort_pairs'
- * id output); exactly one of the two is non-NULL.  3 x 16-byte cp.async per record, issued by the warp that recycles
- * a pipeline stage, completion on the stage's mbarrier; gsr_gather_records* and the [P,12] stream are not needed.
- * Gradient rows are indexed by gaussian id.
+ * contributing (pixel block, record) pairs in, for gsr_render_backward_gather of the same view.  The backward takes
+ * NULL (the kernel finds the candidate records of every pixel block with its own conservative footprint test, like
+ * the forward), or the masks the forward of this view recorded: it then visits exactly the (pixel block, record)
+ * pairs that contributed.
  *
  * Depth and alpha maps from the same walk (precomputed colours), when depth and alpha are non-NULL (both or neither;
  * NULL: colour only, and depth_key / depth_base / depth_bits are not read).  Per pixel, over the splats the colour
@@ -186,10 +175,11 @@ int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* key
                               const int32_t* tile_ranges, const float* background_rgb, int H, int W,
                               int32_t* num_splats_per_pixel, float* final_weight_per_pixel, float* image, float* depth,
                               float* alpha, uint32_t* contribution_masks, void* stream);
-/* Gradient destination: the four planar arrays (grad_rows NULL), or grad_rows [N, GSR_GRAD_ROW_FLOATS] (16-byte
+/* + grad_image [H,W,3].  Gradient destination, accumulated into: the four planar arrays grad_rgb [N,3],
+ * grad_opacity [N], grad_uv [N,2], grad_conic [N,3] (grad_rows NULL), or grad_rows [N, GSR_GRAD_ROW_FLOATS] (16-byte
  * aligned, zero-filled; then the four planar pointers are ignored): one interleaved row per gaussian,
  * rgb3 opacity | uv2 conic0 conic1 | conic2 pad3, accumulated with 16-byte vector reductions — the nine sums of a pair
- * touch two adjacent 32-byte sectors instead of four arrays.  gsr_preprocess_backward reads either form.
+ * touch two adjacent 32-byte sectors instead of four arrays.  gsr_preprocess_backward reads the rows.
  * Depth/alpha mode: grad_depth and grad_alpha [H,W] non-NULL (both or neither; zeros where a map has no gradient),
  * the depth descriptor as in the forward, grad_rows required; the rows are then rgb3 opacity | uv2 conic0 conic1 |
  * conic2 z pad2, z being the gradient on the camera-frame z, which gsr_preprocess_backward consumes with
@@ -297,8 +287,8 @@ int gsr_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, con
  * capacity: 0 when keys / ids hold exactly P entries (the host has read P = scan[N-1] & 0xffffffff); otherwise the
  * number of entries of SPECULATIVELY sized buffers (the host has not synchronised yet): pairs beyond the capacity
  * are dropped (the caller finds P > capacity when it does read P, and redoes the binning), positions [P, capacity)
- * are filled with the all-ones key, which sorts behind every real pair; gsr_sort_*, gsr_tile_ranges and
- * gsr_gather_records* are then called with `capacity` in place of P and ignore the padding. */
+ * are filled with the all-ones key, which sorts behind every real pair; gsr_sort_* and gsr_tile_ranges are then
+ * called with `capacity` in place of P and ignore the padding. */
 int gsr_emit_pairs(int N, const float* records, const uint32_t* depth_key, const uint8_t* visible,
                    const uint64_t* scan, int n_tiles_x, int n_tiles_y, float mh_dist, int depth_bits,
                    uint64_t* keys, uint32_t* ids, int32_t* vis_idx, float* uv_compact, int64_t capacity,
@@ -312,13 +302,7 @@ int gsr_sort_pairs(int P, int n_tiles, int depth_bits, const uint64_t* keys_in, 
 int gsr_tile_ranges(int P, int n_tiles, int depth_bits, const uint64_t* keys_sorted, int32_t* tile_ranges,
                     void* stream);
 
-/* records_sorted[p] = records[ids_sorted[p]] (48-byte rows).  scan / ranks_sorted (both or neither): also
- * ranks_sorted[p] = (scan[ids_sorted[p]] >> 32) - 1, the gaussian's rank among the visible ones = its row in
- * compact per-gaussian gradient arrays (see gsr_preprocess_backward). */
-int gsr_gather_records(int P, const uint32_t* ids_sorted, const float* records, float* records_sorted,
-                       const uint64_t* scan, int32_t* ranks_sorted, void* stream);
-
-/* Keys-only variant of the four calls above: when tile bits + depth_bits + id bits fit in 64, the gaussian id
+/* Keys-only variant of the three calls above: when tile bits + depth_bits + id bits fit in 64, the gaussian id
  * rides in the low id_bits of the key — (tile | depth | id) — and ONE cub::DeviceRadixSort::SortKeys over bits
  * [id_bits, id_bits + depth_bits + tile bits) replaces SortPairs (8 instead of 12 bytes moved per pair and pass;
  * the id bits are not sorted: the sort is stable and pairs are emitted in gaussian order, so ties resolve as
@@ -332,18 +316,14 @@ int gsr_emit_keys(int N, const float* records, const uint32_t* depth_key, const 
 size_t gsr_sort_keys_temp_bytes(int P);
 int gsr_sort_keys(int P, int n_tiles, int depth_bits, int id_bits, const uint64_t* keys_in, uint64_t* keys_out,
                   void* temp, size_t temp_bytes, void* stream);
-/* ids_sorted[p] = the gaussian id of sorted pair p, or — scan != NULL — its rank among the visible gaussians */
-int gsr_gather_records_keys(int P, int id_bits, const uint64_t* keys_sorted, const float* records,
-                            float* records_sorted, int32_t* ids_sorted, const uint64_t* scan, void* stream);
 
-/* backward of the fused per-Gaussian stage.  grad_rgb [N,3] / grad_opacity [N] / grad_uv [N,2] / grad_conic [N,3]
- * are the per-gaussian sums the render backward accumulated (indexed by gaussian).  The gradient on a projected
- * mean is grad_uv[i] (skipped when grad_uv is NULL) PLUS grad_uv_compact[(scan[i] >> 32) - 1] (skipped when NULL):
- * grad_uv_compact [M,2] is a gradient on the compact uv rasterize returned, in its order (scan = the packed
- * inclusive scan of gsr_preprocess_forward) — what a caller added upstream of uv, or the total autograd hands over.
- * grad_rows != NULL: the interleaved rows of gsr_render_backward_gather instead of the four planar arrays
- * (grad_uv == NULL then still means "skip the render backward's uv sums").
- * mode: the GSR_MODE_* bits of the forward and the render backward; any bit requires grad_rows (16-byte aligned).
+/* backward of the fused per-Gaussian stage.  grad_rows [N, GSR_GRAD_ROW_FLOATS] (required, 16-byte aligned) are the
+ * per-gaussian sums gsr_render_backward_gather accumulated into interleaved rows (indexed by gaussian).  The gradient
+ * on a projected mean is the row's uv (skipped when use_rows_uv is 0) PLUS grad_uv_compact[(scan[i] >> 32) - 1]
+ * (skipped when NULL): grad_uv_compact [M,2] is a gradient on the compact uv rasterize returned, in its order
+ * (scan = the packed inclusive scan of gsr_preprocess_forward) — what a caller added upstream of uv, or the total
+ * autograd hands over.
+ * mode: the GSR_MODE_* bits of the forward and the render backward.
  *   GSR_MODE_ABSGRAD changes nothing here (the rows' slots 10-11 are not read).
  *   GSR_MODE_DEPTH_ALPHA: the rows of the depth/alpha render backward: row slot 9, the gradient on the camera-frame z,
  *   joins grad_xyz as camera_T_world[2, :3] * g_z.  No gradient goes to the pose.
@@ -357,9 +337,8 @@ int gsr_gather_records_keys(int P, int id_bits, const uint64_t* keys_sorted, con
 int gsr_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
                             const float* scale, const float* opacity_logit, const float* filter3d,
                             const float* camera_T_world,
-                            const float* K, const float* camera_centre, const uint8_t* visible, const float* grad_rgb,
-                            const float* grad_opacity, const float* grad_uv, const float* grad_conic,
-                            const float* grad_rows, int use_rows_uv,
+                            const float* K, const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                            int use_rows_uv,
                             const float* grad_uv_compact, const uint64_t* scan, float* g_xyz, float* g_quaternion,
                             float* g_scale, float* g_opacity_logit, float* g_rgb_dc, float* g_sh_rest, void* stream);
 

@@ -31,7 +31,7 @@ def declared_symbols():
 def test_header_declares_the_path():
     syms = declared_symbols()
     assert len(syms) >= 25
-    for must in ("gsr_preprocess_forward", "gsr_sort_pairs", "gsr_render_forward", "gsr_render_backward",
+    for must in ("gsr_preprocess_forward", "gsr_sort_pairs", "gsr_render_forward_gather", "gsr_render_backward_gather",
                  "gsr_preprocess_backward", "gsr_binning_emit_sort"):
         assert must in syms
 
@@ -52,10 +52,10 @@ def test_library_is_sm90a_only_and_has_tma():
     archs = set(re.findall(r"sm_(\d+a?)", elfs))
     assert archs == {"90a"}, archs
     names = subprocess.run(["cuobjdump", "-sass", str(so)], capture_output=True, text=True).stdout
-    fwd = re.findall(r"Function : (\S*k_render_fwdILb1ELb0\S*)", names)  # masks on, record stream by bulk copies
-    assert fwd, "k_render_fwd<true, false> not in the library"
+    fwd = re.findall(r"Function : (\S*16k_preprocess_fwdILi16ELb1\S*)", names)  # SH degree 3
+    assert fwd, "k_preprocess_fwd<16, true> not in the library"
     sass = subprocess.run(["cuobjdump", "-sass", "-fun", fwd[0], str(so)], capture_output=True, text=True).stdout
-    assert "UBLKCP" in sass, "render forward kernel should stage records with TMA bulk copies (UBLKCP)"
+    assert "UBLKCP" in sass, "per-gaussian forward kernel should stage through TMA bulk copies (UBLKCP)"
 
 
 def test_binding_exports_reference_surface():

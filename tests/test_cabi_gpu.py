@@ -1,7 +1,7 @@
 """The C ABI driven with RAW device pointers through ctypes — no torch types cross the boundary (torch is only the
 allocator here, any cudaMalloc'd memory would do).  What a cgo / JNI / ctypes host binding would call: the tile
-renderer forward + backward on a packed record stream, and the camera-centre kernel; checked against the torch
-binding of the same library (which the parity tests pin to the reference)."""
+renderer forward + backward on packed per-gaussian records read through a sorted id array, and the camera-centre
+kernel; checked against the torch binding of the same library (which the parity tests pin to the reference)."""
 import ctypes as C
 from pathlib import Path
 
@@ -39,7 +39,7 @@ def test_render_through_ctypes_matches_the_binding():
     bg = torch.full((3,), 0.5, device=dev)
     G = synth.make_upstream_grad("tiny", device=dev)
     # --- the C ABI, raw pointers
-    rec = torch.empty(max(P, 1), 12, device=dev)
+    rec = torch.empty(max(M, 1), 12, device=dev)
     n_px = torch.empty(H, W, dtype=torch.int32, device=dev)
     w_px, image = torch.empty(H, W, device=dev), torch.empty(H, W, 3, device=dev)
     stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -47,17 +47,23 @@ def test_render_through_ctypes_matches_the_binding():
     lib.gsr_contribution_mask_words.argtypes = [C.c_int64, C.c_int, C.c_int]
     words = lib.gsr_contribution_mask_words(P, H, W)
     masks = torch.zeros(words, dtype=torch.int32, device=dev)
-    assert lib.gsr_pack_records(C.c_int(P), ptr(s.sorted_idx), ptr(uv), ptr(opa), ptr(rgb), ptr(conic), ptr(rec), stream) == 0
-    assert lib.gsr_render_forward(ptr(rec), ptr(s.tile_ranges), ptr(bg), C.c_int(H), C.c_int(W), ptr(n_px), ptr(w_px),
-                                  ptr(image), ptr(masks), stream) == 0
+    assert lib.gsr_pack_gaussian_records(C.c_int(M), ptr(uv), ptr(opa), ptr(rgb), ptr(conic), ptr(rec), stream) == 0
+    # pair list as a sorted id array (no keys, id_bits 0), no depth / alpha maps
+    ids = (None, C.c_int(0), ptr(s.sorted_idx), None, C.c_uint32(0), C.c_int(0))
+    assert lib.gsr_render_forward_gather(ptr(rec), *ids, ptr(s.tile_ranges), ptr(bg), C.c_int(H), C.c_int(W),
+                                         ptr(n_px), ptr(w_px), ptr(image), None, None, ptr(masks), stream) == 0
     grads = [torch.zeros(M, 3, device=dev), torch.zeros(M, device=dev), torch.zeros(M, 2, device=dev),
              torch.zeros(M, 3, device=dev)]
-    assert lib.gsr_render_backward(ptr(rec), ptr(s.sorted_idx), ptr(s.tile_ranges), ptr(bg), C.c_int(H), C.c_int(W),
-                                   ptr(n_px), ptr(w_px), ptr(G), *[ptr(t) for t in grads], ptr(masks), stream) == 0
+
+    def backward(out, m):  # planar gradient arrays (grad_rows NULL)
+        return lib.gsr_render_backward_gather(C.c_int(0), ptr(rec), *ids, ptr(s.tile_ranges), ptr(bg), C.c_int(H),
+                                              C.c_int(W), ptr(n_px), ptr(w_px), ptr(G), None, None,
+                                              *[ptr(t) for t in out], None, m, stream)
+
+    assert backward(grads, ptr(masks)) == 0
     # the same without the forward's masks (NULL): the backward finds its candidates itself
     grads0 = [torch.zeros_like(t) for t in grads]
-    assert lib.gsr_render_backward(ptr(rec), ptr(s.sorted_idx), ptr(s.tile_ranges), ptr(bg), C.c_int(H), C.c_int(W),
-                                   ptr(n_px), ptr(w_px), ptr(G), *[ptr(t) for t in grads0], None, stream) == 0
+    assert backward(grads0, None) == 0
     # --- the torch binding (reference surface)
     ext = gsb.native()
     n2, w2, image2 = torch.zeros_like(n_px), torch.zeros_like(w_px), torch.zeros_like(image)
@@ -73,8 +79,8 @@ def test_render_through_ctypes_matches_the_binding():
         assert float((a.reshape(-1) - b.reshape(-1)).abs().max()) <= 2e-5 * scale
         assert float((a0.reshape(-1) - b.reshape(-1)).abs().max()) <= 2e-5 * scale
     # bad arguments come back as status codes, not exceptions or crashes
-    assert lib.gsr_render_forward(ptr(rec), ptr(s.tile_ranges), ptr(bg), C.c_int(0), C.c_int(W), ptr(n_px), ptr(w_px),
-                                  ptr(image), None, stream) != 0
+    assert lib.gsr_render_forward_gather(ptr(rec), *ids, ptr(s.tile_ranges), ptr(bg), C.c_int(0), C.c_int(W),
+                                         ptr(n_px), ptr(w_px), ptr(image), None, None, None, stream) != 0
 
 
 def test_camera_centre_through_ctypes():

@@ -59,7 +59,7 @@ def state_of(g, T, cam, depth_alpha=False, antialiased=False):
         out = rasterize(g, T, cam, 0.3, 500.0, 100, 3.0, True, bg, return_state=True, render_depth_alpha=depth_alpha,
                         antialiased=antialiased)
     st = out[-1]
-    assert st.gather and st.P > 0
+    assert st.P > 0
     return st
 
 

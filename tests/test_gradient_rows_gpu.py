@@ -95,11 +95,8 @@ def flip_pixels(bad_image, w_gpu, o, G):
 
 
 def split_slab(slab, N):
-    if slab.numel() == 12 * N:   # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3
-        v = slab.view(N, 12)
-        return dict(rgb=v[:, 0:3], opacity=v[:, 3], uv=v[:, 4:6], conic=v[:, 6:9])
-    return dict(rgb=slab[:3 * N].view(N, 3), opacity=slab[3 * N:4 * N], uv=slab[4 * N:6 * N].view(N, 2),
-                conic=slab[6 * N:9 * N].view(N, 3))
+    v = slab.view(N, 12)   # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3
+    return dict(rgb=v[:, 0:3], opacity=v[:, 3], uv=v[:, 4:6], conic=v[:, 6:9])
 
 
 def render_results(tag, mine, d, keep, eps, allowed):
@@ -112,12 +109,12 @@ def param_results(tag, g, pr, allowed):
             for k in PARAMS if getattr(g, k) is not None]
 
 
-def fused_vs_oracle(tag, sc, G=None, masks=True, gather=True, check=True, zero_block=None):
+def fused_vs_oracle(tag, sc, G=None, masks=True, check=True, zero_block=None):
     """Fused forward + backward; returns (results, oracle forward, state).  zero_block: (rows, cols) slices where
     the GPU's upstream gradient is zeroed but the oracle's is not (a negative control)."""
     o = oracle_forward(sc)
     G = upstream(sc) if G is None else G
-    R.USE_CONTRIBUTION_MASKS, R.USE_RECORD_GATHER = masks, gather
+    R.USE_CONTRIBUTION_MASKS = masks
     try:
         g = gaussians_from(sc)
         cam = Camera(sc["W"], sc["H"], to_t(sc["K"]))
@@ -133,8 +130,8 @@ def fused_vs_oracle(tag, sc, G=None, masks=True, gather=True, check=True, zero_b
         proj.register_prehook(lambda grad_outputs: seen.append(grad_outputs[1].detach().clone()))
         image.backward(to_t(G_gpu))
     finally:
-        R.USE_CONTRIBUTION_MASKS, R.USE_RECORD_GATHER = True, True
-    assert len(seen) == 1 and st.gather == gather and (st.masks.numel() > 0) == masks
+        R.USE_CONTRIBUTION_MASKS = True
+    assert len(seen) == 1 and (st.masks.numel() > 0) == masks
     slab = {k: v.double().cpu().numpy() for k, v in split_slab(seen[0], st.N).items()}
     d = orc.rasterize_backward(o, G)
     M = int(o.keep.sum())
@@ -201,12 +198,13 @@ def test_fused_720p_100k():
     assert int(o.keep.sum()) > 50_000
 
 
-@pytest.mark.parametrize("masks,gather", [(True, True), (False, True), (True, False), (False, False)])
-def test_fused_deep_tile_variants(masks, gather):
+@pytest.mark.parametrize("masks", [True, False])
+@pytest.mark.parametrize("shd", [0, 3])
+def test_fused_deep_tile_variants(masks, shd):
     """Walks of more than 960 splats over several 128-record batches, with contribution-mask bits in all four
-    words of a batch; every backward variant (masks on / off, record gather / stream) against the oracle."""
-    sc = stack(3000, -5.0)
-    _, o, st = fused_vs_oracle(f"deep masks={masks} gather={gather}", sc, masks=masks, gather=gather)
+    words of a batch; both backward variants (masks on / off) against the oracle, with plain and SH colours."""
+    sc = stack(3000, -5.0, shd=shd)
+    _, o, st = fused_vs_oracle(f"deep masks={masks} sh{shd}", sc, masks=masks)
     assert int(o.n.max()) > 960 and int(np.diff(o.ranges).max()) > 4 * 128
     if masks:
         words = st.masks.view(-1, 4)

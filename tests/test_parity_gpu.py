@@ -402,36 +402,15 @@ def test_tile_hit_masks_and_retested_tiles_give_the_same_lists(sigma):
     assert_bits_equal(out[True][0], out[False][0], "image")
 
 
-def test_record_gather_and_record_stream_agree():
-    """Default: the tile kernels gather their records through the sorted keys with cp.async.  GSR_RECORD_STREAM=1:
-    a separate kernel writes the tile-contiguous record stream they read with bulk copies.  Same records either way,
-    so the same bits in the forward; gradients to atomics noise.  Also the id-array form of the gather (when the
-    gaussian id does not fit the sort key)."""
-    from gaussian_splatting_b200 import rasterize as R
-
-    sc = scenes.np_scene(70_000, "720p", sh_degree=1, seed=8, view=0, n_views=3)
-    G = synth.make_upstream_grad("720p").numpy()
-    assert R.USE_RECORD_GATHER
-    gathered = run_b200(sc, G=G)
-    R.USE_RECORD_GATHER = False
-    try:
-        streamed = run_b200(sc, G=G)
-    finally:
-        R.USE_RECORD_GATHER = True
-    assert_bits_equal(gathered["image"], streamed["image"], "image")
-    assert_bits_equal(gathered["uv"], streamed["uv"], "uv")
-    for k in ("g_xyz", "g_rgb", "g_opacity", "g_scale", "g_quaternion", "g_sh", "g_uv"):
-        assert rel(gathered[k], streamed[k]) < 2e-5, (k, rel(gathered[k], streamed[k]))
-    # far plane at infinity -> full 32-bit depth keys; 4k -> 15 tile bits: 17 bits are left for the id, so 200 000
-    # gaussians do not fit and the sort carries a separate id array (the key/value fallback)
+def test_key_value_fallback_matches_unfused():
+    """The id-array form of the pair list: far plane at infinity -> full 32-bit depth keys; 4k -> 15 tile bits: 17 bits
+    are left for the id, so 200 000 gaussians do not fit and the sort carries a separate id array (the key/value
+    fallback), which the tile kernels read the gaussian ids from.  Same bits in the forward as the operator-by-operator
+    path; gradients to atomics noise."""
     big = scenes.np_scene(200_000, "4k", sh_degree=0, seed=9, view=0, n_views=1)
     G4 = synth.make_upstream_grad("4k").numpy()
     a = run_b200(big, G=G4, far=float("inf"))
-    R.USE_RECORD_GATHER = False
-    try:
-        b = run_b200(big, G=G4, far=float("inf"))
-    finally:
-        R.USE_RECORD_GATHER = True
+    b = run_b200(big, fn=rasterize_unfused, G=G4, far=float("inf"))
     assert_bits_equal(a["image"], b["image"], "image (full-range depth keys)")
     assert rel(a["g_xyz"], b["g_xyz"]) < 2e-5
 

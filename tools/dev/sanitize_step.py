@@ -1,6 +1,6 @@
-"""Workload for compute-sanitizer: three fwd+bwd steps of the fused path on a small scene — the first reads the pair
+"""Workload for compute-sanitizer: four fwd+bwd steps of the fused path on a small scene — the first reads the pair
 count eagerly, the others take the speculative path (padded pair buffers); contribution masks, in-kernel record
-gather (cp.async on the stage barriers), tile-hit masks all on, plus one step of the record-stream form.
+gather (cp.async on the stage barriers), tile-hit masks all on.
 
     compute-sanitizer --tool memcheck  python tools/dev/sanitize_step.py 30000 small
     compute-sanitizer --tool racecheck --racecheck-report analysis python tools/dev/sanitize_step.py 12000 small
@@ -21,8 +21,6 @@ cam = synth.make_camera(res, device=dev)
 G = synth.make_upstream_grad(res, device=dev)
 bg = torch.full((3,), 0.5, device=dev)
 for i in range(4):
-    if i == 3:
-        R.USE_RECORD_GATHER = False
     for p in (g.xyz, g.rgb, g.opacity, g.scale, g.quaternion, g.sh):
         p.grad = None
     T = synth.make_pose(i % 3, 3, device=dev)

@@ -1,6 +1,6 @@
 """Instruction counts of the loops of a kernel in an object file (cuobjdump -sass):
     python tools/dev/sass_loops.py gaussian_splatting_b200/_build/gsr_render.o k_render_bwdILb1
-    python tools/dev/sass_loops.py --inner gaussian_splatting_b200/_build/gsr_render.o k_render_bwdILb1ELb1E
+    python tools/dev/sass_loops.py --inner gaussian_splatting_b200/_build/gsr_render.o k_render_bwdILb1EE
 Default: every backward branch (loop) with its body length and an opcode histogram of the largest loops.
 --inner: the innermost loops instead (the tile walks), in address order.  A compare-and-swap retry loop (how sm_90
 compiles a shared-memory float atomicAdd) does not make the loop around it an outer loop; it is counted as a

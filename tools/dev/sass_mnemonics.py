@@ -10,7 +10,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[2]
 LIB = ROOT / "gaussian_splatting_b200" / "libgsr_b200.so"
-KEEP = ("k_render_fwdILb1ELb1", "k_render_bwdILb1ELb1", "k_render_fwdILb1ELb0", "k_render_bwdILb1ELb0",
+KEEP = ("12k_render_fwdILb1EE", "12k_render_bwdILb1EE", "12k_render_fwdILb0EE", "12k_render_bwdILb0EE",
         "k_preprocess_fwdILi16ELb1", "k_preprocess_bwdILi16ELb1", "k_emit_pairs_fused", "k_tile_ranges",
         "k_camera_centre", "k_adamILb0", "k_adamILb1", "k_densify_apply", "k_densify_accumulate")
 SHOW = ("FFMA", "FMUL", "FADD", "UBLKCP", "LDGSTS", "SYNCS", "ARRIVES", "REDG.F32x4", "REDG", "ATOMG", "ATOMS", "BAR",
@@ -34,8 +34,7 @@ for line in text.splitlines():
 
 print("cuobjdump -sass gaussian_splatting_b200/libgsr_b200.so — static instruction counts of the kernels on the measured path")
 print("(UBLKCP = cp.async.bulk 1-D TMA copy, LDGSTS = cp.async, SYNCS / ARRIVES = mbarrier,")
-print(" REDG.F32x4 = red.global.add.v4.f32; ILb1ELb1 = contribution masks + in-kernel record gather (the default),")
-print(" ILb1ELb0 = contribution masks + record stream)\n")
+print(" REDG.F32x4 = red.global.add.v4.f32; ILb1EE = with contribution masks, ILb0EE = without)\n")
 for name, c in counts.items():
     if not any(k in name for k in KEEP):
         continue
