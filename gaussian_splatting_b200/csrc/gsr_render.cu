@@ -372,6 +372,66 @@ __device__ __forceinline__ void sts_u8(uint32_t addr, uint32_t v) {
     asm volatile("st.shared.u8 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
 }
 
+// Blend-weight statistics (GSR weight_stats, DESIGN.md 3.14): per gaussian, over the pixels it contributes to,
+// sum w, max w and the number of such pixels, w the weight of the colour blend.  Destinations are per-gaussian rows
+// accumulated into; pair_total / capacity guard the speculatively sized pair buffers: when the scan's pair count
+// (low 32 bits of *pair_total) exceeds the capacity the kernel ran with, its output is discarded by the host and
+// nothing is added.
+struct WeightSink {
+    float* sum;
+    uint32_t* max;              // float bits; w >= +0 so the unsigned order is the float order
+    uint32_t* count;
+    const uint64_t* pair_total; // NULL: no guard
+    uint32_t capacity;
+};
+// Per-stage shared accumulator WeightAcc: [sum (f32 bits) | max | count] x BATCH words, indexed by staged record.
+constexpr int WACC_WORDS = 3 * BATCH;
+
+// One walk step: the lane group's 16 pixels reduced (xor shuffles within the group, ballots for the count), one
+// lane per group adds into the record's accumulator.  The sum goes through a shared fp32 atomicAdd (a CAS loop on
+// sm_90); it is issued only by groups where record j contributed.
+__device__ __forceinline__ void weight_stats_step(uint32_t* __restrict__ wacc, int j, F2 w, bool c0, bool c1,
+                                                  int lane) {
+    float s = lo(w) + hi(w);
+    uint32_t m = max(__float_as_uint(lo(w)), __float_as_uint(hi(w)));
+#pragma unroll
+    for (int o = GROUP_LANES / 2; o > 0; o >>= 1) {
+        s += __shfl_xor_sync(0xffffffffu, s, o);
+        m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    }
+    const uint32_t gmask = ((1u << GROUP_LANES) - 1u) << (lane & ~(GROUP_LANES - 1));
+    const uint32_t n = __popc(__ballot_sync(0xffffffffu, c0) & gmask) + __popc(__ballot_sync(0xffffffffu, c1) & gmask);
+    if ((lane % GROUP_LANES) == 0 && n != 0u) {
+        atomicAdd(reinterpret_cast<float*>(wacc + j), s);
+        atomicMax(wacc + BATCH + j, m);
+        atomicAdd(wacc + 2 * BATCH + j, n);
+    }
+}
+
+// By the warp that checked the stage out last: every staged record with a non-zero count goes to HBM (three
+// reductions), and its accumulator is cleared for the stage's next batch.  The caller orders the clearing stores
+// before the stage is re-armed (__threadfence_block ahead of the refill's arrivals), as the backward does.
+__device__ __forceinline__ void weight_stats_flush(uint32_t* __restrict__ wacc, const RecSource& src, int p0, int cnt,
+                                                   const WeightSink& ws, int lane) {
+    const bool keep = ws.pair_total == nullptr || (uint32_t)__ldg(ws.pair_total) <= ws.capacity;
+#pragma unroll
+    for (int k = 0; k < BATCH / 32; ++k) {
+        const int r = k * 32 + lane;
+        if (r >= cnt) break;
+        const uint32_t n = wacc[2 * BATCH + r];
+        if (n == 0u) continue;
+        const float s = __uint_as_float(wacc[r]);
+        const uint32_t m = wacc[BATCH + r];
+        wacc[r] = wacc[BATCH + r] = wacc[2 * BATCH + r] = 0u;
+        if (keep) {
+            const uint32_t id = source_id(src, p0 + r);
+            atomicAdd(ws.sum + id, s);
+            atomicMax(ws.max + id, m);
+            atomicAdd(ws.count + id, n);
+        }
+    }
+}
+
 // MARK: the walk also records, per lane group, WHICH staged records contributed to at least one pixel of the group.
 // Inside the loop the marks are list positions in a register — a store inside the loop costs ptxas's register-pair
 // coalescing (+11 instructions per iteration, measured) — so the walk is split into runs of 32 positions and the
@@ -380,11 +440,12 @@ __device__ __forceinline__ void sts_u8(uint32_t addr, uint32_t v) {
 // entry); after the walk one ballot per 32 records turns the flags into the group's 128-bit record mask, stored to
 // gm_warp[group][word], and the flags are cleared again.
 // DEPTH: also D += w * z, z from the stage's z array zs (same weight w as the colour blend).
-template <bool CHECK, bool MARK, bool DEPTH = false>
+// STATS: also the blend-weight statistics of every walked record (WeightAcc: the stage's accumulator wacc).
+template <bool CHECK, bool MARK, bool DEPTH = false, bool STATS = false>
 __device__ __forceinline__ void fwd_walk(const float4* __restrict__ rec4, uint32_t list_addr, uint32_t dummy_addr,
                                          int my_cnt, int iters, int next_base, F2 fpx, float fpy, FwdState& st,
                                          uint32_t* __restrict__ gm_warp, uint32_t flag_addr, int lane,
-                                         const float* __restrict__ zs = nullptr) {
+                                         const float* __restrict__ zs = nullptr, uint32_t* __restrict__ wacc = nullptr) {
     const float neg_sat = -GSR_SAT_THRESH;
     int lj0 = -1, lj1 = -1;  // record (within this batch) of the last contribution
     for (int t0 = 0; t0 < iters; t0 += (MARK ? 32 : BATCH)) {
@@ -432,6 +493,7 @@ __device__ __forceinline__ void fwd_walk(const float4* __restrict__ rec4, uint32
         st.C1 = fma2(w, bc(q2.z), st.C1);
         st.C2 = fma2(w, bc(q2.w), st.C2);
         if (DEPTH) st.D = fma2(w, bc(zs[j]), st.D);
+        if (STATS) weight_stats_step(wacc, j, w, c0, c1, lane);
         lj0 = c0 ? j : lj0;
         lj1 = c1 ? j : lj1;
         if (MARK) {
@@ -544,19 +606,21 @@ __device__ __noinline__ ExactPixelDepth render_pixel_exact_warp_depth(const RecS
 // MARK: also record, per (batch, warp, lane group), which staged records contributed (contribution masks for
 // the backward; `masks` must be zero-filled by the caller: a warp that skips a batch leaves its masks untouched)
 // DEPTH: also the per-pixel depth D = sum w * z and alpha A (depth / alpha [H,W])
-template <bool MARK, bool DEPTH>
+// STATS: also the per-gaussian blend-weight statistics into ws (weight_stats_step / weight_stats_flush)
+template <bool MARK, bool DEPTH, bool STATS = false>
 __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* __restrict__ ranges,
                                            const float* __restrict__ background, int W, int H,
                                            int32_t* __restrict__ n_out, float* __restrict__ w_out,
                                            float* __restrict__ image, uint32_t* __restrict__ masks,
                                            const DepthSource& ds, float* __restrict__ depth,
-                                           float* __restrict__ alpha) {
+                                           float* __restrict__ alpha, const WeightSink& ws = WeightSink{}) {
     __shared__ __align__(128) float s_rec[STAGES][BATCH * REC];
     __shared__ __align__(8) uint64_t s_full[STAGES];
     __shared__ int s_cnt[STAGES];
     __shared__ __align__(16) uint8_t s_list[CTA_WARPS][LIST_BYTES];
     __shared__ __align__(16) uint8_t s_flag[CTA_WARPS][MARK ? FLAG_BYTES : 16];  // MARK: per-record flags (fwd_walk)
     __shared__ __align__(16) float s_z[STAGES][DEPTH ? BATCH : 1];              // DEPTH: z of the staged records
+    __shared__ __align__(16) uint32_t s_wacc[STAGES][STATS ? WACC_WORDS : 1];   // STATS: WeightAcc per stage
 
     const int tid = threadIdx.x;
     const int lane = tid & 31, warp = tid >> 5;
@@ -588,6 +652,8 @@ __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* _
         }
         fence_mbar_init();
     }
+    if (STATS)
+        for (int k = tid; k < STAGES * WACC_WORDS; k += CTA_THREADS) (&s_wacc[0][0])[k] = 0u;
     __syncthreads();
     // the WHOLE calling warp fetches the records of batch b (gather_batch)
     auto load_batch = [&](int b) {
@@ -625,22 +691,32 @@ __device__ __forceinline__ void render_fwd(const RecSource& rs, const int32_t* _
             const bool small = (live0 && lo(st.nA) > -0.015625f) || (live1 && hi(st.nA) > -0.015625f);
             if (__any_sync(0xffffffffu, small)) {
                 if (lane == 0) STAT(0, iters);
-                fwd_walk<true, MARK, DEPTH>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
-                                            MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane,
-                                            &s_z[s][0]);
+                fwd_walk<true, MARK, DEPTH, STATS>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy,
+                                                   st, MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr,
+                                                   lane, &s_z[s][0], &s_wacc[s][0]);
             } else {
                 if (lane == 0) STAT(1, iters);
-                fwd_walk<false, MARK, DEPTH>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx, fpy, st,
-                                             MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr, flag_addr, lane,
-                                             &s_z[s][0]);
+                fwd_walk<false, MARK, DEPTH, STATS>(rec4, list_addr, dummy_addr, my_cnt, iters, b * BATCH + 1, fpx,
+                                                    fpy, st, MARK ? gm + (size_t)b * MASK_WORDS_PER_SLOT : nullptr,
+                                                    flag_addr, lane, &s_z[s][0], &s_wacc[s][0]);
             }
             if (lane == 0) { STAT(5, cnts[0] + cnts[1]); STAT(6, 2 * cnt); }
 #ifdef GSR_STATS
             if (lane == 0) { int sum = 0; for (int g = 0; g < GROUPS; ++g) sum += cnts[g]; STAT(4, sum); STAT(7, 1); }
 #endif
         }
-        if (stage_checkout(&s_cnt[s], lane) && b + STAGES < nb)  // warp-uniform: this warp left the stage last
+        if (STATS) {
+            if (stage_checkout(&s_cnt[s], lane)) {  // warp-uniform: this warp left the stage last
+                weight_stats_flush(&s_wacc[s][0], rs, start + b * BATCH, min(BATCH, total - b * BATCH), ws, lane);
+                if (b + STAGES < nb) {
+                    __syncwarp();
+                    __threadfence_block();  // every lane: its share of the cleared accumulator before its arrival
+                    load_batch(b + STAGES);
+                }
+            }
+        } else if (stage_checkout(&s_cnt[s], lane) && b + STAGES < nb) {  // warp-uniform: this warp left the stage last
             load_batch(b + STAGES);
+        }
     }
 
     // pixels flagged by the walk: recompute them exactly, one at a time, with the whole warp
@@ -721,6 +797,34 @@ __global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_DEPTH_MINB)
                        float* __restrict__ w_out, float* __restrict__ image, float* __restrict__ depth,
                        float* __restrict__ alpha, uint32_t* __restrict__ masks) {
     render_fwd<MARK, true>(rs, ranges, background, W, H, n_out, w_out, image, masks, ds, depth, alpha);
+}
+
+// Blend-weight statistics (weight_stats): the two forward kernels above plus the per-gaussian sums / maxima / counts.
+// The group reduction keeps three more values live in the walk: at the default kernels' 9 / 8 CTAs per SM the masked
+// builds spill (8-byte frame, reloaded in the walk); one CTA less (64 / 72 registers) keeps every build out of local
+// memory
+#ifndef GSR_FWD_STATS_MINB
+#define GSR_FWD_STATS_MINB 8
+#endif
+#ifndef GSR_FWD_DEPTH_STATS_MINB
+#define GSR_FWD_DEPTH_STATS_MINB 7
+#endif
+template <bool MARK>
+__global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_STATS_MINB)
+    k_render_fwd_stats(const RecSource rs, const int32_t* __restrict__ ranges,
+                       const float* __restrict__ background, int W, int H, int32_t* __restrict__ n_out,
+                       float* __restrict__ w_out, float* __restrict__ image, uint32_t* __restrict__ masks,
+                       const WeightSink ws) {
+    render_fwd<MARK, false, true>(rs, ranges, background, W, H, n_out, w_out, image, masks, DepthSource{}, nullptr,
+                                  nullptr, ws);
+}
+template <bool MARK>
+__global__ void __launch_bounds__(CTA_THREADS, GSR_FWD_DEPTH_STATS_MINB)
+    k_render_fwd_depth_stats(const RecSource rs, const DepthSource ds, const int32_t* __restrict__ ranges,
+                             const float* __restrict__ background, int W, int H, int32_t* __restrict__ n_out,
+                             float* __restrict__ w_out, float* __restrict__ image, float* __restrict__ depth,
+                             float* __restrict__ alpha, uint32_t* __restrict__ masks, const WeightSink ws) {
+    render_fwd<MARK, true, true>(rs, ranges, background, W, H, n_out, w_out, image, masks, ds, depth, alpha, ws);
 }
 
 // (float)(1.0 / (1.0 - (double)alpha)) — src/render_backward.cu:183 — without fp64: 1 - alpha is split
@@ -1360,14 +1464,28 @@ static bool make_depth_source(const uint64_t* keys_sorted, int id_bits, const ui
     return true;
 }
 
-// ds != nullptr: the depth/alpha kernels
+// ds != nullptr: the depth/alpha kernels; ws != nullptr: the blend-weight statistics kernels
 static int launch_forward(const RecSource& src, const DepthSource* ds, const int32_t* ranges, const float* background,
                           int H, int W, int32_t* n_out, float* w_out, float* image, float* depth, float* alpha,
-                          uint32_t* masks, void* stream) {
+                          uint32_t* masks, const WeightSink* ws, void* stream) {
     if (H <= 0 || W <= 0) return GSR_ERR_BAD_ARG;
     const dim3 grid((W + TILE - 1) / TILE, (H + TILE - 1) / TILE), block(CTA_THREADS);
     cudaStream_t st = (cudaStream_t)stream;
-    if (ds != nullptr) {
+    if (ws != nullptr) {
+        const DepthSource d = ds != nullptr ? *ds : DepthSource{};
+        if (ds != nullptr && masks != nullptr)
+            k_render_fwd_depth_stats<true><<<grid, block, 0, st>>>(src, d, ranges, background, W, H, n_out, w_out,
+                                                                   image, depth, alpha, masks, *ws);
+        else if (ds != nullptr)
+            k_render_fwd_depth_stats<false><<<grid, block, 0, st>>>(src, d, ranges, background, W, H, n_out, w_out,
+                                                                    image, depth, alpha, nullptr, *ws);
+        else if (masks != nullptr)
+            k_render_fwd_stats<true><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image, masks,
+                                                             *ws);
+        else
+            k_render_fwd_stats<false><<<grid, block, 0, st>>>(src, ranges, background, W, H, n_out, w_out, image,
+                                                              nullptr, *ws);
+    } else if (ds != nullptr) {
         if (masks != nullptr)
             k_render_fwd_depth<true><<<grid, block, 0, st>>>(src, *ds, ranges, background, W, H, n_out, w_out, image,
                                                              depth, alpha, masks);
@@ -1442,7 +1560,37 @@ int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* key
         return GSR_ERR_BAD_ARG;
     return launch_forward(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
                           depth != nullptr ? &ds : nullptr, ranges, background, H, W, n_out, w_out, image, depth, alpha,
-                          contribution_masks, stream);
+                          contribution_masks, nullptr, stream);
+}
+
+int gsr_render_forward_gather_stats(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                                    const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                                    int depth_bits, const int32_t* ranges, const float* background, int H, int W,
+                                    int32_t* n_out, float* w_out, float* image, float* depth, float* alpha,
+                                    uint32_t* contribution_masks, float* weight_sum, float* weight_max,
+                                    int32_t* pixel_count, const uint64_t* pair_total, int64_t pair_capacity,
+                                    void* stream) {
+    const int given = (weight_sum != nullptr) + (weight_max != nullptr) + (pixel_count != nullptr);
+    if (given == 0)
+        return gsr_render_forward_gather(gaussian_records, keys_sorted, id_bits, ids_sorted, depth_key, depth_base,
+                                         depth_bits, ranges, background, H, W, n_out, w_out, image, depth, alpha,
+                                         contribution_masks, stream);
+    if (given != 3) return GSR_ERR_BAD_ARG;
+    if (pair_total != nullptr && (pair_capacity < 0 || pair_capacity > 0xffffffffll)) return GSR_ERR_BAD_ARG;
+    if ((keys_sorted == nullptr) == (ids_sorted == nullptr)) return GSR_ERR_BAD_ARG;  // exactly one id source
+    if ((depth == nullptr) != (alpha == nullptr)) return GSR_ERR_BAD_ARG;
+    DepthSource ds;
+    if (depth != nullptr && !make_depth_source(keys_sorted, id_bits, depth_key, depth_base, depth_bits, ds))
+        return GSR_ERR_BAD_ARG;
+    WeightSink ws;
+    ws.sum = weight_sum;
+    ws.max = reinterpret_cast<uint32_t*>(weight_max);
+    ws.count = reinterpret_cast<uint32_t*>(pixel_count);
+    ws.pair_total = pair_total;
+    ws.capacity = pair_total != nullptr ? (uint32_t)pair_capacity : 0u;
+    return launch_forward(make_source(gaussian_records, keys_sorted, ids_sorted, id_bits),
+                          depth != nullptr ? &ds : nullptr, ranges, background, H, W, n_out, w_out, image, depth, alpha,
+                          contribution_masks, &ws, stream);
 }
 
 int gsr_render_backward_gather(int mode, const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,

@@ -582,9 +582,31 @@ std::tuple<torch::Tensor, torch::Tensor, torch::Tensor, torch::Tensor, torch::Te
 fused_render_forward(torch::Tensor records, torch::Tensor ranges, torch::Tensor background, int64_t H, int64_t W,
                      int64_t P, bool record_masks, c10::optional<torch::Tensor> keys_sorted,
                      c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
-                     c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits) {
+                     c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits,
+                     c10::optional<torch::Tensor> weight_sum, c10::optional<torch::Tensor> weight_max,
+                     c10::optional<torch::Tensor> pixel_count, c10::optional<torch::Tensor> pair_total,
+                     int64_t pair_capacity) {
     CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
     TORCH_CHECK(background.numel() == 3, "Background RGB must have 3 elements");
+    const int n_stats = weight_sum.has_value() + weight_max.has_value() + pixel_count.has_value();
+    TORCH_CHECK(n_stats == 0 || n_stats == 3, "weight_sum, weight_max and pixel_count go together");
+    if (n_stats == 3) {
+        const int64_t N = records.size(0);
+        for (const torch::Tensor* t : {&*weight_sum, &*weight_max, &*pixel_count}) {
+            CHECK_VALID_INPUT((*t));
+            TORCH_CHECK(t->device() == records.device(), "weight statistics must be on the records' device");
+            TORCH_CHECK(t->dim() == 1 && t->size(0) == N, "weight statistics must have shape [N]");
+        }
+        TORCH_CHECK(weight_sum->scalar_type() == torch::kFloat32 && weight_max->scalar_type() == torch::kFloat32,
+                    "weight_sum and weight_max must be float32");
+        TORCH_CHECK(pixel_count->scalar_type() == torch::kInt32, "pixel_count must be int32");
+    }
+    if (pair_total.has_value()) {
+        CHECK_VALID_INPUT((*pair_total));
+        TORCH_CHECK(pair_total->scalar_type() == torch::kInt64 && pair_total->numel() >= 1,
+                    "pair_total must be an int64 tensor (the pair scan; its last element is read)");
+        TORCH_CHECK(pair_total->device() == records.device(), "pair_total must be on the records' device");
+    }
     c10::cuda::CUDAGuard guard(records.device());
     auto opt = records.options();
     torch::Tensor image = torch::empty({H, W, 3}, opt);
@@ -600,13 +622,18 @@ fused_render_forward(torch::Tensor records, torch::Tensor ranges, torch::Tensor 
                               : torch::empty({0}, opt.dtype(torch::kInt32));
     uint32_t* mptr = record_masks ? (uint32_t*)masks.data_ptr<int>() : nullptr;
     const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
-    check_rc(gsr_render_forward_gather(
+    const bool stats = weight_sum.has_value();
+    check_rc(gsr_render_forward_gather_stats(
                  F32PTR(records), ps.keys, (int)id_bits, ps.ids,
                  depth_key.has_value() ? (const uint32_t*)depth_key->data_ptr<int>() : nullptr,
                  (uint32_t)depth_base, (int)depth_bits, ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
                  n.data_ptr<int>(), F32PTR(w), F32PTR(image), depth.defined() ? F32PTR(depth) : nullptr,
-                 alpha.defined() ? F32PTR(alpha) : nullptr, mptr, cur_stream()),
-             "gsr_render_forward_gather");
+                 alpha.defined() ? F32PTR(alpha) : nullptr, mptr, stats ? F32PTR((*weight_sum)) : nullptr,
+                 stats ? F32PTR((*weight_max)) : nullptr, stats ? pixel_count->data_ptr<int>() : nullptr,
+                 pair_total.has_value() ? (const uint64_t*)(pair_total->data_ptr<int64_t>() + pair_total->numel() - 1)
+                                        : nullptr,
+                 pair_capacity, cur_stream()),
+             "gsr_render_forward_gather_stats");
     return std::make_tuple(image, n, w, masks, depth, alpha);
 }
 
@@ -996,7 +1023,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("mode") = 0, py::arg("filter3d") = py::none());
     m.def("fused_bin", &fused_bin, "pair emission + radix sort + tile ranges");
     m.def("fused_render_forward", &fused_render_forward,
-          "tile renderer forward (with depth_key: also the depth and alpha maps)");
+          "tile renderer forward (with depth_key: also the depth and alpha maps; with weight_sum / weight_max / "
+          "pixel_count: also accumulates the per-gaussian blend-weight statistics, skipped when the last element of "
+          "pair_total exceeds pair_capacity)",
+          py::arg("records"), py::arg("ranges"), py::arg("background"), py::arg("H"), py::arg("W"), py::arg("P"),
+          py::arg("record_masks"), py::arg("keys_sorted"), py::arg("ids_sorted"), py::arg("id_bits"),
+          py::arg("depth_key"), py::arg("depth_base"), py::arg("depth_bits"), py::arg("weight_sum") = py::none(),
+          py::arg("weight_max") = py::none(), py::arg("pixel_count") = py::none(),
+          py::arg("pair_total") = py::none(), py::arg("pair_capacity") = 0);
     m.def("fused_render_backward", &fused_render_backward,
           "tile renderer backward -> per-gaussian gradient slab (with grad_depth / grad_alpha: rows incl. z; "
           "mode: MODE_* bits, MODE_ABSGRAD: rows incl. the absolute uv gradients)",

@@ -50,6 +50,43 @@ class DensificationStats:
                                     self.uv_grad_accum, self.xyz_grad_accum, self.grad_accum_count)
 
 
+class WeightStats:
+    """Blend-weight importance of every Gaussian, accumulated by the render forward: pass it as
+    rasterize(..., weight_stats=ws) and every view adds, over the pixels p where Gaussian i takes part in the colour
+    blend (the pixel is in the image and not yet saturated, alpha > 1/255), with w_ip = T_ip * alpha_ip the blend
+    weight the image uses:
+
+        weight_sum  f32 [N]  sum_p w_ip          (Mini-Splatting; float atomics: determined up to summation order)
+        weight_max  f32 [N]  max_p w_ip          (RadSplat; deterministic)
+        pixel_count i32 [N]  number of such p    (deterministic; wraps past 2^31 - 1)
+
+    Indexed by Gaussian row.  Nothing is ever zeroed by the renderer: a loop over the training views (under
+    torch.no_grad() or during training) leaves the totals here; `reset()` starts again.  A Gaussian that no view
+    reached keeps zeros.  Stale after densification changes N (rasterize raises ValueError): make a new one."""
+
+    def __init__(self, n_gaussians: int, device):
+        self.weight_sum = torch.zeros(n_gaussians, dtype=torch.float32, device=device)
+        self.weight_max = torch.zeros(n_gaussians, dtype=torch.float32, device=device)
+        self.pixel_count = torch.zeros(n_gaussians, dtype=torch.int32, device=device)
+
+    def __len__(self):
+        return int(self.weight_sum.shape[0])
+
+    def reset(self) -> None:
+        self.weight_sum.zero_()
+        self.weight_max.zero_()
+        self.pixel_count.zero_()
+
+    def all_reduce(self, group=None) -> None:
+        """Combine the ranks' statistics in place (SUM, MAX, SUM), so that view-parallel ranks that rendered different
+        views hold the same totals and take the same pruning decision."""
+        import torch.distributed as dist
+
+        dist.all_reduce(self.weight_sum, op=dist.ReduceOp.SUM, group=group)
+        dist.all_reduce(self.weight_max, op=dist.ReduceOp.MAX, group=group)
+        dist.all_reduce(self.pixel_count, op=dist.ReduceOp.SUM, group=group)
+
+
 # ---------------------------------------------------------------------------------------------------------
 # Adaptive density control on the flat buffers (SURVEY.md §8(f) rank 2)
 # ---------------------------------------------------------------------------------------------------------
@@ -221,6 +258,34 @@ def plan_adaptive_density_control(gaussians, stats: DensificationStats, config, 
     return finish(final_rows, clone_row, split_row)
 
 
+def plan_prune(score: torch.Tensor, keep_fraction: float) -> DensificationPlan:
+    """Delete-only plan keeping the ceil(keep_fraction * N) rows of largest `score` ([N], any real dtype, e.g.
+    WeightStats.weight_sum).  Ties are broken by the lower row index; the kept rows stay in ascending original
+    order.  keep_fraction = 1 gives the identity plan.  A NaN score ranks below every other score (it is no evidence
+    that the row matters).  Reads nothing back to the host."""
+    import math
+
+    if score.dim() != 1:
+        raise ValueError(f"score must have shape [N], got {tuple(score.shape)}")
+    if score.is_complex() or score.dtype == torch.bool:
+        raise TypeError(f"score must be real, got {score.dtype}")
+    keep_fraction = float(keep_fraction)
+    if not (0.0 < keep_fraction <= 1.0):
+        raise ValueError(f"keep_fraction must be in (0, 1], got {keep_fraction}")
+    n = int(score.shape[0])
+    plan = DensificationPlan(n)
+    k = min(n, math.ceil(keep_fraction * n))
+    plan.info.update(n_in=n, n_out=k, deleted=n - k)
+    if k == n:
+        return plan
+    # stable sort on the descending score: equal scores keep ascending row order, so the lower row wins a tie
+    if score.is_floating_point():
+        score = torch.nan_to_num(score, nan=float("-inf"))
+    order = torch.sort(score, descending=True, stable=True).indices[:k]
+    plan.src = torch.sort(order).values.to(torch.int32).contiguous()
+    return plan
+
+
 def apply_plan(plan: DensificationPlan, gaussians, optimizer=None, stats: DensificationStats = None, flat=None,
                out_flat=None):
     """Apply a plan with ONE native pass over the flat parameter buffer and (when `optimizer` is a FlatAdam) both of
@@ -283,6 +348,23 @@ class AdaptiveDensityControl:
         from .flat_adam import section_ends
 
         plan = plan_adaptive_density_control(self.gaussians, self.stats, self.config, iteration)
+        out_flat = None
+        if self.alloc_flat is not None and not plan.is_identity():
+            n_rest = 0 if self.gaussians.sh is None else int(self.gaussians.sh.shape[2])
+            out_flat = self.alloc_flat(section_ends(plan.n_out, n_rest)[-1])
+        apply_plan(plan, self.gaussians, self.optimizer, self.stats, out_flat=out_flat)
+        return plan.info
+
+    def prune(self, score: torch.Tensor, keep_fraction: float):
+        """Keep the ceil(keep_fraction * N) Gaussians of largest `score` (plan_prune; e.g. a WeightStats field) with
+        their Adam moments, in one native pass (apply_plan); resets the densification statistics.  Returns the plan's
+        info (n_in, n_out, deleted)."""
+        from .flat_adam import section_ends
+
+        n = self.gaussians.xyz.shape[0]
+        if score.shape != (n,):
+            raise ValueError(f"score has shape {tuple(score.shape)} but there are {n} gaussians")
+        plan = plan_prune(score, keep_fraction)
         out_flat = None
         if self.alloc_flat is not None and not plan.is_identity():
             n_rest = 0 if self.gaussians.sh is None else int(self.gaussians.sh.shape[2])

@@ -240,7 +240,8 @@ class _ViewState:
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "_ids_sorted", "ranges",
                  "records", "keys_sorted", "id_bits",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
-                 "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad", "filter3d")
+                 "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad", "filter3d",
+                 "weight_stats")
 
     @property
     def ids_sorted(self):
@@ -275,6 +276,7 @@ class _ViewState:
         self.filter3d = None
         self.depth = self.alpha = None
         self.uv_absgrad = None  # MODE_ABSGRAD: [M,2], set by every render backward
+        self.weight_stats = None  # optional densify.WeightStats the render forward accumulates into
 
 
 class _stage:
@@ -341,13 +343,20 @@ class _ProjectGaussians(torch.autograd.Function):
 
         depth_keys = zkey if state.mode & ext.MODE_DEPTH_ALPHA else None
 
+        ws = state.weight_stats
+        stats = () if ws is None else (ws.weight_sum, ws.weight_max, ws.pixel_count)
+
         def bin_and_render(M_, P_, speculative):
             with _stage(state, "bin_sort_gather"):
                 binned = ext.fused_bin(records, zkey, visible, scan, M_, P_, H, W, mh, depth_bits, speculative,
                                        tile_mask if USE_TILE_MASKS else None, tile_win if USE_TILE_MASKS else None)
+            # weight statistics of a speculative run: the kernel compares the scan's pair count with the capacity and
+            # adds nothing when the run is discarded for overflowing it
+            guard = (scan, P_) if (stats and speculative) else ()
             with _stage(state, "render_fwd"):
                 rendered = ext.fused_render_forward(records, binned[1], background, H, W, P_, record_masks, binned[4],
-                                                    binned[0], binned[5], depth_keys, depth_base, depth_bits)
+                                                    binned[0], binned[5], depth_keys, depth_base, depth_bits, *stats,
+                                                    *guard)
             return binned, rendered
 
         # The host needs M and P (the shape of the returned uv; the size of the pair buffers).  Reading them right
@@ -474,7 +483,7 @@ class _CompositeTiles(torch.autograd.Function):
 
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
-              render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None):
+              render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
@@ -503,7 +512,31 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     parameter gradients (state.grad_flat as usual) are those of the raw parameters.  Return values and uv.grad keep
     their meaning; combines with antialiased (coef comes before rho), render_depth_alpha, absgrad, return_state and
     grad_out.  After densification changes N the filter must be recomputed: a filter of another length raises
-    ValueError.  fp32 and precomputed SH colours only; the values are not checked (no host synchronisation)."""
+    ValueError.  fp32 and precomputed SH colours only; the values are not checked (no host synchronisation).
+
+    weight_stats: a densify.WeightStats of N Gaussians the render forward accumulates blend-weight importance into:
+    per Gaussian, over the pixels where it takes part in the colour blend, the sum and the max of its blend weight
+    w = T * alpha (the float the image uses; with antialiased / filter3d alpha carries the compensated opacity) and
+    the number of such pixels (DESIGN.md 3.14).  Added to, never zeroed, by every call, with or without gradients, for
+    importance pruning (AdaptiveDensityControl.prune).  Return values, uv.grad, uv.absgrad and all gradients are
+    unchanged and the statistics are not differentiable; combines with render_depth_alpha, antialiased, filter3d,
+    absgrad, return_state and grad_out.  A WeightStats of another length raises ValueError (make a new one after
+    densification changes N).  fp32 and precomputed SH colours only."""
+    if weight_stats is not None:
+        if gaussians.xyz.dtype != torch.float32:
+            raise TypeError("weight_stats needs fp32 inputs (the fused rasterizer's render forward accumulates them)")
+        if gaussians.sh is not None and not use_sh_precompute:
+            raise ValueError("weight_stats needs use_sh_precompute=True (per-pixel SH colours are not supported)")
+        n = gaussians.xyz.shape[0]
+        fields = (weight_stats.weight_sum, weight_stats.weight_max, weight_stats.pixel_count)
+        if any(tuple(f.shape) != (n,) for f in fields):
+            raise ValueError(f"weight_stats holds {tuple(fields[0].shape)} rows but there are {n} gaussians: make a new "
+                             "WeightStats after densification changes the gaussians")
+        for f, dt in zip(fields, (torch.float32, torch.float32, torch.int32)):
+            if f.dtype != dt:
+                raise TypeError(f"weight_stats fields must be float32, float32, int32; got {f.dtype}")
+            if f.device != gaussians.xyz.device or not f.is_contiguous():
+                raise ValueError("weight_stats fields must be contiguous and on the gaussians' device")
     if filter3d is not None:
         if gaussians.xyz.dtype != torch.float32:
             raise TypeError("filter3d needs fp32 inputs (the fused rasterizer's per-gaussian stages apply it)")
@@ -538,6 +571,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
+    state.weight_stats = weight_stats
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))

@@ -175,6 +175,27 @@ int gsr_render_forward_gather(const float* gaussian_records, const uint64_t* key
                               const int32_t* tile_ranges, const float* background_rgb, int H, int W,
                               int32_t* num_splats_per_pixel, float* final_weight_per_pixel, float* image, float* depth,
                               float* alpha, uint32_t* contribution_masks, void* stream);
+/* gsr_render_forward_gather + per-gaussian blend-weight statistics (importance scores for pruning), accumulated into
+ * (never cleared) over every pixel p of the view where gaussian i contributes to the colour blend:
+ *   weight_sum [N]  f32: += sum_p w_ip, w_ip the blend weight of the colour (T_ip * alpha_ip, the walk's float);
+ *   weight_max [N]  f32: max(weight_max, max_p w_ip), taken on the float bits (w >= +0; the array must hold values
+ *                   >= +0.0, e.g. zero-filled);
+ *   pixel_count [N] i32: += the number of such pixels (wraps past 2^31 - 1).
+ * A pixel counts for gaussian i iff the colour blend uses it: the pixel lies in the image and is not yet saturated,
+ * the Mahalanobis term is positive and alpha > 1/255.  The image and every other output are bit-identical to
+ * gsr_render_forward_gather's.  weight_sum is accumulated with float atomics (determined up to summation order);
+ * weight_max and pixel_count are deterministic.  Pixels the walk recomputes exactly contribute the walk's weights.
+ * All three NULL: exactly gsr_render_forward_gather; some but not all NULL: GSR_ERR_BAD_ARG.
+ * Speculatively sized pair buffers: pair_total (NULL: none) points at the pair scan's total, P in its low 32 bits
+ * (the last element of the per-gaussian scan the pair emission reads); when P > pair_capacity (0 <= pair_capacity < 2^32), the pairs the kernel sees
+ * are incomplete and NOTHING is accumulated — the caller renders the view again with the exact count. */
+int gsr_render_forward_gather_stats(const float* gaussian_records, const uint64_t* keys_sorted, int id_bits,
+                                    const int32_t* ids_sorted, const uint32_t* depth_key, uint32_t depth_base,
+                                    int depth_bits, const int32_t* tile_ranges, const float* background_rgb, int H,
+                                    int W, int32_t* num_splats_per_pixel, float* final_weight_per_pixel, float* image,
+                                    float* depth, float* alpha, uint32_t* contribution_masks, float* weight_sum,
+                                    float* weight_max, int32_t* pixel_count, const uint64_t* pair_total,
+                                    int64_t pair_capacity, void* stream);
 /* + grad_image [H,W,3].  Gradient destination, accumulated into: the four planar arrays grad_rgb [N,3],
  * grad_opacity [N], grad_uv [N,2], grad_conic [N,3] (grad_rows NULL), or grad_rows [N, GSR_GRAD_ROW_FLOATS] (16-byte
  * aligned, zero-filled; then the four planar pointers are ignored): one interleaved row per gaussian,

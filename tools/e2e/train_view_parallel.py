@@ -63,7 +63,17 @@ def main():
                     help="Mip-Splatting's 3-D smoothing filter in training and evaluation: computed from the training "
                          "cameras before the first step, after every densification pass and every 100 steps after "
                          "densification ends (not in the last 100); every rank computes the same filter")
+    ap.add_argument("--prune-keep", type=float, default=None,
+                    help="importance pruning: at every --prune-at iteration keep this fraction of the gaussians, ranked "
+                         "by their blend-weight sums over the training views (rasterize(weight_stats=...) under no_grad "
+                         "with the run's antialiased / filter3d settings, views split over the ranks, all-reduced)")
+    ap.add_argument("--prune-at", default="", help="comma-separated iterations for --prune-keep")
+    ap.add_argument("--step-time-from", type=int, default=None,
+                    help="report the mean GPU step time of the sampled steps after this iteration (default: the last "
+                         "--prune-at iteration); give the same value to an unpruned run to compare like with like")
     a = ap.parse_args()
+    prune_at = {int(x) for x in a.prune_at.split(",") if x.strip()}
+    assert (a.prune_keep is None) == (not prune_at), "--prune-keep and --prune-at go together"
 
     real_stdout = os.fdopen(os.dup(1), "w")
     os.dup2(2, 1)
@@ -79,7 +89,7 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
 
     import gaussian_splatting_b200 as gsb
-    from gaussian_splatting_b200.densify import AdaptiveDensityControl, DensificationStats
+    from gaussian_splatting_b200.densify import AdaptiveDensityControl, DensificationStats, WeightStats
     from gaussian_splatting_b200.filter3d import compute_filter3d
     from gaussian_splatting_b200.flat_adam import REFERENCE_LR_MULTIPLIERS as mult, FlatAdam
     from gaussian_splatting_b200.loss import photometric_loss, ssim as fused_ssim
@@ -199,7 +209,9 @@ def main():
         return float(np.mean(psnrs)), float(np.mean(ssims))
 
     fields = ("xyz", "quaternion", "scale", "opacity", "rgb", "sh")
-    curve, adc_log = [], []
+    curve, adc_log, prune_log = [], [], []
+    step_from = a.step_time_from if a.step_time_from is not None else (max(prune_at) if prune_at else None)
+    steps_after = []  # GPU time (CUDA events: rasterize, loss + backward, statistics + reduce + Adam) of sampled steps
     phase_ms = dict(rasterize_fwd=[], loss_and_backward=[], stats_reduce_adam=[])  # CUDA events, every 50th step
     t_adc = 0.0
     if world > 1:
@@ -256,6 +268,8 @@ def main():
             torch.cuda.synchronize()
             for k, (a0, a1) in zip(phase_ms, ((0, 1), (1, 2), (2, 3))):
                 phase_ms[k].append(ev[a0].elapsed_time(ev[a1]))
+            if step_from is not None and i > step_from:
+                steps_after.append(ev[0].elapsed_time(ev[3]))
         if config.adaptive_control_start < i < config.adaptive_control_end and i % config.adaptive_control_interval == 0:
             t_a = time.time()
             all_reduce_statistics([stats.uv_grad_accum, stats.xyz_grad_accum, stats.grad_accum_count])
@@ -266,6 +280,23 @@ def main():
             filt = refresh_filter()
         elif a.filter3d and i >= config.adaptive_control_end and i % 100 == 0 and i < config.num_iters - 100:
             filt = refresh_filter()
+        if i in prune_at:
+            t_a = time.time()
+            ws = WeightStats(g.xyz.shape[0], dev)
+            with torch.no_grad():
+                for k, tim in enumerate(train_ims):
+                    if k % world == rank:
+                        rasterize(g, tim.camera_T_world, cams[tim.camera_id], config.near_thresh, config.far_thresh,
+                                  config.cull_mask_padding, config.mh_dist, config.use_sh_precompute,
+                                  torch.zeros(3, device=dev), antialiased=a.antialiased, filter3d=filt, weight_stats=ws)
+            if world > 1:
+                ws.all_reduce()
+            info = relayout(lambda: adc.prune(ws.weight_sum, a.prune_keep))
+            del ws
+            filt = refresh_filter()
+            torch.cuda.synchronize()
+            t_adc += time.time() - t_a
+            prune_log.append(dict(iter=i, **info))
         if config.reset_opacity_start < i < config.reset_opacity_end and i % config.reset_opacity_interval == 0:
             relayout(adc.reset_opacity)
         if i > 0 and i % config.add_sh_band_interval == 0:
@@ -304,6 +335,10 @@ def main():
             "loss": ("fused: photometric_loss (gsr_photometric_loss_forward / _backward), ssim() in evaluation"
                      if a.loss == "fused" else "shim: l1_loss + SSIM stand-in (tools/e2e/shims) through NCHW views"),
             "antialiased": a.antialiased, "absgrad": a.absgrad, "filter3d": a.filter3d,
+            "prune_keep": a.prune_keep, "prune_log": prune_log,
+            "step_ms_gpu_after": (None if step_from is None else
+                                  dict(from_iter=step_from, samples=len(steps_after),
+                                       mean=round(sum(steps_after) / len(steps_after), 3) if steps_after else None)),
             "device": torch.cuda.get_device_name(local),
         }
         real_stdout.write("E2E " + json.dumps(line) + "\n")
