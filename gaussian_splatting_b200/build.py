@@ -31,6 +31,7 @@ CU_SOURCES = [
     "gsr_render_generic.cu",
     "gsr_adam.cu",
     "gsr_densify.cu",
+    "gsr_mcmc.cu",
     "gsr_loss.cu",
 ]
 HEADERS = [

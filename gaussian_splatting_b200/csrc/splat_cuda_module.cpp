@@ -901,6 +901,99 @@ std::vector<torch::Tensor> densify_apply(torch::Tensor p_in, c10::optional<torch
     return {p_out};
 }
 
+// 3DGS-MCMC relocation of n sampled rows -> (new_opacity [n], new_scale [n,3]) (gsr_mcmc_relocation)
+std::vector<torch::Tensor> mcmc_relocation(torch::Tensor opacity, torch::Tensor scale, torch::Tensor ratio,
+                                           int64_t n_max, double min_opacity) {
+    CHECK_VALID_INPUT(opacity); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(ratio);
+    CHECK_FLOAT_TENSOR(opacity); CHECK_FLOAT_TENSOR(scale); CHECK_INT_TENSOR(ratio);
+    const int64_t n = opacity.numel();
+    TORCH_CHECK(scale.numel() == 3 * n && ratio.numel() == n, "opacity [n], scale [n,3] and ratio [n] must match");
+    TORCH_CHECK(scale.device() == opacity.device() && ratio.device() == opacity.device(), "tensors on different devices");
+    TORCH_CHECK(n_max >= 1, "n_max must be at least 1");
+    c10::cuda::CUDAGuard guard(opacity.device());
+    torch::Tensor new_opacity = torch::empty({n}, opacity.options());
+    torch::Tensor new_scale = torch::empty({n, 3}, opacity.options());
+    check_rc(gsr_mcmc_relocation((int)n, F32PTR(opacity), F32PTR(scale), ratio.data_ptr<int32_t>(), (int)n_max,
+                                 (float)min_opacity, F32PTR(new_opacity), F32PTR(new_scale), cur_stream()),
+             "gsr_mcmc_relocation");
+    return {new_opacity, new_scale};
+}
+
+// a relocation / growth plan applied to the flat parameter buffer and both Adam moments (gsr_mcmc_apply); returns
+// (p_out, m_out, v_out) freshly allocated (p_out: p_out_buf when given; only p_out without moments)
+std::vector<torch::Tensor> mcmc_apply(torch::Tensor p_in, c10::optional<torch::Tensor> m_in,
+                                      c10::optional<torch::Tensor> v_in, int64_t n_in, int64_t n_sh_rest,
+                                      torch::Tensor src, c10::optional<torch::Tensor> set_row,
+                                      c10::optional<torch::Tensor> new_opacity, c10::optional<torch::Tensor> new_scale,
+                                      c10::optional<torch::Tensor> p_out_buf) {
+    CHECK_VALID_INPUT(p_in); CHECK_FLOAT_TENSOR(p_in); CHECK_VALID_INPUT(src); CHECK_INT_TENSOR(src);
+    TORCH_CHECK(n_in >= 0 && n_sh_rest >= 0, "n_in and n_sh_rest must be non-negative");
+    TORCH_CHECK(p_in.numel() == gsr_flat_numel(n_in, (int)n_sh_rest), "p_in does not match the flat layout of n_in gaussians");
+    const int64_t n_out = src.numel();
+    TORCH_CHECK(n_out >= n_in, "mcmc_apply keeps every row: src must have at least n_in entries");
+    const int64_t total = gsr_flat_numel(n_out, (int)n_sh_rest);
+    const bool moments = m_in.has_value();
+    TORCH_CHECK(moments == v_in.has_value(), "m_in and v_in go together");
+    const bool sets = set_row.has_value();
+    TORCH_CHECK(sets == new_opacity.has_value() && sets == new_scale.has_value(),
+                "set_row, new_opacity and new_scale go together");
+    TORCH_CHECK(src.device() == p_in.device(), "src must be on p_in's device");
+    if (sets) {
+        CHECK_VALID_INPUT((*set_row)); CHECK_INT_TENSOR((*set_row));
+        CHECK_VALID_INPUT((*new_opacity)); CHECK_FLOAT_TENSOR((*new_opacity));
+        CHECK_VALID_INPUT((*new_scale)); CHECK_FLOAT_TENSOR((*new_scale));
+        TORCH_CHECK(set_row->numel() == n_out, "set_row must have one entry per output row");
+        TORCH_CHECK(new_scale->numel() == 3 * new_opacity->numel(), "new_opacity [m] and new_scale [m,3] must match");
+        for (auto* t : {&*set_row, &*new_opacity, &*new_scale})
+            TORCH_CHECK(t->device() == p_in.device(), "plan tensors must be on p_in's device");
+    }
+    c10::cuda::CUDAGuard guard(p_in.device());
+    torch::Tensor p_out;
+    if (p_out_buf.has_value()) {  // caller-owned destination (e.g. symmetric memory)
+        p_out = *p_out_buf;
+        CHECK_VALID_INPUT(p_out); CHECK_FLOAT_TENSOR(p_out);
+        TORCH_CHECK(p_out.numel() == total && p_out.device() == p_in.device(), "bad p_out buffer");
+    } else {
+        p_out = torch::empty({total}, p_in.options());
+    }
+    torch::Tensor m_out, v_out;
+    if (moments) {
+        CHECK_VALID_INPUT((*m_in)); CHECK_VALID_INPUT((*v_in)); CHECK_FLOAT_TENSOR((*m_in)); CHECK_FLOAT_TENSOR((*v_in));
+        TORCH_CHECK(m_in->numel() == p_in.numel() && v_in->numel() == p_in.numel(), "moments must match p_in");
+        TORCH_CHECK(m_in->device() == p_in.device() && v_in->device() == p_in.device(), "moments must be on p_in's device");
+        m_out = torch::empty({total}, p_in.options());
+        v_out = torch::empty({total}, p_in.options());
+    }
+    check_rc(gsr_mcmc_apply((int)n_in, (int)n_out, (int)n_sh_rest, F32PTR(p_in), moments ? F32PTR((*m_in)) : nullptr,
+                            moments ? F32PTR((*v_in)) : nullptr, src.data_ptr<int32_t>(),
+                            sets ? set_row->data_ptr<int32_t>() : nullptr, sets ? F32PTR((*new_opacity)) : nullptr,
+                            sets ? F32PTR((*new_scale)) : nullptr, F32PTR(p_out), moments ? F32PTR(m_out) : nullptr,
+                            moments ? F32PTR(v_out) : nullptr, cur_stream()),
+             "gsr_mcmc_apply");
+    if (moments) return {p_out, m_out, v_out};
+    return {p_out};
+}
+
+// SGLD position noise in place on the flat parameter buffer of N gaussians (gsr_mcmc_noise)
+void mcmc_noise(torch::Tensor p, int64_t N, int64_t n_sh_rest, double scaler, double k, double x0, int64_t seed,
+                int64_t offset, c10::optional<torch::Tensor> eps_in, c10::optional<torch::Tensor> eps_out) {
+    CHECK_VALID_INPUT(p); CHECK_FLOAT_TENSOR(p);
+    TORCH_CHECK(N >= 0 && n_sh_rest >= 0, "N and n_sh_rest must be non-negative");
+    TORCH_CHECK(p.numel() == gsr_flat_numel(N, (int)n_sh_rest), "p does not match the flat layout of N gaussians");
+    TORCH_CHECK(offset >= 0, "offset must be non-negative");
+    for (auto* t : {&eps_in, &eps_out}) {
+        if (!t->has_value()) continue;
+        CHECK_VALID_INPUT((**t)); CHECK_FLOAT_TENSOR((**t));
+        TORCH_CHECK((*t)->numel() == 3 * N, "eps_in / eps_out must have shape [N,3]");
+        TORCH_CHECK((*t)->device() == p.device(), "eps_in / eps_out must be on p's device");
+    }
+    c10::cuda::CUDAGuard guard(p.device());
+    check_rc(gsr_mcmc_noise((int)N, (int)n_sh_rest, F32PTR(p), scaler, k, x0, (uint64_t)seed, (uint64_t)offset,
+                            eps_in.has_value() ? F32PTR((*eps_in)) : nullptr,
+                            eps_out.has_value() ? F32PTR((*eps_out)) : nullptr, cur_stream()),
+             "gsr_mcmc_noise");
+}
+
 // inverse(camera_T_world)[:3, 3] with torch's bits (gsr_camera_centre)
 torch::Tensor camera_centre(torch::Tensor camera_T_world) {
     CHECK_VALID_INPUT(camera_T_world); CHECK_FLOAT_TENSOR(camera_T_world);
@@ -1056,6 +1149,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");
     m.def("densify_accumulate", &densify_accumulate, "per-step densification statistics");
     m.def("densify_apply", &densify_apply, "clone / split / delete applied to the flat parameter + Adam buffers");
+    m.def("mcmc_relocation", &mcmc_relocation, "3DGS-MCMC relocation: opacity and scale of N copies (fp64 sum)",
+          py::arg("opacity"), py::arg("scale"), py::arg("ratio"), py::arg("n_max"), py::arg("min_opacity"));
+    m.def("mcmc_apply", &mcmc_apply, "3DGS-MCMC relocation / growth plan applied to the flat parameter + Adam buffers",
+          py::arg("p_in"), py::arg("m_in"), py::arg("v_in"), py::arg("n_in"), py::arg("n_sh_rest"), py::arg("src"),
+          py::arg("set_row"), py::arg("new_opacity"), py::arg("new_scale"), py::arg("p_out") = py::none());
+    m.def("mcmc_noise", &mcmc_noise, "3DGS-MCMC position noise, in place on the flat parameter buffer",
+          py::arg("p"), py::arg("N"), py::arg("n_sh_rest"), py::arg("scaler"), py::arg("k"), py::arg("x0"),
+          py::arg("seed"), py::arg("offset"), py::arg("eps_in") = py::none(), py::arg("eps_out") = py::none());
     m.def("camera_centre", &camera_centre, "inverse(camera_T_world)[:3, 3] with torch's bits, one kernel");
     m.def("photometric_loss_forward", &photometric_loss_forward,
           "(1 - ssim_frac) * L1 + ssim_frac * (1 - SSIM) forward -> (loss, L1, SSIM)");

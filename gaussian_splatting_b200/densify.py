@@ -292,8 +292,6 @@ def apply_plan(plan: DensificationPlan, gaussians, optimizer=None, stats: Densif
     its moment buffers, then re-point the Gaussians' fields (and the optimizer) at the new buffers and reset the
     statistics to the new size (trainer.py:294 `reset_grad_accum`).  `flat`: the flat parameter buffer the fields
     are views of (default: optimizer.p).  Returns the new flat buffer."""
-    from .flat_adam import FIELDS, section_ends
-
     n_rest = 0 if gaussians.sh is None else int(gaussians.sh.shape[2])
     if flat is None:
         assert optimizer is not None, "need the flat parameter buffer"
@@ -305,28 +303,38 @@ def apply_plan(plan: DensificationPlan, gaussians, optimizer=None, stats: Densif
             m, v = optimizer.m, optimizer.v
         out = native().densify_apply(flat, m, v, plan.n_in, n_rest, plan.src, plan.clone_row, plan.split_row,
                                      plan.xyz_sub, plan.xyz_add, plan.q_set, plan.scale_set, out_flat)
-        new_flat = out[0]
-        ends = section_ends(n_out, n_rest)
-        names = [f for f in FIELDS if getattr(gaussians, f, None) is not None]
-        widths = dict(xyz=(3,), quaternion=(4,), scale=(3,), opacity=(1,), rgb=(3,), sh=(3, n_rest))
-        start = 0
-        for name, end in zip(names, ends):
-            shape = (n_out,) + widths[name]
-            numel = n_out
-            for d in widths[name]:
-                numel *= d
-            view = new_flat[start:start + numel].view(shape)
-            old = getattr(gaussians, name)
-            new = torch.nn.Parameter(view) if isinstance(old, torch.nn.Parameter) else view.requires_grad_(True)
-            setattr(gaussians, name, new)
-            start = end
-        if optimizer is not None:
-            optimizer.p, optimizer.m, optimizer.v = new_flat, out[1], out[2]
-            optimizer.ends = [int(e) for e in ends]
-        flat = new_flat
+        flat = adopt_flat(gaussians, optimizer, out, n_out)
     if stats is not None:
         stats.__init__(n_out, flat.device)
     return flat
+
+
+def adopt_flat(gaussians, optimizer, out, n_out: int):
+    """Re-point the Gaussians' fields at views of the new flat parameter buffer out[0] (n_out rows, the Gaussians' SH
+    width) and, when `optimizer` is given, its p / m / v at out[0] / out[1] / out[2] and its section ends.  Returns
+    out[0]."""
+    from .flat_adam import FIELDS, section_ends
+
+    n_rest = 0 if gaussians.sh is None else int(gaussians.sh.shape[2])
+    new_flat = out[0]
+    ends = section_ends(n_out, n_rest)
+    names = [f for f in FIELDS if getattr(gaussians, f, None) is not None]
+    widths = dict(xyz=(3,), quaternion=(4,), scale=(3,), opacity=(1,), rgb=(3,), sh=(3, n_rest))
+    start = 0
+    for name, end in zip(names, ends):
+        shape = (n_out,) + widths[name]
+        numel = n_out
+        for d in widths[name]:
+            numel *= d
+        view = new_flat[start:start + numel].view(shape)
+        old = getattr(gaussians, name)
+        new = torch.nn.Parameter(view) if isinstance(old, torch.nn.Parameter) else view.requires_grad_(True)
+        setattr(gaussians, name, new)
+        start = end
+    if optimizer is not None:
+        optimizer.p, optimizer.m, optimizer.v = new_flat, out[1], out[2]
+        optimizer.ends = [int(e) for e in ends]
+    return new_flat
 
 
 class AdaptiveDensityControl:
@@ -389,46 +397,55 @@ class AdaptiveDensityControl:
     def add_sh_band(self, base_lr: float = 0.002, sh_lr_multiplier: float = 0.1):
         """trainer.py:77-112 + optimizer_manager.py:61-72: SH coefficients per channel 0 -> 3 -> 8 -> 15, new
         coefficients zero, the moments of the WHOLE sh tensor restart from zero (as the reference does)."""
-        from .flat_adam import FIELDS, section_ends
+        return add_sh_band(self.gaussians, self.optimizer, self.config.max_sh_band, self.alloc_flat, base_lr,
+                           sh_lr_multiplier)
 
-        g, opt = self.gaussians, self.optimizer
-        if self.config.max_sh_band == 0:
-            return False
-        old = 0 if g.sh is None else int(g.sh.shape[2])
-        if old == 0:
-            new = 3
-        elif old == 3 and self.config.max_sh_band > 1:
-            new = 8
-        elif old == 8 and self.config.max_sh_band > 2:
-            new = 15
-        else:
-            return False
-        n = g.xyz.shape[0]
-        ends_new = section_ends(n, new)
-        if self.alloc_flat is not None:
-            flat_new = self.alloc_flat(ends_new[-1])
-            flat_new.zero_()
-        else:
-            flat_new = torch.zeros(ends_new[-1], dtype=torch.float32, device=g.xyz.device)
-        m_new = torch.zeros(ends_new[-1], dtype=torch.float32, device=g.xyz.device)
-        v_new = torch.zeros_like(m_new)
-        keep = opt.ends[4]  # xyz .. rgb sections are laid out identically (their ends do not depend on the sh width)
-        flat_new[:keep].copy_(opt.p[:keep])
-        m_new[:keep].copy_(opt.m[:keep])
-        v_new[:keep].copy_(opt.v[:keep])
-        sh_view = flat_new[keep:keep + n * 3 * new].view(n, 3, new)
-        if old:
-            sh_view[:, :, :old].copy_(g.sh.detach())
-        widths = dict(xyz=(3,), quaternion=(4,), scale=(3,), opacity=(1,), rgb=(3,))
-        start = 0
-        for name, end in zip(FIELDS[:5], ends_new[:5]):
-            o = getattr(g, name)
-            view = flat_new[start:start + n * widths[name][0]].view((n,) + widths[name])
-            setattr(g, name, torch.nn.Parameter(view) if isinstance(o, torch.nn.Parameter) else view.requires_grad_(True))
-            start = end
-        was_param = isinstance(g.xyz, torch.nn.Parameter)
-        g.sh = torch.nn.Parameter(sh_view) if was_param else sh_view.requires_grad_(True)
-        opt.p, opt.m, opt.v, opt.ends = flat_new, m_new, v_new, [int(e) for e in ends_new]
-        if len(opt.lrs) == 5:
-            opt.lrs.append(float(base_lr * sh_lr_multiplier))
-        return True
+
+def add_sh_band(gaussians, optimizer, max_sh_band: int, alloc_flat=None, base_lr: float = 0.002,
+                sh_lr_multiplier: float = 0.1):
+    """One more SH band on the flat buffers (AdaptiveDensityControl.add_sh_band, MCMCDensityControl.add_sh_band):
+    SH coefficients per channel 0 -> 3 -> 8 -> 15 up to `max_sh_band`, new coefficients zero, the moments of the
+    WHOLE sh tensor restart from zero.  Returns whether a band was added."""
+    from .flat_adam import FIELDS, section_ends
+
+    g, opt = gaussians, optimizer
+    if max_sh_band == 0:
+        return False
+    old = 0 if g.sh is None else int(g.sh.shape[2])
+    if old == 0:
+        new = 3
+    elif old == 3 and max_sh_band > 1:
+        new = 8
+    elif old == 8 and max_sh_band > 2:
+        new = 15
+    else:
+        return False
+    n = g.xyz.shape[0]
+    ends_new = section_ends(n, new)
+    if alloc_flat is not None:
+        flat_new = alloc_flat(ends_new[-1])
+        flat_new.zero_()
+    else:
+        flat_new = torch.zeros(ends_new[-1], dtype=torch.float32, device=g.xyz.device)
+    m_new = torch.zeros(ends_new[-1], dtype=torch.float32, device=g.xyz.device)
+    v_new = torch.zeros_like(m_new)
+    keep = opt.ends[4]  # xyz .. rgb sections are laid out identically (their ends do not depend on the sh width)
+    flat_new[:keep].copy_(opt.p[:keep])
+    m_new[:keep].copy_(opt.m[:keep])
+    v_new[:keep].copy_(opt.v[:keep])
+    sh_view = flat_new[keep:keep + n * 3 * new].view(n, 3, new)
+    if old:
+        sh_view[:, :, :old].copy_(g.sh.detach())
+    widths = dict(xyz=(3,), quaternion=(4,), scale=(3,), opacity=(1,), rgb=(3,))
+    start = 0
+    for name, end in zip(FIELDS[:5], ends_new[:5]):
+        o = getattr(g, name)
+        view = flat_new[start:start + n * widths[name][0]].view((n,) + widths[name])
+        setattr(g, name, torch.nn.Parameter(view) if isinstance(o, torch.nn.Parameter) else view.requires_grad_(True))
+        start = end
+    was_param = isinstance(g.xyz, torch.nn.Parameter)
+    g.sh = torch.nn.Parameter(sh_view) if was_param else sh_view.requires_grad_(True)
+    opt.p, opt.m, opt.v, opt.ends = flat_new, m_new, v_new, [int(e) for e in ends_new]
+    if len(opt.lrs) == 5:
+        opt.lrs.append(float(base_lr * sh_lr_multiplier))
+    return True

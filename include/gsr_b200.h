@@ -428,6 +428,38 @@ int gsr_densify_apply(int n_in, int n_out, int n_sh_rest, const float* p_in, con
                       const float* xyz_add, const float* q_set, const float* scale_set, float* p_out, float* m_out,
                       float* v_out, void* stream);
 
+/* ---- 3DGS-MCMC densification (Kheradmand et al. 2024) on the flat buffers (csrc/gsr_mcmc.cu) -----------------
+ * Relocation of n sampled rows: opacity [n] (sigmoid opacity o), scale [n,3] (exp scale), ratio int32 [n] (number
+ * of copies, clamped to [1, n_max]) -> new_opacity [n] = clamp(1 - (1 - o)^(1/N), min_opacity, 1 - 2^-23) and
+ * new_scale [n,3] = scale * o / sum_{i=1..N} sum_{k=0..i-1} C(i-1,k) (-1)^k o_hat^(k+1) / sqrt(k+1), the sum and the
+ * power evaluated in fp64 (the sum alternates in sign; see the kernel).  Outputs must not overlap the inputs or each
+ * other; n_max >= 1. */
+int gsr_mcmc_relocation(int n, const float* opacity, const float* scale, const int32_t* ratio, int n_max,
+                        float min_opacity, float* new_opacity, float* new_scale, void* stream);
+
+/* A relocation or growth plan applied to the flat parameter buffer and both Adam moment buffers in ONE pass
+ * (n_out >= n_in; the layout of gsr_flat_numel).  Per OUTPUT row r:
+ *   src[r]      row of the old buffers it is copied from
+ *   set_row[r]  >= 0: opacity <- logit(new_opacity[set_row[r]]), scale <- log(new_scale[set_row[r]][0..2]), both
+ *               formed in the kernel (p / (1 - p), then logf); else -1
+ * Moment contract: m and v are ZERO in every row with set_row[r] >= 0 — the rows whose parameters the pass changes:
+ * the sampled sources, the relocated dead rows and the appended copies.  Every other row keeps its source row's
+ * moments.  A relocated row therefore never inherits a dead row's (or its source's) moments.  Section padding is
+ * zero.  set_row, new_opacity and new_scale go together (all NULL: a plain gather); m_in, v_in, m_out, v_out go
+ * together.  Outputs must not overlap the inputs or each other.  set_row values index the caller's tables. */
+int gsr_mcmc_apply(int n_in, int n_out, int n_sh_rest, const float* p_in, const float* m_in, const float* v_in,
+                   const int32_t* src, const int32_t* set_row, const float* new_opacity, const float* new_scale,
+                   float* p_out, float* m_out, float* v_out, void* stream);
+
+/* SGLD position noise, in place on the flat parameter buffer p of N gaussians (run after the optimizer step):
+ *   xyz_i += scaler * w_i * Sigma_i eps_i,  Sigma_i = R(q_i / |q_i|) diag(exp(2 s_i)) R^T,
+ *   w_i = 1 / (1 + exp(-k ((1 - sigmoid(opacity_i)) - x0)))
+ * eps_i ~ N(0, I_3) from Philox4x32-10 keyed by (seed, subsequence i, offset): the same (seed, offset) gives the
+ * same draws on every device and launch; pass the step as offset.  eps_in [N,3] (optional) replaces the draws;
+ * eps_out [N,3] (optional) receives the draws used.  Only the xyz section is written. */
+int gsr_mcmc_noise(int N, int n_sh_rest, float* p, double scaler, double k, double x0, uint64_t seed, uint64_t offset,
+                   const float* eps_in, float* eps_out, void* stream);
+
 /* ---- photometric loss of the training step (splat_py/trainer.py:363-374) ------------------------------------
  * loss = l1_weight * L1 + ssim_weight * (1 - SSIM), with L1 = mean |pred - target| over all B*C*H*W elements and
  * SSIM the mean over B*C*(H-10)*(W-10) valid window origins of the 11x11 separable Gaussian-window SSIM map

@@ -10,6 +10,9 @@ schedule) with everything the rasterizer hands over kept on this library's fast 
                      summed over ranks and `adaptive_density_control` runs identically on every rank: the plan on
                      per-row scalars with the reference's torch expressions, clone / split / delete applied to the
                      flat parameter + Adam buffers by ONE native pass (gsr_densify_apply); reset_opacity, add_sh_band.
+    --strategy mcmc: 3DGS-MCMC instead of the last line (no statistics, no opacity resets): regularisers into the
+                     flat gradients before the collective, position noise after Adam (gsr_mcmc_noise), relocation +
+                     growth up to --cap-max on the densification window (gsr_mcmc_apply); add_sh_band as before.
 
 Iteration convention (SURVEY.md §8(e)): the reference takes ONE view per optimizer step.  Here an optimizer step
 averages the gradients of `world` views; `--iters` counts optimizer steps and every schedule constant of the
@@ -68,12 +71,22 @@ def main():
                          "by their blend-weight sums over the training views (rasterize(weight_stats=...) under no_grad "
                          "with the run's antialiased / filter3d settings, views split over the ranks, all-reduced)")
     ap.add_argument("--prune-at", default="", help="comma-separated iterations for --prune-keep")
+    ap.add_argument("--strategy", choices=["adc", "mcmc"], default="adc",
+                    help="adc: the reference's adaptive density control with opacity resets; mcmc: 3DGS-MCMC "
+                         "(gaussian_splatting_b200.mcmc): opacity / scale regularisers added to the flat gradients "
+                         "before the exchange, position noise after every optimizer step, relocation of dead "
+                         "gaussians and growth up to --cap-max on the ADC window's schedule, no opacity resets; the "
+                         "refinement draws from one generator seeded with --seed on every rank")
+    ap.add_argument("--cap-max", type=int, default=None, help="--strategy mcmc: the gaussian budget")
     ap.add_argument("--step-time-from", type=int, default=None,
                     help="report the mean GPU step time of the sampled steps after this iteration (default: the last "
                          "--prune-at iteration); give the same value to an unpruned run to compare like with like")
     a = ap.parse_args()
     prune_at = {int(x) for x in a.prune_at.split(",") if x.strip()}
     assert (a.prune_keep is None) == (not prune_at), "--prune-keep and --prune-at go together"
+    mcmc_on = a.strategy == "mcmc"
+    assert (a.cap_max is not None) == mcmc_on, "--cap-max goes with --strategy mcmc"
+    assert not (mcmc_on and prune_at), "--prune-keep needs --strategy adc"
 
     real_stdout = os.fdopen(os.dup(1), "w")
     os.dup2(2, 1)
@@ -93,6 +106,7 @@ def main():
     from gaussian_splatting_b200.filter3d import compute_filter3d
     from gaussian_splatting_b200.flat_adam import REFERENCE_LR_MULTIPLIERS as mult, FlatAdam
     from gaussian_splatting_b200.loss import photometric_loss, ssim as fused_ssim
+    from gaussian_splatting_b200.mcmc import MCMCConfig, MCMCDensityControl
     from gaussian_splatting_b200.rasterize import rasterize
     from gaussian_splatting_b200.structs import Camera
     from gaussian_splatting_b200.view_parallel import GradientBucket, all_reduce_statistics
@@ -147,6 +161,15 @@ def main():
         opt = FlatAdam.for_gaussians(g, base_lr=config.base_lr, multipliers=mult)
     stats = DensificationStats(n0, dev)
     adc = AdaptiveDensityControl(g, opt, stats, config, alloc_flat=alloc_sym if sharded else None)
+    mcmc = None
+    if mcmc_on:  # refinement on the ADC window (scaled with --iters like it), one generator state on every rank
+        mcmc = MCMCDensityControl(
+            g, opt, MCMCConfig(cap_max=a.cap_max, refine_start=config.adaptive_control_start,
+                               refine_stop=config.adaptive_control_end,
+                               refine_every=config.adaptive_control_interval, max_sh_band=config.max_sh_band),
+            alloc_flat=alloc_sym if sharded else None, generator=torch.Generator(device=dev).manual_seed(a.seed))
+    ctl = mcmc if mcmc_on else adc  # the controller whose optimizer relayout() swaps
+    xyz_lr = config.base_lr * mult["xyz"]
 
     def relayout(fn):
         """Run a step that may re-lay-out the parameter buffer (densification, opacity reset, a new SH band).  With
@@ -157,7 +180,7 @@ def main():
             return fn()
         m_full, v_full = opt.full_state()
         shim = types.SimpleNamespace(p=opt.p, m=m_full, v=v_full, ends=list(opt.ends), lrs=list(opt.lrs))
-        adc.optimizer = shim
+        ctl.optimizer = shim
         out = fn()
         if shim.p is not opt.p:
             grads_sym = alloc_sym(shim.p.numel())
@@ -167,7 +190,7 @@ def main():
             opt.load_full_state(shim.m, shim.v, t)
         else:
             opt.load_full_state(shim.m, shim.v, opt.t)
-        adc.optimizer = opt
+        ctl.optimizer = opt
         return out
     ssim = StructuralSimilarityIndexMeasure(data_range=1.0).to(dev)
 
@@ -209,7 +232,7 @@ def main():
         return float(np.mean(psnrs)), float(np.mean(ssims))
 
     fields = ("xyz", "quaternion", "scale", "opacity", "rgb", "sh")
-    curve, adc_log, prune_log = [], [], []
+    curve, adc_log, prune_log, mcmc_log = [], [], [], []
     step_from = a.step_time_from if a.step_time_from is not None else (max(prune_at) if prune_at else None)
     steps_after = []  # GPU time (CUDA events: rasterize, loss + backward, statistics + reduce + Adam) of sampled steps
     phase_ms = dict(rasterize_fwd=[], loss_and_backward=[], stats_reduce_adam=[])  # CUDA events, every 50th step
@@ -241,7 +264,7 @@ def main():
                                            config.use_sh_precompute, background, return_state=True,
                                            grad_out=grads_sym, antialiased=a.antialiased, absgrad=a.absgrad,
                                            filter3d=filt)
-        if not a.absgrad:
+        if not a.absgrad and not mcmc_on:
             uv.retain_grad()
         if timed:
             ev[1].record()
@@ -254,15 +277,20 @@ def main():
         loss.backward()
         if timed:
             ev[2].record()
-        # per-view statistics BEFORE the collective: they are this rank's own view (trainer.py:376-385); the xyz
-        # gradient they use is this view's, so they are taken from the still un-averaged buffer
-        stats.accumulate(state, uv, g.xyz, cams[im.camera_id].K, absgrad=a.absgrad)
+        if mcmc_on:
+            mcmc.regularize(state.grad_flat)  # every rank adds the same terms: the average keeps them once
+        else:
+            # per-view statistics BEFORE the collective: they are this rank's own view (trainer.py:376-385); the
+            # xyz gradient they use is this view's, so they are taken from the still un-averaged buffer
+            stats.accumulate(state, uv, g.xyz, cams[im.camera_id].K, absgrad=a.absgrad)
         if sharded:
             opt.step()  # barrier, reduce-scatter + Adam + all-gather in one kernel over peer memory, barrier
         else:
             bucket = GradientBucket.adopt(state.grad_flat, g)
             bucket.all_reduce(average=True)
             opt.step(bucket)
+        if mcmc_on:
+            mcmc.inject_noise(i, xyz_lr, seed=a.seed)
         if timed:
             ev[3].record()
             torch.cuda.synchronize()
@@ -270,7 +298,14 @@ def main():
                 phase_ms[k].append(ev[a0].elapsed_time(ev[a1]))
             if step_from is not None and i > step_from:
                 steps_after.append(ev[0].elapsed_time(ev[3]))
-        if config.adaptive_control_start < i < config.adaptive_control_end and i % config.adaptive_control_interval == 0:
+        if mcmc_on and mcmc.is_refine_step(i):
+            t_a = time.time()
+            mcmc_log.append(relayout(lambda: mcmc.refine(i)))
+            torch.cuda.synchronize()
+            t_adc += time.time() - t_a
+            filt = refresh_filter()
+        elif (not mcmc_on and config.adaptive_control_start < i < config.adaptive_control_end
+              and i % config.adaptive_control_interval == 0):
             t_a = time.time()
             all_reduce_statistics([stats.uv_grad_accum, stats.xyz_grad_accum, stats.grad_accum_count])
             info = relayout(lambda: adc.adaptive_density_control(i))
@@ -297,10 +332,11 @@ def main():
             torch.cuda.synchronize()
             t_adc += time.time() - t_a
             prune_log.append(dict(iter=i, **info))
-        if config.reset_opacity_start < i < config.reset_opacity_end and i % config.reset_opacity_interval == 0:
+        if (not mcmc_on and config.reset_opacity_start < i < config.reset_opacity_end
+                and i % config.reset_opacity_interval == 0):
             relayout(adc.reset_opacity)
         if i > 0 and i % config.add_sh_band_interval == 0:
-            relayout(lambda: adc.add_sh_band(config.base_lr, config.sh_lr_multiplier))
+            relayout(lambda: ctl.add_sh_band(config.base_lr, config.sh_lr_multiplier))
     torch.cuda.synchronize()
     if world > 1:
         dist.barrier()
@@ -336,6 +372,7 @@ def main():
                      if a.loss == "fused" else "shim: l1_loss + SSIM stand-in (tools/e2e/shims) through NCHW views"),
             "antialiased": a.antialiased, "absgrad": a.absgrad, "filter3d": a.filter3d,
             "prune_keep": a.prune_keep, "prune_log": prune_log,
+            "strategy": a.strategy, "cap_max": a.cap_max, "mcmc_passes": len(mcmc_log), "mcmc_last": mcmc_log[-3:],
             "step_ms_gpu_after": (None if step_from is None else
                                   dict(from_iter=step_from, samples=len(steps_after),
                                        mean=round(sum(steps_after) / len(steps_after), 3) if steps_after else None)),
