@@ -1,9 +1,10 @@
 """In-tree build of the native code (no JIT cache: the .so files ship with the tree).
 
   libgsr_b200.so            CUDA kernels + C ABI (include/gsr_b200.h), nvcc, sm_90a only, no torch
+  libgsr_selective_adam.so  the visibility-masked Adam step (include/gsr_selective_adam.h), same flags
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds both; `build(force=False)` is incremental.
+`python -m gaussian_splatting_b200.build` builds all three; `build(force=False)` is incremental.
 """
 from __future__ import annotations
 
@@ -21,6 +22,7 @@ CSRC = PKG / "csrc"
 OBJ = PKG / "_build"
 EXT_DIR = PKG / "_ext"
 LIB = PKG / "libgsr_b200.so"
+SELECTIVE_LIB = PKG / "libgsr_selective_adam.so"
 
 CU_SOURCES = [
     "gsr_pergaussian.cu",
@@ -42,6 +44,10 @@ HEADERS = [
     CSRC / "gsr_f32x2.cuh",
     ROOT / "include" / "gsr_b200.h",
 ]
+# A library of its own, so that libgsr_b200.so keeps exactly its kernels (and their SASS).
+SELECTIVE_SOURCES = ["gsr_adam_selective.cu"]
+SELECTIVE_HEADERS = [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h",
+                     ROOT / "include" / "gsr_selective_adam.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -76,12 +82,12 @@ def ext_path() -> Path:
     return EXT_DIR / f"splat_cuda{suffix}"
 
 
-def build_lib(force: bool = False, verbose: bool = False) -> Path:
+def _build_cuda_lib(lib: Path, sources, headers, stamp_name: str, force: bool, verbose: bool) -> Path:
     OBJ.mkdir(exist_ok=True)
-    stamp = OBJ / "lib.sha256"
-    want = _digest([CSRC / s for s in CU_SOURCES] + HEADERS, " ".join(NVCC_FLAGS))
-    if not force and LIB.exists() and stamp.exists() and stamp.read_text() == want:
-        return LIB
+    stamp = OBJ / stamp_name
+    want = _digest([CSRC / s for s in sources] + headers, " ".join(NVCC_FLAGS))
+    if not force and lib.exists() and stamp.exists() and stamp.read_text() == want:
+        return lib
 
     def compile_one(src):
         obj = OBJ / (Path(src).stem + ".o")
@@ -93,12 +99,21 @@ def build_lib(force: bool = False, verbose: bool = False) -> Path:
             print(out)
         return obj
 
-    with ThreadPoolExecutor(max_workers=min(len(CU_SOURCES), os.cpu_count() or 1)) as ex:
-        objs = list(ex.map(compile_one, CU_SOURCES))
-    _run([_nvcc(), "-shared", "-o", str(LIB), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a",
+    with ThreadPoolExecutor(max_workers=min(len(sources), os.cpu_count() or 1)) as ex:
+        objs = list(ex.map(compile_one, sources))
+    _run([_nvcc(), "-shared", "-o", str(lib), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a",
           "-cudart", "shared"])
     stamp.write_text(want)
-    return LIB
+    return lib
+
+
+def build_lib(force: bool = False, verbose: bool = False) -> Path:
+    return _build_cuda_lib(LIB, CU_SOURCES, HEADERS, "lib.sha256", force, verbose)
+
+
+def build_selective_lib(force: bool = False, verbose: bool = False) -> Path:
+    return _build_cuda_lib(SELECTIVE_LIB, SELECTIVE_SOURCES, SELECTIVE_HEADERS, "selective_lib.sha256", force,
+                           verbose)
 
 
 def build_ext(force: bool = False) -> Path:
@@ -110,7 +125,8 @@ def build_ext(force: bool = False) -> Path:
     out = ext_path()
     src = CSRC / "splat_cuda_module.cpp"
     stamp = OBJ / "ext.sha256"
-    want = _digest([src, ROOT / "include" / "gsr_b200.h"], torch.__version__)
+    want = _digest([src, ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h"],
+                   torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -121,7 +137,7 @@ def build_ext(force: bool = False) -> Path:
         "-DTORCH_EXTENSION_NAME=splat_cuda", "-DTORCH_API_INCLUDE_EXTENSION_H",
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
-        f"-L{PKG}", "-lgsr_b200", f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
+        f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",
     ]
@@ -141,6 +157,7 @@ def build_render_variant(out_dir, flags) -> Path:
 
 def build(force: bool = False, verbose: bool = False):
     lib = build_lib(force=force, verbose=verbose)
+    build_selective_lib(force=force, verbose=verbose)
     ext = build_ext(force=force)
     return lib, ext
 

@@ -11,6 +11,7 @@
 #include <tuple>
 
 #include "../../include/gsr_b200.h"
+#include "../../include/gsr_selective_adam.h"
 
 namespace {
 
@@ -821,6 +822,57 @@ void adam_step_sharded(int64_t lo, int64_t hi, std::vector<int64_t> peer_grad_pt
              "gsr_adam_step_sharded");
 }
 
+// visible: CUDA bool / uint8 [N], nonzero = the row is updated (rasterize's state.visible); N = visible.numel()
+void adam_step_selective(torch::Tensor p, torch::Tensor g, torch::Tensor m, torch::Tensor v, torch::Tensor visible,
+                         int64_t n_sh_rest, std::vector<int64_t> section_end, std::vector<double> section_lr,
+                         double beta1, double beta2, double eps, int64_t step) {
+    CHECK_VALID_INPUT(p); CHECK_VALID_INPUT(g); CHECK_VALID_INPUT(m); CHECK_VALID_INPUT(v);
+    CHECK_FLOAT_TENSOR(p); CHECK_FLOAT_TENSOR(g); CHECK_FLOAT_TENSOR(m); CHECK_FLOAT_TENSOR(v);
+    CHECK_VALID_INPUT(visible);
+    TORCH_CHECK(visible.dtype() == torch::kBool || visible.dtype() == torch::kUInt8, "visible must be bool or uint8");
+    TORCH_CHECK(visible.device() == p.device() && g.device() == p.device() && m.device() == p.device() &&
+                    v.device() == p.device(), "p, g, m, v and visible must be on one device");
+    const int64_t n = p.numel();
+    TORCH_CHECK(g.numel() == n && m.numel() == n && v.numel() == n, "p, g, m, v must have the same length");
+    TORCH_CHECK(section_end.size() == section_lr.size() && !section_end.empty() && section_end.back() == n,
+                "sections must cover the buffer");
+    const int64_t rows = visible.numel();
+    TORCH_CHECK(n_sh_rest >= 0 && flat_section_ends(rows, n_sh_rest) == section_end,
+                "visible has ", rows, " rows, which do not match the flat layout of the buffer");
+    c10::cuda::CUDAGuard guard(p.device());
+    check_rc(gsr_adam_step_selective(rows, (int)n_sh_rest, F32PTR(p), F32PTR(g), F32PTR(m), F32PTR(v),
+                                     reinterpret_cast<const uint8_t*>(visible.data_ptr()), (int)section_end.size(),
+                                     section_end.data(), section_lr.data(), beta1, beta2, eps, (int)step,
+                                     cur_stream()),
+             "gsr_adam_step_selective");
+}
+
+void adam_step_selective_sharded(int64_t lo, int64_t hi, std::vector<int64_t> peer_grad_ptrs,
+                                 std::vector<int64_t> peer_param_ptrs, std::vector<int64_t> peer_visible_ptrs,
+                                 int64_t self_rank, torch::Tensor m_shard, torch::Tensor v_shard, int64_t n_rows,
+                                 int64_t n_sh_rest, std::vector<int64_t> section_end, std::vector<double> section_lr,
+                                 double beta1, double beta2, double eps, int64_t step) {
+    CHECK_VALID_INPUT(m_shard); CHECK_VALID_INPUT(v_shard); CHECK_FLOAT_TENSOR(m_shard); CHECK_FLOAT_TENSOR(v_shard);
+    TORCH_CHECK(peer_grad_ptrs.size() == peer_param_ptrs.size() && peer_grad_ptrs.size() == peer_visible_ptrs.size() &&
+                    !peer_grad_ptrs.empty(), "one pointer per rank");
+    TORCH_CHECK(m_shard.numel() == hi - lo && v_shard.numel() == hi - lo, "state shards must hold hi - lo elements");
+    TORCH_CHECK(section_end.size() == section_lr.size() && !section_end.empty(), "bad sections");
+    std::vector<const float*> gp;
+    std::vector<float*> pp;
+    std::vector<const uint8_t*> vp;
+    for (size_t q = 0; q < peer_grad_ptrs.size(); ++q) {
+        gp.push_back(reinterpret_cast<const float*>(peer_grad_ptrs[q]));
+        pp.push_back(reinterpret_cast<float*>(peer_param_ptrs[q]));
+        vp.push_back(reinterpret_cast<const uint8_t*>(peer_visible_ptrs[q]));
+    }
+    c10::cuda::CUDAGuard guard(m_shard.device());
+    check_rc(gsr_adam_step_selective_sharded(lo, hi, (int)gp.size(), gp.data(), pp.data(), vp.data(), (int)self_rank,
+                                             F32PTR(m_shard), F32PTR(v_shard), n_rows, (int)n_sh_rest,
+                                             (int)section_end.size(), section_end.data(), section_lr.data(), beta1,
+                                             beta2, eps, (int)step, cur_stream()),
+             "gsr_adam_step_selective_sharded");
+}
+
 void densify_accumulate(torch::Tensor vis_idx, torch::Tensor uv_grad, torch::Tensor xyz_grad, torch::Tensor K,
                         torch::Tensor uv_grad_accum, torch::Tensor xyz_grad_accum, torch::Tensor grad_accum_count) {
     CHECK_VALID_INPUT(vis_idx); CHECK_VALID_INPUT(uv_grad); CHECK_VALID_INPUT(xyz_grad); CHECK_VALID_INPUT(K);
@@ -1147,6 +1199,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");
+    m.def("adam_step_selective", &adam_step_selective,
+          "Adam on the flat parameter buffer, only the rows whose visible byte is nonzero (gsr_adam_step_selective)");
+    m.def("adam_step_selective_sharded", &adam_step_selective_sharded,
+          "reduce-scatter + Adam + all-gather of the rows any rank's view saw (gsr_adam_step_selective_sharded)");
     m.def("densify_accumulate", &densify_accumulate, "per-step densification statistics");
     m.def("densify_apply", &densify_apply, "clone / split / delete applied to the flat parameter + Adam buffers");
     m.def("mcmc_relocation", &mcmc_relocation, "3DGS-MCMC relocation: opacity and scale of N copies (fp64 sum)",

@@ -164,6 +164,19 @@ def all_reduce_statistics(tensors: Iterable[torch.Tensor], group=None) -> None:
         dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
 
 
+def all_reduce_visibility(visible: torch.Tensor, group=None) -> torch.Tensor:
+    """OR of the ranks' visibility masks (bool or uint8 [N], `state.visible`), in place, as a MAX all-reduce: what
+    FlatAdam.step(bucket, visible=...) needs after the gradient all-reduce, so that every replica updates the same rows
+    (a row is updated when any rank's view saw it).  A bool mask is reduced through its uint8 view.  No-op without an
+    initialised process group or with a single rank.  Returns `visible`."""
+    if not dist.is_available() or not dist.is_initialized() or dist.get_world_size(group) == 1:
+        return visible
+    assert visible.dtype in (torch.bool, torch.uint8) and visible.is_contiguous(), "a contiguous bool / uint8 mask"
+    buf = visible.view(torch.uint8) if visible.dtype == torch.bool else visible
+    dist.all_reduce(buf, op=dist.ReduceOp.MAX, group=group)
+    return visible
+
+
 def broadcast_parameters(gaussians, src: int = 0, group=None) -> None:
     """Make every rank start from rank `src`'s Gaussians (after initialisation or densification on `src`)."""
     if not dist.is_available() or not dist.is_initialized() or dist.get_world_size(group) == 1:

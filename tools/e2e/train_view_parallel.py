@@ -13,6 +13,8 @@ schedule) with everything the rasterizer hands over kept on this library's fast 
     --strategy mcmc: 3DGS-MCMC instead of the last line (no statistics, no opacity resets): regularisers into the
                      flat gradients before the collective, position noise after Adam (gsr_mcmc_noise), relocation +
                      growth up to --cap-max on the densification window (gsr_mcmc_apply); add_sh_band as before.
+    --selective-adam: the Adam step updates only the gaussians the step's views saw (the OR of the ranks'
+                     state.visible masks), gsr_adam_step_selective[_sharded]; every other row keeps p, m and v.
 
 Iteration convention (SURVEY.md §8(e)): the reference takes ONE view per optimizer step.  Here an optimizer step
 averages the gradients of `world` views; `--iters` counts optimizer steps and every schedule constant of the
@@ -78,6 +80,10 @@ def main():
                          "gaussians and growth up to --cap-max on the ADC window's schedule, no opacity resets; the "
                          "refinement draws from one generator seeded with --seed on every rank")
     ap.add_argument("--cap-max", type=int, default=None, help="--strategy mcmc: the gaussian budget")
+    ap.add_argument("--selective-adam", action="store_true",
+                    help="visibility-masked Adam: update only the gaussians the step's views saw (the OR of the ranks' "
+                         "state.visible masks); the others keep their parameters and moments. Works with --optimizer "
+                         "flat (MAX all-reduce of the masks) and sharded (masks in symmetric memory, read by the kernel)")
     ap.add_argument("--step-time-from", type=int, default=None,
                     help="report the mean GPU step time of the sampled steps after this iteration (default: the last "
                          "--prune-at iteration); give the same value to an unpruned run to compare like with like")
@@ -109,7 +115,7 @@ def main():
     from gaussian_splatting_b200.mcmc import MCMCConfig, MCMCDensityControl
     from gaussian_splatting_b200.rasterize import rasterize
     from gaussian_splatting_b200.structs import Camera
-    from gaussian_splatting_b200.view_parallel import GradientBucket, all_reduce_statistics
+    from gaussian_splatting_b200.view_parallel import GradientBucket, all_reduce_statistics, all_reduce_visibility
     from oracle import ref_loader
 
     gsb.install_as_splat_cuda()                 # the reference's loader imports splat_py.* which imports splat_cuda
@@ -140,7 +146,7 @@ def main():
     for name in ("xyz", "quaternion", "scale", "opacity", "rgb"):
         getattr(g, name).requires_grad_(True)
     sharded = a.optimizer == "sharded"
-    grads_sym = None
+    grads_sym = vis_sym = None
     if sharded:
         assert world > 1, "--optimizer sharded needs torchrun with at least 2 ranks"
         import types
@@ -156,7 +162,13 @@ def main():
         flat, ends, names = flatten_gaussians(g, flat=params_sym)
         grads_sym = alloc_sym(flat.numel())
         grads_sym.zero_()
-        opt = ShardedFlatAdam(params_sym, grads_sym, ends, [config.base_lr * mult[f] for f in names])
+
+        def alloc_vis(n):  # this rank's mask, read by every rank's kernel
+            return symm_mem.empty(int(n), dtype=torch.uint8, device=dev) if a.selective_adam else None
+
+        vis_sym = alloc_vis(n0)
+        opt = ShardedFlatAdam(params_sym, grads_sym, ends, [config.base_lr * mult[f] for f in names],
+                              visible_sym=vis_sym)
     else:
         opt = FlatAdam.for_gaussians(g, base_lr=config.base_lr, multipliers=mult)
     stats = DensificationStats(n0, dev)
@@ -175,7 +187,7 @@ def main():
         """Run a step that may re-lay-out the parameter buffer (densification, opacity reset, a new SH band).  With
         the sharded optimizer the Adam state is first gathered to full size, the step runs on a full-state stand-in
         of the optimizer, and the state is sharded again — over new symmetric buffers if the layout changed."""
-        nonlocal opt, grads_sym
+        nonlocal opt, grads_sym, vis_sym
         if not sharded:
             return fn()
         m_full, v_full = opt.full_state()
@@ -185,8 +197,9 @@ def main():
         if shim.p is not opt.p:
             grads_sym = alloc_sym(shim.p.numel())
             grads_sym.zero_()
+            vis_sym = alloc_vis(g.xyz.shape[0])  # N may have changed: the mask buffer follows the new layout
             t = opt.t
-            opt = ShardedFlatAdam(shim.p, grads_sym, shim.ends, shim.lrs)
+            opt = ShardedFlatAdam(shim.p, grads_sym, shim.ends, shim.lrs, visible_sym=vis_sym)
             opt.load_full_state(shim.m, shim.v, t)
         else:
             opt.load_full_state(shim.m, shim.v, opt.t)
@@ -236,6 +249,9 @@ def main():
     step_from = a.step_time_from if a.step_time_from is not None else (max(prune_at) if prune_at else None)
     steps_after = []  # GPU time (CUDA events: rasterize, loss + backward, statistics + reduce + Adam) of sampled steps
     phase_ms = dict(rasterize_fwd=[], loss_and_backward=[], stats_reduce_adam=[])  # CUDA events, every 50th step
+    # share of the gaussians in state.visible on the timed steps: this rank's view, or with --selective-adam
+    # --optimizer flat the OR over the ranks (all_reduce_visibility works in place)
+    visible_frac = []
     t_adc = 0.0
     if world > 1:
         dist.barrier()
@@ -284,11 +300,16 @@ def main():
             # xyz gradient they use is this view's, so they are taken from the still un-averaged buffer
             stats.accumulate(state, uv, g.xyz, cams[im.camera_id].K, absgrad=a.absgrad)
         if sharded:
+            if a.selective_adam:
+                vis_sym.copy_(state.visible)  # the kernel ORs every rank's mask after the step's first barrier
             opt.step()  # barrier, reduce-scatter + Adam + all-gather in one kernel over peer memory, barrier
         else:
             bucket = GradientBucket.adopt(state.grad_flat, g)
             bucket.all_reduce(average=True)
-            opt.step(bucket)
+            if a.selective_adam:
+                opt.step(bucket, visible=all_reduce_visibility(state.visible))
+            else:
+                opt.step(bucket)
         if mcmc_on:
             mcmc.inject_noise(i, xyz_lr, seed=a.seed)
         if timed:
@@ -296,6 +317,7 @@ def main():
             torch.cuda.synchronize()
             for k, (a0, a1) in zip(phase_ms, ((0, 1), (1, 2), (2, 3))):
                 phase_ms[k].append(ev[a0].elapsed_time(ev[a1]))
+            visible_frac.append(float((state.visible != 0).float().mean()))
             if step_from is not None and i > step_from:
                 steps_after.append(ev[0].elapsed_time(ev[3]))
         if mcmc_on and mcmc.is_refine_step(i):
@@ -372,6 +394,8 @@ def main():
                      if a.loss == "fused" else "shim: l1_loss + SSIM stand-in (tools/e2e/shims) through NCHW views"),
             "antialiased": a.antialiased, "absgrad": a.absgrad, "filter3d": a.filter3d,
             "prune_keep": a.prune_keep, "prune_log": prune_log,
+            "selective_adam": a.selective_adam,
+            "visible_fraction_mean": round(sum(visible_frac) / max(len(visible_frac), 1), 4),
             "strategy": a.strategy, "cap_max": a.cap_max, "mcmc_passes": len(mcmc_log), "mcmc_last": mcmc_log[-3:],
             "step_ms_gpu_after": (None if step_from is None else
                                   dict(from_iter=step_from, samples=len(steps_after),
