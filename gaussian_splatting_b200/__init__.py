@@ -32,7 +32,8 @@ def native():
         from .build import ext_path
 
         path = ext_path()
-        if not path.exists() or not all((_PKG / lib).exists() for lib in ("libgsr_b200.so", "libgsr_selective_adam.so")):
+        if not path.exists() or not all((_PKG / lib).exists() for lib in ("libgsr_b200.so", "libgsr_selective_adam.so",
+                                                                    "libgsr_features.so")):
             raise ImportError(
                 f"gaussian_splatting_b200 native code is not built ({path} missing); "
                 "run `python -m gaussian_splatting_b200.build` (needs nvcc, sm_90a)"

@@ -2,9 +2,10 @@
 
   libgsr_b200.so            CUDA kernels + C ABI (include/gsr_b200.h), nvcc, sm_90a only, no torch
   libgsr_selective_adam.so  the visibility-masked Adam step (include/gsr_selective_adam.h), same flags
+  libgsr_features.so        the feature-channel tile kernels (include/gsr_features.h), same flags
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all three; `build(force=False)` is incremental.
+`python -m gaussian_splatting_b200.build` builds all four; `build(force=False)` is incremental.
 """
 from __future__ import annotations
 
@@ -23,6 +24,7 @@ OBJ = PKG / "_build"
 EXT_DIR = PKG / "_ext"
 LIB = PKG / "libgsr_b200.so"
 SELECTIVE_LIB = PKG / "libgsr_selective_adam.so"
+FEATURES_LIB = PKG / "libgsr_features.so"
 
 CU_SOURCES = [
     "gsr_pergaussian.cu",
@@ -42,12 +44,16 @@ HEADERS = [
     CSRC / "gsr_math_bwd.cuh",
     CSRC / "gsr_record.cuh",
     CSRC / "gsr_f32x2.cuh",
+    CSRC / "gsr_tile_walk.cuh",
     ROOT / "include" / "gsr_b200.h",
 ]
 # A library of its own, so that libgsr_b200.so keeps exactly its kernels (and their SASS).
 SELECTIVE_SOURCES = ["gsr_adam_selective.cu"]
 SELECTIVE_HEADERS = [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h",
                      ROOT / "include" / "gsr_selective_adam.h"]
+FEATURES_SOURCES = ["gsr_features.cu"]
+FEATURES_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [ROOT / "include" / "gsr_b200.h",
+                                                                  ROOT / "include" / "gsr_features.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -116,6 +122,10 @@ def build_selective_lib(force: bool = False, verbose: bool = False) -> Path:
                            verbose)
 
 
+def build_features_lib(force: bool = False, verbose: bool = False) -> Path:
+    return _build_cuda_lib(FEATURES_LIB, FEATURES_SOURCES, FEATURES_HEADERS, "features_lib.sha256", force, verbose)
+
+
 def build_ext(force: bool = False) -> Path:
     import torch  # noqa: F401  (needed for include/library paths)
     from torch.utils import cpp_extension as ce
@@ -125,8 +135,8 @@ def build_ext(force: bool = False) -> Path:
     out = ext_path()
     src = CSRC / "splat_cuda_module.cpp"
     stamp = OBJ / "ext.sha256"
-    want = _digest([src, ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h"],
-                   torch.__version__)
+    want = _digest([src, ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h",
+                    ROOT / "include" / "gsr_features.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -137,7 +147,7 @@ def build_ext(force: bool = False) -> Path:
         "-DTORCH_EXTENSION_NAME=splat_cuda", "-DTORCH_API_INCLUDE_EXTENSION_H",
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
-        f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
+        f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",
     ]
@@ -158,6 +168,7 @@ def build_render_variant(out_dir, flags) -> Path:
 def build(force: bool = False, verbose: bool = False):
     lib = build_lib(force=force, verbose=verbose)
     build_selective_lib(force=force, verbose=verbose)
+    build_features_lib(force=force, verbose=verbose)
     ext = build_ext(force=force)
     return lib, ext
 

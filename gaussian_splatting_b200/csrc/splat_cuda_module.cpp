@@ -12,6 +12,7 @@
 
 #include "../../include/gsr_b200.h"
 #include "../../include/gsr_selective_adam.h"
+#include "../../include/gsr_features.h"
 
 namespace {
 
@@ -679,6 +680,53 @@ torch::Tensor fused_render_backward(torch::Tensor grad_image, int64_t N, int64_t
     return slab;
 }
 
+// feature_map [H,W,D]: features [N, stride] (stride = D rounded up to a multiple of 4, the padding columns 0) blended
+// with the colour forward's weights over the same pair list (gsr_render_features_forward)
+torch::Tensor fused_render_features_forward(torch::Tensor records, torch::Tensor ranges, int64_t H, int64_t W,
+                                            int64_t P, c10::optional<torch::Tensor> keys_sorted,
+                                            c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                            torch::Tensor features, int64_t D) {
+    CHECK_VALID_INPUT(features); CHECK_FLOAT_TENSOR(features);
+    TORCH_CHECK(features.dim() == 2 && features.size(0) == records.size(0), "features must be [N, stride]");
+    TORCH_CHECK(features.device() == records.device(), "features must be on the records' device");
+    c10::cuda::CUDAGuard guard(records.device());
+    torch::Tensor fmap = torch::empty({H, W, D}, records.options());
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    check_rc(gsr_render_features_forward(F32PTR(records), ps.keys, (int)id_bits, ps.ids, ranges.data_ptr<int>(), (int)H,
+                                         (int)W, F32PTR(features), (int)features.size(1), (int)D, F32PTR(fmap),
+                                         cur_stream()),
+             "gsr_render_features_forward");
+    return fmap;
+}
+
+// the feature backward (gsr_render_features_backward): adds the feature loss's opacity / uv / conic part into the
+// gradient slab of fused_render_backward and returns grad_features [N, stride]
+torch::Tensor fused_render_features_backward(torch::Tensor grad_map, torch::Tensor slab, int64_t P,
+                                             torch::Tensor records, torch::Tensor ids_sorted, torch::Tensor ranges,
+                                             torch::Tensor n, torch::Tensor w, torch::Tensor masks,
+                                             c10::optional<torch::Tensor> keys_sorted, int64_t id_bits,
+                                             torch::Tensor features) {
+    CHECK_VALID_INPUT(grad_map); CHECK_FLOAT_TENSOR(grad_map);
+    CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
+    CHECK_VALID_INPUT(features); CHECK_FLOAT_TENSOR(features);
+    const int64_t N = records.size(0);
+    TORCH_CHECK(grad_map.dim() == 3 && grad_map.size(0) == n.size(0) && grad_map.size(1) == n.size(1),
+                "grad_map must be [H, W, D]");
+    TORCH_CHECK(features.dim() == 2 && features.size(0) == N, "features must be [N, stride]");
+    TORCH_CHECK(slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ", GSR_GRAD_ROW_FLOATS,
+                " floats per gaussian");
+    c10::cuda::CUDAGuard guard(grad_map.device());
+    torch::Tensor grad_features = torch::zeros_like(features);
+    const uint32_t* mptr = masks.numel() > 0 ? (const uint32_t*)masks.data_ptr<int>() : nullptr;
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    check_rc(gsr_render_features_backward(F32PTR(records), ps.keys, (int)id_bits, ps.ids, ranges.data_ptr<int>(),
+                                          (int)n.size(0), (int)n.size(1), n.data_ptr<int>(), F32PTR(w),
+                                          F32PTR(features), (int)features.size(1), (int)grad_map.size(2),
+                                          F32PTR(grad_map), F32PTR(grad_features), F32PTR(slab), mptr, cur_stream()),
+             "gsr_render_features_backward");
+    return grad_features;
+}
+
 // grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab of fused_render_backward:
 // interleaved rows [N,12] by gaussian.  grad_uv_compact [M,2] (optional): gradient on the compact uv,
 // added to — or, with use_slab_uv false, replacing — the slab's uv section.  mode: the GSR_MODE_* bits of the forward
@@ -1183,6 +1231,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("ranges"), py::arg("background"), py::arg("n"), py::arg("w"), py::arg("masks"),
           py::arg("keys_sorted"), py::arg("id_bits"), py::arg("grad_depth"), py::arg("grad_alpha"),
           py::arg("depth_key"), py::arg("depth_base"), py::arg("depth_bits"), py::arg("mode") = 0);
+    m.def("fused_render_features_forward", &fused_render_features_forward,
+          "feature map [H,W,D] blended with the colour's weights (gsr_render_features_forward)");
+    m.def("fused_render_features_backward", &fused_render_features_backward,
+          "feature backward: grad_features [N, stride], and the geometry part added into the slab");
     m.def("fused_preprocess_backward", &fused_preprocess_backward,
           "fused per-gaussian backward (mode: MODE_* bits; filter3d: the forward's, with MODE_FILTER3D)",
           py::arg("slab"), py::arg("xyz"), py::arg("quaternion"), py::arg("scale"), py::arg("opacity_logit"),

@@ -8,7 +8,8 @@ densification (splat_py/trainer.py:360,379-385).
 Implementation: two autograd nodes around the native fused kernels
 
     _ProjectGaussians   params -> uv [M,2], carrier          (gsr_preprocess_forward + binning)
-    _CompositeTiles     uv, carrier -> image                  (gsr_render_forward_gather)
+    _CompositeTiles     uv, carrier[, features] -> image[, depth, alpha][, feature map]
+                                                          (gsr_render_forward_gather; gsr_render_features_*)
 
 (The tile renderer's forward kernel is enqueued by the projection node, right behind the binning and BEFORE the
 host reads the pair count; `_CompositeTiles` only ties its image into the graph.)
@@ -439,20 +440,41 @@ class _ProjectGaussians(torch.autograd.Function):
 
 
 class _CompositeTiles(torch.autograd.Function):
-    """uv, carrier -> image, or (image, depth, alpha) with the depth/alpha maps."""
+    """uv, carrier[, features] -> image, or (image, depth, alpha) with the depth/alpha maps, then the feature map."""
 
     @staticmethod
-    def forward(ctx, uv, carrier, background_rgb, state):
+    def forward(ctx, uv, carrier, background_rgb, state, features=None):
         # the tile renderer was already enqueued by the projection node (right behind the binning, before the host
         # learned the pair count): this node only ties its outputs to uv and to the gradient carrier
-        outs = state.image if state.depth is None else (state.image, state.depth, state.alpha)
+        outs = (state.image,) if state.depth is None else (state.image, state.depth, state.alpha)
         state.image = state.depth = state.alpha = None
         ctx.state = state
-        return outs
+        ctx.n_features = 0
+        if features is not None:
+            # the feature kernels read 4 channels per CTA with 16-byte copies: rows padded to a multiple of 4 columns
+            D = features.shape[1]
+            stride = (D + 3) // 4 * 4
+            fpad = features
+            if stride != D:
+                fpad = torch.nn.functional.pad(features, (0, stride - D))
+            elif features.data_ptr() % 16 != 0:
+                fpad = features.clone()
+            # P is final here: the projection node reran binning and the renderer if the speculative guess overflowed
+            with _stage(state, "features_fwd"):
+                fmap = native().fused_render_features_forward(state.records, state.ranges, state.H, state.W, state.P,
+                                                              state.keys_sorted, state._ids_sorted, state.id_bits,
+                                                              fpad, D)
+            ctx.n_features = D
+            ctx.save_for_backward(fpad)
+            outs = outs + (fmap,)
+        return outs if len(outs) > 1 else outs[0]
 
     @staticmethod
-    def backward(ctx, grad_image, grad_depth=None, grad_alpha=None):
+    def backward(ctx, grad_image, *grad_maps):
         st = ctx.state
+        grad_depth = grad_alpha = None
+        if st.mode & native().MODE_DEPTH_ALPHA:
+            grad_depth, grad_alpha = grad_maps[:2]
         with _stage(st, "render_bwd"):
             slab = native().fused_render_backward(
                 grad_image.contiguous(), st.N, st.P, st.records, st._ids_sorted, st.ranges, st.background,
@@ -460,6 +482,16 @@ class _CompositeTiles(torch.autograd.Function):
                 None if grad_depth is None else grad_depth.contiguous(),
                 None if grad_alpha is None else grad_alpha.contiguous(), st.zkey, st.depth_base, st.depth_bits,
                 st.mode)
+        grad_features = None
+        if ctx.n_features:
+            # into the same slab, before the per-gaussian backward reads it: the feature loss's part of d alpha
+            (fpad,) = ctx.saved_tensors
+            with _stage(st, "features_bwd"):
+                gpad = native().fused_render_features_backward(
+                    grad_maps[-1].contiguous(), slab, st.P, st.records, st._ids_sorted, st.ranges, st.n_per_pixel,
+                    st.w_per_pixel, st.masks, st.keys_sorted, st.id_bits, fpad)
+            if ctx.needs_input_grad[4]:
+                grad_features = gpad if gpad.shape[1] == ctx.n_features else gpad[:, :ctx.n_features]
         uv_t = st.uv_ref() if st.uv_ref is not None else None
         if st.mode & native().MODE_ABSGRAD:
             # sum over pixels of |d loss_p / d uv| (rows' slots 10-11), in the compact order of uv; replaced, not
@@ -475,15 +507,16 @@ class _CompositeTiles(torch.autograd.Function):
         watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
         st.uv_grad_emitted = bool(watched)
         if not watched:
-            return None, slab, None, None
+            return None, slab, None, None, grad_features
         # interleaved rows: rgb3 opa | uv2 conic0 conic1 | conic2 pad3 (depth mode: z pad2)
         grad_uv = slab.view(st.N, 12).index_select(0, st.vis_idx)[:, 4:6].contiguous()
-        return grad_uv, slab, None, None
+        return grad_uv, slab, None, None, grad_features
 
 
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
-              render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None):
+              render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
+              features=None):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
@@ -521,7 +554,38 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     importance pruning (AdaptiveDensityControl.prune).  Return values, uv.grad, uv.absgrad and all gradients are
     unchanged and the statistics are not differentiable; combines with render_depth_alpha, antialiased, filter3d,
     absgrad, return_state and grad_out.  A WeightStats of another length raises ValueError (make a new one after
-    densification changes N).  fp32 and precomputed SH colours only."""
+    densification changes N).  fp32 and precomputed SH colours only.
+
+    features: an fp32 CUDA tensor [N, D] (D >= 1, contiguous, on the gaussians' device; it may require grad) of
+    per-gaussian feature vectors to blend with the colour's weights, for feature or semantic distillation,
+    instance channels or rendered normals.  The return tuple gains feature_map [H,W,D] after depth/alpha and before
+    state: (image, culling_mask, uv[, depth, alpha][, feature_map][, state]).  Per pixel feature_map[p, c] =
+    sum_i w_i * F[i, c] over exactly the splats, in exactly the order and with exactly the blend weights w_i = T * alpha
+    (the same floats) as the colour, with no background term (composite with alpha, render_depth_alpha=True, for one).
+    The gradient reaches F (sum_p w_ip * G[p, c], zero for culled gaussians) and, through alpha, opacity and the
+    geometry: uv.grad is the total loss's gradient on the projected means (DESIGN.md 3.17).  Separate tile kernels
+    process the channels in chunks of 4, each chunk walking the tile's pairs again.  The image, mask, uv, depth /
+    alpha, weight statistics and all other gradients are unchanged; combines with render_depth_alpha, antialiased,
+    filter3d, weight_stats, return_state and grad_out, not with absgrad (ValueError).  fp32 and precomputed SH colours
+    only."""
+    if features is not None:
+        if not torch.is_tensor(features):
+            raise TypeError("features must be a torch tensor [N, D]")
+        if gaussians.xyz.dtype != torch.float32:
+            raise TypeError("features needs fp32 inputs (the fused rasterizer's tile kernels blend them)")
+        if gaussians.sh is not None and not use_sh_precompute:
+            raise ValueError("features needs use_sh_precompute=True (per-pixel SH colours are not supported)")
+        if features.dtype != torch.float32:
+            raise TypeError(f"features must be float32, got {features.dtype}")
+        n = gaussians.xyz.shape[0]
+        if features.dim() != 2 or features.shape[0] != n or features.shape[1] < 1:
+            raise ValueError(f"features has shape {tuple(features.shape)} but must be [{n}, D] with D >= 1 (one row "
+                             "per gaussian)")
+        if features.device != gaussians.xyz.device or not features.is_contiguous():
+            raise ValueError("features must be contiguous and on the gaussians' device")
+        if absgrad:
+            raise ValueError("absgrad with features is not supported: the per-pixel |d loss / d uv| cannot be "
+                             "split across the colour and the feature kernels")
     if weight_stats is not None:
         if gaussians.xyz.dtype != torch.float32:
             raise TypeError("weight_stats needs fp32 inputs (the fused rasterizer's render forward accumulates them)")
@@ -582,8 +646,8 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
         camera_T_world.contiguous(), camera.K.contiguous(), state, cfg)
     state.uv_ref = weakref.ref(uv)
     culling_mask = state.visible == 0
-    outs = _CompositeTiles.apply(uv, carrier, state.background, state)
-    image, maps = (outs[0], outs[1:]) if render_depth_alpha else (outs, ())
+    outs = _CompositeTiles.apply(uv, carrier, state.background, state, features)
+    image, maps = (outs[0], outs[1:]) if isinstance(outs, tuple) else (outs, ())
     result = (image, culling_mask, uv, *maps)
     return (*result, state) if return_state else result
 
