@@ -8,6 +8,7 @@ Drop-in for the rasterization path of joeyan/gaussian_splatting:
     reference's own ``splat_py`` package runs on it unmodified.
   * ``gaussian_splatting_b200.rasterize.rasterize`` — same signature and return values as
     ``splat_py.rasterize.rasterize`` (splat_py/rasterize.py:18-112), fused implementation.
+  * ``gaussian_splatting_b200.rasterize_batch`` — C cameras of one scene in one fused forward and backward.
   * ``cuda_autograd_functions`` / ``tile_culling`` / ``structs`` / ``utils`` / ``depth`` — host-side
     mirror of the reference modules of the same names.
 
@@ -33,7 +34,7 @@ def native():
 
         path = ext_path()
         if not path.exists() or not all((_PKG / lib).exists() for lib in ("libgsr_b200.so", "libgsr_selective_adam.so",
-                                                                    "libgsr_features.so")):
+                                                                    "libgsr_features.so", "libgsr_batch.so")):
             raise ImportError(
                 f"gaussian_splatting_b200 native code is not built ({path} missing); "
                 "run `python -m gaussian_splatting_b200.build` (needs nvcc, sm_90a)"
@@ -54,6 +55,10 @@ def install_as_splat_cuda():
 def __getattr__(name):
     if name == "splat_cuda":
         return native()
+    if name == "rasterize_batch":
+        from .rasterize import rasterize_batch
+
+        return rasterize_batch
     raise AttributeError(name)
 
 

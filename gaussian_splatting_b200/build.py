@@ -3,9 +3,10 @@
   libgsr_b200.so            CUDA kernels + C ABI (include/gsr_b200.h), nvcc, sm_90a only, no torch
   libgsr_selective_adam.so  the visibility-masked Adam step (include/gsr_selective_adam.h), same flags
   libgsr_features.so        the feature-channel tile kernels (include/gsr_features.h), same flags
+  libgsr_batch.so           the multi-view per-gaussian kernels of rasterize_batch (include/gsr_batch.h), same flags
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all four; `build(force=False)` is incremental.
+`python -m gaussian_splatting_b200.build` builds all five; `build(force=False)` is incremental.
 """
 from __future__ import annotations
 
@@ -25,6 +26,7 @@ EXT_DIR = PKG / "_ext"
 LIB = PKG / "libgsr_b200.so"
 SELECTIVE_LIB = PKG / "libgsr_selective_adam.so"
 FEATURES_LIB = PKG / "libgsr_features.so"
+BATCH_LIB = PKG / "libgsr_batch.so"
 
 CU_SOURCES = [
     "gsr_pergaussian.cu",
@@ -45,6 +47,7 @@ HEADERS = [
     CSRC / "gsr_record.cuh",
     CSRC / "gsr_f32x2.cuh",
     CSRC / "gsr_tile_walk.cuh",
+    CSRC / "gsr_preprocess.cuh",
     ROOT / "include" / "gsr_b200.h",
 ]
 # A library of its own, so that libgsr_b200.so keeps exactly its kernels (and their SASS).
@@ -54,6 +57,9 @@ SELECTIVE_HEADERS = [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h",
 FEATURES_SOURCES = ["gsr_features.cu"]
 FEATURES_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [ROOT / "include" / "gsr_b200.h",
                                                                   ROOT / "include" / "gsr_features.h"]
+BATCH_SOURCES = ["gsr_batch.cu"]
+BATCH_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [ROOT / "include" / "gsr_b200.h",
+                                                               ROOT / "include" / "gsr_batch.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -126,6 +132,10 @@ def build_features_lib(force: bool = False, verbose: bool = False) -> Path:
     return _build_cuda_lib(FEATURES_LIB, FEATURES_SOURCES, FEATURES_HEADERS, "features_lib.sha256", force, verbose)
 
 
+def build_batch_lib(force: bool = False, verbose: bool = False) -> Path:
+    return _build_cuda_lib(BATCH_LIB, BATCH_SOURCES, BATCH_HEADERS, "batch_lib.sha256", force, verbose)
+
+
 def build_ext(force: bool = False) -> Path:
     import torch  # noqa: F401  (needed for include/library paths)
     from torch.utils import cpp_extension as ce
@@ -136,7 +146,7 @@ def build_ext(force: bool = False) -> Path:
     src = CSRC / "splat_cuda_module.cpp"
     stamp = OBJ / "ext.sha256"
     want = _digest([src, ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h",
-                    ROOT / "include" / "gsr_features.h"], torch.__version__)
+                    ROOT / "include" / "gsr_features.h", ROOT / "include" / "gsr_batch.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -147,7 +157,7 @@ def build_ext(force: bool = False) -> Path:
         "-DTORCH_EXTENSION_NAME=splat_cuda", "-DTORCH_API_INCLUDE_EXTENSION_H",
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
-        f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
+        f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",
     ]
@@ -169,6 +179,7 @@ def build(force: bool = False, verbose: bool = False):
     lib = build_lib(force=force, verbose=verbose)
     build_selective_lib(force=force, verbose=verbose)
     build_features_lib(force=force, verbose=verbose)
+    build_batch_lib(force=force, verbose=verbose)
     ext = build_ext(force=force)
     return lib, ext
 

@@ -13,6 +13,7 @@
 #include "../../include/gsr_b200.h"
 #include "../../include/gsr_selective_adam.h"
 #include "../../include/gsr_features.h"
+#include "../../include/gsr_batch.h"
 
 namespace {
 
@@ -799,6 +800,221 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
     return out;
 }
 
+// ---------------------------------------------------------------------------------------------
+// multi-view fused path (rasterize_batch): C views of one scene, per-view arrays stacked view-major
+// ---------------------------------------------------------------------------------------------
+static int64_t check_views(const torch::Tensor& camera_T_world, const torch::Tensor& K) {
+    CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
+    CHECK_FLOAT_TENSOR(camera_T_world); CHECK_FLOAT_TENSOR(K);
+    const int64_t C = camera_T_world.size(0);
+    TORCH_CHECK(camera_T_world.dim() == 3 && C >= 1 && camera_T_world.size(1) == 4 && camera_T_world.size(2) == 4,
+                "camera_T_world must have shape Cx4x4, C >= 1");
+    TORCH_CHECK(K.dim() == 3 && K.size(0) == C && K.size(1) == 3 && K.size(2) == 3, "K must have shape Cx3x3");
+    return C;
+}
+
+// fused_preprocess_forward of every view into stacked outputs: [records [C,N,12], depth_key [C,N], visible [C,N],
+// scan [C,N] (each view's own packed inclusive scan), tile_mask [C,N], tile_win [C,N]].  xyz_camera_frame [C,R,3]:
+// camera-frame positions of the LAST R gaussians of every view; camera_centre [C,3].
+std::vector<torch::Tensor> batch_preprocess_forward(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
+    c10::optional<torch::Tensor> filter3d) {
+    CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
+    CHECK_VALID_INPUT(rgb_dc);
+    CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
+    CHECK_FLOAT_TENSOR(opacity_logit); CHECK_FLOAT_TENSOR(rgb_dc);
+    const int64_t C = check_views(camera_T_world, K);
+    const int N = xyz.size(0);
+    TORCH_CHECK(xyz.dim() == 2 && xyz.size(1) == 3, "xyz must have shape Nx3");
+    TORCH_CHECK(quaternion.size(0) == N && quaternion.size(1) == 4, "quaternion must have shape Nx4");
+    TORCH_CHECK(scale.size(0) == N && scale.size(1) == 3, "scale must have shape Nx3");
+    TORCH_CHECK(opacity_logit.numel() == N, "opacity must have shape Nx1");
+    TORCH_CHECK(rgb_dc.size(0) == N && rgb_dc.size(1) == 3, "rgb must have shape Nx3");
+    const float* cam_ptr = nullptr;
+    int64_t R = 0;
+    if (xyz_camera_frame.has_value()) {
+        const torch::Tensor& pc = *xyz_camera_frame;
+        CHECK_VALID_INPUT(pc); CHECK_FLOAT_TENSOR(pc);
+        TORCH_CHECK(pc.dim() == 3 && pc.size(0) == C && pc.size(1) <= N && pc.size(2) == 3,
+                    "xyz_camera_frame must have shape CxRx3, R <= N");
+        cam_ptr = pc.data_ptr<float>();
+        R = pc.size(1);
+    }
+    const float* centre_ptr = nullptr;
+    if (camera_centre.has_value()) {
+        CHECK_VALID_INPUT((*camera_centre)); CHECK_FLOAT_TENSOR((*camera_centre));
+        TORCH_CHECK(camera_centre->numel() == 3 * C, "camera_centre must have shape Cx3");
+        centre_ptr = camera_centre->data_ptr<float>();
+    }
+    int n_rest = 0;
+    const float* sh_ptr = nullptr;
+    if (sh_rest.has_value()) {
+        const torch::Tensor& sh = *sh_rest;
+        CHECK_VALID_INPUT(sh); CHECK_FLOAT_TENSOR(sh);
+        TORCH_CHECK(sh.dim() == 3 && sh.size(0) == N && sh.size(1) == 3, "sh must have shape Nx3xK");
+        n_rest = sh.size(2);
+        TORCH_CHECK(n_rest == 3 || n_rest == 8 || n_rest == 15, "sh must hold 3, 8 or 15 coefficients per channel");
+        sh_ptr = sh.data_ptr<float>();
+    }
+    c10::cuda::CUDAGuard guard(xyz.device());
+    auto opt = xyz.options();
+    torch::Tensor records = torch::empty({C, N, GSR_REC_FLOATS}, opt);
+    torch::Tensor zkey = torch::empty({C, N}, opt.dtype(torch::kInt32));
+    torch::Tensor visible = torch::empty({C, N}, opt.dtype(torch::kUInt8));
+    torch::Tensor scan = torch::empty({C, N}, opt.dtype(torch::kInt64));
+    torch::Tensor tile_mask = torch::empty({C, N}, opt.dtype(torch::kInt64));
+    torch::Tensor tile_win = torch::empty({C, N}, opt.dtype(torch::kInt32));
+    const size_t tb = gsr_preprocess_temp_bytes(N);
+    torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
+    const float* f3d = filter3d_ptr(filter3d, N);
+    for (int64_t c = 0; c < C && N > 0; ++c) {
+        check_rc(gsr_preprocess_forward(
+                     (int)mode, N, n_rest, F32PTR(xyz), cam_ptr ? cam_ptr + c * R * 3 : nullptr, N - (int)R,
+                     F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(rgb_dc), sh_ptr,
+                     F32PTR(camera_T_world) + 16 * c, F32PTR(K) + 9 * c, centre_ptr ? centre_ptr + 3 * c : nullptr,
+                     (int)H, (int)W, (float)near_thresh, (float)far_thresh, (float)cull_mask_padding, (float)mh_dist,
+                     (uint32_t)depth_base, F32PTR(records[c]), (uint32_t*)zkey[c].data_ptr<int>(),
+                     visible[c].data_ptr<uint8_t>(), (uint64_t*)scan[c].data_ptr<int64_t>(),
+                     (uint64_t*)tile_mask[c].data_ptr<int64_t>(), (uint32_t*)tile_win[c].data_ptr<int>(),
+                     temp.data_ptr(), tb, cur_stream()),
+                 "gsr_preprocess_forward");
+    }
+    return {records, zkey, visible, scan, tile_mask, tile_win};
+}
+
+// fused_render_backward of every view into one stacked slab [C, N*12]: grad_image [C,H,W,3], per view the forward's
+// pair list (keys_sorted or ids_sorted, the other one empty), ranges, n, w and masks (empty: none); records [C,N,12],
+// background [C,3]; with grad_depth / grad_alpha [C,H,W,1] also depth_key [C,N].
+torch::Tensor batch_render_backward(torch::Tensor grad_image, int64_t N, std::vector<int64_t> P, torch::Tensor records,
+                                    std::vector<torch::Tensor> ids_sorted, std::vector<torch::Tensor> keys_sorted,
+                                    std::vector<int64_t> id_bits, std::vector<torch::Tensor> ranges,
+                                    torch::Tensor background, std::vector<torch::Tensor> n,
+                                    std::vector<torch::Tensor> w, std::vector<torch::Tensor> masks,
+                                    c10::optional<torch::Tensor> grad_depth, c10::optional<torch::Tensor> grad_alpha,
+                                    c10::optional<torch::Tensor> depth_key, int64_t depth_base, int64_t depth_bits,
+                                    int64_t mode) {
+    CHECK_VALID_INPUT(grad_image); CHECK_FLOAT_TENSOR(grad_image);
+    CHECK_VALID_INPUT(records); CHECK_FLOAT_TENSOR(records);
+    CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
+    const int64_t C = (int64_t)P.size();
+    TORCH_CHECK(C >= 1 && (int64_t)ids_sorted.size() == C && (int64_t)keys_sorted.size() == C &&
+                    (int64_t)id_bits.size() == C && (int64_t)ranges.size() == C && (int64_t)n.size() == C &&
+                    (int64_t)w.size() == C && (int64_t)masks.size() == C,
+                "every per-view list must hold C >= 1 entries");
+    const int H = n[0].size(0), W = n[0].size(1);
+    TORCH_CHECK(grad_image.dim() == 4 && grad_image.size(0) == C && grad_image.size(1) == H &&
+                    grad_image.size(2) == W && grad_image.size(3) == 3,
+                "grad_image must be CxHxWx3");
+    TORCH_CHECK(records.numel() == C * N * (int64_t)GSR_REC_FLOATS, "records must have shape CxNx12");
+    TORCH_CHECK(background.numel() == 3 * C, "background must have shape Cx3");
+    const bool depth = grad_depth.has_value();
+    if (depth) {
+        TORCH_CHECK(grad_alpha.has_value() && depth_key.has_value(),
+                    "the depth/alpha backward needs grad_alpha and depth_key");
+        CHECK_VALID_INPUT((*grad_depth)); CHECK_FLOAT_TENSOR((*grad_depth));
+        CHECK_VALID_INPUT((*grad_alpha)); CHECK_FLOAT_TENSOR((*grad_alpha));
+        CHECK_VALID_INPUT((*depth_key));
+        TORCH_CHECK(grad_depth->numel() == C * H * W && grad_alpha->numel() == C * H * W,
+                    "grad_depth and grad_alpha must hold C*H*W values");
+        TORCH_CHECK(depth_key->numel() == C * N, "depth_key must have shape CxN");
+    }
+    c10::cuda::CUDAGuard guard(grad_image.device());
+    torch::Tensor slab = torch::zeros({C, N * (int64_t)GSR_GRAD_ROW_FLOATS}, grad_image.options());
+    const int64_t HW = (int64_t)H * W;
+    for (int64_t c = 0; c < C && N > 0; ++c) {
+        TORCH_CHECK(n[c].size(0) == H && n[c].size(1) == W, "every view must have the same image size");
+        const uint32_t* mptr = masks[c].numel() > 0 ? (const uint32_t*)masks[c].data_ptr<int>() : nullptr;
+        const PairSource ps = pair_source(keys_sorted[c], ids_sorted[c], P[c]);
+        check_rc(gsr_render_backward_gather(
+                     (int)mode, F32PTR(records) + c * N * GSR_REC_FLOATS, ps.keys, (int)id_bits[c], ps.ids,
+                     depth ? (const uint32_t*)depth_key->data_ptr<int>() + c * N : nullptr, (uint32_t)depth_base,
+                     (int)depth_bits, ranges[c].data_ptr<int>(), F32PTR(background) + 3 * c, H, W,
+                     n[c].data_ptr<int>(), F32PTR(w[c]), F32PTR(grad_image) + c * HW * 3,
+                     depth ? F32PTR((*grad_depth)) + c * HW : nullptr, depth ? F32PTR((*grad_alpha)) + c * HW : nullptr,
+                     nullptr, nullptr, nullptr, nullptr, F32PTR(slab[c]), mptr, cur_stream()),
+                 "gsr_render_backward_gather");
+    }
+    return slab;
+}
+
+// the per-gaussian backward of C views in one pass (gsr_batch_preprocess_backward): slab [C, N*12] of
+// batch_render_backward, visible / scan [C,N] of batch_preprocess_forward, grad_uv_compact [sum M_c, 2] (optional).
+// Same outputs and flat layout as fused_preprocess_backward, holding the gradient summed over the views.
+std::vector<torch::Tensor> batch_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
+                                                     torch::Tensor scale, torch::Tensor opacity_logit,
+                                                     c10::optional<torch::Tensor> sh_rest,
+                                                     torch::Tensor camera_T_world, torch::Tensor K,
+                                                     c10::optional<torch::Tensor> camera_centre,
+                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+                                                     c10::optional<torch::Tensor> grad_uv_compact,
+                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
+                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
+    CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
+    CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
+    CHECK_VALID_INPUT(visible);
+    const int64_t C = check_views(camera_T_world, K);
+    const int64_t N = xyz.size(0);
+    TORCH_CHECK(slab.numel() == C * N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold C*N*",
+                GSR_GRAD_ROW_FLOATS, " floats");
+    TORCH_CHECK(visible.numel() == C * N && visible.scalar_type() == torch::kUInt8, "visible must be a CxN uint8 tensor");
+    const float* centre_ptr = nullptr;
+    if (camera_centre.has_value()) {
+        CHECK_VALID_INPUT((*camera_centre)); CHECK_FLOAT_TENSOR((*camera_centre));
+        TORCH_CHECK(camera_centre->numel() == 3 * C, "camera_centre must have shape Cx3");
+        centre_ptr = camera_centre->data_ptr<float>();
+    }
+    c10::cuda::CUDAGuard guard(xyz.device());
+    auto opt = xyz.options();
+    const int n_rest = sh_rest.has_value() ? (int)sh_rest->size(2) : 0;
+    const float* g_uv_compact = nullptr;
+    const uint64_t* scan_ptr = nullptr;
+    if (grad_uv_compact.has_value() && grad_uv_compact->numel() > 0) {
+        CHECK_VALID_INPUT((*grad_uv_compact)); CHECK_FLOAT_TENSOR((*grad_uv_compact));
+        TORCH_CHECK(scan.has_value() && scan->numel() == C * N && scan->scalar_type() == torch::kInt64,
+                    "grad_uv_compact needs the packed scans of the forward pass");
+        CHECK_VALID_INPUT((*scan));
+        TORCH_CHECK(grad_uv_compact->dim() == 2 && grad_uv_compact->size(1) == 2, "grad_uv_compact must be Mx2");
+        g_uv_compact = grad_uv_compact->data_ptr<float>();
+        scan_ptr = (const uint64_t*)scan->data_ptr<int64_t>();
+    }
+    const int64_t widths[6] = {3, 4, 3, 1, 3, 3 * (int64_t)n_rest};
+    int64_t offs[7];
+    offs[0] = 0;
+    for (int i = 0; i < 6; ++i) offs[i + 1] = (offs[i] + N * widths[i] + 3) & ~(int64_t)3;
+    torch::Tensor flat;
+    if (out_flat.has_value()) {
+        flat = *out_flat;
+        CHECK_VALID_INPUT(flat); CHECK_FLOAT_TENSOR(flat);
+        TORCH_CHECK(flat.numel() == offs[6], "out_flat must hold ", offs[6], " floats");
+        TORCH_CHECK((reinterpret_cast<uintptr_t>(flat.data_ptr()) & 15u) == 0, "out_flat must be 16-byte aligned");
+    } else {
+        flat = torch::empty({offs[6]}, opt);
+    }
+    for (int i = 0; i < 6; ++i)
+        if (offs[i + 1] > offs[i] + N * widths[i]) flat.narrow(0, offs[i] + N * widths[i], offs[i + 1] - offs[i] - N * widths[i]).zero_();
+    auto section = [&](int i, std::vector<int64_t> shape) {
+        return flat.narrow(0, offs[i], N * widths[i]).view(shape);
+    };
+    torch::Tensor o_xyz = section(0, {N, 3}), o_q = section(1, {N, 4}), o_s = section(2, {N, 3}),
+                  o_o = section(3, {N}), o_dc = section(4, {N, 3});
+    torch::Tensor g_sh;
+    if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
+    const float* f3d = filter3d_ptr(filter3d, N);
+    check_rc(gsr_batch_preprocess_backward((int)mode, (int)C, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion),
+                                           F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(camera_T_world), F32PTR(K),
+                                           centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab), use_slab_uv ? 1 : 0,
+                                           g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s),
+                                           F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr, cur_stream()),
+             "gsr_batch_preprocess_backward");
+    std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
+    if (n_rest) out.push_back(g_sh);
+    out.push_back(flat);
+    return out;
+}
+
 // Mip-Splatting's 3-D filter size per gaussian (gsr_filter3d): xyz [N,3], camera_T_world [C,4,4], K [C,3,3],
 // width / height int32 [C], all on xyz's device -> filter3d [N]
 torch::Tensor filter3d(torch::Tensor xyz, torch::Tensor camera_T_world, torch::Tensor K, torch::Tensor width,
@@ -1241,6 +1457,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"), py::arg("camera_centre"), py::arg("visible"),
           py::arg("out_flat"), py::arg("grad_uv_compact"), py::arg("scan"), py::arg("use_slab_uv"), py::arg("mode"),
           py::arg("filter3d") = py::none());
+    m.def("batch_preprocess_forward", &batch_preprocess_forward,
+          "per-gaussian forward of C views into stacked records / keys / visibility / scans (rasterize_batch)");
+    m.def("batch_render_backward", &batch_render_backward,
+          "render backward of C views into one stacked gradient slab [C, N*12]");
+    m.def("batch_preprocess_backward", &batch_preprocess_backward,
+          "per-gaussian backward of C views in one pass: the gradient summed over the views (gsr_batch)");
     m.def("filter3d", &filter3d, "Mip-Splatting's 3-D filter size per gaussian from the training cameras (gsr_filter3d)",
           py::arg("xyz"), py::arg("camera_T_world"), py::arg("K"), py::arg("width"), py::arg("height"),
           py::arg("near"), py::arg("margin"), py::arg("variance"));

@@ -695,3 +695,301 @@ def rasterize_unfused(gaussians, camera_T_world, camera, near_thresh, far_thresh
     image = RenderImage.apply(render_rgb, s.opacity, s.uv, s.conic, rays, s.tile_ranges, s.sorted_idx,
                               (camera.height, camera.width), background_rgb)
     return image, s.culling_mask, s.uv
+
+
+# ---- multi-view: C cameras of one scene in one call ------------------------------------------------------------------
+class _BatchView:
+    """What one view of a rasterize_batch call exposes (state.views[c]): the fields DensificationStats.accumulate
+    reads (vis_idx32, uv_absgrad, N, M) and the view's pair list."""
+
+    __slots__ = ("N", "M", "P", "vis_idx", "vis_idx32", "uv_absgrad", "ranges", "keys_sorted", "_ids_sorted", "id_bits",
+                 "n_per_pixel", "w_per_pixel", "masks")
+
+    ids_sorted = _ViewState.ids_sorted
+
+    def __init__(self):
+        self.uv_absgrad = None
+
+
+class _BatchState:
+    """Non-differentiable buffers of a rasterize_batch call shared by its two autograd nodes; per-view arrays are
+    stacked view-major ([C, N, ...])."""
+
+    def __init__(self, profile=None):
+        self.profile = profile
+        self.grad_flat = None    # set by the backward pass: the gradient summed over the views (flat layout)
+        self.grad_out = None
+        self.uv_refs = None      # weak references to the C uv tensors handed to the caller
+        self.uv_grad_emitted = False
+        self.speculation_overflowed = False
+        self.mode = 0
+        self.filter3d = None
+        self.views = []
+        self.images = self.depth = self.alpha = None
+
+
+class _ProjectBatch(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg):
+        ext = native()
+        H, W, near, far, pad, mh = cfg
+        C, N = camera_T_world.shape[0], xyz.shape[0]
+        depth_base, depth_bits = _depth_key_params(near, far)
+        opacity_flat = opacity.reshape(-1)
+        # per view exactly the camera-frame positions and camera centre rasterize() forms (DESIGN.md 4)
+        if IN_KERNEL_TRANSFORM and N >= IN_KERNEL_TRANSFORM_MIN_N and in_kernel_transform_ok(xyz.device):
+            tails = [tail_positions(xyz, camera_T_world[c]) for c in range(C)]
+            xyz_cam = None if tails[0] is None else torch.stack(tails)
+        else:
+            xyz_cam = torch.stack([transform_points_torch(xyz, camera_T_world[c]) for c in range(C)])
+        centre = None
+        if sh is not None:
+            if native_centre_ok(xyz.device):
+                centre = torch.stack([ext.camera_centre(camera_T_world[c]) for c in range(C)])
+            else:
+                centre = torch.stack([torch.linalg.inv_ex(camera_T_world[c])[0][:3, 3] for c in range(C)])
+        with _stage(state, "preprocess_fwd"):
+            records, zkey, visible, scan, tile_mask, tile_win = ext.batch_preprocess_forward(
+                xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
+                pad, mh, depth_base, state.mode, state.filter3d)
+        record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])
+        background = state.background
+        depth_mode = bool(state.mode & ext.MODE_DEPTH_ALPHA)
+
+        def counts(totals):
+            Ms, Ps = [t >> 32 for t in totals], [t & 0xFFFFFFFF for t in totals]
+            # the native entry points index pairs with int32: the batch's pairs, over all views, must stay below 2^31
+            if any(m > N for m in Ms) or sum(Ps) >= 2**31:
+                raise RuntimeError(f"rasterize_batch: {sum(Ps)} (gaussian, tile) pairs over {C} views exceed the int32 "
+                                   "pair index of the native path (the batch's P must be < 2^31)")
+            return Ms, Ps
+
+        def bin_and_render(c, M_, P_, speculative):
+            with _stage(state, "bin_sort_gather"):
+                binned = ext.fused_bin(records[c], zkey[c], visible[c], scan[c], M_, P_, H, W, mh, depth_bits,
+                                       speculative, tile_mask[c] if USE_TILE_MASKS else None,
+                                       tile_win[c] if USE_TILE_MASKS else None)
+            with _stage(state, "render_fwd"):
+                rendered = ext.fused_render_forward(records[c], binned[1], background[c], H, W, P_, record_masks,
+                                                    binned[4], binned[0], binned[5], zkey[c] if depth_mode else None,
+                                                    depth_base, depth_bits)
+            return binned, rendered
+
+        # One host read for the whole batch: every view's pair buffers are sized from the recent views of this
+        # (N, H, W, C) and enqueued, and only then the C (M, P) totals, copied together to pinned memory on a side
+        # stream right behind the scans, are read (DESIGN.md 3.5 and 3.18).  Views that overflowed their guess run
+        # again with exact sizes.
+        key = (xyz.device.index, N, H, W, C)
+        cap = _pair_capacity(key) if (SPECULATIVE_BINNING and N > 0) else None
+        out = [None] * C
+        if N == 0:
+            Ms, Ps = [0] * C, [0] * C
+            out = [bin_and_render(c, 0, 0, False) for c in range(C)]
+        elif cap is None:
+            Ms, Ps = counts(scan[:, -1].tolist())
+            out = [bin_and_render(c, Ms[c], Ps[c], False) for c in range(C)]
+        else:
+            totals = scan[:, -1].contiguous()
+            slot = torch.empty(C, dtype=torch.int64, pin_memory=True)
+            side = _side_stream(xyz.device)
+            scanned = torch.cuda.Event()
+            scanned.record()
+            with torch.cuda.stream(side):
+                side.wait_event(scanned)
+                slot.copy_(totals, non_blocking=True)
+                ready = torch.cuda.Event()
+                ready.record(side)
+            totals.record_stream(side)
+            out = [bin_and_render(c, N, cap, True) for c in range(C)]
+            ready.synchronize()
+            Ms, Ps = counts(slot.tolist())
+            for c in range(C):
+                if Ps[c] > cap:
+                    out[c] = bin_and_render(c, Ms[c], Ps[c], False)
+                    state.speculation_overflowed = True
+                else:
+                    (ids_c, ranges_c, vis_c, uv_c, keys_c, idb), rendered = out[c]
+                    out[c] = ((ids_c.narrow(0, 0, Ps[c]) if ids_c.numel() else ids_c, ranges_c,
+                               vis_c.narrow(0, 0, Ms[c]), uv_c.narrow(0, 0, Ms[c]), keys_c, idb), rendered)
+        for P_ in Ps:
+            _note_pairs(key, P_)
+        views, uvs = [], []
+        for c in range(C):
+            (ids_sorted, ranges, vis_idx, uv, keys_sorted, id_bits), rendered = out[c]
+            v = _BatchView()
+            v.N, v.M, v.P = N, Ms[c], Ps[c]
+            v.vis_idx = v.vis_idx32 = vis_idx
+            v._ids_sorted, v.ranges, v.keys_sorted, v.id_bits = ids_sorted, ranges, keys_sorted, int(id_bits)
+            _, v.n_per_pixel, v.w_per_pixel, v.masks, _, _ = rendered
+            views.append(v)
+            uvs.append(uv)
+        state.images = torch.stack([o[1][0] for o in out])
+        if depth_mode:
+            state.depth = torch.stack([o[1][4] for o in out])
+            state.alpha = torch.stack([o[1][5] for o in out])
+        state.views, state.C, state.N, state.H, state.W = views, C, N, H, W
+        state.records, state.zkey, state.visible, state.scan = records, zkey, visible, scan
+        state.depth_base, state.depth_bits = depth_base, depth_bits
+        uv_all = torch.cat(uvs) if C > 1 else uvs[0].contiguous()
+        carrier = torch.empty(C * 12 * N, dtype=xyz.dtype, device=xyz.device)
+        ctx.state = state
+        ctx.has_sh = sh is not None
+        ctx.save_for_backward(xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre)
+        return uv_all, carrier
+
+    @staticmethod
+    def backward(ctx, grad_uv, grad_carrier):
+        xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre = ctx.saved_tensors
+        st = ctx.state
+        C, N = st.C, st.N
+        if grad_carrier is None:
+            grad_carrier = torch.zeros(C * 12 * N, dtype=xyz.dtype, device=xyz.device)
+        slab = grad_carrier.contiguous()
+        # as in _ProjectGaussians.backward: the uv gradient is either only what the caller added on the uvs (added to
+        # the rows' uv sums) or the total (it replaces them); view c's rows of the compact uv follow views 0..c-1
+        guv = None
+        if grad_uv is not None and grad_uv.shape[0] > 0:
+            guv = grad_uv.contiguous()
+        with _stage(st, "preprocess_bwd"):
+            grads = native().batch_preprocess_backward(slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world,
+                                                       K, centre, st.visible, st.grad_out, guv,
+                                                       st.scan if guv is not None else None, not st.uv_grad_emitted,
+                                                       st.mode, st.filter3d)
+        g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
+        g_sh = grads[5] if ctx.has_sh else None
+        st.grad_flat = grads[-1]
+        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, None, None, None, None
+
+
+class _CompositeBatch(torch.autograd.Function):
+    """carrier, uv_0 .. uv_{C-1} -> images [C,H,W,3], or (images, depth, alpha) [C,H,W,1] each.  The per-view uvs
+    (views of the projection node's compact uv) are the inputs, so that their .grad is the render pass's gradient."""
+
+    @staticmethod
+    def forward(ctx, carrier, background_rgb, state, *uvs):
+        outs = (state.images,) if state.depth is None else (state.images, state.depth, state.alpha)
+        state.images = state.depth = state.alpha = None
+        ctx.state = state
+        return outs if len(outs) > 1 else outs[0]
+
+    @staticmethod
+    def backward(ctx, grad_images, *grad_maps):
+        ext = native()
+        st = ctx.state
+        grad_depth = grad_alpha = None
+        if st.mode & ext.MODE_DEPTH_ALPHA:
+            grad_depth, grad_alpha = grad_maps[:2]
+        vs = st.views
+        empty = torch.empty(0, dtype=torch.int64, device=grad_images.device)
+        with _stage(st, "render_bwd"):
+            slab = ext.batch_render_backward(
+                grad_images.contiguous(), st.N, [v.P for v in vs], st.records,
+                [v._ids_sorted for v in vs], [v.keys_sorted if v.keys_sorted is not None else empty for v in vs],
+                [v.id_bits for v in vs], [v.ranges for v in vs], st.background, [v.n_per_pixel for v in vs],
+                [v.w_per_pixel for v in vs], [v.masks for v in vs],
+                None if grad_depth is None else grad_depth.contiguous(),
+                None if grad_alpha is None else grad_alpha.contiguous(), st.zkey, st.depth_base, st.depth_bits,
+                st.mode)
+        rows = slab.view(st.C, st.N, 12)
+        uvs = [r() for r in st.uv_refs] if st.uv_refs is not None else [None] * st.C
+        if st.mode & ext.MODE_ABSGRAD:
+            for c, v in enumerate(vs):
+                v.uv_absgrad = rows[c][:, 10:12].index_select(0, v.vis_idx)
+                if uvs[c] is not None:
+                    uvs[c].absgrad = v.uv_absgrad
+        watched = any(u is None or u.retains_grad or bool(u._backward_hooks) for u in uvs)
+        st.uv_grad_emitted = bool(watched)
+        if not watched:
+            return (slab.view(-1), None, None) + (None,) * st.C
+        return (slab.view(-1), None, None) + tuple(rows[c].index_select(0, v.vis_idx)[:, 4:6].contiguous()
+                                                   for c, v in enumerate(vs))
+
+
+def _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, background_rgb, filter3d, weight_stats,
+                      features):
+    xyz = gaussians.xyz
+    if weight_stats is not None:
+        raise ValueError("weight_stats is not supported by rasterize_batch: use rasterize per view")
+    if features is not None:
+        raise ValueError("features is not supported by rasterize_batch: use rasterize per view")
+    if gaussians.sh is not None and not use_sh_precompute:
+        raise ValueError("rasterize_batch needs use_sh_precompute=True (per-pixel SH colours are not supported)")
+    if xyz.dtype != torch.float32:
+        raise TypeError("rasterize_batch is fp32 (the fused rasterizer); use rasterize_unfused per view for float64")
+    if not torch.is_tensor(camera_T_world) or camera_T_world.dim() != 3 or tuple(camera_T_world.shape[1:]) != (4, 4) \
+            or camera_T_world.shape[0] < 1:
+        raise ValueError("camera_T_world must be a [C,4,4] tensor with C >= 1")
+    C = camera_T_world.shape[0]
+    K = camera.K
+    if not torch.is_tensor(K) or tuple(K.shape) not in ((3, 3), (C, 3, 3)):
+        raise ValueError(f"camera.K must be [3,3] or [{C},3,3]")
+    if not torch.is_tensor(background_rgb) or tuple(background_rgb.shape) not in ((3,), (C, 3)):
+        raise ValueError(f"background_rgb must be [3] or [{C},3]")
+    for name, t in (("camera_T_world", camera_T_world), ("camera.K", K), ("background_rgb", background_rgb)):
+        if t.dtype != torch.float32:
+            raise TypeError(f"{name} must be float32, got {t.dtype}")
+        if t.device != xyz.device:
+            raise ValueError(f"{name} must be on the gaussians' device")
+    if filter3d is not None:
+        if filter3d.requires_grad:
+            raise ValueError("filter3d is a constant of the scene (no gradient flows to it): pass filter3d.detach()")
+        if filter3d.dtype != torch.float32:
+            raise TypeError(f"filter3d must be float32, got {filter3d.dtype}")
+        n = xyz.shape[0]
+        if not (tuple(filter3d.shape) in ((n,), (n, 1))):
+            raise ValueError(f"filter3d has shape {tuple(filter3d.shape)} but there are {n} gaussians: recompute it "
+                             "(compute_filter3d) after densification changes the gaussians")
+    return C
+
+
+def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
+                    use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
+                    render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
+                    features=None):
+    """C cameras of one scene in one call: rasterize()'s nine positional arguments with camera_T_world [C,4,4]
+    (C >= 1), camera.K [3,3] (shared) or [C,3,3], camera.height / width shared, background_rgb [3] or [C,3].
+
+    Returns (images [C,H,W,3], culling_mask [C,N] bool, uvs[, depth [C,H,W,1], alpha [C,H,W,1]][, state]).  uvs is a
+    tuple of C tensors [M_c,2], views of one compact tensor in view order; uvs[c].retain_grad() gives uvs[c].grad
+    after backward, and with absgrad=True uvs[c].absgrad is set, as rasterize() does for its uv.
+
+    Forward: view c is bit-identical to rasterize(gaussians, camera_T_world[c], K_c, ..., background_c) with the same
+    flags (image, mask, uv, depth / alpha): every view gets exactly the single-view camera-frame positions, camera
+    centre, depth keys, pair list and tile kernels.  Backward: one gradient for the batch, the sum over the views of
+    each view's parameter gradient, added per gaussian in view order in fp32 (g = g_0; g += g_1; ...), which is what
+    autograd's accumulation over C rasterize() calls gives for the same render-stage rows.  The per-gaussian backward
+    reads the parameters once and writes the gradient once for all views (libgsr_batch.so, DESIGN.md 3.18).  Camera
+    poses and filter3d get no gradient.
+
+    state (return_state=True): state.views[c] has vis_idx32, uv_absgrad, N and M, so that
+    DensificationStats.accumulate(state.views[c], uvs[c], xyz, K_c) works per view; state.grad_flat (or grad_out, a
+    caller-owned buffer of the flat layout) holds the batch's one gradient.
+
+    Supports render_depth_alpha, antialiased, absgrad, filter3d ([N], one filter for all views), return_state,
+    profile and grad_out.  weight_stats and features raise ValueError (use rasterize per view), fp64 inputs
+    TypeError, per-pixel SH (use_sh_precompute=False) ValueError, and so do poses, K or backgrounds of the wrong
+    shape (ValueError), dtype (TypeError) or device (ValueError)."""
+    C = _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, background_rgb, filter3d, weight_stats,
+                          features)
+    ext = native()
+    K = camera.K if camera.K.dim() == 3 else camera.K.expand(C, 3, 3)
+    state = _BatchState(profile)
+    state.grad_out = grad_out
+    state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
+                  | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
+    state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
+    state.background = (background_rgb if background_rgb.dim() == 2 else background_rgb.expand(C, 3)).contiguous()
+    cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
+           float(cull_mask_padding), float(mh_dist))
+    uv_all, carrier = _ProjectBatch.apply(
+        gaussians.xyz.contiguous(), gaussians.quaternion.contiguous(), gaussians.scale.contiguous(),
+        gaussians.opacity.contiguous(), gaussians.rgb.contiguous(),
+        None if gaussians.sh is None else gaussians.sh.contiguous(),
+        camera_T_world.contiguous(), K.contiguous(), state, cfg)
+    uvs = torch.split(uv_all, [v.M for v in state.views])
+    state.uv_refs = [weakref.ref(u) for u in uvs]
+    culling_mask = state.visible == 0
+    outs = _CompositeBatch.apply(carrier, state.background, state, *uvs)
+    images, maps = (outs[0], outs[1:]) if isinstance(outs, tuple) else (outs, ())
+    result = (images, culling_mask, uvs, *maps)
+    return (*result, state) if return_state else result
