@@ -1,0 +1,318 @@
+// gsr_fisheye.cu — the fused per-gaussian stages for fisheye cameras (rasterize(..., fisheye=k), libgsr_fisheye.so).
+//
+// The bodies are the pinhole ones of gsr_preprocess.cuh — forward, single-view backward and batched backward —
+// compiled with the camera-model hooks defined for COLMAP's OPENCV_FISHEYE model (gsr_fisheye.cuh).  Each view's
+// {k1, k2, k3, k4, theta_max} is read into shared memory next to the view constants, by threads 32..36 while threads
+// 0..27 fetch T, K and the camera centre.  The records these kernels write are ordinary records: binning and the
+// tile kernels run unchanged.
+#include <cub/cub.cuh>
+
+#include <cmath>
+
+#include "gsr_fisheye.cuh"
+
+#include "../../include/gsr_fisheye.h"
+
+#define GSR_PROJECTION_HOOKS
+#define GSR_VIEW_PARAM , const float* __restrict__ fisheye
+#define GSR_VIEW_DECL __shared__ float vfe[GSR_FISHEYE_CONSTS];
+#define GSR_LOAD_VIEW(T, K, cam, view)                                                                          \
+    do {                                                                                                        \
+        if (threadIdx.x >= 32 && threadIdx.x < 32 + GSR_FISHEYE_CONSTS)                                         \
+            vfe[threadIdx.x - 32] = fisheye[GSR_FISHEYE_CONSTS * (view) + threadIdx.x - 32];                     \
+        load_view_cta(T, K, cam, vc, HAS_SH); /* ends with a CTA barrier */                                     \
+    } while (0)
+#define GSR_PROJECT(px, py, pz, u, v) \
+    float fe_theta;                   \
+    fisheye_project(px, py, pz, vc.K[0], vc.K[2], vc.K[4], vc.K[5], vfe, u, v, fe_theta)
+#define GSR_CULL_MORE | (fe_theta >= vfe[4])
+#define GSR_JACOBIAN(px, py, pz, J) fisheye_jacobian(px, py, pz, vc.K[0], vc.K[4], vfe, J)
+#define GSR_JACOBIAN_BWD(px, py, pz, gJ, g) fisheye_jacobian_bwd(px, py, pz, vc.K[0], vc.K[4], vfe, gJ, g)
+#define GSR_PROJECT_BWD(px, py, pz, gu, gv, g) fisheye_project_bwd(J, gu, gv, g)
+#include "gsr_preprocess.cuh"
+
+namespace gsr {
+
+// CTAs per SM the register budget is sized for (-Xptxas -v: no local memory at these bounds, DESIGN.md 3.19)
+#ifndef GSR_FE_FWD_MINB
+#define GSR_FE_FWD_MINB 6
+#endif
+#ifndef GSR_FE_BWD_MINB
+#define GSR_FE_BWD_MINB 4
+#endif
+#ifndef GSR_FE_BATCH_MINB
+#define GSR_FE_BATCH_MINB 3
+#endif
+
+template <int N_SH, bool HAS_SH, bool ANTIALIAS, bool FILTER3D>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_FE_FWD_MINB)
+    k_fisheye_preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* __restrict__ filter3d, const float* __restrict__ fisheye) {
+    preprocess_fwd<N_SH, HAS_SH, ANTIALIAS, FILTER3D>(GSR_PRE_FWD_FORWARD, filter3d, fisheye);
+}
+
+#define GSR_PRE_BWD_PARAMS                                                                                          \
+    int N, const float* __restrict__ xyz, const float* __restrict__ quat, const float* __restrict__ scale,          \
+        const float* __restrict__ opa_logit, const float* __restrict__ Tdev, const float* __restrict__ Kdev,        \
+        const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rows,    \
+        int rows_uv, const float* __restrict__ g_uv_compact, const uint64_t* __restrict__ scan,                      \
+        float* __restrict__ o_xyz, float* __restrict__ o_quat, float* __restrict__ o_scale,                         \
+        float* __restrict__ o_opa, float* __restrict__ o_dc, float* __restrict__ o_sh, int use_tma,                 \
+        const float* __restrict__ filter3d, const float* __restrict__ fisheye
+template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS, bool FILTER3D>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_FE_BWD_MINB) k_fisheye_preprocess_bwd(GSR_PRE_BWD_PARAMS) {
+    preprocess_bwd<N_SH, HAS_SH, DEPTH, ANTIALIAS, FILTER3D>(N, xyz, quat, scale, opa_logit, Tdev, Kdev, camdev,
+                                                             visible, g_rows, rows_uv, g_uv_compact, scan, o_xyz,
+                                                             o_quat, o_scale, o_opa, o_dc, o_sh, use_tma, filter3d,
+                                                             fisheye);
+}
+template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS, bool FILTER3D>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_FE_BATCH_MINB)
+    k_fisheye_batch_preprocess_bwd(int C, GSR_PRE_BWD_PARAMS) {
+    batch_preprocess_bwd<N_SH, HAS_SH, DEPTH, ANTIALIAS, FILTER3D>(C, N, xyz, quat, scale, opa_logit, Tdev, Kdev,
+                                                                   camdev, visible, g_rows, rows_uv, g_uv_compact,
+                                                                   scan, o_xyz, o_quat, o_scale, o_opa, o_dc, o_sh,
+                                                                   use_tma, filter3d, fisheye);
+}
+#undef GSR_PRE_BWD_PARAMS
+
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD | GSR_MODE_FILTER3D;
+
+// n_sh_rest -> the SH template arguments
+#define GSR_FE_SH_SWITCH(LAUNCH)            \
+    switch (n_sh_rest) {                    \
+        case 0: LAUNCH(1, false); break;    \
+        case 3: LAUNCH(4, true); break;     \
+        case 8: LAUNCH(9, true); break;     \
+        case 15: LAUNCH(16, true); break;   \
+        default: return GSR_ERR_UNSUPPORTED; \
+    }
+
+template <bool AA, bool F3D>
+static int launch_fwd(int n_sh_rest, dim3 grid, cudaStream_t st, int N, const float* xyz, const float* xyz_cam,
+                      int cam_first, const float* quat, const float* scale, const float* opa, const float* dc,
+                      const float* sh, const float* T, const float* K, const float* cam, float width, float height,
+                      float near_t, float far_t, float pad, float mh, int ntx, int nty, uint32_t depth_base,
+                      float* records, uint32_t* zkey, uint8_t* visible, uint64_t* packed, uint64_t* tile_mask,
+                      uint32_t* tile_win, int use_tma, const float* filter3d, const float* fisheye) {
+#define GSR_FE_FWD(NSH, HSH)                                                                                        \
+    k_fisheye_preprocess_fwd<NSH, HSH, AA, F3D><<<grid, PRE_THREADS, 0, st>>>(                                      \
+        N, xyz, xyz_cam, cam_first, quat, scale, opa, dc, sh, T, K, cam, width, height, near_t, far_t, pad, mh, ntx, \
+        nty, depth_base, records, zkey, visible, packed, tile_mask, tile_win, use_tma, filter3d, fisheye)
+    GSR_FE_SH_SWITCH(GSR_FE_FWD)
+#undef GSR_FE_FWD
+    return GSR_OK;
+}
+
+#define GSR_FE_BWD_ARGS_DECL                                                                                       \
+    int n_sh_rest, dim3 grid, cudaStream_t st, int N, const float *xyz, const float *quat, const float *scale,     \
+        const float *opa, const float *T, const float *K, const float *cam, const uint8_t *visible,                \
+        const float *rows, int rows_uv, const float *g_uv, const uint64_t *scan, float *o_xyz, float *o_quat,      \
+        float *o_scale, float *o_opa, float *o_dc, float *o_sh, int use_tma, const float *filter3d,                \
+        const float *fisheye
+#define GSR_FE_BWD_ARGS                                                                                             \
+    N, xyz, quat, scale, opa, T, K, cam, visible, rows, rows_uv, g_uv, scan, o_xyz, o_quat, o_scale, o_opa, o_dc,    \
+        o_sh, use_tma, filter3d, fisheye
+
+template <bool DEPTH, bool AA, bool F3D>
+static int launch_bwd(GSR_FE_BWD_ARGS_DECL) {
+#define GSR_FE_BWD(NSH, HSH) \
+    k_fisheye_preprocess_bwd<NSH, HSH, DEPTH, AA, F3D><<<grid, PRE_THREADS, 0, st>>>(GSR_FE_BWD_ARGS)
+    GSR_FE_SH_SWITCH(GSR_FE_BWD)
+#undef GSR_FE_BWD
+    return GSR_OK;
+}
+
+template <bool DEPTH, bool AA, bool F3D>
+static int launch_batch_bwd(int C, GSR_FE_BWD_ARGS_DECL) {
+#define GSR_FE_BWD(NSH, HSH) \
+    k_fisheye_batch_preprocess_bwd<NSH, HSH, DEPTH, AA, F3D><<<grid, PRE_THREADS, 0, st>>>(C, GSR_FE_BWD_ARGS)
+    GSR_FE_SH_SWITCH(GSR_FE_BWD)
+#undef GSR_FE_BWD
+    return GSR_OK;
+}
+
+// the 8 (depth, antialiased, filter3d) instantiations of a backward launcher, selected by the mode bits
+#define GSR_FE_MODE_DISPATCH(launcher, ...)                                                             \
+    (f3d ? (aa ? (depth ? launcher<true, true, true>(__VA_ARGS__) : launcher<false, true, true>(__VA_ARGS__))   \
+               : (depth ? launcher<true, false, true>(__VA_ARGS__) : launcher<false, false, true>(__VA_ARGS__))) \
+         : (aa ? (depth ? launcher<true, true, false>(__VA_ARGS__) : launcher<false, true, false>(__VA_ARGS__))  \
+               : (depth ? launcher<true, false, false>(__VA_ARGS__) : launcher<false, false, false>(__VA_ARGS__))))
+
+// p(t) = c[0] + c[1] t + ... + c[n] t^n
+static double poly(const double* c, int n, double t) {
+    double r = c[n];
+    for (int i = n - 1; i >= 0; --i) r = r * t + c[i];
+    return r;
+}
+
+// The real roots of p in [lo, hi], ascending: p is monotone between consecutive roots of p' (found the same way),
+// so every piece with a sign change holds exactly one root, found by bisection to full precision.
+static int roots_in(const double* c, int n, double lo, double hi, double* out) {
+    while (n > 0 && c[n] == 0.0) --n;
+    if (n == 0) return 0;
+    double pts[8];
+    int np = 0;
+    pts[np++] = lo;
+    if (n > 1) {
+        double dc[4], cr[4];
+        for (int i = 1; i <= n; ++i) dc[i - 1] = i * c[i];
+        const int m = roots_in(dc, n - 1, lo, hi, cr);
+        for (int j = 0; j < m; ++j)
+            if (cr[j] > pts[np - 1]) pts[np++] = cr[j];
+    }
+    if (hi > pts[np - 1]) pts[np++] = hi;
+    int r = 0;
+    for (int j = 0; j < np; ++j) {
+        const double a = pts[j], fa = poly(c, n, a);
+        if (fa == 0.0) {
+            if (r == 0 || out[r - 1] != a) out[r++] = a;
+            continue;
+        }
+        if (j + 1 == np) break;
+        double b = pts[j + 1];
+        const double fb = poly(c, n, b);
+        if (fb == 0.0 || (fa < 0.0) == (fb < 0.0)) continue;
+        double x0 = a, x1 = b;
+        for (int it = 0; it < 200 && x1 > x0; ++it) {
+            const double mid = 0.5 * (x0 + x1);
+            if (mid <= x0 || mid >= x1) break;
+            if ((poly(c, n, mid) < 0.0) == (fa < 0.0)) x0 = mid;
+            else x1 = mid;
+        }
+        out[r++] = x0;
+    }
+    return r;
+}
+
+}  // namespace gsr
+
+using namespace gsr;
+
+extern "C" {
+
+float gsr_fisheye_theta_max(const float* k) {
+    if (k == nullptr) return NAN;
+    for (int i = 0; i < 4; ++i)
+        if (!std::isfinite(k[i])) return NAN;
+    const double half_pi = 1.5707963267948966;
+    // d theta_d / d theta as a polynomial in t = theta^2
+    const double c[5] = {1.0, 3.0 * k[0], 5.0 * k[1], 7.0 * k[2], 9.0 * k[3]};
+    double roots[4];
+    const int n = roots_in(c, 4, 0.0, half_pi * half_pi, roots);
+    double th = half_pi;
+    for (int i = 0; i < n; ++i)
+        if (roots[i] > 0.0) { th = std::sqrt(roots[i]); break; }
+    float f = (float)th;
+    if ((double)f > th) f = std::nextafter(f, 0.0f);  // round down: the cull never admits a folded theta
+    return f;
+}
+
+int gsr_fisheye_preprocess_forward(int mode, int N, int n_sh_rest, const float* xyz, const float* xyz_camera_frame,
+                                   int cam_first, const float* quaternion, const float* scale,
+                                   const float* opacity_logit, const float* filter3d, const float* rgb_dc,
+                                   const float* sh_rest, const float* camera_T_world, const float* K,
+                                   const float* camera_centre, int H, int W, float near_thresh, float far_thresh,
+                                   float cull_mask_padding, float mh_dist, uint32_t depth_base, float* records,
+                                   uint32_t* depth_key, uint8_t* visible, uint64_t* scan, uint64_t* tile_mask,
+                                   uint32_t* tile_win, void* temp, size_t temp_bytes, const float* fisheye,
+                                   void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if ((mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
+    if (((mode & GSR_MODE_FILTER3D) != 0) != (filter3d != nullptr)) return GSR_ERR_BAD_ARG;
+    if (N < 0 || fisheye == nullptr) return GSR_ERR_BAD_ARG;
+    if (N == 0) return GSR_OK;
+    size_t scan_bytes = 0;
+    cub::DeviceScan::InclusiveSum((void*)nullptr, scan_bytes, (uint64_t*)nullptr, (uint64_t*)nullptr, N);
+    if (temp == nullptr || temp_bytes < align256(scan_bytes) + align256(sizeof(uint64_t) * (size_t)N))
+        return GSR_ERR_BAD_ARG;
+    if ((tile_mask == nullptr) != (tile_win == nullptr)) return GSR_ERR_BAD_ARG;
+    uint64_t* packed = reinterpret_cast<uint64_t*>((char*)temp + align256(scan_bytes));
+    const int ntx = (W + TILE - 1) / TILE, nty = (H + TILE - 1) / TILE;
+    const dim3 grid((N + PRE_THREADS - 1) / PRE_THREADS);
+    const int use_tma = (aligned16(records) && (sh_rest == nullptr || aligned16(sh_rest))) ? 1 : 0;
+    const bool aa = (mode & GSR_MODE_ANTIALIASED) != 0, f3d = (mode & GSR_MODE_FILTER3D) != 0;
+#define GSR_FE_FWD_ARGS                                                                                             \
+    n_sh_rest, grid, st, N, xyz, xyz_camera_frame, cam_first, quaternion, scale, opacity_logit, rgb_dc, sh_rest,     \
+        camera_T_world, K, camera_centre, (float)W, (float)H, near_thresh, far_thresh, cull_mask_padding, mh_dist,   \
+        ntx, nty, depth_base, records, depth_key, visible, packed, tile_mask, tile_win, use_tma, filter3d, fisheye
+    const int rc = f3d ? (aa ? launch_fwd<true, true>(GSR_FE_FWD_ARGS) : launch_fwd<false, true>(GSR_FE_FWD_ARGS))
+                       : (aa ? launch_fwd<true, false>(GSR_FE_FWD_ARGS) : launch_fwd<false, false>(GSR_FE_FWD_ARGS));
+#undef GSR_FE_FWD_ARGS
+    if (rc != GSR_OK) return rc;
+    cudaError_t e = cub::DeviceScan::InclusiveSum(temp, scan_bytes, packed, scan, N, st);
+    if (e != cudaSuccess) return (int)e;
+    return (int)cudaGetLastError();
+}
+
+}  // extern "C"
+
+// single: the single-view kernels (C is 1, no running sums); else the batched ones over C views
+static int fisheye_backward(bool single, int mode, int C, int N, int n_sh_rest, const float* xyz,
+                                          const float* quaternion, const float* scale, const float* opacity_logit,
+                                          const float* filter3d, const float* camera_T_world, const float* K,
+                                          const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                                          int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
+                                          float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit,
+                                          float* g_rgb_dc, float* g_sh_rest, const float* fisheye, void* stream) {
+    if (C < 1 || N < 0 || (mode & ~KNOWN_MODES) != 0) return GSR_ERR_BAD_ARG;
+    if (((mode & GSR_MODE_FILTER3D) != 0) != (filter3d != nullptr)) return GSR_ERR_BAD_ARG;
+    if (N == 0) return GSR_OK;  // nothing to launch (the arrays of an empty scene may be NULL)
+    if (xyz == nullptr || quaternion == nullptr || scale == nullptr || opacity_logit == nullptr ||
+        camera_T_world == nullptr || K == nullptr || visible == nullptr || grad_rows == nullptr || g_xyz == nullptr ||
+        g_quaternion == nullptr || g_scale == nullptr || g_opacity_logit == nullptr || g_rgb_dc == nullptr ||
+        fisheye == nullptr)
+        return GSR_ERR_BAD_ARG;
+    if ((n_sh_rest > 0) != (g_sh_rest != nullptr)) return GSR_ERR_BAD_ARG;
+    if (!aligned16(grad_rows)) return GSR_ERR_BAD_ARG;
+    if (grad_uv_compact != nullptr && scan == nullptr) return GSR_ERR_BAD_ARG;
+    if (n_sh_rest != 0 && n_sh_rest != 3 && n_sh_rest != 8 && n_sh_rest != 15) return GSR_ERR_UNSUPPORTED;
+    cudaStream_t st = (cudaStream_t)stream;
+    const dim3 grid((N + PRE_THREADS - 1) / PRE_THREADS);
+    const int use_tma = (aligned16(g_xyz) && aligned16(g_quaternion) && aligned16(g_scale) &&
+                         aligned16(g_opacity_logit) && aligned16(g_rgb_dc) &&
+                         (g_sh_rest == nullptr || aligned16(g_sh_rest)))
+                            ? 1
+                            : 0;
+    const bool depth = (mode & GSR_MODE_DEPTH_ALPHA) != 0, aa = (mode & GSR_MODE_ANTIALIASED) != 0,
+               f3d = (mode & GSR_MODE_FILTER3D) != 0;
+#define GSR_FE_ARGS                                                                                                \
+    n_sh_rest, grid, st, N, xyz, quaternion, scale, opacity_logit, camera_T_world, K, camera_centre, visible,        \
+        grad_rows, use_rows_uv, grad_uv_compact, scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc,      \
+        g_sh_rest, use_tma, filter3d, fisheye
+    const int rc = single ? GSR_FE_MODE_DISPATCH(launch_bwd, GSR_FE_ARGS)
+                          : GSR_FE_MODE_DISPATCH(launch_batch_bwd, C, GSR_FE_ARGS);
+#undef GSR_FE_ARGS
+    if (rc != GSR_OK) return rc;
+    return (int)cudaGetLastError();
+}
+
+extern "C" {
+
+int gsr_fisheye_preprocess_backward(int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
+                                    const float* scale, const float* opacity_logit, const float* filter3d,
+                                    const float* camera_T_world, const float* K, const float* camera_centre,
+                                    const uint8_t* visible, const float* grad_rows, int use_rows_uv,
+                                    const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
+                                    float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                                    float* g_sh_rest, const float* fisheye, void* stream) {
+    return fisheye_backward(true, mode, 1, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
+                            camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
+                            g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, fisheye, stream);
+}
+
+int gsr_fisheye_batch_preprocess_backward(int mode, int C, int N, int n_sh_rest, const float* xyz,
+                                          const float* quaternion, const float* scale, const float* opacity_logit,
+                                          const float* filter3d, const float* camera_T_world, const float* K,
+                                          const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                                          int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
+                                          float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit,
+                                          float* g_rgb_dc, float* g_sh_rest, const float* fisheye, void* stream) {
+    return fisheye_backward(false, mode, C, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
+                            camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
+                            g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, fisheye, stream);
+}
+
+}  // extern "C"

@@ -1,7 +1,8 @@
-// gsr_preprocess.cuh — the per-Gaussian backward of the fused path and the view constants it reads, shared by the
-// single-view kernels (gsr_preprocess.cu, libgsr_b200.so) and the multi-view kernels (gsr_batch.cu,
-// libgsr_batch.so).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian; the single-view kernels store its
-// result, the batched kernels add it up over the views.
+// gsr_preprocess.cuh — the per-Gaussian stages of the fused path and the view constants they read, shared by the
+// single-view kernels (gsr_preprocess.cu, libgsr_b200.so), the multi-view kernels (gsr_batch.cu, libgsr_batch.so)
+// and the fisheye kernels (gsr_fisheye.cu, libgsr_fisheye.so).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian;
+// the single-view kernels store its result, the batched kernels add it up over the views.  The camera model enters
+// only through the GSR_PROJECT / GSR_JACOBIAN hooks below.
 #pragma once
 #include "gsr_common.cuh"
 #include "gsr_math.cuh"
@@ -103,6 +104,29 @@ __device__ __forceinline__ void coop_copy(float* __restrict__ dst, const float* 
     for (int k = threadIdx.x; k < n_floats; k += PRE_THREADS) dst[k] = src[k];
 }
 
+// Camera-model hooks.  The per-gaussian bodies below name the camera model only through these macros.  The pinhole
+// defaults expand to exactly the calls the bodies made before the hooks existed, so every pinhole kernel keeps its
+// instructions; a translation unit that defines GSR_PROJECTION_HOOKS (and the macros) before including this header
+// compiles the same bodies for another model (gsr_fisheye.cu).
+//   GSR_VIEW_PARAM                       extra trailing parameters of the bodies
+//   GSR_VIEW_DECL                        extra CTA-wide view constants, next to `vc`
+//   GSR_LOAD_VIEW(T, K, cam, view)       fill `vc` (and the extra constants) for view index `view`; ends with a barrier
+//   GSR_PROJECT(px, py, pz, u, v)        the projected mean
+//   GSR_CULL_MORE                        extra `| (...)` terms of the forward's cull
+//   GSR_JACOBIAN(px, py, pz, J)          J = d(u, v) / d(px, py, pz), 2x3 row-major
+//   GSR_JACOBIAN_BWD(px, py, pz, gJ, g)  g = contraction of dJ / dp with the gradient on J
+//   GSR_PROJECT_BWD(px, py, pz, gu, gv, g)  g = (d(u, v) / dp)^T (gu, gv); may read the body's `J`
+#ifndef GSR_PROJECTION_HOOKS
+#define GSR_VIEW_PARAM
+#define GSR_VIEW_DECL
+#define GSR_LOAD_VIEW(T, K, cam, view) load_view_cta(T, K, cam, vc, HAS_SH)
+#define GSR_PROJECT(px, py, pz, u, v) project_uv<float>(px, py, pz, vc.K[0], vc.K[2], vc.K[4], vc.K[5], u, v)
+#define GSR_CULL_MORE
+#define GSR_JACOBIAN(px, py, pz, J) proj_jacobian<float>(px, py, pz, vc.K[0], vc.K[4], J)
+#define GSR_JACOBIAN_BWD(px, py, pz, gJ, g) proj_jacobian_bwd<float>(px, py, pz, vc.K[0], vc.K[4], gJ, g)
+#define GSR_PROJECT_BWD(px, py, pz, gu, gv, g) project_uv_bwd<float>(px, py, pz, vc.K[0], vc.K[4], gu, gv, g)
+#endif
+
 // One view's fused VJP for one visible gaussian, as a statement block: it reads the view constants `vc`, the
 // parameters x y z qw qx qy qz s0 s1 s2 opl (f: the 3-D filter) and the view's gradient row (grv rgb, gov opacity,
 // guv uv, gcv conic, gzc camera-frame z; gov and gcv are modified) and assigns gx gq gs go gdc and the SH rest
@@ -134,7 +158,7 @@ _Pragma("unroll")                                                               
             sigma_world<float>(qw, qx, qy, qz, s0, s1, s2, S6);                                                          \
         }                                                                                                                \
         sym6_to_full(S6, S9);                                                                                            \
-        proj_jacobian<float>(px, py, pz, vc.K[0], vc.K[4], J);                                                           \
+        GSR_JACOBIAN(px, py, pz, J);                                                                                     \
         W[0] = vc.T[0]; W[1] = vc.T[1]; W[2] = vc.T[2];                                                                  \
         W[3] = vc.T[4]; W[4] = vc.T[5]; W[5] = vc.T[6];                                                                  \
         W[6] = vc.T[8]; W[7] = vc.T[9]; W[8] = vc.T[10];                                                                 \
@@ -168,8 +192,8 @@ _Pragma("unroll")                                                               
             sigma_world_bwd<float>(qw, qx, qy, qz, s0, s1, s2, gS, gq, gs);                                              \
         }                                                                                                                \
         float gp_j[3], gp_uv[3] = {0.f, 0.f, 0.f};                                                                       \
-        proj_jacobian_bwd<float>(px, py, pz, vc.K[0], vc.K[4], gJ, gp_j);                                                \
-        project_uv_bwd<float>(px, py, pz, vc.K[0], vc.K[4], guv[0], guv[1], gp_uv);                                      \
+        GSR_JACOBIAN_BWD(px, py, pz, gJ, gp_j);                                                                          \
+        GSR_PROJECT_BWD(px, py, pz, guv[0], guv[1], gp_uv);                                                              \
         float gp[3] = {gp_j[0] + gp_uv[0], gp_j[1] + gp_uv[1], gp_j[2] + gp_uv[2]};                                      \
         if (DEPTH) gp[2] += gzc;                                                                                         \
         /* xyz_cam = W xyz + t  =>  grad_xyz = W^T grad_xyz_cam */                                                       \
@@ -218,11 +242,12 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
                      const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
                      float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa,
                      float* __restrict__ o_dc, float* __restrict__ o_sh, int use_tma,
-                     const float* __restrict__ filter3d) {
+                     const float* __restrict__ filter3d GSR_VIEW_PARAM) {
     constexpr int NR = N_SH - 1;
     constexpr int NR3 = HAS_SH ? 3 * NR : 1;
     // all outputs of the CTA's 128 gaussians are staged in shared memory and leave as six bulk stores
     __shared__ ViewConsts vc;
+    GSR_VIEW_DECL
     __shared__ __align__(128) float s_sh[PRE_THREADS * NR3];
     __shared__ __align__(128) float s_xyz[PRE_THREADS * 3];
     __shared__ __align__(128) float s_quat[PRE_THREADS * 4];
@@ -272,7 +297,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
             guv[1] = __fadd_rn(guv[1], t.y);
         }
     }
-    load_view_cta(Tdev, Kdev, camdev, vc, HAS_SH);
+    GSR_LOAD_VIEW(Tdev, Kdev, camdev, 0);
     if (vis) GSR_PRE_BWD_VIEW else if (HAS_SH) {
 #pragma unroll
         for (int k = 0; k < NR3; ++k) my_sh[k] = 0.f;
@@ -281,6 +306,308 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
     for (int k = 0; k < 3; ++k) { s_xyz[tid * 3 + k] = gx[k]; s_scale[tid * 3 + k] = gs[k]; s_dc[tid * 3 + k] = gdc[k]; }
     *reinterpret_cast<float4*>(s_quat + tid * 4) = make_float4(gq[0], gq[1], gq[2], gq[3]);
     s_opa[tid] = go;
+    if (tma) {
+        fence_proxy_async_smem();
+        __syncthreads();
+        if (tid == 0) {
+            tma_store_1d(o_xyz + (size_t)i0 * 3, s_xyz, PRE_THREADS * 3 * 4);
+            tma_store_1d(o_quat + (size_t)i0 * 4, s_quat, PRE_THREADS * 4 * 4);
+            tma_store_1d(o_scale + (size_t)i0 * 3, s_scale, PRE_THREADS * 3 * 4);
+            tma_store_1d(o_opa + (size_t)i0, s_opa, PRE_THREADS * 4);
+            tma_store_1d(o_dc + (size_t)i0 * 3, s_dc, PRE_THREADS * 3 * 4);
+            if (HAS_SH) tma_store_1d(o_sh + (size_t)i0 * NR3, s_sh, PRE_THREADS * NR3 * 4);
+            tma_store_commit_and_wait();
+        }
+    } else {
+        __syncthreads();
+        coop_copy(o_xyz + (size_t)i0 * 3, s_xyz, cnt * 3);
+        coop_copy(o_quat + (size_t)i0 * 4, s_quat, cnt * 4);
+        coop_copy(o_scale + (size_t)i0 * 3, s_scale, cnt * 3);
+        coop_copy(o_opa + (size_t)i0, s_opa, cnt);
+        coop_copy(o_dc + (size_t)i0 * 3, s_dc, cnt * 3);
+        if (HAS_SH) coop_copy(o_sh + (size_t)i0 * NR3, s_sh, cnt * NR3);
+    }
+}
+
+// SH -> RGB exactly as src/precompute_sh.cu:29-56 evaluates it on cat(rgb_dc, sh_rest)
+template <int N_SH>
+__device__ __forceinline__ void sh_rgb_fused(const float* __restrict__ dc, const float* __restrict__ rest,
+                                             float px, float py, float pz, const float* cam,
+                                             float* __restrict__ out) {
+    if (N_SH == 1) {
+        out[0] = dc[0]; out[1] = dc[1]; out[2] = dc[2];
+        return;
+    }
+    float dx, dy, dz, Y[N_SH];
+    view_dir<float>(px, py, pz, cam[0], cam[1], cam[2], dx, dy, dz);
+    sh_basis<float, N_SH>(dx, dy, dz, Y);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        float acc = __fmaf_rn(Y[0], dc[c], 0.0f);
+#pragma unroll
+        for (int k = 1; k < N_SH; ++k) acc = __fmaf_rn(Y[k], rest[c * (N_SH - 1) + (k - 1)], acc);
+        out[c] = __fmul_rn(acc, GSR_RSH0);
+    }
+}
+
+#define GSR_PRE_FWD_PARAMS                                                                                         \
+    int N, const float* __restrict__ xyz, const float* __restrict__ xyz_cam, int cam_first,                        \
+        const float* __restrict__ quat, const float* __restrict__ scale, const float* __restrict__ opa_logit,      \
+        const float* __restrict__ rgb_dc, const float* __restrict__ sh_rest, const float* __restrict__ Tdev,       \
+        const float* __restrict__ Kdev, const float* __restrict__ camdev, float width, float height, float near_t, \
+        float far_t, float pad, float mh, int ntx, int nty, uint32_t depth_base, float* __restrict__ records,      \
+        uint32_t* __restrict__ zkey, uint8_t* __restrict__ visible, uint64_t* __restrict__ packed,                 \
+        uint64_t* __restrict__ tile_mask, uint32_t* __restrict__ tile_win, int use_tma
+#define GSR_PRE_FWD_FORWARD                                                                                        \
+    N, xyz, xyz_cam, cam_first, quat, scale, opa_logit, rgb_dc, sh_rest, Tdev, Kdev, camdev, width, height, near_t, \
+        far_t, pad, mh, ntx, nty, depth_base, records, zkey, visible, packed, tile_mask, tile_win, use_tma
+// The fused per-gaussian forward of one view (gsr_preprocess.cu).
+// ANTIALIAS: the record's opacity is sigmoid(o) * aa_rho(conic) (gsr_record.cuh); the culling bound tau' is formed
+// from that compensated opacity
+// FILTER3D: Mip-Splatting's 3-D filter, f = filter3d[i]: Sigma_world is formed from the variances exp(s)^2 + f^2 and
+// the opacity is multiplied by coef before rho (gsr_record.cuh f3d_filter)
+template <int N_SH, bool HAS_SH, bool ANTIALIAS, bool FILTER3D>
+__device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* __restrict__ filter3d GSR_VIEW_PARAM) {
+    constexpr int NR3 = HAS_SH ? 3 * (N_SH - 1) : 1;
+    __shared__ ViewConsts vc;
+    GSR_VIEW_DECL
+    __shared__ __align__(128) float s_sh[PRE_THREADS * NR3];       // SH coefficients of the CTA's gaussians
+    __shared__ __align__(128) float s_rec[PRE_THREADS * REC];      // output records
+    __shared__ __align__(8) uint64_t s_bar;
+    const int tid = threadIdx.x;
+    const int i0 = blockIdx.x * PRE_THREADS;
+    const int cnt = min(PRE_THREADS, N - i0);
+    const bool tma = use_tma && cnt == PRE_THREADS;
+    // Latencies overlap instead of queueing up: the SH slice's bulk copy is issued first, every thread then
+    // fetches its own gaussian's parameters, and only then the view constants are fetched (cooperatively).
+    if (tid == 0 && HAS_SH && tma) {
+        mbar_init(&s_bar, 1);
+        fence_mbar_init();
+        const uint32_t bytes = (uint32_t)(PRE_THREADS * NR3 * sizeof(float));
+        mbar_arrive_expect_tx(&s_bar, bytes);
+        tma_load_1d(s_sh, sh_rest + (size_t)i0 * NR3, bytes, &s_bar);
+    }
+    if (HAS_SH && !tma) coop_copy(s_sh, sh_rest + (size_t)i0 * NR3, cnt * NR3);
+    const int i = i0 + tid;
+    float x = 0.f, y = 0.f, z = 0.f, q0 = 1.f, q1 = 0.f, q2 = 0.f, q3 = 0.f, sc0 = 0.f, sc1 = 0.f, sc2 = 0.f,
+          opl = 0.f, dc0 = 0.f, dc1 = 0.f, dc2 = 0.f;
+    if (i < N) {
+        x = xyz[i * 3 + 0]; y = xyz[i * 3 + 1]; z = xyz[i * 3 + 2];
+        q0 = quat[i * 4 + 0]; q1 = quat[i * 4 + 1]; q2 = quat[i * 4 + 2]; q3 = quat[i * 4 + 3];
+        sc0 = scale[i * 3 + 0]; sc1 = scale[i * 3 + 1]; sc2 = scale[i * 3 + 2];
+        opl = opa_logit[i];
+        dc0 = rgb_dc[i * 3 + 0]; dc1 = rgb_dc[i * 3 + 1]; dc2 = rgb_dc[i * 3 + 2];
+    }
+    GSR_LOAD_VIEW(Tdev, Kdev, camdev, 0);
+    float rec[REC];
+#pragma unroll
+    for (int k = 0; k < REC; ++k) rec[k] = 0.0f;
+    if (i < N) {
+        float px, py, pz, u, v;
+        if (xyz_cam != nullptr && i >= cam_first) {
+            const float* pc = xyz_cam + (size_t)(i - cam_first) * 3;
+            px = pc[0]; py = pc[1]; pz = pc[2];
+        } else {
+            transform_point<float>(vc.T, x, y, z, px, py, pz);
+        }
+        GSR_PROJECT(px, py, pz, u, v);
+        // splat_py/rasterize.py:38-49 (strict compares, fp32)
+        const bool culled = (pz < near_t) | (pz > far_t) | (u < -pad) | (u > width + pad) | (v < -pad) |
+                            (v > height + pad) GSR_CULL_MORE;
+        // visible => pz >= near > 0: float bits are monotone, and relative to bits(near) only a few low
+        // bits are significant (shorter radix sort)
+        zkey[i] = depth_base ? (__float_as_uint(pz) - depth_base) : depth_key(pz);
+        // NaN coordinates compare false everywhere and would survive; the reference aborts on them
+        // (splat_py/tile_culling.py:15-18) — treat as culled instead.
+        const bool vis = !culled && (pz == pz) && (u == u) && (v == v);
+        visible[i] = vis ? 1 : 0;
+        uint64_t pk = 0ull;
+        if (vis) {
+            float S6[6], S9[9], J[6], W[9], conic[3], coef = 1.0f;
+            if (FILTER3D) {
+                const float f = filter3d[i];
+                const float F = __fmul_rn(f, f);
+                const float e0 = expf(sc0), e1 = expf(sc1), e2 = expf(sc2);
+                const float v[3] = {__fmul_rn(e0, e0), __fmul_rn(e1, e1), __fmul_rn(e2, e2)};
+                float vp[3], t[3];
+                coef = f3d_filter(v, F, vp, t);
+                sigma_world_var<float>(q0, q1, q2, q3, vp[0], vp[1], vp[2], S6);
+            } else {
+                sigma_world<float>(q0, q1, q2, q3, sc0, sc1, sc2, S6);
+            }
+            sym6_to_full(S6, S9);
+            GSR_JACOBIAN(px, py, pz, J);
+            W[0] = vc.T[0]; W[1] = vc.T[1]; W[2] = vc.T[2];
+            W[3] = vc.T[4]; W[4] = vc.T[5]; W[5] = vc.T[6];
+            W[6] = vc.T[8]; W[7] = vc.T[9]; W[8] = vc.T[10];
+            conic_from<float>(S9, J, W, conic, nullptr);
+
+            float opa = sigmoid_torch(opl);
+            if (FILTER3D) opa = __fmul_rn(opa, coef);
+            if (ANTIALIAS) opa = __fmul_rn(opa, aa_rho(conic[0], conic[1], conic[2]));
+            float dc[3] = {dc0, dc1, dc2};
+            float col[3];
+            if (HAS_SH) {
+                if (tma) mbar_wait(&s_bar, 0);
+                sh_rgb_fused<N_SH>(dc, s_sh + tid * NR3, x, y, z, vc.cam, col);  // stride 3*(N_SH-1): odd, no conflicts
+            } else {
+                col[0] = dc[0]; col[1] = dc[1]; col[2] = dc[2];
+            }
+            make_record(u, v, conic[0], conic[1], conic[2], opa, col[0], col[1], col[2], rec);
+
+            // tiles touched (src/tile_culling.cu:139-176)
+            Obb ob;
+            compute_obb(u, v, rec[R_A], __fmul_rn(rec[R_B2], 0.5f), rec[R_C], mh, ob);
+            int x0, x1, y0, y1, c = 0;
+            tile_window(u, v, ob.radius_tiles, ntx, nty, x0, x1, y0, y1);
+            // The tiles hit are remembered as a bit mask over the window (bit = (tx - x0) * height + (ty - y0), the
+            // enumeration order) when the window has at most 64 tiles — footprints up to 3 sigma = 48 px — so that
+            // the pair emission does not repeat the OBB / separating-axis tests (gsr_binning.cu); larger windows
+            // are flagged and re-tested there.
+            const int wx = x1 - x0, wy = y1 - y0;
+            const bool small = (wx * wy <= 64) & (x0 < 256) & (y0 < 256);
+            uint64_t hits = 0ull;
+            for (int tx = x0; tx < x1; ++tx) {
+                const float left = __fmul_rn(__int2float_rn(tx), 16.0f);
+                const float right = __fmul_rn(__int2float_rn(tx + 1), 16.0f);
+                for (int ty = y0; ty < y1; ++ty) {
+                    const float top = __fmul_rn(__int2float_rn(ty), 16.0f);
+                    const float bottom = __fmul_rn(__int2float_rn(ty + 1), 16.0f);
+                    if (obb_hits_tile(ob, left, right, top, bottom)) {
+                        ++c;
+                        if (small) hits |= 1ull << ((tx - x0) * wy + (ty - y0));
+                    }
+                }
+            }
+            if (tile_mask != nullptr) {
+                tile_mask[i] = hits;
+                tile_win[i] = small ? ((uint32_t)x0 | ((uint32_t)y0 << 8) | ((uint32_t)wx << 16) | ((uint32_t)wy << 24))
+                                    : 0xffffffffu;
+            }
+            pk = (1ull << 32) | (uint64_t)(uint32_t)c;
+        }
+        packed[i] = pk;
+    }
+    // records leave through shared memory: one 6 KB bulk store per CTA instead of 48-byte strided stores
+    float4* sr = reinterpret_cast<float4*>(s_rec + tid * REC);
+    sr[0] = make_float4(rec[0], rec[1], rec[2], rec[3]);
+    sr[1] = make_float4(rec[4], rec[5], rec[6], rec[7]);
+    sr[2] = make_float4(rec[8], rec[9], rec[10], rec[11]);
+    if (tma) {
+        fence_proxy_async_smem();
+        __syncthreads();
+        if (tid == 0) {
+            tma_store_1d(records + (size_t)i0 * REC, s_rec, (uint32_t)(PRE_THREADS * REC * sizeof(float)));
+            tma_store_commit_and_wait();
+        }
+    } else {
+        __syncthreads();
+        coop_copy(records + (size_t)i0 * REC, s_rec, cnt * REC);
+    }
+    if (HAS_SH && tma && tid == 0) mbar_wait(&s_bar, 0);  // never exit with the SH load still in flight
+}
+
+// The per-gaussian backward of C views in one pass (gsr_batch.cu).  A CTA takes 128 gaussians, reads their parameters
+// once and walks the views in order.  For every view that sees a gaussian it forms that view's VJP with the
+// single-view kernel's own statement block (GSR_PRE_BWD_VIEW) and adds it to the running sums with one rounded fp32
+// add, so the result is the view-order sum of the single-view gradients bit for bit (up to the sign of zero).  The
+// sums of the SH rest coefficients live in the shared-memory staging the single-view kernel stores from; everything
+// leaves once, by the same bulk stores.
+template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS, bool FILTER3D>
+__device__ __forceinline__ void batch_preprocess_bwd(
+    int C, int N, const float* __restrict__ xyz, const float* __restrict__ quat, const float* __restrict__ scale,
+    const float* __restrict__ opa_logit, const float* __restrict__ Tdev, const float* __restrict__ Kdev,
+    const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rows,
+    int rows_uv, const float* __restrict__ g_uv_compact, const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
+    float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa, float* __restrict__ o_dc,
+    float* __restrict__ o_sh, int use_tma, const float* __restrict__ filter3d GSR_VIEW_PARAM) {
+    constexpr int NR = N_SH - 1;
+    constexpr int NR3 = HAS_SH ? 3 * NR : 1;
+    __shared__ ViewConsts vc;
+    GSR_VIEW_DECL
+    __shared__ __align__(128) float s_sh[PRE_THREADS * NR3];
+    __shared__ __align__(128) float s_xyz[PRE_THREADS * 3];
+    __shared__ __align__(128) float s_quat[PRE_THREADS * 4];
+    __shared__ __align__(128) float s_scale[PRE_THREADS * 3];
+    __shared__ __align__(128) float s_opa[PRE_THREADS];
+    __shared__ __align__(128) float s_dc[PRE_THREADS * 3];
+    const int tid = threadIdx.x;
+    const int i0 = blockIdx.x * PRE_THREADS;
+    const int cnt = min(PRE_THREADS, N - i0);
+    const bool tma = use_tma && cnt == PRE_THREADS;
+    const int i = i0 + tid;
+    // running sums over the views
+    float ax[3] = {0.f, 0.f, 0.f}, aq[4] = {0.f, 0.f, 0.f, 0.f}, as[3] = {0.f, 0.f, 0.f}, ao = 0.f,
+          adc[3] = {0.f, 0.f, 0.f};
+    float* acc_sh = s_sh + tid * NR3;
+    if (HAS_SH) {
+#pragma unroll
+        for (int k = 0; k < NR3; ++k) acc_sh[k] = 0.f;
+    }
+    bool any = false;
+    if (i < N)
+        for (int c = 0; c < C; ++c) any |= visible[(size_t)c * N + i] != 0;
+    float x = 0.f, y = 0.f, z = 0.f, qw = 1.f, qx = 0.f, qy = 0.f, qz = 0.f, s0 = 0.f, s1 = 0.f, s2 = 0.f, opl = 0.f,
+          f = 0.f;
+    if (any) {
+        if (FILTER3D) f = filter3d[i];
+        x = xyz[i * 3 + 0]; y = xyz[i * 3 + 1]; z = xyz[i * 3 + 2];
+        qw = quat[i * 4 + 0]; qx = quat[i * 4 + 1]; qy = quat[i * 4 + 2]; qz = quat[i * 4 + 3];
+        s0 = scale[i * 3 + 0]; s1 = scale[i * 3 + 1]; s2 = scale[i * 3 + 2];
+        opl = opa_logit[i];
+    }
+    size_t uv_base = 0;  // first compact uv row of view c
+    for (int c = 0; c < C; ++c) {
+        const size_t ci = (size_t)c * N + i;
+        const bool vis = any && visible[ci] != 0;
+        float gcv[3] = {0.f, 0.f, 0.f}, guv[2] = {0.f, 0.f}, gov = 0.f, grv[3] = {0.f, 0.f, 0.f}, gzc = 0.f;
+        if (vis) {
+            // view c's row, read exactly as the single-view kernel reads it
+            const float4* row = reinterpret_cast<const float4*>(g_rows + ci * GSR_GRAD_ROW_FLOATS);
+            const float4 r0 = row[0], r1 = row[1];
+            grv[0] = r0.x; grv[1] = r0.y; grv[2] = r0.z; gov = r0.w;
+            if (rows_uv) { guv[0] = r1.x; guv[1] = r1.y; }
+            gcv[0] = r1.z; gcv[1] = r1.w;
+            if (DEPTH) {
+                const float2 r2 = *reinterpret_cast<const float2*>(g_rows + ci * GSR_GRAD_ROW_FLOATS + 8);
+                gcv[2] = r2.x;
+                gzc = r2.y;
+            } else {
+                gcv[2] = g_rows[ci * GSR_GRAD_ROW_FLOATS + 8];
+            }
+            if (g_uv_compact != nullptr) {
+                const size_t r = uv_base + (size_t)(scan[ci] >> 32) - 1;
+                const float2 t = *reinterpret_cast<const float2*>(g_uv_compact + r * 2);
+                guv[0] = __fadd_rn(guv[0], t.x);
+                guv[1] = __fadd_rn(guv[1], t.y);
+            }
+        }
+        if (g_uv_compact != nullptr) uv_base += (size_t)(scan[(size_t)c * N + N - 1] >> 32);
+        if (c > 0) __syncthreads();  // every thread is done with the previous view's constants
+        GSR_LOAD_VIEW(Tdev + 16 * c, Kdev + 9 * c, camdev != nullptr ? camdev + 3 * c : nullptr, c);
+        if (vis) {
+            float gx[3], gq[4], gs[3], go, gdc[3], v_sh[NR3];
+            float* my_sh = v_sh;
+            GSR_PRE_BWD_VIEW
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                ax[k] = __fadd_rn(ax[k], gx[k]);
+                as[k] = __fadd_rn(as[k], gs[k]);
+                adc[k] = __fadd_rn(adc[k], gdc[k]);
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) aq[k] = __fadd_rn(aq[k], gq[k]);
+            ao = __fadd_rn(ao, go);
+            if (HAS_SH) {
+#pragma unroll
+                for (int k = 0; k < NR3; ++k) acc_sh[k] = __fadd_rn(acc_sh[k], v_sh[k]);
+            }
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { s_xyz[tid * 3 + k] = ax[k]; s_scale[tid * 3 + k] = as[k]; s_dc[tid * 3 + k] = adc[k]; }
+    *reinterpret_cast<float4*>(s_quat + tid * 4) = make_float4(aq[0], aq[1], aq[2], aq[3]);
+    s_opa[tid] = ao;
     if (tma) {
         fence_proxy_async_smem();
         __syncthreads();

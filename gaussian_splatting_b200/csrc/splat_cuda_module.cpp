@@ -14,6 +14,7 @@
 #include "../../include/gsr_selective_adam.h"
 #include "../../include/gsr_features.h"
 #include "../../include/gsr_batch.h"
+#include "../../include/gsr_fisheye.h"
 
 namespace {
 
@@ -444,12 +445,24 @@ static const float* filter3d_ptr(const c10::optional<torch::Tensor>& filter3d, i
 
 // returns [records [N,12], depth_key [N] i32-viewed u32, visible [N] u8, scan [N] i64-viewed u64] and, with_tiles,
 // also [tile_mask [N] i64-viewed u64, tile_win [N] i32-viewed u32].  mode: GSR_MODE_* bits
-std::vector<torch::Tensor> fused_preprocess_forward(
+// the fisheye constants of C views ({k1, k2, k3, k4, theta_max} each, fp32 on xyz's device), or NULL
+static const float* fisheye_ptr(const c10::optional<torch::Tensor>& fisheye, int64_t C, const torch::Tensor& xyz) {
+    if (!fisheye.has_value()) return nullptr;
+    const torch::Tensor& f = *fisheye;
+    CHECK_VALID_INPUT(f); CHECK_FLOAT_TENSOR(f);
+    TORCH_CHECK(f.numel() == C * GSR_FISHEYE_CONSTS, "fisheye constants must hold ", GSR_FISHEYE_CONSTS,
+                " floats per view");
+    TORCH_CHECK(f.device() == xyz.device(), "fisheye constants must be on the gaussians' device");
+    return f.data_ptr<float>();
+}
+
+// fe: the fisheye constants (gsr_fisheye_preprocess_forward) or NULL (the pinhole gsr_preprocess_forward)
+static std::vector<torch::Tensor> preprocess_forward(
     torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d) {
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, c10::optional<torch::Tensor> fisheye) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc); CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -498,18 +511,44 @@ std::vector<torch::Tensor> fused_preprocess_forward(
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
     const float* f3d = filter3d_ptr(filter3d, N);
-    check_rc(gsr_preprocess_forward((int)mode, N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion),
-                                    F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world),
-                                    F32PTR(K), centre_ptr, (int)H, (int)W, (float)near_thresh, (float)far_thresh,
-                                    (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base, F32PTR(records),
-                                    (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),
-                                    (uint64_t*)scan.data_ptr<int64_t>(),
-                                    with_tiles && N > 0 ? (uint64_t*)tile_mask.data_ptr<int64_t>() : nullptr,
-                                    with_tiles && N > 0 ? (uint32_t*)tile_win.data_ptr<int>() : nullptr, temp.data_ptr(), tb,
-                                    cur_stream()),
-             "gsr_preprocess_forward");
+    const float* fe = fisheye_ptr(fisheye, 1, xyz);
+#define GSR_FWD_ARGS                                                                                                  \
+    (int)mode, N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), \
+        f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world), F32PTR(K), centre_ptr, (int)H, (int)W,                   \
+        (float)near_thresh, (float)far_thresh, (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base,        \
+        F32PTR(records), (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),                                \
+        (uint64_t*)scan.data_ptr<int64_t>(), with_tiles && N > 0 ? (uint64_t*)tile_mask.data_ptr<int64_t>() : nullptr, \
+        with_tiles && N > 0 ? (uint32_t*)tile_win.data_ptr<int>() : nullptr, temp.data_ptr(), tb
+    if (fe != nullptr)
+        check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, fe, cur_stream()), "gsr_fisheye_preprocess_forward");
+    else
+        check_rc(gsr_preprocess_forward(GSR_FWD_ARGS, cur_stream()), "gsr_preprocess_forward");
+#undef GSR_FWD_ARGS
     if (!with_tiles) return {records, zkey, visible, scan};
     return {records, zkey, visible, scan, tile_mask, tile_win};
+}
+
+std::vector<torch::Tensor> fused_preprocess_forward(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d) {
+    return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
+                              K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
+                              with_tiles, mode, filter3d, c10::nullopt);
+}
+
+// fused_preprocess_forward for a fisheye camera: fisheye [5] = {k1, k2, k3, k4, theta_max} on xyz's device
+std::vector<torch::Tensor> fisheye_preprocess_forward(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
+    return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
+                              K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
+                              with_tiles, mode, filter3d, fisheye);
 }
 
 // (M, P known) -> the sorted pair list the tile renderers read records through, tile ranges [n_tiles+1] i32,
@@ -733,15 +772,16 @@ torch::Tensor fused_render_features_backward(torch::Tensor grad_map, torch::Tens
 // added to — or, with use_slab_uv false, replacing — the slab's uv section.  mode: the GSR_MODE_* bits of the forward
 // (gsr_preprocess_backward): GSR_MODE_DEPTH_ALPHA reads the z gradient of the depth/alpha rows, GSR_MODE_ANTIALIASED
 // takes the rows' opacity slot as the gradient on the compensated opacity, GSR_MODE_FILTER3D needs the forward's filter3d.
-std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
-                                                     torch::Tensor scale, torch::Tensor opacity_logit,
-                                                     c10::optional<torch::Tensor> sh_rest,
-                                                     torch::Tensor camera_T_world, torch::Tensor K,
-                                                     c10::optional<torch::Tensor> camera_centre,
-                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-                                                     c10::optional<torch::Tensor> grad_uv_compact,
-                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
-                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
+static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
+                                                      torch::Tensor scale, torch::Tensor opacity_logit,
+                                                      c10::optional<torch::Tensor> sh_rest,
+                                                      torch::Tensor camera_T_world, torch::Tensor K,
+                                                      c10::optional<torch::Tensor> camera_centre,
+                                                      torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+                                                      c10::optional<torch::Tensor> grad_uv_compact,
+                                                      c10::optional<torch::Tensor> scan, bool use_slab_uv,
+                                                      int64_t mode, c10::optional<torch::Tensor> filter3d,
+                                                      c10::optional<torch::Tensor> fisheye) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     const int64_t N = xyz.size(0);
     TORCH_CHECK(slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ", GSR_GRAD_ROW_FLOATS,
@@ -786,18 +826,49 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
     const float* f3d = filter3d_ptr(filter3d, N);
-    check_rc(gsr_preprocess_backward((int)mode, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
-                                     F32PTR(opacity_logit), f3d, F32PTR(camera_T_world), F32PTR(K),
-                                     camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,
-                                     visible.data_ptr<uint8_t>(), slab.data_ptr<float>(), use_slab_uv ? 1 : 0, g_uv_compact,
-                                     scan_ptr, F32PTR(o_xyz),
-                                     F32PTR(o_q), F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc),
-                                     n_rest ? F32PTR(g_sh) : nullptr, cur_stream()),
-             "gsr_preprocess_backward");
+    const float* fe = fisheye_ptr(fisheye, 1, xyz);
+#define GSR_BWD_ARGS                                                                                                 \
+    (int)mode, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d,          \
+        F32PTR(camera_T_world), F32PTR(K), camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,   \
+        visible.data_ptr<uint8_t>(), slab.data_ptr<float>(), use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr,            \
+        F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
+    if (fe != nullptr)
+        check_rc(gsr_fisheye_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()), "gsr_fisheye_preprocess_backward");
+    else
+        check_rc(gsr_preprocess_backward(GSR_BWD_ARGS, cur_stream()), "gsr_preprocess_backward");
+#undef GSR_BWD_ARGS
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
     out.push_back(flat);  // last: the allocation all the others are views of
     return out;
+}
+
+std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
+                                                     torch::Tensor scale, torch::Tensor opacity_logit,
+                                                     c10::optional<torch::Tensor> sh_rest,
+                                                     torch::Tensor camera_T_world, torch::Tensor K,
+                                                     c10::optional<torch::Tensor> camera_centre,
+                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+                                                     c10::optional<torch::Tensor> grad_uv_compact,
+                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
+                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
+    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, c10::nullopt);
+}
+
+// fused_preprocess_backward for a fisheye camera (the forward's fisheye constants)
+std::vector<torch::Tensor> fisheye_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
+                                                       torch::Tensor scale, torch::Tensor opacity_logit,
+                                                       c10::optional<torch::Tensor> sh_rest,
+                                                       torch::Tensor camera_T_world, torch::Tensor K,
+                                                       c10::optional<torch::Tensor> camera_centre,
+                                                       torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+                                                       c10::optional<torch::Tensor> grad_uv_compact,
+                                                       c10::optional<torch::Tensor> scan, bool use_slab_uv,
+                                                       int64_t mode, c10::optional<torch::Tensor> filter3d,
+                                                       torch::Tensor fisheye) {
+    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, fisheye);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -816,12 +887,12 @@ static int64_t check_views(const torch::Tensor& camera_T_world, const torch::Ten
 // fused_preprocess_forward of every view into stacked outputs: [records [C,N,12], depth_key [C,N], visible [C,N],
 // scan [C,N] (each view's own packed inclusive scan), tile_mask [C,N], tile_win [C,N]].  xyz_camera_frame [C,R,3]:
 // camera-frame positions of the LAST R gaussians of every view; camera_centre [C,3].
-std::vector<torch::Tensor> batch_preprocess_forward(
+static std::vector<torch::Tensor> batch_forward(
     torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
-    c10::optional<torch::Tensor> filter3d) {
+    c10::optional<torch::Tensor> filter3d, c10::optional<torch::Tensor> fisheye) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -870,19 +941,46 @@ std::vector<torch::Tensor> batch_preprocess_forward(
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
     const float* f3d = filter3d_ptr(filter3d, N);
+    const float* fe = fisheye_ptr(fisheye, C, xyz);
     for (int64_t c = 0; c < C && N > 0; ++c) {
-        check_rc(gsr_preprocess_forward(
-                     (int)mode, N, n_rest, F32PTR(xyz), cam_ptr ? cam_ptr + c * R * 3 : nullptr, N - (int)R,
-                     F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(rgb_dc), sh_ptr,
-                     F32PTR(camera_T_world) + 16 * c, F32PTR(K) + 9 * c, centre_ptr ? centre_ptr + 3 * c : nullptr,
-                     (int)H, (int)W, (float)near_thresh, (float)far_thresh, (float)cull_mask_padding, (float)mh_dist,
-                     (uint32_t)depth_base, F32PTR(records[c]), (uint32_t*)zkey[c].data_ptr<int>(),
-                     visible[c].data_ptr<uint8_t>(), (uint64_t*)scan[c].data_ptr<int64_t>(),
-                     (uint64_t*)tile_mask[c].data_ptr<int64_t>(), (uint32_t*)tile_win[c].data_ptr<int>(),
-                     temp.data_ptr(), tb, cur_stream()),
-                 "gsr_preprocess_forward");
+#define GSR_FWD_ARGS                                                                                                \
+    (int)mode, N, n_rest, F32PTR(xyz), cam_ptr ? cam_ptr + c * R * 3 : nullptr, N - (int)R, F32PTR(quaternion),     \
+        F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world) + 16 * c,          \
+        F32PTR(K) + 9 * c, centre_ptr ? centre_ptr + 3 * c : nullptr, (int)H, (int)W, (float)near_thresh,            \
+        (float)far_thresh, (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base, F32PTR(records[c]),       \
+        (uint32_t*)zkey[c].data_ptr<int>(), visible[c].data_ptr<uint8_t>(), (uint64_t*)scan[c].data_ptr<int64_t>(),  \
+        (uint64_t*)tile_mask[c].data_ptr<int64_t>(), (uint32_t*)tile_win[c].data_ptr<int>(), temp.data_ptr(), tb
+        if (fe != nullptr)
+            check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, fe + GSR_FISHEYE_CONSTS * c, cur_stream()),
+                     "gsr_fisheye_preprocess_forward");
+        else
+            check_rc(gsr_preprocess_forward(GSR_FWD_ARGS, cur_stream()), "gsr_preprocess_forward");
+#undef GSR_FWD_ARGS
     }
     return {records, zkey, visible, scan, tile_mask, tile_win};
+}
+
+std::vector<torch::Tensor> batch_preprocess_forward(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
+    c10::optional<torch::Tensor> filter3d) {
+    return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
+                         camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
+                         filter3d, c10::nullopt);
+}
+
+// batch_preprocess_forward for fisheye cameras: fisheye [C,5] = {k1, k2, k3, k4, theta_max} per view
+std::vector<torch::Tensor> batch_fisheye_preprocess_forward(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
+    return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
+                         camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
+                         filter3d, fisheye);
 }
 
 // fused_render_backward of every view into one stacked slab [C, N*12]: grad_image [C,H,W,3], per view the forward's
@@ -943,15 +1041,15 @@ torch::Tensor batch_render_backward(torch::Tensor grad_image, int64_t N, std::ve
 // the per-gaussian backward of C views in one pass (gsr_batch_preprocess_backward): slab [C, N*12] of
 // batch_render_backward, visible / scan [C,N] of batch_preprocess_forward, grad_uv_compact [sum M_c, 2] (optional).
 // Same outputs and flat layout as fused_preprocess_backward, holding the gradient summed over the views.
-std::vector<torch::Tensor> batch_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
-                                                     torch::Tensor scale, torch::Tensor opacity_logit,
-                                                     c10::optional<torch::Tensor> sh_rest,
-                                                     torch::Tensor camera_T_world, torch::Tensor K,
-                                                     c10::optional<torch::Tensor> camera_centre,
-                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-                                                     c10::optional<torch::Tensor> grad_uv_compact,
-                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
-                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
+static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
+                                                 torch::Tensor scale, torch::Tensor opacity_logit,
+                                                 c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
+                                                 torch::Tensor K, c10::optional<torch::Tensor> camera_centre,
+                                                 torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+                                                 c10::optional<torch::Tensor> grad_uv_compact,
+                                                 c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+                                                 c10::optional<torch::Tensor> filter3d,
+                                                 c10::optional<torch::Tensor> fisheye) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(visible);
@@ -1003,16 +1101,53 @@ std::vector<torch::Tensor> batch_preprocess_backward(torch::Tensor slab, torch::
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
     const float* f3d = filter3d_ptr(filter3d, N);
-    check_rc(gsr_batch_preprocess_backward((int)mode, (int)C, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion),
-                                           F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(camera_T_world), F32PTR(K),
-                                           centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab), use_slab_uv ? 1 : 0,
-                                           g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s),
-                                           F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr, cur_stream()),
-             "gsr_batch_preprocess_backward");
+    const float* fe = fisheye_ptr(fisheye, C, xyz);
+#define GSR_BWD_ARGS                                                                                                \
+    (int)mode, (int)C, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d,  \
+        F32PTR(camera_T_world), F32PTR(K), centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab),                    \
+        use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o),           \
+        F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
+    if (fe != nullptr)
+        check_rc(gsr_fisheye_batch_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
+                 "gsr_fisheye_batch_preprocess_backward");
+    else
+        check_rc(gsr_batch_preprocess_backward(GSR_BWD_ARGS, cur_stream()), "gsr_batch_preprocess_backward");
+#undef GSR_BWD_ARGS
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
     out.push_back(flat);
     return out;
+}
+
+std::vector<torch::Tensor> batch_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
+                                                     torch::Tensor scale, torch::Tensor opacity_logit,
+                                                     c10::optional<torch::Tensor> sh_rest,
+                                                     torch::Tensor camera_T_world, torch::Tensor K,
+                                                     c10::optional<torch::Tensor> camera_centre,
+                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+                                                     c10::optional<torch::Tensor> grad_uv_compact,
+                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
+                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
+    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, c10::nullopt);
+}
+
+// batch_preprocess_backward for fisheye cameras (the forward's [C,5] fisheye constants)
+std::vector<torch::Tensor> batch_fisheye_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
+    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, fisheye);
+}
+
+// gsr_fisheye_theta_max of 4 coefficients (host floats)
+double fisheye_theta_max(std::vector<double> k) {
+    TORCH_CHECK(k.size() == 4, "fisheye needs 4 coefficients k1 k2 k3 k4");
+    const float kf[4] = {(float)k[0], (float)k[1], (float)k[2], (float)k[3]};
+    return (double)gsr_fisheye_theta_max(kf);
 }
 
 // Mip-Splatting's 3-D filter size per gaussian (gsr_filter3d): xyz [N,3], camera_T_world [C,4,4], K [C,3,3],
@@ -1463,6 +1598,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "render backward of C views into one stacked gradient slab [C, N*12]");
     m.def("batch_preprocess_backward", &batch_preprocess_backward,
           "per-gaussian backward of C views in one pass: the gradient summed over the views (gsr_batch)");
+    m.def("fisheye_preprocess_forward", &fisheye_preprocess_forward,
+          "fused_preprocess_forward for an OPENCV_FISHEYE camera (gsr_fisheye_preprocess_forward)");
+    m.def("fisheye_preprocess_backward", &fisheye_preprocess_backward,
+          "fused_preprocess_backward for an OPENCV_FISHEYE camera (gsr_fisheye_preprocess_backward)");
+    m.def("batch_fisheye_preprocess_forward", &batch_fisheye_preprocess_forward,
+          "batch_preprocess_forward for OPENCV_FISHEYE cameras, [C,5] constants");
+    m.def("batch_fisheye_preprocess_backward", &batch_fisheye_preprocess_backward,
+          "batch_preprocess_backward for OPENCV_FISHEYE cameras (gsr_fisheye_batch_preprocess_backward)");
+    m.def("fisheye_theta_max", &fisheye_theta_max, "the fisheye cull limit of 4 coefficients (gsr_fisheye_theta_max)");
     m.def("filter3d", &filter3d, "Mip-Splatting's 3-D filter size per gaussian from the training cameras (gsr_filter3d)",
           py::arg("xyz"), py::arg("camera_T_world"), py::arg("K"), py::arg("width"), py::arg("height"),
           py::arg("near"), py::arg("margin"), py::arg("variance"));

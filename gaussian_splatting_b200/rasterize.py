@@ -242,7 +242,7 @@ class _ViewState:
                  "records", "keys_sorted", "id_bits",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
                  "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad", "filter3d",
-                 "weight_stats")
+                 "weight_stats", "fisheye")
 
     @property
     def ids_sorted(self):
@@ -275,6 +275,7 @@ class _ViewState:
         # per-gaussian stages: filter3d [N], a constant)
         self.mode = 0
         self.filter3d = None
+        self.fisheye = None     # fisheye cameras: {k1, k2, k3, k4, theta_max} on the device (_fisheye_constants)
         self.depth = self.alpha = None
         self.uv_absgrad = None  # MODE_ABSGRAD: [M,2], set by every render backward
         self.weight_stats = None  # optional densify.WeightStats the render forward accumulates into
@@ -297,6 +298,62 @@ class _stage:
         if self.rec is not None:
             self.e1.record()
             self.rec.append((self.name, self.e0, self.e1))
+
+
+# ---- fisheye cameras ---------------------------------------------------------------------------------------------------
+def fisheye_theta_max(k) -> float:
+    """The cull limit of COLMAP's OPENCV_FISHEYE model with coefficients k = (k1, k2, k3, k4): the first theta in
+    (0, pi/2) where d theta_d / d theta = 1 + 3 k1 theta^2 + 5 k2 theta^4 + 7 k3 theta^6 + 9 k4 theta^8 reaches 0 (beyond
+    it the model folds points back into the image), else pi/2; found in fp64 for the fp32 coefficients and rounded down
+    to fp32 (gsr_fisheye_theta_max, the value the kernels cull with)."""
+    return native().fisheye_theta_max([float(v) for v in _fisheye_coefficients(k)])
+
+
+def _fisheye_coefficients(fisheye, C=None):
+    """The host coefficients as float32 numpy [4] (C None) or [C,4]; ValueError for a CUDA tensor, a wrong shape or
+    non-finite values.  Batches take [4] (shared) or [C,4]."""
+    import numpy as np
+
+    if torch.is_tensor(fisheye):
+        if fisheye.device.type != "cpu":
+            raise ValueError("fisheye coefficients are camera constants read on the host: pass a CPU tensor or a "
+                             "sequence, not a tensor on " + str(fisheye.device))
+        k = fisheye.detach().to(torch.float64).numpy()
+    else:
+        try:
+            k = np.asarray(fisheye, dtype=np.float64)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"fisheye must be 4 numbers k1 k2 k3 k4: {e}") from None
+    shapes = ((4,),) if C is None else ((4,), (C, 4))
+    if k.shape not in shapes:
+        want = "[4]" if C is None else f"[4] or [{C},4]"
+        raise ValueError(f"fisheye has shape {list(k.shape)} but must be {want} (COLMAP's k1 k2 k3 k4)")
+    with np.errstate(over="ignore"):
+        k32 = k.astype(np.float32)
+    if not np.isfinite(k32).all():
+        raise ValueError("fisheye coefficients must be finite (in fp32)")
+    return k32 if C is None or k.ndim == 2 else np.broadcast_to(k32, (C, 4))
+
+
+_FISHEYE_CONSTS = {}  # (device, coefficient bytes) -> [C,5] device constants
+
+
+def _fisheye_constants(k, device):
+    """[C,5] fp32 on the device: each row k1 k2 k3 k4 theta_max.  Copied from pinned memory without blocking the host
+    and kept per (device, coefficients), so a camera's constants are uploaded once."""
+    import numpy as np
+
+    k = np.ascontiguousarray(np.reshape(k, (-1, 4)), np.float32)
+    key = (str(device), k.tobytes())
+    t = _FISHEYE_CONSTS.get(key)
+    if t is None:
+        lim = [native().fisheye_theta_max([float(v) for v in row]) for row in k]
+        host = torch.from_numpy(np.concatenate([k, np.asarray(lim, np.float32)[:, None]], 1)).pin_memory()
+        t = host.to(device, non_blocking=True)
+        if len(_FISHEYE_CONSTS) >= 64:
+            _FISHEYE_CONSTS.clear()
+        _FISHEYE_CONSTS[key] = t
+    return t
 
 
 class _ProjectGaussians(torch.autograd.Function):
@@ -327,9 +384,12 @@ class _ProjectGaussians(torch.autograd.Function):
                 centre = torch.linalg.inv_ex(camera_T_world)[0][:3, 3].contiguous()
         with _stage(state, "preprocess_fwd"):
             # tile_mask / tile_win: the tiles each gaussian hits, tested once here and only expanded by the pair emission
-            records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(
-                xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
-                pad, mh, depth_base, True, state.mode, state.filter3d)
+            args = (xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
+                    pad, mh, depth_base, True, state.mode, state.filter3d)
+            if state.fisheye is None:
+                records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(*args)
+            else:
+                records, zkey, visible, scan, tile_mask, tile_win = ext.fisheye_preprocess_forward(*args, state.fisheye)
         record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])  # a backward pass can follow
         background = state.background
 
@@ -429,10 +489,12 @@ class _ProjectGaussians(torch.autograd.Function):
         if grad_uv is not None and st.M > 0:
             guv = grad_uv.contiguous()
         with _stage(st, "preprocess_bwd"):
-            grads = native().fused_preprocess_backward(slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K,
-                                                       centre, st.visible, st.grad_out, guv,
-                                                       st.scan if guv is not None else None, not st.uv_grad_emitted,
-                                                       st.mode, st.filter3d)
+            args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
+                    guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
+            if st.fisheye is None:
+                grads = native().fused_preprocess_backward(*args)
+            else:
+                grads = native().fisheye_preprocess_backward(*args, st.fisheye)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
@@ -516,7 +578,7 @@ class _CompositeTiles(torch.autograd.Function):
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
               render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
-              features=None):
+              features=None, fisheye=None):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
@@ -567,7 +629,25 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     process the channels in chunks of 4, each chunk walking the tile's pairs again.  The image, mask, uv, depth /
     alpha, weight statistics and all other gradients are unchanged; combines with render_depth_alpha, antialiased,
     filter3d, weight_stats, return_state and grad_out, not with absgrad (ValueError).  fp32 and precomputed SH colours
-    only."""
+    only.
+
+    fisheye: COLMAP's OPENCV_FISHEYE (Kannala-Brandt) camera instead of the pinhole, k = (k1, k2, k3, k4) =
+    params[4:8] of the COLMAP camera as 4 host numbers (a sequence or a CPU tensor [4]; fx fy cx cy stay in camera.K).
+    A camera-frame point (x, y, z) projects to u = fx (theta_d / rho) x + cx, v = fy (theta_d / rho) y + cy with
+    rho = |(x, y)|, theta = atan2(rho, z), theta_d = theta (1 + k1 theta^2 + k2 theta^4 + k3 theta^6 + k4 theta^8);
+    k = 0 is the equidistant fisheye, not the pinhole.  The 2-D covariance uses the Jacobian of that projection at the
+    mean (EWA), and a gaussian at theta >= fisheye_theta_max(k), where the model folds back, is culled on top of the
+    near / far / padding rules.  Depth keys, the depth map and the SH view direction keep camera-frame z and the
+    position; uv and uv.grad are the fisheye pixel coordinates and their gradient; K, the pose and k get no gradient
+    (DESIGN.md 3.19).  The coefficients are constants of the camera, uploaded once per camera without synchronising
+    with the device.  Combines with every other option.  None (the default) is the pinhole.  A CUDA tensor, a wrong
+    shape or non-finite coefficients raise ValueError; fp32 and precomputed SH colours only."""
+    if fisheye is not None:
+        if gaussians.xyz.dtype != torch.float32:
+            raise TypeError("fisheye needs fp32 inputs (the fused rasterizer's per-gaussian stages project through it)")
+        if gaussians.sh is not None and not use_sh_precompute:
+            raise ValueError("fisheye needs use_sh_precompute=True (per-pixel SH colours are not supported)")
+        fisheye = _fisheye_coefficients(fisheye)
     if features is not None:
         if not torch.is_tensor(features):
             raise TypeError("features must be a torch tensor [N, D]")
@@ -635,6 +715,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
+    state.fisheye = None if fisheye is None else _fisheye_constants(fisheye, gaussians.xyz.device)
     state.weight_stats = weight_stats
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
@@ -724,6 +805,7 @@ class _BatchState:
         self.speculation_overflowed = False
         self.mode = 0
         self.filter3d = None
+        self.fisheye = None      # fisheye cameras: [C,5] constants on the device (_fisheye_constants)
         self.views = []
         self.images = self.depth = self.alpha = None
 
@@ -749,9 +831,13 @@ class _ProjectBatch(torch.autograd.Function):
             else:
                 centre = torch.stack([torch.linalg.inv_ex(camera_T_world[c])[0][:3, 3] for c in range(C)])
         with _stage(state, "preprocess_fwd"):
-            records, zkey, visible, scan, tile_mask, tile_win = ext.batch_preprocess_forward(
-                xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
-                pad, mh, depth_base, state.mode, state.filter3d)
+            args = (xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
+                    pad, mh, depth_base, state.mode, state.filter3d)
+            if state.fisheye is None:
+                records, zkey, visible, scan, tile_mask, tile_win = ext.batch_preprocess_forward(*args)
+            else:
+                records, zkey, visible, scan, tile_mask, tile_win = ext.batch_fisheye_preprocess_forward(
+                    *args, state.fisheye)
         record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])
         background = state.background
         depth_mode = bool(state.mode & ext.MODE_DEPTH_ALPHA)
@@ -851,10 +937,12 @@ class _ProjectBatch(torch.autograd.Function):
         if grad_uv is not None and grad_uv.shape[0] > 0:
             guv = grad_uv.contiguous()
         with _stage(st, "preprocess_bwd"):
-            grads = native().batch_preprocess_backward(slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world,
-                                                       K, centre, st.visible, st.grad_out, guv,
-                                                       st.scan if guv is not None else None, not st.uv_grad_emitted,
-                                                       st.mode, st.filter3d)
+            args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
+                    guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
+            if st.fisheye is None:
+                grads = native().batch_preprocess_backward(*args)
+            else:
+                grads = native().batch_fisheye_preprocess_backward(*args, st.fisheye)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]
@@ -945,7 +1033,7 @@ def _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, back
 def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
                     use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
                     render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
-                    features=None):
+                    features=None, fisheye=None):
     """C cameras of one scene in one call: rasterize()'s nine positional arguments with camera_T_world [C,4,4]
     (C >= 1), camera.K [3,3] (shared) or [C,3,3], camera.height / width shared, background_rgb [3] or [C,3].
 
@@ -968,9 +1056,14 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
     Supports render_depth_alpha, antialiased, absgrad, filter3d ([N], one filter for all views), return_state,
     profile and grad_out.  weight_stats and features raise ValueError (use rasterize per view), fp64 inputs
     TypeError, per-pixel SH (use_sh_precompute=False) ValueError, and so do poses, K or backgrounds of the wrong
-    shape (ValueError), dtype (TypeError) or device (ValueError)."""
+    shape (ValueError), dtype (TypeError) or device (ValueError).
+
+    fisheye: OPENCV_FISHEYE cameras as in rasterize(), k [4] shared by every view or [C,4] one row per view (host
+    values: a sequence or a CPU tensor); view c is then bit-identical to rasterize(..., fisheye=k_c)."""
     C = _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, background_rgb, filter3d, weight_stats,
                           features)
+    if fisheye is not None:
+        fisheye = _fisheye_coefficients(fisheye, C)
     ext = native()
     K = camera.K if camera.K.dim() == 3 else camera.K.expand(C, 3, 3)
     state = _BatchState(profile)
@@ -978,6 +1071,7 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
+    state.fisheye = None if fisheye is None else _fisheye_constants(fisheye, gaussians.xyz.device)
     state.background = (background_rgb if background_rgb.dim() == 2 else background_rgb.expand(C, 3)).contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))
