@@ -5,9 +5,10 @@
   libgsr_features.so        the feature-channel tile kernels (include/gsr_features.h), same flags
   libgsr_batch.so           the multi-view per-gaussian kernels of rasterize_batch (include/gsr_batch.h), same flags
   libgsr_fisheye.so         the per-gaussian kernels for fisheye cameras (include/gsr_fisheye.h), same flags
+  libgsr_distortion.so      the per-gaussian kernels for radial-tangential lens distortion (include/gsr_distortion.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all six; `build(force=False)` is incremental.
+`python -m gaussian_splatting_b200.build` builds all seven; `build(force=False)` is incremental.
 """
 from __future__ import annotations
 
@@ -29,6 +30,7 @@ SELECTIVE_LIB = PKG / "libgsr_selective_adam.so"
 FEATURES_LIB = PKG / "libgsr_features.so"
 BATCH_LIB = PKG / "libgsr_batch.so"
 FISHEYE_LIB = PKG / "libgsr_fisheye.so"
+DISTORTION_LIB = PKG / "libgsr_distortion.so"
 
 CU_SOURCES = [
     "gsr_pergaussian.cu",
@@ -64,8 +66,14 @@ BATCH_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [ROOT / "include" /
                                                                ROOT / "include" / "gsr_batch.h"]
 FISHEYE_SOURCES = ["gsr_fisheye.cu"]
 FISHEYE_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_fisheye.cuh",
+                                                                 CSRC / "gsr_poly_roots.h",
                                                                  ROOT / "include" / "gsr_b200.h",
                                                                  ROOT / "include" / "gsr_fisheye.h"]
+DISTORTION_SOURCES = ["gsr_distortion.cu"]
+DISTORTION_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_distortion.cuh",
+                                                                    CSRC / "gsr_poly_roots.h",
+                                                                    ROOT / "include" / "gsr_b200.h",
+                                                                    ROOT / "include" / "gsr_distortion.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -146,6 +154,11 @@ def build_fisheye_lib(force: bool = False, verbose: bool = False) -> Path:
     return _build_cuda_lib(FISHEYE_LIB, FISHEYE_SOURCES, FISHEYE_HEADERS, "fisheye_lib.sha256", force, verbose)
 
 
+def build_distortion_lib(force: bool = False, verbose: bool = False) -> Path:
+    return _build_cuda_lib(DISTORTION_LIB, DISTORTION_SOURCES, DISTORTION_HEADERS, "distortion_lib.sha256", force,
+                           verbose)
+
+
 def build_ext(force: bool = False) -> Path:
     import torch  # noqa: F401  (needed for include/library paths)
     from torch.utils import cpp_extension as ce
@@ -157,7 +170,7 @@ def build_ext(force: bool = False) -> Path:
     stamp = OBJ / "ext.sha256"
     want = _digest([src, ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h",
                     ROOT / "include" / "gsr_features.h", ROOT / "include" / "gsr_batch.h",
-                    ROOT / "include" / "gsr_fisheye.h"], torch.__version__)
+                    ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -169,6 +182,7 @@ def build_ext(force: bool = False) -> Path:
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
         f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", "-lgsr_fisheye",
+        "-lgsr_distortion",
         f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",
@@ -193,6 +207,7 @@ def build(force: bool = False, verbose: bool = False):
     build_features_lib(force=force, verbose=verbose)
     build_batch_lib(force=force, verbose=verbose)
     build_fisheye_lib(force=force, verbose=verbose)
+    build_distortion_lib(force=force, verbose=verbose)
     ext = build_ext(force=force)
     return lib, ext
 

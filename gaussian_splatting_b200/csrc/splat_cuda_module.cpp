@@ -15,6 +15,7 @@
 #include "../../include/gsr_features.h"
 #include "../../include/gsr_batch.h"
 #include "../../include/gsr_fisheye.h"
+#include "../../include/gsr_distortion.h"
 
 namespace {
 
@@ -445,24 +446,32 @@ static const float* filter3d_ptr(const c10::optional<torch::Tensor>& filter3d, i
 
 // returns [records [N,12], depth_key [N] i32-viewed u32, visible [N] u8, scan [N] i64-viewed u64] and, with_tiles,
 // also [tile_mask [N] i64-viewed u64, tile_win [N] i32-viewed u32].  mode: GSR_MODE_* bits
-// the fisheye constants of C views ({k1, k2, k3, k4, theta_max} each, fp32 on xyz's device), or NULL
-static const float* fisheye_ptr(const c10::optional<torch::Tensor>& fisheye, int64_t C, const torch::Tensor& xyz) {
-    if (!fisheye.has_value()) return nullptr;
-    const torch::Tensor& f = *fisheye;
+// The camera model of the per-gaussian stages: the pinhole (libgsr_b200.so, libgsr_batch.so) or a lens whose
+// per-view constants the lens library's entry points read: OPENCV_FISHEYE (libgsr_fisheye.so, {k1, k2, k3, k4,
+// theta_max}) or OPENCV radial-tangential distortion (libgsr_distortion.so, {k1, k2, p1, p2, k3, r2_max}).
+enum class Lens { Pinhole, Fisheye, Distortion };
+
+// the lens constants of C views (fp32 on xyz's device), or NULL for the pinhole
+static const float* lens_ptr(Lens lens, const c10::optional<torch::Tensor>& consts, int64_t C,
+                             const torch::Tensor& xyz) {
+    if (lens == Lens::Pinhole) return nullptr;
+    TORCH_CHECK(consts.has_value(), "a lens needs its constants");
+    const torch::Tensor& f = *consts;
+    const int64_t per_view = lens == Lens::Fisheye ? GSR_FISHEYE_CONSTS : GSR_DISTORTION_CONSTS;
+    const char* name = lens == Lens::Fisheye ? "fisheye" : "distortion";
     CHECK_VALID_INPUT(f); CHECK_FLOAT_TENSOR(f);
-    TORCH_CHECK(f.numel() == C * GSR_FISHEYE_CONSTS, "fisheye constants must hold ", GSR_FISHEYE_CONSTS,
-                " floats per view");
-    TORCH_CHECK(f.device() == xyz.device(), "fisheye constants must be on the gaussians' device");
+    TORCH_CHECK(f.numel() == C * per_view, name, " constants must hold ", per_view, " floats per view");
+    TORCH_CHECK(f.device() == xyz.device(), name, " constants must be on the gaussians' device");
     return f.data_ptr<float>();
 }
 
-// fe: the fisheye constants (gsr_fisheye_preprocess_forward) or NULL (the pinhole gsr_preprocess_forward)
+// lens: the camera model; lc: its constants (gsr_fisheye_ / gsr_distortion_preprocess_forward), none for the pinhole
 static std::vector<torch::Tensor> preprocess_forward(
     torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, c10::optional<torch::Tensor> fisheye) {
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, Lens lens, c10::optional<torch::Tensor> lc) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc); CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -511,7 +520,7 @@ static std::vector<torch::Tensor> preprocess_forward(
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
     const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = fisheye_ptr(fisheye, 1, xyz);
+    const float* fe = lens_ptr(lens, lc, 1, xyz);
 #define GSR_FWD_ARGS                                                                                                  \
     (int)mode, N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), \
         f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world), F32PTR(K), centre_ptr, (int)H, (int)W,                   \
@@ -519,8 +528,11 @@ static std::vector<torch::Tensor> preprocess_forward(
         F32PTR(records), (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),                                \
         (uint64_t*)scan.data_ptr<int64_t>(), with_tiles && N > 0 ? (uint64_t*)tile_mask.data_ptr<int64_t>() : nullptr, \
         with_tiles && N > 0 ? (uint32_t*)tile_win.data_ptr<int>() : nullptr, temp.data_ptr(), tb
-    if (fe != nullptr)
+    if (lens == Lens::Fisheye)
         check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, fe, cur_stream()), "gsr_fisheye_preprocess_forward");
+    else if (lens == Lens::Distortion)
+        check_rc(gsr_distortion_preprocess_forward(GSR_FWD_ARGS, fe, cur_stream()),
+                 "gsr_distortion_preprocess_forward");
     else
         check_rc(gsr_preprocess_forward(GSR_FWD_ARGS, cur_stream()), "gsr_preprocess_forward");
 #undef GSR_FWD_ARGS
@@ -536,7 +548,7 @@ std::vector<torch::Tensor> fused_preprocess_forward(
     bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d) {
     return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
                               K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
-                              with_tiles, mode, filter3d, c10::nullopt);
+                              with_tiles, mode, filter3d, Lens::Pinhole, c10::nullopt);
 }
 
 // fused_preprocess_forward for a fisheye camera: fisheye [5] = {k1, k2, k3, k4, theta_max} on xyz's device
@@ -548,7 +560,7 @@ std::vector<torch::Tensor> fisheye_preprocess_forward(
     bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
     return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
                               K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
-                              with_tiles, mode, filter3d, fisheye);
+                              with_tiles, mode, filter3d, Lens::Fisheye, fisheye);
 }
 
 // (M, P known) -> the sorted pair list the tile renderers read records through, tile ranges [n_tiles+1] i32,
@@ -781,7 +793,7 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
                                                       c10::optional<torch::Tensor> grad_uv_compact,
                                                       c10::optional<torch::Tensor> scan, bool use_slab_uv,
                                                       int64_t mode, c10::optional<torch::Tensor> filter3d,
-                                                      c10::optional<torch::Tensor> fisheye) {
+                                                      Lens lens, c10::optional<torch::Tensor> lc) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     const int64_t N = xyz.size(0);
     TORCH_CHECK(slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ", GSR_GRAD_ROW_FLOATS,
@@ -826,14 +838,17 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
     const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = fisheye_ptr(fisheye, 1, xyz);
+    const float* fe = lens_ptr(lens, lc, 1, xyz);
 #define GSR_BWD_ARGS                                                                                                 \
     (int)mode, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d,          \
         F32PTR(camera_T_world), F32PTR(K), camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,   \
         visible.data_ptr<uint8_t>(), slab.data_ptr<float>(), use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr,            \
         F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    if (fe != nullptr)
+    if (lens == Lens::Fisheye)
         check_rc(gsr_fisheye_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()), "gsr_fisheye_preprocess_backward");
+    else if (lens == Lens::Distortion)
+        check_rc(gsr_distortion_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
+                 "gsr_distortion_preprocess_backward");
     else
         check_rc(gsr_preprocess_backward(GSR_BWD_ARGS, cur_stream()), "gsr_preprocess_backward");
 #undef GSR_BWD_ARGS
@@ -853,7 +868,8 @@ std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::
                                                      c10::optional<torch::Tensor> scan, bool use_slab_uv,
                                                      int64_t mode, c10::optional<torch::Tensor> filter3d) {
     return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, c10::nullopt);
+                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Pinhole,
+                               c10::nullopt);
 }
 
 // fused_preprocess_backward for a fisheye camera (the forward's fisheye constants)
@@ -868,7 +884,8 @@ std::vector<torch::Tensor> fisheye_preprocess_backward(torch::Tensor slab, torch
                                                        int64_t mode, c10::optional<torch::Tensor> filter3d,
                                                        torch::Tensor fisheye) {
     return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, fisheye);
+                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Fisheye,
+                               fisheye);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -892,7 +909,7 @@ static std::vector<torch::Tensor> batch_forward(
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, c10::optional<torch::Tensor> fisheye) {
+    c10::optional<torch::Tensor> filter3d, Lens lens, c10::optional<torch::Tensor> lc) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -941,7 +958,7 @@ static std::vector<torch::Tensor> batch_forward(
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
     const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = fisheye_ptr(fisheye, C, xyz);
+    const float* fe = lens_ptr(lens, lc, C, xyz);
     for (int64_t c = 0; c < C && N > 0; ++c) {
 #define GSR_FWD_ARGS                                                                                                \
     (int)mode, N, n_rest, F32PTR(xyz), cam_ptr ? cam_ptr + c * R * 3 : nullptr, N - (int)R, F32PTR(quaternion),     \
@@ -950,9 +967,12 @@ static std::vector<torch::Tensor> batch_forward(
         (float)far_thresh, (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base, F32PTR(records[c]),       \
         (uint32_t*)zkey[c].data_ptr<int>(), visible[c].data_ptr<uint8_t>(), (uint64_t*)scan[c].data_ptr<int64_t>(),  \
         (uint64_t*)tile_mask[c].data_ptr<int64_t>(), (uint32_t*)tile_win[c].data_ptr<int>(), temp.data_ptr(), tb
-        if (fe != nullptr)
+        if (lens == Lens::Fisheye)
             check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, fe + GSR_FISHEYE_CONSTS * c, cur_stream()),
                      "gsr_fisheye_preprocess_forward");
+        else if (lens == Lens::Distortion)
+            check_rc(gsr_distortion_preprocess_forward(GSR_FWD_ARGS, fe + GSR_DISTORTION_CONSTS * c, cur_stream()),
+                     "gsr_distortion_preprocess_forward");
         else
             check_rc(gsr_preprocess_forward(GSR_FWD_ARGS, cur_stream()), "gsr_preprocess_forward");
 #undef GSR_FWD_ARGS
@@ -968,7 +988,7 @@ std::vector<torch::Tensor> batch_preprocess_forward(
     c10::optional<torch::Tensor> filter3d) {
     return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
                          camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
-                         filter3d, c10::nullopt);
+                         filter3d, Lens::Pinhole, c10::nullopt);
 }
 
 // batch_preprocess_forward for fisheye cameras: fisheye [C,5] = {k1, k2, k3, k4, theta_max} per view
@@ -980,7 +1000,7 @@ std::vector<torch::Tensor> batch_fisheye_preprocess_forward(
     c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
     return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
                          camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
-                         filter3d, fisheye);
+                         filter3d, Lens::Fisheye, fisheye);
 }
 
 // fused_render_backward of every view into one stacked slab [C, N*12]: grad_image [C,H,W,3], per view the forward's
@@ -1048,8 +1068,8 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
                                                  torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
                                                  c10::optional<torch::Tensor> grad_uv_compact,
                                                  c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-                                                 c10::optional<torch::Tensor> filter3d,
-                                                 c10::optional<torch::Tensor> fisheye) {
+                                                 c10::optional<torch::Tensor> filter3d, Lens lens,
+                                                 c10::optional<torch::Tensor> lc) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(visible);
@@ -1101,15 +1121,18 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
     const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = fisheye_ptr(fisheye, C, xyz);
+    const float* fe = lens_ptr(lens, lc, C, xyz);
 #define GSR_BWD_ARGS                                                                                                \
     (int)mode, (int)C, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d,  \
         F32PTR(camera_T_world), F32PTR(K), centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab),                    \
         use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o),           \
         F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    if (fe != nullptr)
+    if (lens == Lens::Fisheye)
         check_rc(gsr_fisheye_batch_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
                  "gsr_fisheye_batch_preprocess_backward");
+    else if (lens == Lens::Distortion)
+        check_rc(gsr_distortion_batch_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
+                 "gsr_distortion_batch_preprocess_backward");
     else
         check_rc(gsr_batch_preprocess_backward(GSR_BWD_ARGS, cur_stream()), "gsr_batch_preprocess_backward");
 #undef GSR_BWD_ARGS
@@ -1129,7 +1152,8 @@ std::vector<torch::Tensor> batch_preprocess_backward(torch::Tensor slab, torch::
                                                      c10::optional<torch::Tensor> scan, bool use_slab_uv,
                                                      int64_t mode, c10::optional<torch::Tensor> filter3d) {
     return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, c10::nullopt);
+                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Pinhole,
+                          c10::nullopt);
 }
 
 // batch_preprocess_backward for fisheye cameras (the forward's [C,5] fisheye constants)
@@ -1140,7 +1164,8 @@ std::vector<torch::Tensor> batch_fisheye_preprocess_backward(
     c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
     c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
     return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, fisheye);
+                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Fisheye,
+                          fisheye);
 }
 
 // gsr_fisheye_theta_max of 4 coefficients (host floats)
@@ -1148,6 +1173,59 @@ double fisheye_theta_max(std::vector<double> k) {
     TORCH_CHECK(k.size() == 4, "fisheye needs 4 coefficients k1 k2 k3 k4");
     const float kf[4] = {(float)k[0], (float)k[1], (float)k[2], (float)k[3]};
     return (double)gsr_fisheye_theta_max(kf);
+}
+
+// The radial-tangential (COLMAP OPENCV) counterparts: distortion [C,6] = {k1, k2, p1, p2, k3, r2_max} per view on
+// xyz's device, C = 1 for the single-view functions.
+std::vector<torch::Tensor> distortion_preprocess_forward(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
+    return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
+                              K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
+                              with_tiles, mode, filter3d, Lens::Distortion, distortion);
+}
+
+std::vector<torch::Tensor> distortion_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
+    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Distortion,
+                               distortion);
+}
+
+std::vector<torch::Tensor> batch_distortion_preprocess_forward(
+    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
+    return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
+                         camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
+                         filter3d, Lens::Distortion, distortion);
+}
+
+std::vector<torch::Tensor> batch_distortion_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
+    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Distortion,
+                          distortion);
+}
+
+// gsr_distortion_r2_max of 5 coefficients k1 k2 p1 p2 k3 (host floats)
+double distortion_r2_max(std::vector<double> k) {
+    TORCH_CHECK(k.size() == 5, "distortion needs 5 coefficients k1 k2 p1 p2 k3");
+    const float kf[5] = {(float)k[0], (float)k[1], (float)k[2], (float)k[3], (float)k[4]};
+    return (double)gsr_distortion_r2_max(kf);
 }
 
 // Mip-Splatting's 3-D filter size per gaussian (gsr_filter3d): xyz [N,3], camera_T_world [C,4,4], K [C,3,3],
@@ -1607,6 +1685,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("batch_fisheye_preprocess_backward", &batch_fisheye_preprocess_backward,
           "batch_preprocess_backward for OPENCV_FISHEYE cameras (gsr_fisheye_batch_preprocess_backward)");
     m.def("fisheye_theta_max", &fisheye_theta_max, "the fisheye cull limit of 4 coefficients (gsr_fisheye_theta_max)");
+    m.def("distortion_preprocess_forward", &distortion_preprocess_forward,
+          "fused_preprocess_forward for an OPENCV (radial-tangential) camera (gsr_distortion_preprocess_forward)");
+    m.def("distortion_preprocess_backward", &distortion_preprocess_backward,
+          "fused_preprocess_backward for an OPENCV (radial-tangential) camera (gsr_distortion_preprocess_backward)");
+    m.def("batch_distortion_preprocess_forward", &batch_distortion_preprocess_forward,
+          "batch_preprocess_forward for OPENCV (radial-tangential) cameras, [C,6] constants");
+    m.def("batch_distortion_preprocess_backward", &batch_distortion_preprocess_backward,
+          "batch_preprocess_backward for OPENCV cameras (gsr_distortion_batch_preprocess_backward)");
+    m.def("distortion_r2_max", &distortion_r2_max,
+          "the radial fold limit s = r^2 of 5 coefficients k1 k2 p1 p2 k3 (gsr_distortion_r2_max)");
     m.def("filter3d", &filter3d, "Mip-Splatting's 3-D filter size per gaussian from the training cameras (gsr_filter3d)",
           py::arg("xyz"), py::arg("camera_T_world"), py::arg("K"), py::arg("width"), py::arg("height"),
           py::arg("near"), py::arg("margin"), py::arg("variance"));

@@ -242,7 +242,7 @@ class _ViewState:
                  "records", "keys_sorted", "id_bits",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
                  "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad", "filter3d",
-                 "weight_stats", "fisheye")
+                 "weight_stats", "lens")
 
     @property
     def ids_sorted(self):
@@ -275,7 +275,7 @@ class _ViewState:
         # per-gaussian stages: filter3d [N], a constant)
         self.mode = 0
         self.filter3d = None
-        self.fisheye = None     # fisheye cameras: {k1, k2, k3, k4, theta_max} on the device (_fisheye_constants)
+        self.lens = None        # a lens model: (name, its constants on the device) (_lens_constants)
         self.depth = self.alpha = None
         self.uv_absgrad = None  # MODE_ABSGRAD: [M,2], set by every render backward
         self.weight_stats = None  # optional densify.WeightStats the render forward accumulates into
@@ -300,59 +300,86 @@ class _stage:
             self.rec.append((self.name, self.e0, self.e1))
 
 
-# ---- fisheye cameras ---------------------------------------------------------------------------------------------------
+# ---- lens models: fisheye and radial-tangential distortion -------------------------------------------------------------
+# name -> (coefficient names, the native cull limit of one row of coefficients)
+_LENSES = {"fisheye": ("k1 k2 k3 k4", "fisheye_theta_max"), "distortion": ("k1 k2 p1 p2 k3", "distortion_r2_max")}
+
+
 def fisheye_theta_max(k) -> float:
     """The cull limit of COLMAP's OPENCV_FISHEYE model with coefficients k = (k1, k2, k3, k4): the first theta in
     (0, pi/2) where d theta_d / d theta = 1 + 3 k1 theta^2 + 5 k2 theta^4 + 7 k3 theta^6 + 9 k4 theta^8 reaches 0 (beyond
     it the model folds points back into the image), else pi/2; found in fp64 for the fp32 coefficients and rounded down
     to fp32 (gsr_fisheye_theta_max, the value the kernels cull with)."""
-    return native().fisheye_theta_max([float(v) for v in _fisheye_coefficients(k)])
+    return native().fisheye_theta_max([float(v) for v in _lens_coefficients("fisheye", k)])
 
 
-def _fisheye_coefficients(fisheye, C=None):
-    """The host coefficients as float32 numpy [4] (C None) or [C,4]; ValueError for a CUDA tensor, a wrong shape or
-    non-finite values.  Batches take [4] (shared) or [C,4]."""
+def distortion_r2_max(k) -> float:
+    """The cull limit of COLMAP's OPENCV (radial-tangential) model with coefficients k = (k1, k2, p1, p2, k3): the
+    smallest positive s = r^2 where d (r radial(r^2)) / dr = 1 + 3 k1 s + 5 k2 s^2 + 7 k3 s^3 reaches 0 (beyond it
+    barrel distortion folds points back into the image), else +inf; found in fp64 for the fp32 coefficients and
+    rounded down to fp32 (gsr_distortion_r2_max, the value the kernels cull with).  The tangential p1 p2 do not enter
+    it: COLMAP's are of order 1e-3."""
+    return native().distortion_r2_max([float(v) for v in _lens_coefficients("distortion", k)])
+
+
+def _lens_coefficients(lens, k, C=None):
+    """A lens's host coefficients as float32 numpy [n] (C None) or [C,n]; ValueError for a CUDA tensor, a wrong shape
+    or non-finite values.  Batches take [n] (shared) or [C,n]."""
     import numpy as np
 
-    if torch.is_tensor(fisheye):
-        if fisheye.device.type != "cpu":
-            raise ValueError("fisheye coefficients are camera constants read on the host: pass a CPU tensor or a "
-                             "sequence, not a tensor on " + str(fisheye.device))
-        k = fisheye.detach().to(torch.float64).numpy()
+    names = _LENSES[lens][0]
+    n = len(names.split())
+    if torch.is_tensor(k):
+        if k.device.type != "cpu":
+            raise ValueError(f"{lens} coefficients are camera constants read on the host: pass a CPU tensor or a "
+                             "sequence, not a tensor on " + str(k.device))
+        k = k.detach().to(torch.float64).numpy()
     else:
         try:
-            k = np.asarray(fisheye, dtype=np.float64)
+            k = np.asarray(k, dtype=np.float64)
         except (TypeError, ValueError) as e:
-            raise ValueError(f"fisheye must be 4 numbers k1 k2 k3 k4: {e}") from None
-    shapes = ((4,),) if C is None else ((4,), (C, 4))
+            raise ValueError(f"{lens} must be {n} numbers {names}: {e}") from None
+    shapes = ((n,),) if C is None else ((n,), (C, n))
     if k.shape not in shapes:
-        want = "[4]" if C is None else f"[4] or [{C},4]"
-        raise ValueError(f"fisheye has shape {list(k.shape)} but must be {want} (COLMAP's k1 k2 k3 k4)")
+        want = f"[{n}]" if C is None else f"[{n}] or [{C},{n}]"
+        raise ValueError(f"{lens} has shape {list(k.shape)} but must be {want} ({names})")
     with np.errstate(over="ignore"):
         k32 = k.astype(np.float32)
     if not np.isfinite(k32).all():
-        raise ValueError("fisheye coefficients must be finite (in fp32)")
-    return k32 if C is None or k.ndim == 2 else np.broadcast_to(k32, (C, 4))
+        raise ValueError(f"{lens} coefficients must be finite (in fp32)")
+    return k32 if C is None or k.ndim == 2 else np.broadcast_to(k32, (C, n))
 
 
-_FISHEYE_CONSTS = {}  # (device, coefficient bytes) -> [C,5] device constants
+def _lens_arg(fisheye, distortion, C=None):
+    """None (the pinhole) or (lens name, coefficients as _lens_coefficients returns them)."""
+    if fisheye is not None and distortion is not None:
+        raise ValueError("pass either fisheye or distortion: a camera has one lens model")
+    if fisheye is not None:
+        return "fisheye", _lens_coefficients("fisheye", fisheye, C)
+    if distortion is not None:
+        return "distortion", _lens_coefficients("distortion", distortion, C)
+    return None
 
 
-def _fisheye_constants(k, device):
-    """[C,5] fp32 on the device: each row k1 k2 k3 k4 theta_max.  Copied from pinned memory without blocking the host
-    and kept per (device, coefficients), so a camera's constants are uploaded once."""
+_LENS_CONSTS = {}  # (lens, device, coefficient bytes) -> [C, n+1] device constants
+
+
+def _lens_constants(lens, k, device):
+    """[C, n+1] fp32 on the device: each row the n coefficients and the lens's cull limit.  Copied from pinned memory
+    without blocking the host and kept per (lens, device, coefficients), so a camera's constants are uploaded once."""
     import numpy as np
 
-    k = np.ascontiguousarray(np.reshape(k, (-1, 4)), np.float32)
-    key = (str(device), k.tobytes())
-    t = _FISHEYE_CONSTS.get(key)
+    limit = getattr(native(), _LENSES[lens][1])
+    k = np.ascontiguousarray(np.reshape(k, (-1, np.shape(k)[-1])), np.float32)
+    key = (lens, str(device), k.tobytes())
+    t = _LENS_CONSTS.get(key)
     if t is None:
-        lim = [native().fisheye_theta_max([float(v) for v in row]) for row in k]
+        lim = [limit([float(v) for v in row]) for row in k]
         host = torch.from_numpy(np.concatenate([k, np.asarray(lim, np.float32)[:, None]], 1)).pin_memory()
         t = host.to(device, non_blocking=True)
-        if len(_FISHEYE_CONSTS) >= 64:
-            _FISHEYE_CONSTS.clear()
-        _FISHEYE_CONSTS[key] = t
+        if len(_LENS_CONSTS) >= 64:
+            _LENS_CONSTS.clear()
+        _LENS_CONSTS[key] = t
     return t
 
 
@@ -386,10 +413,12 @@ class _ProjectGaussians(torch.autograd.Function):
             # tile_mask / tile_win: the tiles each gaussian hits, tested once here and only expanded by the pair emission
             args = (xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
                     pad, mh, depth_base, True, state.mode, state.filter3d)
-            if state.fisheye is None:
+            if state.lens is None:
                 records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(*args)
             else:
-                records, zkey, visible, scan, tile_mask, tile_win = ext.fisheye_preprocess_forward(*args, state.fisheye)
+                lens, consts = state.lens
+                fwd = ext.fisheye_preprocess_forward if lens == "fisheye" else ext.distortion_preprocess_forward
+                records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
         record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])  # a backward pass can follow
         background = state.background
 
@@ -491,10 +520,13 @@ class _ProjectGaussians(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            if st.fisheye is None:
+            if st.lens is None:
                 grads = native().fused_preprocess_backward(*args)
             else:
-                grads = native().fisheye_preprocess_backward(*args, st.fisheye)
+                lens, consts = st.lens
+                ext = native()
+                bwd = ext.fisheye_preprocess_backward if lens == "fisheye" else ext.distortion_preprocess_backward
+                grads = bwd(*args, consts)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
@@ -578,7 +610,7 @@ class _CompositeTiles(torch.autograd.Function):
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
               render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
-              features=None, fisheye=None):
+              features=None, fisheye=None, distortion=None):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
@@ -641,13 +673,24 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     position; uv and uv.grad are the fisheye pixel coordinates and their gradient; K, the pose and k get no gradient
     (DESIGN.md 3.19).  The coefficients are constants of the camera, uploaded once per camera without synchronising
     with the device.  Combines with every other option.  None (the default) is the pinhole.  A CUDA tensor, a wrong
-    shape or non-finite coefficients raise ValueError; fp32 and precomputed SH colours only."""
-    if fisheye is not None:
+    shape or non-finite coefficients raise ValueError; fp32 and precomputed SH colours only.
+
+    distortion: COLMAP's OPENCV radial-tangential camera (OpenCV's 5-coefficient model) instead of the pinhole,
+    k = (k1, k2, p1, p2, k3) in OpenCV's distCoeffs order as 5 host numbers; structs.camera_from_colmap builds it from
+    a COLMAP camera (OPENCV, FULL_OPENCV without rational terms, RADIAL, SIMPLE_RADIAL).  With a = x / z, b = y / z,
+    s = a^2 + b^2 and radial = 1 + k1 s + k2 s^2 + k3 s^3 a camera-frame point projects to u = fx a_d + cx,
+    v = fy b_d + cy, a_d = a radial + 2 p1 a b + p2 (s + 2 a^2), b_d = b radial + p1 (s + 2 b^2) + 2 p2 a b.  The 2-D
+    covariance uses the exact Jacobian of that projection at the mean, and a gaussian at s >= distortion_r2_max(k),
+    where barrel distortion folds back, is culled on top of the other rules.  Everything else is as for fisheye
+    (DESIGN.md 3.20); k = 0 runs the distortion kernels and gives the pinhole up to fp32 rounding.  Passing both
+    fisheye and distortion raises ValueError."""
+    lens = _lens_arg(fisheye, distortion)
+    if lens is not None:
         if gaussians.xyz.dtype != torch.float32:
-            raise TypeError("fisheye needs fp32 inputs (the fused rasterizer's per-gaussian stages project through it)")
+            raise TypeError(f"{lens[0]} needs fp32 inputs (the fused rasterizer's per-gaussian stages project through "
+                            "it)")
         if gaussians.sh is not None and not use_sh_precompute:
-            raise ValueError("fisheye needs use_sh_precompute=True (per-pixel SH colours are not supported)")
-        fisheye = _fisheye_coefficients(fisheye)
+            raise ValueError(f"{lens[0]} needs use_sh_precompute=True (per-pixel SH colours are not supported)")
     if features is not None:
         if not torch.is_tensor(features):
             raise TypeError("features must be a torch tensor [N, D]")
@@ -715,7 +758,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
-    state.fisheye = None if fisheye is None else _fisheye_constants(fisheye, gaussians.xyz.device)
+    state.lens = None if lens is None else (lens[0], _lens_constants(*lens, gaussians.xyz.device))
     state.weight_stats = weight_stats
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
@@ -805,7 +848,7 @@ class _BatchState:
         self.speculation_overflowed = False
         self.mode = 0
         self.filter3d = None
-        self.fisheye = None      # fisheye cameras: [C,5] constants on the device (_fisheye_constants)
+        self.lens = None         # a lens model: (name, [C, n+1] constants on the device) (_lens_constants)
         self.views = []
         self.images = self.depth = self.alpha = None
 
@@ -833,11 +876,13 @@ class _ProjectBatch(torch.autograd.Function):
         with _stage(state, "preprocess_fwd"):
             args = (xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
                     pad, mh, depth_base, state.mode, state.filter3d)
-            if state.fisheye is None:
+            if state.lens is None:
                 records, zkey, visible, scan, tile_mask, tile_win = ext.batch_preprocess_forward(*args)
             else:
-                records, zkey, visible, scan, tile_mask, tile_win = ext.batch_fisheye_preprocess_forward(
-                    *args, state.fisheye)
+                lens, consts = state.lens
+                fwd = (ext.batch_fisheye_preprocess_forward if lens == "fisheye"
+                       else ext.batch_distortion_preprocess_forward)
+                records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
         record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])
         background = state.background
         depth_mode = bool(state.mode & ext.MODE_DEPTH_ALPHA)
@@ -939,10 +984,14 @@ class _ProjectBatch(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            if st.fisheye is None:
+            if st.lens is None:
                 grads = native().batch_preprocess_backward(*args)
             else:
-                grads = native().batch_fisheye_preprocess_backward(*args, st.fisheye)
+                lens, consts = st.lens
+                ext = native()
+                bwd = (ext.batch_fisheye_preprocess_backward if lens == "fisheye"
+                       else ext.batch_distortion_preprocess_backward)
+                grads = bwd(*args, consts)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]
@@ -1033,7 +1082,7 @@ def _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, back
 def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
                     use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
                     render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
-                    features=None, fisheye=None):
+                    features=None, fisheye=None, distortion=None):
     """C cameras of one scene in one call: rasterize()'s nine positional arguments with camera_T_world [C,4,4]
     (C >= 1), camera.K [3,3] (shared) or [C,3,3], camera.height / width shared, background_rgb [3] or [C,3].
 
@@ -1059,11 +1108,11 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
     shape (ValueError), dtype (TypeError) or device (ValueError).
 
     fisheye: OPENCV_FISHEYE cameras as in rasterize(), k [4] shared by every view or [C,4] one row per view (host
-    values: a sequence or a CPU tensor); view c is then bit-identical to rasterize(..., fisheye=k_c)."""
+    values: a sequence or a CPU tensor); view c is then bit-identical to rasterize(..., fisheye=k_c).  distortion:
+    radial-tangential cameras likewise, k [5] or [C,5] (rasterize(..., distortion=k_c))."""
     C = _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, background_rgb, filter3d, weight_stats,
                           features)
-    if fisheye is not None:
-        fisheye = _fisheye_coefficients(fisheye, C)
+    lens = _lens_arg(fisheye, distortion, C)
     ext = native()
     K = camera.K if camera.K.dim() == 3 else camera.K.expand(C, 3, 3)
     state = _BatchState(profile)
@@ -1071,7 +1120,7 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
-    state.fisheye = None if fisheye is None else _fisheye_constants(fisheye, gaussians.xyz.device)
+    state.lens = None if lens is None else (lens[0], _lens_constants(*lens, gaussians.xyz.device))
     state.background = (background_rgb if background_rgb.dim() == 2 else background_rgb.expand(C, 3)).contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))

@@ -20,6 +20,54 @@ class Camera:
         self.K = K
 
 
+# COLMAP camera model -> its parameter names (colmap/src/colmap/sensor/models.h), for the models the fused rasterizer
+# projects through
+_COLMAP_PARAMS = {
+    "SIMPLE_PINHOLE": ("f", "cx", "cy"),
+    "PINHOLE": ("fx", "fy", "cx", "cy"),
+    "SIMPLE_RADIAL": ("f", "cx", "cy", "k"),
+    "RADIAL": ("f", "cx", "cy", "k1", "k2"),
+    "OPENCV": ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2"),
+    "FULL_OPENCV": ("fx", "fy", "cx", "cy", "k1", "k2", "p1", "p2", "k3", "k4", "k5", "k6"),
+    "OPENCV_FISHEYE": ("fx", "fy", "cx", "cy", "k1", "k2", "k3", "k4"),
+}
+
+
+def camera_from_colmap(model, width, height, params, device="cpu"):
+    """(Camera, lens_kwargs) for a COLMAP camera: `model` is COLMAP's model name, `params` its parameter list in
+    COLMAP's order.  K [3,3] fp32 on `device` holds fx fy cx cy; lens_kwargs is the keyword the lens needs for
+    rasterize / rasterize_batch: {} for SIMPLE_PINHOLE and PINHOLE, {"distortion": (k1, k2, p1, p2, k3)} for
+    SIMPLE_RADIAL, RADIAL, OPENCV and FULL_OPENCV, {"fisheye": (k1, k2, k3, k4)} for OPENCV_FISHEYE:
+
+        cam, lens = camera_from_colmap(c.model, c.width, c.height, c.params, "cuda")
+        image, mask, uv = rasterize(gaussians, T, cam, 0.3, 500.0, 100, 3.0, True, bg, **lens)
+
+    FULL_OPENCV is accepted only with k4 = k5 = k6 = 0 (the rational terms are not modelled).  Any other model, or a
+    parameter list of the wrong length, raises ValueError."""
+    name = str(model).upper()
+    if name not in _COLMAP_PARAMS:
+        raise ValueError(f"COLMAP camera model {model!r} is not supported: use one of {', '.join(_COLMAP_PARAMS)}")
+    params = [float(v) for v in params]
+    if len(params) != len(_COLMAP_PARAMS[name]):
+        raise ValueError(f"COLMAP {name} has {len(_COLMAP_PARAMS[name])} parameters "
+                         f"({' '.join(_COLMAP_PARAMS[name])}), got {len(params)}")
+    p = dict(zip(_COLMAP_PARAMS[name], params))
+    if "f" in p:
+        p["fx"] = p["fy"] = p["f"]
+    if name == "FULL_OPENCV" and (p["k4"], p["k5"], p["k6"]) != (0.0, 0.0, 0.0):
+        raise ValueError("COLMAP FULL_OPENCV with rational terms k4 k5 k6 != 0 is not supported")
+    K = torch.tensor([[p["fx"], 0.0, p["cx"]], [0.0, p["fy"], p["cy"]], [0.0, 0.0, 1.0]], dtype=torch.float32,
+                     device=device)
+    cam = Camera(int(width), int(height), K)
+    if name == "OPENCV_FISHEYE":
+        return cam, {"fisheye": (p["k1"], p["k2"], p["k3"], p["k4"])}
+    if name in ("SIMPLE_PINHOLE", "PINHOLE"):
+        return cam, {}
+    if name == "SIMPLE_RADIAL":
+        p["k1"] = p["k"]
+    return cam, {"distortion": tuple(p.get(k, 0.0) for k in ("k1", "k2", "p1", "p2", "k3"))}
+
+
 class Image:
     """An 8-bit RGB image with its camera id and world->camera pose (splat_py/structs.py:14-27)."""
 
