@@ -1724,4 +1724,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "(1 - ssim_frac) * L1 + ssim_frac * (1 - SSIM) forward -> (loss, L1, SSIM)");
     m.def("photometric_loss_backward", &photometric_loss_backward, "photometric loss backward -> gradient on pred");
     m.def("version", &version, "library version string");
+    m.def("contribution_mask_words",
+          [](int64_t P, int64_t H, int64_t W) { return (int64_t)gsr_contribution_mask_words(P, (int)H, (int)W); },
+          "32-bit words of the contribution masks of P pairs over an H x W image");
 }

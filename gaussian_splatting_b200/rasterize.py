@@ -143,6 +143,17 @@ def _pair_capacity(key):
     return min((cap + 127) // 128 * 128, 2**31 - 128)
 
 
+def _fit_masks(ext, rendered, P, H, W):
+    """The renderer's outputs of a speculative run that fitted its capacity, with the contribution masks cut to the
+    words of the P pairs actually binned (the buffer was sized for the capacity; the words past them stay zero), so that
+    the state does not depend on the pair counts of earlier views."""
+    rendered = tuple(rendered)
+    masks = rendered[3]
+    if masks.numel() == 0:
+        return rendered
+    return rendered[:3] + (masks.narrow(0, 0, ext.contribution_mask_words(P, H, W)),) + rendered[4:]
+
+
 def _note_pairs(key, P):
     hist = _PAIR_HISTORY.setdefault(key, [])
     hist.append(int(P))
@@ -484,6 +495,7 @@ class _ProjectGaussians(torch.autograd.Function):
                 ids_c, ranges_c, vis_c, uv_c, keys_c, idb = binned
                 binned = (ids_c.narrow(0, 0, P) if ids_c.numel() else ids_c, ranges_c, vis_c.narrow(0, 0, M),
                           uv_c.narrow(0, 0, M), keys_c, idb)
+                rendered = _fit_masks(ext, rendered, P, H, W)
         _note_pairs(key, P)
         ids_sorted, ranges, vis_idx, uv, keys_sorted, id_bits = binned
         state.records, state.keys_sorted, state.id_bits = records, keys_sorted, int(id_bits)
@@ -941,7 +953,8 @@ class _ProjectBatch(torch.autograd.Function):
                 else:
                     (ids_c, ranges_c, vis_c, uv_c, keys_c, idb), rendered = out[c]
                     out[c] = ((ids_c.narrow(0, 0, Ps[c]) if ids_c.numel() else ids_c, ranges_c,
-                               vis_c.narrow(0, 0, Ms[c]), uv_c.narrow(0, 0, Ms[c]), keys_c, idb), rendered)
+                               vis_c.narrow(0, 0, Ms[c]), uv_c.narrow(0, 0, Ms[c]), keys_c, idb),
+                              _fit_masks(ext, rendered, Ps[c], H, W))
         for P_ in Ps:
             _note_pairs(key, P_)
         views, uvs = [], []

@@ -71,19 +71,40 @@ def general_pose():
     return T.astype(np.float32)
 
 
-def exact_arithmetic_scene(n_exact=300, n_huge=12):
-    """Splats whose centre falls EXACTLY on a pixel centre and splats whose 2-D covariance determinant exceeds 1e18."""
+def exact_arithmetic_scene(n_exact=300, n_huge=12, H=64, W=64):
+    """Splats whose centre falls EXACTLY on a pixel centre and splats whose 2-D covariance determinant exceeds 1e18.
+
+    The tile renderers recompute a flagged pixel with the exact arithmetic (gsr_render.cu render_fwd): a listed
+    record with |det| outside [1e-18, 1e18] flags its whole warp, an exact centre (Mahalanobis numerator 0) the
+    pixels of its lane.  The n_huge splats are ~1800 world units wide at z = 2 with opacity sigmoid(-3) ~ 0.047:
+    those near the axis reach det ~ 1e19 px^4 and every pixel, those off the axis project to needles; together they
+    flag about two thirds of the 64 x 64 frame's warps and contribute to every pixel.  H x W other than 64 x 64: the
+    principal point stays an integer (W // 2, H // 2), so the exact centres still land on pixel centres."""
     rng = np.random.default_rng(7)
     sc = np_scene(3000, "tiny", sh_degree=0, seed=3, sigma_px=(2.0, 0.5, 0.5, 8.0))
-    sc["K"] = np.array([[64, 0, 32], [0, 64, 32], [0, 0, 1]], np.float32)  # powers of two: u = 64*x/z + 32 is exact
+    cx, cy = W // 2, H // 2
+    # powers of two: u = 64*x/z + cx is exact
+    sc["K"] = np.array([[64, 0, cx], [0, 64, cy], [0, 0, 1]], np.float32)
     sc["T"] = np.eye(4, dtype=np.float32)
+    sc["H"], sc["W"] = H, W
     z = np.full(n_exact, 2.0, np.float32)
-    px, py = rng.integers(0, 64, n_exact), rng.integers(0, 64, n_exact)
-    sc["xyz"][:n_exact] = np.stack([(px - 32) / 64.0 * z, (py - 32) / 64.0 * z, z], 1).astype(np.float32)
+    px, py = rng.integers(0, W, n_exact), rng.integers(0, H, n_exact)
+    sc["xyz"][:n_exact] = np.stack([(px - cx) / 64.0 * z, (py - cy) / 64.0 * z, z], 1).astype(np.float32)
     sc["xyz"][n_exact:n_exact + n_huge, 2] = 2.0
     sc["scale"][n_exact:n_exact + n_huge] = 7.5       # exp(7.5) = 1808 world units -> det(Sigma_2D) ~ 1e19
     sc["opacity"][n_exact:n_exact + n_huge] = -3.0
     return sc
+
+
+# Scenes whose pixels the tile renderers recompute with the exact arithmetic: "huge" flags whole warps (huge splats)
+# plus exact centres, "scattered" only the pixels at exact centres (n_huge = 0), in the same warps as pixels the walk
+# computes; the 37 x 61 variants add an odd width (a lane's second pixel outside the image) and partial edge tiles.
+FLAGGED = {"exact huge": dict(), "exact scattered": dict(n_huge=0),
+           "exact huge 37x61": dict(H=37, W=61), "exact scattered 37x61": dict(n_huge=0, H=37, W=61)}
+
+
+def flagged_scene(name):
+    return exact_arithmetic_scene(**FLAGGED[name])
 
 
 def headline_inputs(H, device):

@@ -119,6 +119,7 @@ SCENES = [(f"sh{s}", lambda s=s: small(s)) for s in range(4)]
 SCENES += [("50x37", lambda: ragged(50, 37, 1)), ("17x33", lambda: ragged(17, 33, 2)),
            ("720p", lambda: np_scene(100_000, "720p", 3, seed=0)), ("deep", lambda: stack(3000, -5.0)),
            ("saturated", lambda: stack(6000, 3.0, spread=0.05, scale=(0.03, 0.07)))]
+SCENES += [(n, lambda n=n: scenes.flagged_scene(n)) for n in scenes.FLAGGED]   # the exact recompute
 VARIANTS = [("masks", dict()), ("no masks", dict(masks=False)), ("depth", dict(depth_alpha=True)),
             ("aa", dict(antialiased=True))]
 ROW_CASES = [(f"{s} {v}", make, kw) for s, make in SCENES for v, kw in VARIANTS

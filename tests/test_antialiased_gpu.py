@@ -8,7 +8,7 @@ from gaussian_splatting_b200 import rasterize as R
 from gaussian_splatting_b200.rasterize import rasterize
 from gaussian_splatting_b200.structs import Camera
 from tests import antialiased_oracle as aao
-from tests import gradrows
+from tests import gradrows, scenes
 from tests.gradrows import PARAM_FLOOR, PARAM_RTOL, RENDER_C
 from tests.test_gradient_rows_gpu import check_forward, flip_pixels, gaussians_from, np_scene, ragged
 
@@ -167,7 +167,8 @@ def rows_cases():
               ("720p", True, False, lambda: np_scene(100_000, "720p", 3, seed=0)),
               ("sh3 no masks", False, False, lambda: small(3)),
               ("sh3 depth+alpha", True, True, lambda: small(3)),
-              ("sh0 depth+alpha no masks", False, True, lambda: small(0))]
+              ("sh0 depth+alpha no masks", False, True, lambda: small(0)),
+              ("exact huge", True, False, lambda: scenes.flagged_scene("exact huge"))]
     return cases
 
 

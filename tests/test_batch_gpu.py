@@ -33,6 +33,8 @@ def bits(t):
 
 
 def scene(name, sh_degree=None):
+    if name == "exact":   # most warps recomputed with the exact arithmetic (tests/scenes.py FLAGGED)
+        return scenes.flagged_scene("exact huge")
     n, res, sig = SCENES[name]
     sc = scenes.np_scene(n, res, sh_degree=SH_DEGREE[name] if sh_degree is None else sh_degree, seed=0, view=0,
                          n_views=3, sigma_px=sig)
@@ -54,6 +56,17 @@ def poses(C, away=()):
         T[c, 0, :3] *= -1.0
         T[c, 2, 3] = -T[c, 2, 3] - 50.0
     return T.contiguous()
+
+
+def exact_views(sc, C):
+    """C views of the "exact" scene that keep its exact centres on pixel centres: the identity pose, the principal
+    point moved by whole pixels per view."""
+    T = torch.eye(4, device=dev()).expand(C, 4, 4).contiguous()
+    K = to_t(sc["K"]).expand(C, 3, 3).clone()
+    for c in range(C):
+        K[c, 0, 2] += c
+        K[c, 1, 2] -= 2 * c
+    return T, K
 
 
 def intrinsics(sc, C, distinct):
@@ -133,11 +146,12 @@ def rel(a, b):
 
 # 1. per-view forward parity ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("C", [1, 2, 3, 4, 8])
-@pytest.mark.parametrize("name", ["tiny", "small", "deep"])
+@pytest.mark.parametrize("name", ["tiny", "small", "deep", "exact"])
 def test_every_view_is_bit_identical_to_rasterize(name, C):
     sc = scene(name)
     H, W = sc["H"], sc["W"]
-    T, K, bg = poses(C), intrinsics(sc, C, C > 1), backgrounds(C, C > 2)
+    T, K = exact_views(sc, C) if name == "exact" else (poses(C), intrinsics(sc, C, C > 1))
+    bg = backgrounds(C, C > 2)
     check_forward_equal(run_loop(sc, T, K, bg, H, W), run_batch(sc, T, K, bg, H, W), False)
 
 
@@ -234,11 +248,12 @@ def test_batched_per_gaussian_backward_is_the_view_order_sum(sh_degree, mode):
 
 # 4-6. gradients, speculation, densification statistics -------------------------------------------------------------
 @pytest.mark.parametrize("C", [1, 2, 4])
-@pytest.mark.parametrize("name", ["tiny", "small"])
+@pytest.mark.parametrize("name", ["tiny", "small", "exact"])
 def test_gradients_equal_the_loop_within_the_atomics_noise(name, C):
     sc = scene(name)
     H, W = sc["H"], sc["W"]
-    T, K, bg = poses(C), intrinsics(sc, C, True), backgrounds(C, True)
+    T, K = exact_views(sc, C) if name == "exact" else (poses(C), intrinsics(sc, C, True))
+    bg = backgrounds(C, True)
     G = upstream(C, H, W)
     loop, loop2, batch = (run_loop(sc, T, K, bg, H, W, G), run_loop(sc, T, K, bg, H, W, G),
                           run_batch(sc, T, K, bg, H, W, G))

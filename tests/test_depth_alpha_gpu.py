@@ -79,9 +79,11 @@ def bits(a):
 
 
 # 1. ------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("kind", ["sh3", "deep"])
+@pytest.mark.parametrize("kind", ["sh3", "deep", "exact huge"])
 def test_image_mask_uv_and_image_gradients_unchanged(kind):
-    sc = np_scene(2000, "tiny", 3, sigma_px=(2.0, 0.5, 0.5, 8.0)) if kind == "sh3" else stack(3000, -5.0)
+    """"exact huge": most pixels come from the recompute, render_pixel_exact_warp_depth against render_pixel_exact_warp."""
+    sc = {"sh3": lambda: np_scene(2000, "tiny", 3, sigma_px=(2.0, 0.5, 0.5, 8.0)), "deep": lambda: stack(3000, -5.0),
+          "exact huge": lambda: scenes.flagged_scene("exact huge")}[kind]()
     G = upstream3(sc)[0]
     (img0, m0, uv0, st0), g0, _ = run(sc, (G,), depth_alpha=False)
     (img1, m1, uv1, d1, a1, st1), g1, _ = run(sc, (G, None, None))
@@ -94,15 +96,18 @@ def test_image_mask_uv_and_image_gradients_unchanged(kind):
 
 # 2. ------------------------------------------------------------------------------------------------------------
 def bitwise_cases():
-    cases = [(f"sh{s}", lambda s=s: np_scene(2000, "tiny", s, sigma_px=(2.0, 0.5, 0.5, 8.0))) for s in range(4)]
-    cases += [(f"{H}x{W}", lambda H=H, W=W, s=s: ragged(H, W, s))
+    cases = [(f"sh{s}", lambda s=s: np_scene(2000, "tiny", s, sigma_px=(2.0, 0.5, 0.5, 8.0)), 500.0) for s in range(4)]
+    cases += [(f"{H}x{W}", lambda H=H, W=W, s=s: ragged(H, W, s), 500.0)
               for H, W, s in [(50, 37, 1), (17, 33, 2), (1, 64, 0), (64, 1, 3)]]
-    cases.append(("deep", lambda: stack(3000, -5.0)))
+    cases.append(("deep", lambda: stack(3000, -5.0), 500.0))
+    # the exact recompute (tests/scenes.py FLAGGED); far = inf: it decodes z from base-0 (full-range) depth keys
+    cases += [(n, lambda n=n: scenes.flagged_scene(n), 500.0) for n in scenes.FLAGGED]
+    cases.append(("exact huge far=inf", lambda: scenes.flagged_scene("exact huge"), float("inf")))
     return cases
 
 
-@pytest.mark.parametrize("name,make", bitwise_cases(), ids=[c[0] for c in bitwise_cases()])
-def test_depth_and_alpha_match_the_oracle_where_the_walk_does(name, make):
+@pytest.mark.parametrize("name,make,far", bitwise_cases(), ids=[c[0] for c in bitwise_cases()])
+def test_depth_and_alpha_match_the_oracle_where_the_walk_does(name, make, far):
     """Where the walk matches the fp32 oracle bit for bit — image, final transmittance weight and splat count — alpha
     is bit-identical on at least 90 % of them and within 1e-6 on all, and depth within 1e-5 relative (the oracle's walk
     fed the z the kernels decode from the keys).  Matching outputs do not pin every blend weight: the oracle's exp2f and
@@ -112,7 +117,8 @@ def test_depth_and_alpha_match_the_oracle_where_the_walk_does(name, make):
     Elsewhere both agree to fp32 rounding.  The kernels' own depth is checked bit for bit across two z sources in the
     4k test below."""
     sc = make()
-    (img, _, _, depth, alpha, st), _, _ = run(sc)
+    (img, _, _, depth, alpha, st), _, _ = run(sc, far=far)
+    assert (st.depth_base == 0) == (far == float("inf"))
     o = oracle(sc)
     z = gpu_z(st)[o.keep]
     assert gradrows.global_rel(z, o.z) < 1e-6
@@ -167,6 +173,8 @@ def rows_cases():
               ("saturated", True, lambda: stack(6000, 3.0, spread=0.05, scale=(0.03, 0.07))),
               ("deep masks", True, lambda: stack(3000, -5.0)), ("deep no masks", False, lambda: stack(3000, -5.0)),
               ("sh3 no masks", False, lambda: np_scene(2000, "tiny", 3, sigma_px=(2.0, 0.5, 0.5, 8.0)))]
+    cases += [(n, True, lambda n=n: scenes.flagged_scene(n)) for n in scenes.FLAGGED]
+    cases.append(("exact huge no masks", False, lambda: scenes.flagged_scene("exact huge")))
     return cases
 
 

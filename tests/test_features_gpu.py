@@ -41,6 +41,8 @@ GOLDEN = {"tiny": ("synth_tiny", 2000, "tiny", (2.0, 0.5, 0.5, 8.0)),
 
 
 def golden_scene(name):
+    if name in scenes.FLAGGED:   # SH degree 0 already
+        return scenes.flagged_scene(name)
     _, n, res, sig = GOLDEN[name]
     sc = scenes.np_scene(n, res, sh_degree=0, seed=0, view=0, n_views=3, sigma_px=sig)
     sc["sh"] = None
@@ -70,7 +72,7 @@ def colour_features(g):
 @pytest.mark.parametrize("masks", [True, False])
 @pytest.mark.parametrize("filter3d", [False, True])
 @pytest.mark.parametrize("antialiased", [False, True])
-@pytest.mark.parametrize("name", list(GOLDEN))
+@pytest.mark.parametrize("name", list(GOLDEN) + list(scenes.FLAGGED))
 def test_colour_features_render_the_image_on_black_bit_for_bit(name, antialiased, filter3d, masks):
     sc = golden_scene(name)
     g = gaussians(sc)
@@ -81,6 +83,22 @@ def test_colour_features_render_the_image_on_black_bit_for_bit(name, antialiased
     assert float(img.detach().abs().max()) > 0
     if name == "deep":  # the weight recurrence's chunk-local index wraps (> 960 splats in the busiest tiles)
         assert int((st.ranges[1:] - st.ranges[:-1]).max()) > 960
+
+
+@pytest.mark.parametrize("masks", [True, False])
+@pytest.mark.parametrize("name", ["tiny"] + list(scenes.FLAGGED))
+def test_two_chunk_colour_features_render_the_image_twice(name, masks):
+    """F = SH0 * [rgb, rgb], D = 6: channels 3-5 come from the second 4-channel chunk (blockIdx.z = 1, also in the
+    exact recompute of flagged pixels) and must equal the image bit for bit, as channels 0-2 do."""
+    sc = golden_scene(name)
+    g = gaussians(sc)
+    F = colour_features(g)
+    img, _, _, fmap, _ = render(sc, g, torch.cat([F, F], 1).contiguous(), masks=masks)
+    assert fmap.shape == img.shape[:2] + (6,)
+    for c0 in (0, 3):
+        b = bits(fmap[..., c0:c0 + 3])
+        assert np.array_equal(b, bits(img)), (c0, int((b != bits(img)).sum()))
+    assert float(img.detach().abs().max()) > 0
 
 
 # 2. gradient identity ----------------------------------------------------------------------------------------------
@@ -125,9 +143,11 @@ def feature_run(sc, F, G=None, masks=True):
     return out, g, Ft, (seen[0].view(-1, 12).double().cpu().numpy() if seen else None)
 
 
-@pytest.mark.parametrize("D", [1, 4, 7, 16, 33, 64])
-def test_feature_map_and_gradients_match_the_oracle(D):
-    sc = np_scene(2000, "tiny", 3, sigma_px=(2.0, 0.5, 0.5, 8.0))
+@pytest.mark.parametrize("D,scene", [pytest.param(D, None, id=str(D)) for D in (1, 4, 7, 16, 33, 64)]
+                         + [pytest.param(D, "exact huge", id=f"exact huge-{D}") for D in (5, 33)])
+def test_feature_map_and_gradients_match_the_oracle(D, scene):
+    """scene "exact huge": most pixels' feature sums come from feature_pixel_exact_warp, chunks 0 .. (D - 1) / 4."""
+    sc = np_scene(2000, "tiny", 3, sigma_px=(2.0, 0.5, 0.5, 8.0)) if scene is None else scenes.flagged_scene(scene)
     N, H, W = sc["xyz"].shape[0], sc["H"], sc["W"]
     rng = np.random.default_rng(D)
     F = rng.standard_normal((N, D)).astype(np.float32)
@@ -152,7 +172,7 @@ def test_feature_map_and_gradients_match_the_oracle(D):
     res += [gradrows.param_rows(f"D={D} {k}", getattr(g, k).grad, getattr(pr, k), PARAM_RTOL, PARAM_FLOOR, allowed)
             for k in ("xyz", "quaternion", "scale", "opacity")]
     gradrows.assert_all(res)
-    assert not g.rgb.grad.any() and not g.sh.grad.any()
+    assert not g.rgb.grad.any() and (g.sh is None or not g.sh.grad.any())
     assert not Ft.grad[torch.from_numpy(~o.keep).to(dev())].any()
 
 

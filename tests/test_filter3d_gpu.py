@@ -13,7 +13,7 @@ from gaussian_splatting_b200.flat_adam import FlatAdam
 from gaussian_splatting_b200.rasterize import rasterize
 from gaussian_splatting_b200.structs import Camera
 from tests import filter3d_oracle as fo
-from tests import gradrows
+from tests import gradrows, scenes
 from tests.gradrows import PARAM_FLOOR, PARAM_RTOL, RENDER_C
 from oracle import cpu_oracle as orc
 from tests.test_gradient_rows_gpu import gaussians_from, np_scene, ragged
@@ -249,7 +249,8 @@ def rows_cases():
               ("sh3 antialiased", dict(antialiased=True), lambda: small(3)),
               ("sh2 antialiased depth+alpha", dict(antialiased=True, depth_alpha=True), lambda: small(2)),
               ("720p antialiased", dict(antialiased=True), lambda: np_scene(100_000, "720p", 3, seed=0)),
-              ("sh3 absgrad", dict(absgrad=True), lambda: small(3))]
+              ("sh3 absgrad", dict(absgrad=True), lambda: small(3)),
+              ("exact huge", dict(), lambda: scenes.flagged_scene("exact huge"))]
     return cases
 
 

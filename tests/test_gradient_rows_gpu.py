@@ -211,6 +211,15 @@ def test_fused_deep_tile_variants(masks, shd):
         assert bool((words != 0).any(0).all()), "some word of the 128-bit masks is never used"
 
 
+@pytest.mark.parametrize("masks", [True, False])
+@pytest.mark.parametrize("name", list(scenes.FLAGGED))
+def test_fused_flagged_pixels(name, masks):
+    """Scenes whose pixels the forward recomputes with the exact arithmetic (tests/scenes.py FLAGGED): every warp
+    ("all") or single pixels among walked ones ("scattered").  The image and the final weights come from the
+    recompute, the contribution masks the masked backward walks from the walk itself."""
+    fused_vs_oracle(f"{name} masks={masks}", scenes.flagged_scene(name), masks=masks)
+
+
 def test_fused_saturating_stack():
     """Opaque splats stacked in one tile: every pixel saturates and the backward starts at the saturation depth."""
     sc = stack(6000, 3.0, spread=0.05, scale=(0.03, 0.07))

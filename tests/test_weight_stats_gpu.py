@@ -112,11 +112,15 @@ def check_against_oracle(tag, ws, r):
 SCENES = [("sh0", lambda: small(0)), ("sh3", lambda: small(3)), ("50x37", lambda: ragged(50, 37, 1)),
           ("720p", lambda: np_scene(100_000, "720p", 3, seed=0)), ("deep", lambda: stack(3000, -5.0)),
           ("saturated", lambda: stack(6000, 3.0, spread=0.05, scale=(0.03, 0.07)))]
+# the exact recompute (tests/scenes.py FLAGGED): the statistics of flagged pixels come from the walk, the image from the
+# recompute
+SCENES += [(n, lambda n=n: scenes.flagged_scene(n)) for n in scenes.FLAGGED]
 VARIANTS = [("masks", dict()), ("no masks", dict(masks=False)), ("no_grad", dict(grad=False)),
             ("depth", dict(depth_alpha=True)), ("aa", dict(antialiased=True)), ("f3d", dict(f3d=True)),
             ("f3d aa depth", dict(f3d=True, antialiased=True, depth_alpha=True))]
 CASES = [(f"{s} {v}", make, kw) for s, make in SCENES for v, kw in VARIANTS
-         if v in ("masks", "no masks") or s in ("sh3", "720p", "saturated")]
+         if v in ("masks", "no masks") or s in ("sh3", "720p", "saturated")
+         or (s in scenes.FLAGGED and v in ("depth", "aa"))]
 
 
 @pytest.mark.parametrize("tag,make,kw", CASES, ids=[c[0] for c in CASES])
@@ -195,7 +199,7 @@ def test_eager_fitting_and_overflowing_speculation_agree(depth_alpha):
     N = sc["xyz"].shape[0]
     key = (dev().index if dev().index is not None else torch.cuda.current_device(), N, sc["H"], sc["W"])
     R._PAIR_HISTORY.pop(key, None)
-    res = {}
+    res, masks = {}, {}
     for name in ("eager", "fitting", "overflow"):
         if name == "overflow":
             R._PAIR_HISTORY[key] = [1000]
@@ -203,9 +207,12 @@ def test_eager_fitting_and_overflowing_speculation_agree(depth_alpha):
         out, _ = run(sc, ws, depth_alpha=depth_alpha)
         assert out[-1].speculation_overflowed == (name == "overflow"), name
         res[name] = ws
+        masks[name] = out[-1].masks
     R._PAIR_HISTORY.pop(key, None)
     e = res["eager"]
     for name in ("fitting", "overflow"):
+        # the state's contribution masks hold the words of the binned pairs, whatever capacity the run was sized for
+        assert torch.equal(masks[name], masks["eager"]), name
         assert torch.equal(res[name].pixel_count, e.pixel_count), name
         assert torch.equal(res[name].weight_max, e.weight_max), name
         assert gradrows.global_rel(res[name].weight_sum, e.weight_sum) < 1e-6, name
