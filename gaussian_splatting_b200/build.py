@@ -6,9 +6,10 @@
   libgsr_batch.so           the multi-view per-gaussian kernels of rasterize_batch (include/gsr_batch.h), same flags
   libgsr_fisheye.so         the per-gaussian kernels for fisheye cameras (include/gsr_fisheye.h), same flags
   libgsr_distortion.so      the per-gaussian kernels for radial-tangential lens distortion (include/gsr_distortion.h)
+  libgsr_pose.so            the per-gaussian backward with the camera pose gradient, every lens (include/gsr_pose.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all seven; `build(force=False)` is incremental.
+`python -m gaussian_splatting_b200.build` builds all eight; `build(force=False)` is incremental.
 """
 from __future__ import annotations
 
@@ -31,6 +32,7 @@ FEATURES_LIB = PKG / "libgsr_features.so"
 BATCH_LIB = PKG / "libgsr_batch.so"
 FISHEYE_LIB = PKG / "libgsr_fisheye.so"
 DISTORTION_LIB = PKG / "libgsr_distortion.so"
+POSE_LIB = PKG / "libgsr_pose.so"
 
 CU_SOURCES = [
     "gsr_pergaussian.cu",
@@ -74,6 +76,14 @@ DISTORTION_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_d
                                                                     CSRC / "gsr_poly_roots.h",
                                                                     ROOT / "include" / "gsr_b200.h",
                                                                     ROOT / "include" / "gsr_distortion.h"]
+# gsr_pose.cu once per camera model (GSR_POSE_LENS: 0 pinhole, 1 fisheye, 2 distortion): (source, object, -D flags)
+POSE_SOURCES = [("gsr_pose.cu", f"gsr_pose_{i}", [f"-DGSR_POSE_LENS={i}"]) for i in range(3)]
+POSE_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_pose.cuh", CSRC / "gsr_fisheye.cuh",
+                                                             CSRC / "gsr_distortion.cuh",
+                                                             ROOT / "include" / "gsr_b200.h",
+                                                             ROOT / "include" / "gsr_fisheye.h",
+                                                             ROOT / "include" / "gsr_distortion.h",
+                                                             ROOT / "include" / "gsr_pose.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -109,15 +119,19 @@ def ext_path() -> Path:
 
 
 def _build_cuda_lib(lib: Path, sources, headers, stamp_name: str, force: bool, verbose: bool) -> Path:
+    """sources: file names, or (file name, object stem, extra nvcc flags) for a file compiled more than once."""
     OBJ.mkdir(exist_ok=True)
     stamp = OBJ / stamp_name
-    want = _digest([CSRC / s for s in sources] + headers, " ".join(NVCC_FLAGS))
+    units = [s if isinstance(s, tuple) else (s, Path(s).stem, []) for s in sources]
+    want = _digest(sorted({CSRC / s for s, _, _ in units}) + headers,
+                   " ".join(NVCC_FLAGS + [f for _, _, fl in units for f in fl]))
     if not force and lib.exists() and stamp.exists() and stamp.read_text() == want:
         return lib
 
-    def compile_one(src):
-        obj = OBJ / (Path(src).stem + ".o")
-        cmd = [_nvcc(), *NVCC_FLAGS, "-c", str(CSRC / src), "-o", str(obj)]
+    def compile_one(unit):
+        src, stem, flags = unit
+        obj = OBJ / (stem + ".o")
+        cmd = [_nvcc(), *NVCC_FLAGS, *flags, "-c", str(CSRC / src), "-o", str(obj)]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         out = _run(cmd)
@@ -126,7 +140,7 @@ def _build_cuda_lib(lib: Path, sources, headers, stamp_name: str, force: bool, v
         return obj
 
     with ThreadPoolExecutor(max_workers=min(len(sources), os.cpu_count() or 1)) as ex:
-        objs = list(ex.map(compile_one, sources))
+        objs = list(ex.map(compile_one, units))
     _run([_nvcc(), "-shared", "-o", str(lib), *map(str, objs), "-gencode", "arch=compute_90a,code=sm_90a",
           "-cudart", "shared"])
     stamp.write_text(want)
@@ -159,6 +173,10 @@ def build_distortion_lib(force: bool = False, verbose: bool = False) -> Path:
                            verbose)
 
 
+def build_pose_lib(force: bool = False, verbose: bool = False) -> Path:
+    return _build_cuda_lib(POSE_LIB, POSE_SOURCES, POSE_HEADERS, "pose_lib.sha256", force, verbose)
+
+
 def build_ext(force: bool = False) -> Path:
     import torch  # noqa: F401  (needed for include/library paths)
     from torch.utils import cpp_extension as ce
@@ -170,7 +188,8 @@ def build_ext(force: bool = False) -> Path:
     stamp = OBJ / "ext.sha256"
     want = _digest([src, ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h",
                     ROOT / "include" / "gsr_features.h", ROOT / "include" / "gsr_batch.h",
-                    ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h"], torch.__version__)
+                    ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h",
+                    ROOT / "include" / "gsr_pose.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -182,7 +201,7 @@ def build_ext(force: bool = False) -> Path:
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
         f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", "-lgsr_fisheye",
-        "-lgsr_distortion",
+        "-lgsr_distortion", "-lgsr_pose",
         f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",
@@ -208,6 +227,7 @@ def build(force: bool = False, verbose: bool = False):
     build_batch_lib(force=force, verbose=verbose)
     build_fisheye_lib(force=force, verbose=verbose)
     build_distortion_lib(force=force, verbose=verbose)
+    build_pose_lib(force=force, verbose=verbose)
     ext = build_ext(force=force)
     return lib, ext
 

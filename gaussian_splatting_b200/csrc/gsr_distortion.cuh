@@ -106,3 +106,25 @@ __device__ __forceinline__ void distortion_project_bwd(const float* __restrict__
 }
 
 }  // namespace gsr
+
+// The camera-model hooks of gsr_preprocess.cuh for this lens, for a translation unit that defines GSR_DISTORTION_HOOKS
+// before including this header and then includes gsr_preprocess.cuh (gsr_distortion.cu, gsr_pose.cu).  The lens
+// constants of view `view` are read into shared memory next to the view constants.
+#ifdef GSR_DISTORTION_HOOKS
+#define GSR_PROJECTION_HOOKS
+#define GSR_VIEW_PARAM , const float* __restrict__ distortion
+#define GSR_VIEW_DECL __shared__ float vdc[GSR_DISTORTION_CONSTS];
+#define GSR_LOAD_VIEW(T, K, cam, view)                                                                          \
+    do {                                                                                                        \
+        if (threadIdx.x >= 32 && threadIdx.x < 32 + GSR_DISTORTION_CONSTS)                                      \
+            vdc[threadIdx.x - 32] = distortion[GSR_DISTORTION_CONSTS * (view) + threadIdx.x - 32];              \
+        load_view_cta(T, K, cam, vc, HAS_SH); /* ends with a CTA barrier */                                     \
+    } while (0)
+#define GSR_PROJECT(px, py, pz, u, v) \
+    float dt_s;                       \
+    distortion_project(px, py, pz, vc.K[0], vc.K[2], vc.K[4], vc.K[5], vdc, u, v, dt_s)
+#define GSR_CULL_MORE | (dt_s >= vdc[5])
+#define GSR_JACOBIAN(px, py, pz, J) distortion_jacobian(px, py, pz, vc.K[0], vc.K[4], vdc, J)
+#define GSR_JACOBIAN_BWD(px, py, pz, gJ, g) distortion_jacobian_bwd(px, py, pz, vc.K[0], vc.K[4], vdc, gJ, g)
+#define GSR_PROJECT_BWD(px, py, pz, gu, gv, g) distortion_project_bwd(J, gu, gv, g)
+#endif

@@ -134,3 +134,25 @@ __device__ __forceinline__ void fisheye_project_bwd(const float* __restrict__ J,
 }
 
 }  // namespace gsr
+
+// The camera-model hooks of gsr_preprocess.cuh for this lens, for a translation unit that defines GSR_FISHEYE_HOOKS
+// before including this header and then includes gsr_preprocess.cuh (gsr_fisheye.cu, gsr_pose.cu).  The lens
+// constants of view `view` are read into shared memory next to the view constants.
+#ifdef GSR_FISHEYE_HOOKS
+#define GSR_PROJECTION_HOOKS
+#define GSR_VIEW_PARAM , const float* __restrict__ fisheye
+#define GSR_VIEW_DECL __shared__ float vfe[GSR_FISHEYE_CONSTS];
+#define GSR_LOAD_VIEW(T, K, cam, view)                                                                          \
+    do {                                                                                                        \
+        if (threadIdx.x >= 32 && threadIdx.x < 32 + GSR_FISHEYE_CONSTS)                                         \
+            vfe[threadIdx.x - 32] = fisheye[GSR_FISHEYE_CONSTS * (view) + threadIdx.x - 32];                     \
+        load_view_cta(T, K, cam, vc, HAS_SH); /* ends with a CTA barrier */                                     \
+    } while (0)
+#define GSR_PROJECT(px, py, pz, u, v) \
+    float fe_theta;                   \
+    fisheye_project(px, py, pz, vc.K[0], vc.K[2], vc.K[4], vc.K[5], vfe, u, v, fe_theta)
+#define GSR_CULL_MORE | (fe_theta >= vfe[4])
+#define GSR_JACOBIAN(px, py, pz, J) fisheye_jacobian(px, py, pz, vc.K[0], vc.K[4], vfe, J)
+#define GSR_JACOBIAN_BWD(px, py, pz, gJ, g) fisheye_jacobian_bwd(px, py, pz, vc.K[0], vc.K[4], vfe, gJ, g)
+#define GSR_PROJECT_BWD(px, py, pz, gu, gv, g) fisheye_project_bwd(J, gu, gv, g)
+#endif

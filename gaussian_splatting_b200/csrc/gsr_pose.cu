@@ -1,0 +1,279 @@
+// gsr_pose.cu — the per-gaussian backward with the camera pose gradient (libgsr_pose.so): rasterize(...) and
+// rasterize_batch(...) when camera_T_world requires grad.
+//
+// The bodies are those of gsr_preprocess.cuh — single-view and batched backward, so the gaussian gradients are the
+// existing arithmetic — compiled with the pose hooks of gsr_pose.cuh.  This file is compiled once per camera model:
+// GSR_POSE_LENS 0 (pinhole, the default hooks), 1 (gsr_fisheye.cuh's hooks) or 2 (gsr_distortion.cuh's hooks).  Each
+// compile puts its kernels in a namespace of its own and exports one hidden launcher; the compile with
+// GSR_POSE_LENS == 0 also holds the fp64 finishing kernel and the C ABI of include/gsr_pose.h, which dispatch on the
+// lens.
+#include <cstdint>
+
+#include "../../include/gsr_distortion.h"
+#include "../../include/gsr_fisheye.h"
+
+#ifndef GSR_POSE_LENS
+#define GSR_POSE_LENS 0
+#endif
+
+#if GSR_POSE_LENS == 1
+#define GSR_FISHEYE_HOOKS
+#include "gsr_fisheye.cuh"
+#define GSR_POSE_NS pose_fisheye
+#define GSR_POSE_LAUNCH gsr_pose_launch_fisheye
+#define GSR_POSE_LENS_ARG , lens
+#elif GSR_POSE_LENS == 2
+#define GSR_DISTORTION_HOOKS
+#include "gsr_distortion.cuh"
+#define GSR_POSE_NS pose_distortion
+#define GSR_POSE_LAUNCH gsr_pose_launch_distortion
+#define GSR_POSE_LENS_ARG , lens
+#else
+#define GSR_POSE_NS pose_pinhole
+#define GSR_POSE_LAUNCH gsr_pose_launch_pinhole
+#define GSR_POSE_LENS_ARG
+#endif
+
+// gsr_preprocess.cuh's one non-inline device function has a host-side symbol: one name per compile, so that the
+// three objects link into one library
+#if GSR_POSE_LENS == 1
+#define camera_centre camera_centre_pose_fisheye
+#elif GSR_POSE_LENS == 2
+#define camera_centre camera_centre_pose_distortion
+#endif
+#include "gsr_common.cuh"
+#include "gsr_pose.cuh"
+#include "gsr_preprocess.cuh"
+
+#include "../../include/gsr_pose.h"
+
+// CTAs per SM the register budget is sized for (-Xptxas -v: no local memory at these bounds, DESIGN.md 3.21)
+#ifndef GSR_POSE_BWD_MINB
+#define GSR_POSE_BWD_MINB 4
+#endif
+#ifndef GSR_POSE_BATCH_MINB
+#define GSR_POSE_BATCH_MINB 3
+#endif
+
+// the launcher of one camera model: the per-gaussian kernel of `single` (C == 1) or of C views, writing the
+// partials [C, grid, 12]
+#define GSR_POSE_LAUNCH_DECL(name)                                                                                   \
+    __attribute__((visibility("hidden"))) int name(                                                                 \
+        bool single, int mode, int C, int N, int n_sh_rest, const float* xyz, const float* quat, const float* scale, \
+        const float* opa, const float* filter3d, const float* T, const float* K, const float* cam,                  \
+        const uint8_t* visible, const float* rows, int rows_uv, const float* g_uv, const uint64_t* scan,            \
+        float* o_xyz, float* o_quat, float* o_scale, float* o_opa, float* o_dc, float* o_sh, int use_tma,           \
+        const float* lens, float* partials, cudaStream_t st)
+
+namespace gsr {
+static_assert(POSE_CTA_THREADS == PRE_THREADS, "pose_cta_reduce sums one CTA of the bodies");
+namespace GSR_POSE_NS {
+
+#define GSR_POSE_BWD_PARAMS                                                                                         \
+    int N, const float* __restrict__ xyz, const float* __restrict__ quat, const float* __restrict__ scale,          \
+        const float* __restrict__ opa_logit, const float* __restrict__ Tdev, const float* __restrict__ Kdev,        \
+        const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rows,    \
+        int rows_uv, const float* __restrict__ g_uv_compact, const uint64_t* __restrict__ scan,                      \
+        float* __restrict__ o_xyz, float* __restrict__ o_quat, float* __restrict__ o_scale,                         \
+        float* __restrict__ o_opa, float* __restrict__ o_dc, float* __restrict__ o_sh, int use_tma,                 \
+        const float* __restrict__ filter3d, const float* __restrict__ lens, float* __restrict__ partials
+#define GSR_POSE_BWD_FORWARD                                                                                        \
+    N, xyz, quat, scale, opa_logit, Tdev, Kdev, camdev, visible, g_rows, rows_uv, g_uv_compact, scan, o_xyz, o_quat, \
+        o_scale, o_opa, o_dc, o_sh, use_tma, filter3d GSR_POSE_LENS_ARG, partials
+template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS, bool FILTER3D>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_POSE_BWD_MINB) k_pose_preprocess_bwd(GSR_POSE_BWD_PARAMS) {
+    preprocess_bwd<N_SH, HAS_SH, DEPTH, ANTIALIAS, FILTER3D>(GSR_POSE_BWD_FORWARD);
+}
+template <int N_SH, bool HAS_SH, bool DEPTH, bool ANTIALIAS, bool FILTER3D>
+__global__ void __launch_bounds__(PRE_THREADS, GSR_POSE_BATCH_MINB)
+    k_pose_batch_preprocess_bwd(int C, GSR_POSE_BWD_PARAMS) {
+    batch_preprocess_bwd<N_SH, HAS_SH, DEPTH, ANTIALIAS, FILTER3D>(C, GSR_POSE_BWD_FORWARD);
+}
+#undef GSR_POSE_BWD_PARAMS
+#undef GSR_POSE_BWD_FORWARD
+
+template <bool DEPTH, bool AA, bool F3D>
+static int launch(bool single, int n_sh_rest, dim3 grid, cudaStream_t st, int C, int N, const float* xyz,
+                  const float* quat, const float* scale, const float* opa, const float* T, const float* K,
+                  const float* cam, const uint8_t* visible, const float* rows, int rows_uv, const float* g_uv,
+                  const uint64_t* scan, float* o_xyz, float* o_quat, float* o_scale, float* o_opa, float* o_dc,
+                  float* o_sh, int use_tma, const float* filter3d, const float* lens, float* partials) {
+#define GSR_POSE_ARGS                                                                                                \
+    N, xyz, quat, scale, opa, T, K, cam, visible, rows, rows_uv, g_uv, scan, o_xyz, o_quat, o_scale, o_opa, o_dc,    \
+        o_sh, use_tma, filter3d, lens, partials
+#define GSR_POSE_SH(NSH, HSH)                                                                                        \
+    if (single)                                                                                                      \
+        k_pose_preprocess_bwd<NSH, HSH, DEPTH, AA, F3D><<<grid, PRE_THREADS, 0, st>>>(GSR_POSE_ARGS);                \
+    else                                                                                                             \
+        k_pose_batch_preprocess_bwd<NSH, HSH, DEPTH, AA, F3D><<<grid, PRE_THREADS, 0, st>>>(C, GSR_POSE_ARGS);
+    switch (n_sh_rest) {
+        case 0: GSR_POSE_SH(1, false) break;
+        case 3: GSR_POSE_SH(4, true) break;
+        case 8: GSR_POSE_SH(9, true) break;
+        case 15: GSR_POSE_SH(16, true) break;
+        default: return GSR_ERR_UNSUPPORTED;
+    }
+#undef GSR_POSE_SH
+#undef GSR_POSE_ARGS
+    return GSR_OK;
+}
+
+}  // namespace GSR_POSE_NS
+}  // namespace gsr
+
+GSR_POSE_LAUNCH_DECL(GSR_POSE_LAUNCH) {
+    using namespace gsr::GSR_POSE_NS;
+    const dim3 grid((N + gsr::PRE_THREADS - 1) / gsr::PRE_THREADS);
+    const bool depth = (mode & GSR_MODE_DEPTH_ALPHA) != 0, aa = (mode & GSR_MODE_ANTIALIASED) != 0,
+               f3d = (mode & GSR_MODE_FILTER3D) != 0;
+#define GSR_POSE_ARGS                                                                                                \
+    single, n_sh_rest, grid, st, C, N, xyz, quat, scale, opa, T, K, cam, visible, rows, rows_uv, g_uv, scan, o_xyz,  \
+        o_quat, o_scale, o_opa, o_dc, o_sh, use_tma, filter3d, lens, partials
+    return f3d ? (aa ? (depth ? launch<true, true, true>(GSR_POSE_ARGS) : launch<false, true, true>(GSR_POSE_ARGS))
+                     : (depth ? launch<true, false, true>(GSR_POSE_ARGS) : launch<false, false, true>(GSR_POSE_ARGS)))
+               : (aa ? (depth ? launch<true, true, false>(GSR_POSE_ARGS) : launch<false, true, false>(GSR_POSE_ARGS))
+                     : (depth ? launch<true, false, false>(GSR_POSE_ARGS)
+                              : launch<false, false, false>(GSR_POSE_ARGS)));
+#undef GSR_POSE_ARGS
+}
+
+#if GSR_POSE_LENS == 0
+
+GSR_POSE_LAUNCH_DECL(gsr_pose_launch_fisheye);
+GSR_POSE_LAUNCH_DECL(gsr_pose_launch_distortion);
+
+namespace gsr {
+
+constexpr int POSE_FINISH_THREADS = 256;
+
+// one CTA per view: thread t adds the partials t, t + 256, ... in fp64, then the CTA adds the 256 sums in a fixed
+// order (a shuffle tree per warp, then the warps in order) and rounds once.  Writes the view's [4, 4] gradient, the
+// last row 0.
+__global__ void __launch_bounds__(POSE_FINISH_THREADS) k_pose_finish(int nblk, const float* __restrict__ partials,
+                                                                    float* __restrict__ g_pose) {
+    __shared__ double s_sum[POSE_FINISH_THREADS / 32][POSE_VALUES];
+    const int c = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const float* src = partials + (size_t)c * nblk * POSE_VALUES;
+    double acc[POSE_VALUES];
+#pragma unroll
+    for (int k = 0; k < POSE_VALUES; ++k) acc[k] = 0.0;
+    for (int b = t; b < nblk; b += POSE_FINISH_THREADS) {
+        const float4* row = reinterpret_cast<const float4*>(src + (size_t)b * POSE_VALUES);
+#pragma unroll
+        for (int q = 0; q < POSE_VALUES / 4; ++q) {
+            const float4 v = row[q];
+            acc[4 * q + 0] += (double)v.x;
+            acc[4 * q + 1] += (double)v.y;
+            acc[4 * q + 2] += (double)v.z;
+            acc[4 * q + 3] += (double)v.w;
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < POSE_VALUES; ++k) {
+        double v = acc[k];
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
+        if (lane == 0) s_sum[warp][k] = v;
+    }
+    __syncthreads();
+    if (t < 16) {
+        float out = 0.f;
+        if (t < POSE_VALUES) {
+            double v = s_sum[0][t];
+            for (int w = 1; w < POSE_FINISH_THREADS / 32; ++w) v += s_sum[w][t];
+            out = (float)v;
+        }
+        g_pose[(size_t)c * 16 + t] = out;
+    }
+}
+
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MODE_ABSGRAD | GSR_MODE_FILTER3D;
+
+}  // namespace gsr
+
+using namespace gsr;
+
+static int pose_backward(bool single, int lens, int mode, int C, int N, int n_sh_rest, const float* xyz,
+                         const float* quaternion, const float* scale, const float* opacity_logit, const float* filter3d,
+                         const float* camera_T_world, const float* K, const float* camera_centre,
+                         const uint8_t* visible, const float* grad_rows, int use_rows_uv,
+                         const float* grad_uv_compact, const uint64_t* scan, float* g_xyz, float* g_quaternion,
+                         float* g_scale, float* g_opacity_logit, float* g_rgb_dc, float* g_sh_rest,
+                         const float* lens_consts, float* g_pose, void* temp, size_t temp_bytes, void* stream) {
+    if (C < 1 || N < 0 || (mode & ~KNOWN_MODES) != 0 || g_pose == nullptr) return GSR_ERR_BAD_ARG;
+    if (lens != GSR_LENS_PINHOLE && lens != GSR_LENS_FISHEYE && lens != GSR_LENS_DISTORTION) return GSR_ERR_BAD_ARG;
+    if ((lens != GSR_LENS_PINHOLE) != (lens_consts != nullptr)) return GSR_ERR_BAD_ARG;
+    if (((mode & GSR_MODE_FILTER3D) != 0) != (filter3d != nullptr)) return GSR_ERR_BAD_ARG;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int nblk = (N + PRE_THREADS - 1) / PRE_THREADS;
+    float* partials = reinterpret_cast<float*>(temp);
+    if (N > 0) {
+        if (xyz == nullptr || quaternion == nullptr || scale == nullptr || opacity_logit == nullptr ||
+            camera_T_world == nullptr || K == nullptr || visible == nullptr || grad_rows == nullptr ||
+            g_xyz == nullptr || g_quaternion == nullptr || g_scale == nullptr || g_opacity_logit == nullptr ||
+            g_rgb_dc == nullptr)
+            return GSR_ERR_BAD_ARG;
+        if ((n_sh_rest > 0) != (g_sh_rest != nullptr)) return GSR_ERR_BAD_ARG;
+        if (!aligned16(grad_rows)) return GSR_ERR_BAD_ARG;
+        if (grad_uv_compact != nullptr && scan == nullptr) return GSR_ERR_BAD_ARG;
+        if (n_sh_rest != 0 && n_sh_rest != 3 && n_sh_rest != 8 && n_sh_rest != 15) return GSR_ERR_UNSUPPORTED;
+        if (temp == nullptr || !aligned16(temp) || temp_bytes < gsr_pose_temp_bytes(C, N)) return GSR_ERR_BAD_ARG;
+        const int use_tma = (aligned16(g_xyz) && aligned16(g_quaternion) && aligned16(g_scale) &&
+                             aligned16(g_opacity_logit) && aligned16(g_rgb_dc) &&
+                             (g_sh_rest == nullptr || aligned16(g_sh_rest)))
+                                ? 1
+                                : 0;
+        const auto launcher = lens == GSR_LENS_FISHEYE      ? gsr_pose_launch_fisheye
+                              : lens == GSR_LENS_DISTORTION ? gsr_pose_launch_distortion
+                                                            : gsr_pose_launch_pinhole;
+        const int rc = launcher(single, mode, C, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
+                                camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact,
+                                scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, use_tma,
+                                lens_consts, partials, st);
+        if (rc != GSR_OK) return rc;
+    }
+    k_pose_finish<<<C, POSE_FINISH_THREADS, 0, st>>>(nblk, partials, g_pose);
+    return (int)cudaGetLastError();
+}
+
+extern "C" {
+
+size_t gsr_pose_temp_bytes(int C, int N) {
+    const size_t nblk = (size_t)((N > 0 ? N : 0) + PRE_THREADS - 1) / PRE_THREADS;
+    return align256(sizeof(float) * POSE_VALUES * nblk * (size_t)(C > 0 ? C : 0));
+}
+
+int gsr_pose_preprocess_backward(int lens, int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
+                                 const float* scale, const float* opacity_logit, const float* filter3d,
+                                 const float* camera_T_world, const float* K, const float* camera_centre,
+                                 const uint8_t* visible, const float* grad_rows, int use_rows_uv,
+                                 const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
+                                 float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                                 float* g_sh_rest, const float* lens_consts, float* g_pose, void* temp,
+                                 size_t temp_bytes, void* stream) {
+    return pose_backward(true, lens, mode, 1, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
+                         camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
+                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose, temp,
+                         temp_bytes, stream);
+}
+
+int gsr_pose_batch_preprocess_backward(int lens, int mode, int C, int N, int n_sh_rest, const float* xyz,
+                                       const float* quaternion, const float* scale, const float* opacity_logit,
+                                       const float* filter3d, const float* camera_T_world, const float* K,
+                                       const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                                       int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
+                                       float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit,
+                                       float* g_rgb_dc, float* g_sh_rest, const float* lens_consts, float* g_pose,
+                                       void* temp, size_t temp_bytes, void* stream) {
+    return pose_backward(false, lens, mode, C, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
+                         camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
+                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose, temp,
+                         temp_bytes, stream);
+}
+
+}  // extern "C"
+
+#endif  // GSR_POSE_LENS == 0

@@ -1,6 +1,6 @@
 // gsr_preprocess.cuh — the per-Gaussian stages of the fused path and the view constants they read, shared by the
 // single-view kernels (gsr_preprocess.cu, libgsr_b200.so), the multi-view kernels (gsr_batch.cu, libgsr_batch.so)
-// and the fisheye kernels (gsr_fisheye.cu, libgsr_fisheye.so).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian;
+// the lens kernels (gsr_fisheye.cu, gsr_distortion.cu) and the pose-gradient kernels (gsr_pose.cu).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian;
 // the single-view kernels store its result, the batched kernels add it up over the views.  The camera model enters
 // only through the GSR_PROJECT / GSR_JACOBIAN hooks below.
 #pragma once
@@ -107,7 +107,7 @@ __device__ __forceinline__ void coop_copy(float* __restrict__ dst, const float* 
 // Camera-model hooks.  The per-gaussian bodies below name the camera model only through these macros.  The pinhole
 // defaults expand to exactly the calls the bodies made before the hooks existed, so every pinhole kernel keeps its
 // instructions; a translation unit that defines GSR_PROJECTION_HOOKS (and the macros) before including this header
-// compiles the same bodies for another model (gsr_fisheye.cu).
+// compiles the same bodies for another model (the hook sets of gsr_fisheye.cuh and gsr_distortion.cuh).
 //   GSR_VIEW_PARAM                       extra trailing parameters of the bodies
 //   GSR_VIEW_DECL                        extra CTA-wide view constants, next to `vc`
 //   GSR_LOAD_VIEW(T, K, cam, view)       fill `vc` (and the extra constants) for view index `view`; ends with a barrier
@@ -125,6 +125,19 @@ __device__ __forceinline__ void coop_copy(float* __restrict__ dst, const float* 
 #define GSR_JACOBIAN(px, py, pz, J) proj_jacobian<float>(px, py, pz, vc.K[0], vc.K[4], J)
 #define GSR_JACOBIAN_BWD(px, py, pz, gJ, g) proj_jacobian_bwd<float>(px, py, pz, vc.K[0], vc.K[4], gJ, g)
 #define GSR_PROJECT_BWD(px, py, pz, gu, gv, g) project_uv_bwd<float>(px, py, pz, vc.K[0], vc.K[4], gu, gv, g)
+#endif
+
+// Pose-gradient hooks, empty by default: every kernel that does not define GSR_POSE_HOOKS keeps its instructions.
+// gsr_pose.cuh defines them (gsr_pose.cu, libgsr_pose.so).
+//   GSR_POSE_PARAM          extra trailing parameters of the backward bodies
+//   GSR_POSE_DECL           per-thread pose accumulators, zero (single view: once; batched: per view)
+//   GSR_POSE_VIEW           inside GSR_PRE_BWD_VIEW once gp, the gradient on the camera-frame mean, is complete
+//   GSR_POSE_REDUCE(view)   after the view's `if (vis)` block, reached by every thread of the CTA
+#ifndef GSR_POSE_HOOKS
+#define GSR_POSE_PARAM
+#define GSR_POSE_DECL
+#define GSR_POSE_VIEW
+#define GSR_POSE_REDUCE(view)
 #endif
 
 // One view's fused VJP for one visible gaussian, as a statement block: it reads the view constants `vc`, the
@@ -196,6 +209,7 @@ _Pragma("unroll")                                                               
         GSR_PROJECT_BWD(px, py, pz, guv[0], guv[1], gp_uv);                                                              \
         float gp[3] = {gp_j[0] + gp_uv[0], gp_j[1] + gp_uv[1], gp_j[2] + gp_uv[2]};                                      \
         if (DEPTH) gp[2] += gzc;                                                                                         \
+        GSR_POSE_VIEW                                                                                                    \
         /* xyz_cam = W xyz + t  =>  grad_xyz = W^T grad_xyz_cam */                                                       \
 _Pragma("unroll")                                                                                                        \
         for (int k = 0; k < 3; ++k) gx[k] = W[0 + k] * gp[0] + W[3 + k] * gp[1] + W[6 + k] * gp[2];                      \
@@ -242,7 +256,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
                      const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
                      float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa,
                      float* __restrict__ o_dc, float* __restrict__ o_sh, int use_tma,
-                     const float* __restrict__ filter3d GSR_VIEW_PARAM) {
+                     const float* __restrict__ filter3d GSR_VIEW_PARAM GSR_POSE_PARAM) {
     constexpr int NR = N_SH - 1;
     constexpr int NR3 = HAS_SH ? 3 * NR : 1;
     // all outputs of the CTA's 128 gaussians are staged in shared memory and leave as six bulk stores
@@ -261,6 +275,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
     const int i = i0 + tid;
     float gx[3] = {0.f, 0.f, 0.f}, gq[4] = {0.f, 0.f, 0.f, 0.f}, gs[3] = {0.f, 0.f, 0.f}, go = 0.f,
           gdc[3] = {0.f, 0.f, 0.f};
+    GSR_POSE_DECL
     float* my_sh = s_sh + tid * NR3;
     bool vis = false;
     if (i < N) vis = visible[i] != 0;
@@ -302,6 +317,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
 #pragma unroll
         for (int k = 0; k < NR3; ++k) my_sh[k] = 0.f;
     }
+    GSR_POSE_REDUCE(0)
 #pragma unroll
     for (int k = 0; k < 3; ++k) { s_xyz[tid * 3 + k] = gx[k]; s_scale[tid * 3 + k] = gs[k]; s_dc[tid * 3 + k] = gdc[k]; }
     *reinterpret_cast<float4*>(s_quat + tid * 4) = make_float4(gq[0], gq[1], gq[2], gq[3]);
@@ -520,7 +536,7 @@ __device__ __forceinline__ void batch_preprocess_bwd(
     const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rows,
     int rows_uv, const float* __restrict__ g_uv_compact, const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
     float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa, float* __restrict__ o_dc,
-    float* __restrict__ o_sh, int use_tma, const float* __restrict__ filter3d GSR_VIEW_PARAM) {
+    float* __restrict__ o_sh, int use_tma, const float* __restrict__ filter3d GSR_VIEW_PARAM GSR_POSE_PARAM) {
     constexpr int NR = N_SH - 1;
     constexpr int NR3 = HAS_SH ? 3 * NR : 1;
     __shared__ ViewConsts vc;
@@ -561,6 +577,7 @@ __device__ __forceinline__ void batch_preprocess_bwd(
         const size_t ci = (size_t)c * N + i;
         const bool vis = any && visible[ci] != 0;
         float gcv[3] = {0.f, 0.f, 0.f}, guv[2] = {0.f, 0.f}, gov = 0.f, grv[3] = {0.f, 0.f, 0.f}, gzc = 0.f;
+        GSR_POSE_DECL
         if (vis) {
             // view c's row, read exactly as the single-view kernel reads it
             const float4* row = reinterpret_cast<const float4*>(g_rows + ci * GSR_GRAD_ROW_FLOATS);
@@ -603,6 +620,7 @@ __device__ __forceinline__ void batch_preprocess_bwd(
                 for (int k = 0; k < NR3; ++k) acc_sh[k] = __fadd_rn(acc_sh[k], v_sh[k]);
             }
         }
+        GSR_POSE_REDUCE(c)
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) { s_xyz[tid * 3 + k] = ax[k]; s_scale[tid * 3 + k] = as[k]; s_dc[tid * 3 + k] = adc[k]; }

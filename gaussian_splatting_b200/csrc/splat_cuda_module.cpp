@@ -16,6 +16,7 @@
 #include "../../include/gsr_batch.h"
 #include "../../include/gsr_fisheye.h"
 #include "../../include/gsr_distortion.h"
+#include "../../include/gsr_pose.h"
 
 namespace {
 
@@ -793,7 +794,8 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
                                                       c10::optional<torch::Tensor> grad_uv_compact,
                                                       c10::optional<torch::Tensor> scan, bool use_slab_uv,
                                                       int64_t mode, c10::optional<torch::Tensor> filter3d,
-                                                      Lens lens, c10::optional<torch::Tensor> lc) {
+                                                      Lens lens, c10::optional<torch::Tensor> lc,
+                                                      bool pose = false) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     const int64_t N = xyz.size(0);
     TORCH_CHECK(slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ", GSR_GRAD_ROW_FLOATS,
@@ -844,7 +846,14 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
         F32PTR(camera_T_world), F32PTR(K), camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,   \
         visible.data_ptr<uint8_t>(), slab.data_ptr<float>(), use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr,            \
         F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    if (lens == Lens::Fisheye)
+    torch::Tensor g_pose;
+    if (pose) {
+        g_pose = torch::empty({4, 4}, opt);
+        torch::Tensor temp = torch::empty({(int64_t)gsr_pose_temp_bytes(1, (int)N)}, opt.dtype(torch::kUInt8));
+        check_rc(gsr_pose_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), temp.data_ptr(),
+                                              (size_t)temp.numel(), cur_stream()),
+                 "gsr_pose_preprocess_backward");
+    } else if (lens == Lens::Fisheye)
         check_rc(gsr_fisheye_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()), "gsr_fisheye_preprocess_backward");
     else if (lens == Lens::Distortion)
         check_rc(gsr_distortion_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
@@ -854,7 +863,8 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
 #undef GSR_BWD_ARGS
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
-    out.push_back(flat);  // last: the allocation all the others are views of
+    out.push_back(flat);  // the allocation all the gaussian gradients are views of
+    if (pose) out.push_back(g_pose);  // last: d loss / d camera_T_world [4,4]
     return out;
 }
 
@@ -1069,7 +1079,7 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
                                                  c10::optional<torch::Tensor> grad_uv_compact,
                                                  c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
                                                  c10::optional<torch::Tensor> filter3d, Lens lens,
-                                                 c10::optional<torch::Tensor> lc) {
+                                                 c10::optional<torch::Tensor> lc, bool pose = false) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(visible);
@@ -1127,7 +1137,14 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
         F32PTR(camera_T_world), F32PTR(K), centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab),                    \
         use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o),           \
         F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    if (lens == Lens::Fisheye)
+    torch::Tensor g_pose;
+    if (pose) {
+        g_pose = torch::empty({C, 4, 4}, opt);
+        torch::Tensor temp = torch::empty({(int64_t)gsr_pose_temp_bytes((int)C, (int)N)}, opt.dtype(torch::kUInt8));
+        check_rc(gsr_pose_batch_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), temp.data_ptr(),
+                                                    (size_t)temp.numel(), cur_stream()),
+                 "gsr_pose_batch_preprocess_backward");
+    } else if (lens == Lens::Fisheye)
         check_rc(gsr_fisheye_batch_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
                  "gsr_fisheye_batch_preprocess_backward");
     else if (lens == Lens::Distortion)
@@ -1139,6 +1156,7 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
     out.push_back(flat);
+    if (pose) out.push_back(g_pose);  // last: d loss / d camera_T_world [C,4,4]
     return out;
 }
 
@@ -1219,6 +1237,41 @@ std::vector<torch::Tensor> batch_distortion_preprocess_backward(
     return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
                           visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Distortion,
                           distortion);
+}
+
+// The per-gaussian backward with the camera pose gradient (libgsr_pose.so): the arguments of fused_preprocess_backward /
+// batch_preprocess_backward plus the lens (0 pinhole, 1 fisheye, 2 distortion; GSR_LENS_*) and its constants (the
+// forward's, none for the pinhole).  Returns the same outputs followed by d loss / d camera_T_world, [4,4] / [C,4,4]
+// (last row 0).
+static Lens pose_lens(int64_t lens) {
+    TORCH_CHECK(lens == GSR_LENS_PINHOLE || lens == GSR_LENS_FISHEYE || lens == GSR_LENS_DISTORTION,
+                "lens must be 0 (pinhole), 1 (fisheye) or 2 (distortion)");
+    static_assert((int)Lens::Pinhole == GSR_LENS_PINHOLE && (int)Lens::Fisheye == GSR_LENS_FISHEYE &&
+                      (int)Lens::Distortion == GSR_LENS_DISTORTION,
+                  "Lens and GSR_LENS_* agree");
+    return (Lens)lens;
+}
+
+std::vector<torch::Tensor> pose_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
+    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
+                               lens_consts, true);
+}
+
+std::vector<torch::Tensor> batch_pose_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
+    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
+                          lens_consts, true);
 }
 
 // gsr_distortion_r2_max of 5 coefficients k1 k2 p1 p2 k3 (host floats)
@@ -1693,6 +1746,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "batch_preprocess_forward for OPENCV (radial-tangential) cameras, [C,6] constants");
     m.def("batch_distortion_preprocess_backward", &batch_distortion_preprocess_backward,
           "batch_preprocess_backward for OPENCV cameras (gsr_distortion_batch_preprocess_backward)");
+    m.def("pose_preprocess_backward", &pose_preprocess_backward,
+          "fused_preprocess_backward plus d loss / d camera_T_world [4,4], any lens (gsr_pose_preprocess_backward)");
+    m.def("batch_pose_preprocess_backward", &batch_pose_preprocess_backward,
+          "batch_preprocess_backward plus d loss / d camera_T_world [C,4,4], any lens "
+          "(gsr_pose_batch_preprocess_backward)");
     m.def("distortion_r2_max", &distortion_r2_max,
           "the radial fold limit s = r^2 of 5 coefficients k1 k2 p1 p2 k3 (gsr_distortion_r2_max)");
     m.def("filter3d", &filter3d, "Mip-Splatting's 3-D filter size per gaussian from the training cameras (gsr_filter3d)",

@@ -394,10 +394,20 @@ def _lens_constants(lens, k, device):
     return t
 
 
+def _pose_lens(lens):
+    """(lens enum, constants) of the pose bindings for a state's lens (None: the pinhole)"""
+    if lens is None:
+        return 0, None
+    return (1 if lens[0] == "fisheye" else 2), lens[1]
+
+
 class _ProjectGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg):
         ext = native()
+        # torch.matmul takes another path (other rounding) for an operand that requires grad: the forward's bits must
+        # not depend on whether the pose does
+        camera_T_world = camera_T_world.detach()
         H, W, near, far, pad, mh = cfg
         depth_base, depth_bits = _depth_key_params(near, far)
         opacity_flat = opacity.reshape(-1)
@@ -430,7 +440,8 @@ class _ProjectGaussians(torch.autograd.Function):
                 lens, consts = state.lens
                 fwd = ext.fisheye_preprocess_forward if lens == "fisheye" else ext.distortion_preprocess_forward
                 records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
-        record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])  # a backward pass can follow
+        # a backward pass can follow (the pose counts: a pose-only refinement needs the masks too)
+        record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:7])
         background = state.background
 
         def counts(total):
@@ -532,7 +543,11 @@ class _ProjectGaussians(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            if st.lens is None:
+            g_pose = None
+            if ctx.needs_input_grad[6]:
+                # the same kernels' arithmetic plus the pose reduction (libgsr_pose.so)
+                *grads, g_pose = native().pose_preprocess_backward(*args, *_pose_lens(st.lens))
+            elif st.lens is None:
                 grads = native().fused_preprocess_backward(*args)
             else:
                 lens, consts = st.lens
@@ -542,7 +557,7 @@ class _ProjectGaussians(torch.autograd.Function):
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
-        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, None, None, None, None
+        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, None, None, None
 
 
 class _CompositeTiles(torch.autograd.Function):
@@ -682,7 +697,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     k = 0 is the equidistant fisheye, not the pinhole.  The 2-D covariance uses the Jacobian of that projection at the
     mean (EWA), and a gaussian at theta >= fisheye_theta_max(k), where the model folds back, is culled on top of the
     near / far / padding rules.  Depth keys, the depth map and the SH view direction keep camera-frame z and the
-    position; uv and uv.grad are the fisheye pixel coordinates and their gradient; K, the pose and k get no gradient
+    position; uv and uv.grad are the fisheye pixel coordinates and their gradient; K and k get no gradient
     (DESIGN.md 3.19).  The coefficients are constants of the camera, uploaded once per camera without synchronising
     with the device.  Combines with every other option.  None (the default) is the pinhole.  A CUDA tensor, a wrong
     shape or non-finite coefficients raise ValueError; fp32 and precomputed SH colours only.
@@ -695,7 +710,17 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     covariance uses the exact Jacobian of that projection at the mean, and a gaussian at s >= distortion_r2_max(k),
     where barrel distortion folds back, is culled on top of the other rules.  Everything else is as for fisheye
     (DESIGN.md 3.20); k = 0 runs the distortion kernels and gives the pinhole up to fp32 rounding.  Passing both
-    fisheye and distortion raises ValueError."""
+    fisheye and distortion raises ValueError.
+
+    camera_T_world: when it requires grad (a leaf, or e.g. pose.PoseDelta's se3_exp(xi) @ T0), the backward also gives
+    d loss / d camera_T_world [4,4], for pose refinement, with every lens and option above.  With W = T[:3,:3] and
+    p_i = W x_i + t: dL/dT[:3,:3] = sum_i (g_p,i x_i^T + J_i^T (2 G_i M_i Sigma_i)), dL/dT[:3,3] = sum_i g_p,i,
+    dL/dT[3,:] = 0, over the visible gaussians, g_p the gradient on the camera-frame mean (projection, lens, depth and
+    any gradient on uv), G the gradient on the 2-D covariance M Sigma M^T, M = J W.  The camera centre of the SH view
+    direction is held constant, as it is for xyz (exact with SH degree 0).  Reduced natively in a fixed order, so the
+    same render-stage rows give the same bits (DESIGN.md 3.21).  Everything else is unchanged.  A pose that does not
+    require grad runs exactly the kernels without it.  rasterize_unfused (and fp64 / per-pixel SH) gives the pose only
+    what autograd gets through its torch transform of the means."""
     lens = _lens_arg(fisheye, distortion)
     if lens is not None:
         if gaussians.xyz.dtype != torch.float32:
@@ -868,6 +893,7 @@ class _BatchState:
 class _ProjectBatch(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg):
+        camera_T_world = camera_T_world.detach()  # as in _ProjectGaussians.forward
         ext = native()
         H, W, near, far, pad, mh = cfg
         C, N = camera_T_world.shape[0], xyz.shape[0]
@@ -895,7 +921,7 @@ class _ProjectBatch(torch.autograd.Function):
                 fwd = (ext.batch_fisheye_preprocess_forward if lens == "fisheye"
                        else ext.batch_distortion_preprocess_forward)
                 records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
-        record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:6])
+        record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:7])
         background = state.background
         depth_mode = bool(state.mode & ext.MODE_DEPTH_ALPHA)
 
@@ -997,7 +1023,10 @@ class _ProjectBatch(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            if st.lens is None:
+            g_pose = None
+            if ctx.needs_input_grad[6]:
+                *grads, g_pose = native().batch_pose_preprocess_backward(*args, *_pose_lens(st.lens))
+            elif st.lens is None:
                 grads = native().batch_preprocess_backward(*args)
             else:
                 lens, consts = st.lens
@@ -1008,7 +1037,7 @@ class _ProjectBatch(torch.autograd.Function):
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]
-        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, None, None, None, None
+        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, None, None, None
 
 
 class _CompositeBatch(torch.autograd.Function):
@@ -1108,8 +1137,9 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
     centre, depth keys, pair list and tile kernels.  Backward: one gradient for the batch, the sum over the views of
     each view's parameter gradient, added per gaussian in view order in fp32 (g = g_0; g += g_1; ...), which is what
     autograd's accumulation over C rasterize() calls gives for the same render-stage rows.  The per-gaussian backward
-    reads the parameters once and writes the gradient once for all views (libgsr_batch.so, DESIGN.md 3.18).  Camera
-    poses and filter3d get no gradient.
+    reads the parameters once and writes the gradient once for all views (libgsr_batch.so, DESIGN.md 3.18).  filter3d
+    gets no gradient.  A camera_T_world that requires grad gets one gradient per view [C,4,4], as rasterize() defines
+    it; view c's is bit-identical to the single-view kernel's on view c's rows (DESIGN.md 3.21).
 
     state (return_state=True): state.views[c] has vis_idx32, uv_absgrad, N and M, so that
     DensificationStats.accumulate(state.views[c], uvs[c], xyz, K_c) works per view; state.grad_flat (or grad_out, a
