@@ -9,6 +9,7 @@ Drop-in for the rasterization path of joeyan/gaussian_splatting:
   * ``gaussian_splatting_b200.rasterize.rasterize`` — same signature and return values as
     ``splat_py.rasterize.rasterize`` (splat_py/rasterize.py:18-112), fused implementation.
   * ``gaussian_splatting_b200.rasterize_batch`` — C cameras of one scene in one fused forward and backward.
+  * ``gaussian_splatting_b200.appearance`` — per-image bilateral grids (appearance correction) on native kernels.
   * ``cuda_autograd_functions`` / ``tile_culling`` / ``structs`` / ``utils`` / ``depth`` — host-side
     mirror of the reference modules of the same names.
 

@@ -17,6 +17,7 @@
 #include "../../include/gsr_fisheye.h"
 #include "../../include/gsr_distortion.h"
 #include "../../include/gsr_pose.h"
+#include "../../include/gsr_bilagrid.h"
 
 namespace {
 
@@ -1663,6 +1664,93 @@ torch::Tensor photometric_loss_backward(torch::Tensor pred, torch::Tensor target
     return grad;
 }
 
+// ---------------------------------------------------------------------------------------------
+// bilateral-grid appearance correction (gsr_bilagrid_*): rgb [C,H,W,3] any strides, grids [N,12,L,GY,GX] contiguous,
+// ids [C] int32 on the device (range-checked by the caller)
+// ---------------------------------------------------------------------------------------------
+void check_bilagrid_grids(const torch::Tensor& grids) {
+    CHECK_VALID_INPUT(grids);
+    CHECK_FLOAT_TENSOR(grids);
+    TORCH_CHECK(grids.dim() == 5 && grids.size(1) == 12, "grids must be [N,12,L,GY,GX]");
+}
+
+void check_bilagrid_slice(const torch::Tensor& rgb, const torch::Tensor& grids, const torch::Tensor& ids) {
+    check_bilagrid_grids(grids);
+    TORCH_CHECK(rgb.is_cuda() && rgb.device() == grids.device(), "rgb must be on the grids' device");
+    CHECK_FLOAT_TENSOR(rgb);
+    TORCH_CHECK(rgb.dim() == 4 && rgb.size(3) == 3, "rgb must be [C,H,W,3]");
+    CHECK_VALID_INPUT(ids);
+    CHECK_INT_TENSOR(ids);
+    TORCH_CHECK(ids.device() == grids.device() && ids.dim() == 1 && ids.size(0) == rgb.size(0),
+                "ids must be [C] on the grids' device");
+}
+
+torch::Tensor bilagrid_slice_forward(torch::Tensor rgb, torch::Tensor grids, torch::Tensor ids) {
+    check_bilagrid_slice(rgb, grids, ids);
+    c10::cuda::CUDAGuard guard(rgb.device());
+    torch::Tensor out = torch::empty(rgb.sizes(), rgb.options().memory_format(torch::MemoryFormat::Contiguous));
+    const int64_t rs[4] = {rgb.stride(0), rgb.stride(1), rgb.stride(2), rgb.stride(3)};
+    check_rc(gsr_bilagrid_slice_forward((int)rgb.size(0), (int)rgb.size(1), (int)rgb.size(2), F32PTR(rgb), rs,
+                                        F32PTR(grids), (int)grids.size(0), (int)grids.size(2), (int)grids.size(3),
+                                        (int)grids.size(4), ids.data_ptr<int32_t>(), F32PTR(out), cur_stream()),
+             "gsr_bilagrid_slice_forward");
+    return out;
+}
+
+// returns (grad_rgb [C,H,W,3] contiguous or None, grad_grids [N,12,L,GY,GX] or None)
+std::vector<torch::Tensor> bilagrid_slice_backward(torch::Tensor rgb, torch::Tensor grids, torch::Tensor ids,
+                                                   torch::Tensor grad_out, bool need_rgb, bool need_grids) {
+    check_bilagrid_slice(rgb, grids, ids);
+    TORCH_CHECK(grad_out.is_cuda() && grad_out.device() == rgb.device(), "grad_out must be on rgb's device");
+    CHECK_FLOAT_TENSOR(grad_out);
+    TORCH_CHECK(grad_out.sizes() == rgb.sizes(), "grad_out must have rgb's shape");
+    c10::cuda::CUDAGuard guard(rgb.device());
+    const int C = rgb.size(0), H = rgb.size(1), W = rgb.size(2);
+    const int L = grids.size(2), GY = grids.size(3), GX = grids.size(4);
+    torch::Tensor grad_rgb, grad_grids, temp;
+    if (need_rgb) grad_rgb = torch::empty(rgb.sizes(), rgb.options().memory_format(torch::MemoryFormat::Contiguous));
+    size_t tb = 0;
+    if (need_grids) {
+        grad_grids = torch::empty_like(grids);
+        tb = gsr_bilagrid_slice_backward_temp_bytes(C, H, L, GY, GX);
+        temp = torch::empty({(int64_t)tb}, grids.options().dtype(torch::kUInt8));
+    }
+    const int64_t rs[4] = {rgb.stride(0), rgb.stride(1), rgb.stride(2), rgb.stride(3)};
+    const int64_t gs[4] = {grad_out.stride(0), grad_out.stride(1), grad_out.stride(2), grad_out.stride(3)};
+    check_rc(gsr_bilagrid_slice_backward(C, H, W, F32PTR(rgb), rs, F32PTR(grids), (int)grids.size(0), L, GY, GX,
+                                         ids.data_ptr<int32_t>(), F32PTR(grad_out), gs,
+                                         need_rgb ? F32PTR(grad_rgb) : nullptr,
+                                         need_grids ? F32PTR(grad_grids) : nullptr,
+                                         need_grids ? temp.data_ptr() : nullptr, tb, cur_stream()),
+             "gsr_bilagrid_slice_backward");
+    return {grad_rgb, grad_grids};
+}
+
+// returns tv(grids) as a 0-dim float tensor on the device
+torch::Tensor bilagrid_tv_forward(torch::Tensor grids) {
+    check_bilagrid_grids(grids);
+    c10::cuda::CUDAGuard guard(grids.device());
+    const int N = grids.size(0), L = grids.size(2), GY = grids.size(3), GX = grids.size(4);
+    torch::Tensor out = torch::empty({}, grids.options());
+    const size_t tb = gsr_bilagrid_tv_temp_bytes(N, L, GY, GX);
+    torch::Tensor temp = torch::empty({(int64_t)tb}, grids.options().dtype(torch::kUInt8));
+    check_rc(gsr_bilagrid_tv_forward(N, L, GY, GX, F32PTR(grids), F32PTR(out), temp.data_ptr(), tb, cur_stream()),
+             "gsr_bilagrid_tv_forward");
+    return out;
+}
+
+torch::Tensor bilagrid_tv_backward(torch::Tensor grids, torch::Tensor grad_tv) {
+    check_bilagrid_grids(grids);
+    TORCH_CHECK(grad_tv.is_cuda() && grad_tv.device() == grids.device(), "grad_tv must be on the grids' device");
+    TORCH_CHECK(grad_tv.numel() == 1 && grad_tv.dtype() == torch::kFloat32, "grad_tv must be a float scalar");
+    c10::cuda::CUDAGuard guard(grids.device());
+    torch::Tensor grad = torch::empty_like(grids);
+    check_rc(gsr_bilagrid_tv_backward((int)grids.size(0), (int)grids.size(2), (int)grids.size(3), (int)grids.size(4),
+                                      F32PTR(grids), F32PTR(grad_tv), F32PTR(grad), cur_stream()),
+             "gsr_bilagrid_tv_backward");
+    return grad;
+}
+
 std::string version() { return gsr_version(); }
 
 }  // namespace
@@ -1781,6 +1869,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("photometric_loss_forward", &photometric_loss_forward,
           "(1 - ssim_frac) * L1 + ssim_frac * (1 - SSIM) forward -> (loss, L1, SSIM)");
     m.def("photometric_loss_backward", &photometric_loss_backward, "photometric loss backward -> gradient on pred");
+    m.def("bilagrid_slice_forward", &bilagrid_slice_forward,
+          "bilateral-grid slice: per-pixel affine colour transform from grids[ids[c]] (gsr_bilagrid_slice_forward)",
+          py::arg("rgb"), py::arg("grids"), py::arg("ids"));
+    m.def("bilagrid_slice_backward", &bilagrid_slice_backward,
+          "bilateral-grid slice backward -> (grad_rgb or None, grad_grids or None) (gsr_bilagrid_slice_backward)",
+          py::arg("rgb"), py::arg("grids"), py::arg("ids"), py::arg("grad_out"), py::arg("need_rgb"),
+          py::arg("need_grids"));
+    m.def("bilagrid_tv_forward", &bilagrid_tv_forward, "total variation of the grids, on the device");
+    m.def("bilagrid_tv_backward", &bilagrid_tv_backward, "total variation backward -> gradient on the grids");
     m.def("version", &version, "library version string");
     m.def("contribution_mask_words",
           [](int64_t P, int64_t H, int64_t W) { return (int64_t)gsr_contribution_mask_words(P, (int)H, (int)W); },
