@@ -10,6 +10,7 @@ Drop-in for the rasterization path of joeyan/gaussian_splatting:
     ``splat_py.rasterize.rasterize`` (splat_py/rasterize.py:18-112), fused implementation.
   * ``gaussian_splatting_b200.rasterize_batch`` — C cameras of one scene in one fused forward and backward.
   * ``gaussian_splatting_b200.appearance`` — per-image bilateral grids (appearance correction) on native kernels.
+  * ``gaussian_splatting_b200.calib`` — ``IntrinsicsDelta``, camera self-calibration with the fused path's K gradient.
   * ``cuda_autograd_functions`` / ``tile_culling`` / ``structs`` / ``utils`` / ``depth`` — host-side
     mirror of the reference modules of the same names.
 

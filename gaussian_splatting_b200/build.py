@@ -7,11 +7,13 @@
   libgsr_fisheye.so         the per-gaussian kernels for fisheye cameras (include/gsr_fisheye.h), same flags
   libgsr_distortion.so      the per-gaussian kernels for radial-tangential lens distortion (include/gsr_distortion.h)
   libgsr_pose.so            the per-gaussian backward with the camera pose gradient, every lens (include/gsr_pose.h)
+  libgsr_calib.so           the same sources compiled with the pose, intrinsics and lens-coefficient gradients
+                            (include/gsr_calib.h)
   libgsr_bilagrid.so        bilateral-grid appearance correction: slice forward / backward, total variation
                             (include/gsr_bilagrid.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all nine; `build(force=False)` is incremental.
+`python -m gaussian_splatting_b200.build` builds all ten; `build(force=False)` is incremental.
 """
 from __future__ import annotations
 
@@ -35,6 +37,7 @@ BATCH_LIB = PKG / "libgsr_batch.so"
 FISHEYE_LIB = PKG / "libgsr_fisheye.so"
 DISTORTION_LIB = PKG / "libgsr_distortion.so"
 POSE_LIB = PKG / "libgsr_pose.so"
+CALIB_LIB = PKG / "libgsr_calib.so"
 BILAGRID_LIB = PKG / "libgsr_bilagrid.so"
 
 CU_SOURCES = [
@@ -79,14 +82,18 @@ DISTORTION_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_d
                                                                     CSRC / "gsr_poly_roots.h",
                                                                     ROOT / "include" / "gsr_b200.h",
                                                                     ROOT / "include" / "gsr_distortion.h"]
-# gsr_pose.cu once per camera model (GSR_POSE_LENS: 0 pinhole, 1 fisheye, 2 distortion): (source, object, -D flags)
+# gsr_pose.cu once per camera model (GSR_POSE_LENS: 0 pinhole, 1 fisheye, 2 distortion): (source, object, -D flags);
+# libgsr_calib.so compiles the same three with GSR_POSE_CAMERA (the camera-gradient kernels)
 POSE_SOURCES = [("gsr_pose.cu", f"gsr_pose_{i}", [f"-DGSR_POSE_LENS={i}"]) for i in range(3)]
-POSE_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_pose.cuh", CSRC / "gsr_fisheye.cuh",
+CALIB_SOURCES = [("gsr_pose.cu", f"gsr_camera_{i}", [f"-DGSR_POSE_LENS={i}", "-DGSR_POSE_CAMERA"]) for i in range(3)]
+POSE_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_pose.cuh", CSRC / "gsr_calib.cuh",
+                                                             CSRC / "gsr_fisheye.cuh",
                                                              CSRC / "gsr_distortion.cuh",
                                                              ROOT / "include" / "gsr_b200.h",
                                                              ROOT / "include" / "gsr_fisheye.h",
                                                              ROOT / "include" / "gsr_distortion.h",
-                                                             ROOT / "include" / "gsr_pose.h"]
+                                                             ROOT / "include" / "gsr_pose.h",
+                                                             ROOT / "include" / "gsr_calib.h"]
 BILAGRID_SOURCES = ["gsr_bilagrid.cu"]
 BILAGRID_HEADERS = [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_bilagrid.h"]
 
@@ -182,6 +189,10 @@ def build_pose_lib(force: bool = False, verbose: bool = False) -> Path:
     return _build_cuda_lib(POSE_LIB, POSE_SOURCES, POSE_HEADERS, "pose_lib.sha256", force, verbose)
 
 
+def build_calib_lib(force: bool = False, verbose: bool = False) -> Path:
+    return _build_cuda_lib(CALIB_LIB, CALIB_SOURCES, POSE_HEADERS, "calib_lib.sha256", force, verbose)
+
+
 def build_bilagrid_lib(force: bool = False, verbose: bool = False) -> Path:
     return _build_cuda_lib(BILAGRID_LIB, BILAGRID_SOURCES, BILAGRID_HEADERS, "bilagrid_lib.sha256", force, verbose)
 
@@ -198,7 +209,8 @@ def build_ext(force: bool = False) -> Path:
     want = _digest([src, ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h",
                     ROOT / "include" / "gsr_features.h", ROOT / "include" / "gsr_batch.h",
                     ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h",
-                    ROOT / "include" / "gsr_pose.h", ROOT / "include" / "gsr_bilagrid.h"], torch.__version__)
+                    ROOT / "include" / "gsr_pose.h", ROOT / "include" / "gsr_bilagrid.h",
+                    ROOT / "include" / "gsr_calib.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -210,7 +222,7 @@ def build_ext(force: bool = False) -> Path:
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
         f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", "-lgsr_fisheye",
-        "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid",
+        "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid", "-lgsr_calib",
         f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",
@@ -237,6 +249,7 @@ def build(force: bool = False, verbose: bool = False):
     build_fisheye_lib(force=force, verbose=verbose)
     build_distortion_lib(force=force, verbose=verbose)
     build_pose_lib(force=force, verbose=verbose)
+    build_calib_lib(force=force, verbose=verbose)
     build_bilagrid_lib(force=force, verbose=verbose)
     ext = build_ext(force=force)
     return lib, ext

@@ -6,7 +6,8 @@
 // GSR_POSE_LENS 0 (pinhole, the default hooks), 1 (gsr_fisheye.cuh's hooks) or 2 (gsr_distortion.cuh's hooks).  Each
 // compile puts its kernels in a namespace of its own and exports one hidden launcher; the compile with
 // GSR_POSE_LENS == 0 also holds the fp64 finishing kernel and the C ABI of include/gsr_pose.h, which dispatch on the
-// lens.
+// lens.  With GSR_POSE_CAMERA the same three compiles make libgsr_calib.so: the same bodies, whose rows also carry the
+// intrinsics and lens-coefficient gradients of gsr_calib.cuh, with the C ABI of include/gsr_calib.h.
 #include <cstdint>
 
 #include "../../include/gsr_distortion.h"
@@ -19,44 +20,86 @@
 #if GSR_POSE_LENS == 1
 #define GSR_FISHEYE_HOOKS
 #include "gsr_fisheye.cuh"
-#define GSR_POSE_NS pose_fisheye
-#define GSR_POSE_LAUNCH gsr_pose_launch_fisheye
 #define GSR_POSE_LENS_ARG , lens
 #elif GSR_POSE_LENS == 2
 #define GSR_DISTORTION_HOOKS
 #include "gsr_distortion.cuh"
-#define GSR_POSE_NS pose_distortion
-#define GSR_POSE_LAUNCH gsr_pose_launch_distortion
 #define GSR_POSE_LENS_ARG , lens
 #else
-#define GSR_POSE_NS pose_pinhole
-#define GSR_POSE_LAUNCH gsr_pose_launch_pinhole
 #define GSR_POSE_LENS_ARG
 #endif
 
-// gsr_preprocess.cuh's one non-inline device function has a host-side symbol: one name per compile, so that the
-// three objects link into one library
+// one namespace, launcher and name of gsr_preprocess.cuh's one non-inline device function (it has a host-side symbol)
+// per compile, so that the three objects of a library (and the two libraries) link side by side
+#ifdef GSR_POSE_CAMERA
 #if GSR_POSE_LENS == 1
+#define GSR_POSE_NS camera_fisheye
+#define GSR_POSE_LAUNCH gsr_camera_launch_fisheye
+#define camera_centre camera_centre_camera_fisheye
+#elif GSR_POSE_LENS == 2
+#define GSR_POSE_NS camera_distortion
+#define GSR_POSE_LAUNCH gsr_camera_launch_distortion
+#define camera_centre camera_centre_camera_distortion
+#else
+#define GSR_POSE_NS camera_pinhole
+#define GSR_POSE_LAUNCH gsr_camera_launch_pinhole
+#define camera_centre camera_centre_camera_pinhole
+#endif
+#else
+#if GSR_POSE_LENS == 1
+#define GSR_POSE_NS pose_fisheye
+#define GSR_POSE_LAUNCH gsr_pose_launch_fisheye
 #define camera_centre camera_centre_pose_fisheye
 #elif GSR_POSE_LENS == 2
+#define GSR_POSE_NS pose_distortion
+#define GSR_POSE_LAUNCH gsr_pose_launch_distortion
 #define camera_centre camera_centre_pose_distortion
+#else
+#define GSR_POSE_NS pose_pinhole
+#define GSR_POSE_LAUNCH gsr_pose_launch_pinhole
+#endif
 #endif
 #include "gsr_common.cuh"
+#ifdef GSR_POSE_CAMERA
+#include "gsr_calib.cuh"
+namespace gsr {
+// a row: 12 pose values, fx fy cx cy, the lens's coefficients, zero padding to a multiple of 4 (float4 loads)
+#if GSR_POSE_LENS == 1
+constexpr int CAMERA_VALUES = 20;
+#define GSR_CAMERA_VIEW(px, py, pz, guv, gJ, out) \
+    fisheye_calib(px, py, pz, vc.K[0], vc.K[4], vfe, guv[0], guv[1], gJ, out)
+#elif GSR_POSE_LENS == 2
+constexpr int CAMERA_VALUES = 24;
+#define GSR_CAMERA_VIEW(px, py, pz, guv, gJ, out) \
+    distortion_calib(px, py, pz, vc.K[0], vc.K[4], vdc, guv[0], guv[1], gJ, out)
+#else
+constexpr int CAMERA_VALUES = 16;
+#define GSR_CAMERA_VIEW(px, py, pz, guv, gJ, out) pinhole_calib(px, py, pz, guv[0], guv[1], gJ, out)
+#endif
+}  // namespace gsr
+#endif
 #include "gsr_pose.cuh"
 #include "gsr_preprocess.cuh"
 
 #include "../../include/gsr_pose.h"
+#ifdef GSR_POSE_CAMERA
+#include "../../include/gsr_calib.h"
+#endif
 
-// CTAs per SM the register budget is sized for (-Xptxas -v: no local memory at these bounds, DESIGN.md 3.21)
+// CTAs per SM the register budget is sized for (-Xptxas -v: no local memory at these bounds, DESIGN.md 3.21, 3.23)
 #ifndef GSR_POSE_BWD_MINB
 #define GSR_POSE_BWD_MINB 4
 #endif
 #ifndef GSR_POSE_BATCH_MINB
 #define GSR_POSE_BATCH_MINB 3
 #endif
+#ifdef GSR_POSE_CAMERA
+#define k_pose_preprocess_bwd k_camera_preprocess_bwd
+#define k_pose_batch_preprocess_bwd k_camera_batch_preprocess_bwd
+#endif
 
 // the launcher of one camera model: the per-gaussian kernel of `single` (C == 1) or of C views, writing the
-// partials [C, grid, 12]
+// partials [C, grid, 12] (the camera-gradient kernels: [C, grid, CAMERA_VALUES])
 #define GSR_POSE_LAUNCH_DECL(name)                                                                                   \
     __attribute__((visibility("hidden"))) int name(                                                                 \
         bool single, int mode, int C, int N, int n_sh_rest, const float* xyz, const float* quat, const float* scale, \
@@ -139,28 +182,34 @@ GSR_POSE_LAUNCH_DECL(GSR_POSE_LAUNCH) {
 
 #if GSR_POSE_LENS == 0
 
-GSR_POSE_LAUNCH_DECL(gsr_pose_launch_fisheye);
-GSR_POSE_LAUNCH_DECL(gsr_pose_launch_distortion);
+// the launchers of the other two lenses, compiled in the same library
+#ifdef GSR_POSE_CAMERA
+#define GSR_LAUNCH_FISHEYE gsr_camera_launch_fisheye
+#define GSR_LAUNCH_DISTORTION gsr_camera_launch_distortion
+#else
+#define GSR_LAUNCH_FISHEYE gsr_pose_launch_fisheye
+#define GSR_LAUNCH_DISTORTION gsr_pose_launch_distortion
+#endif
+GSR_POSE_LAUNCH_DECL(GSR_LAUNCH_FISHEYE);
+GSR_POSE_LAUNCH_DECL(GSR_LAUNCH_DISTORTION);
 
 namespace gsr {
 
 constexpr int POSE_FINISH_THREADS = 256;
 
-// one CTA per view: thread t adds the partials t, t + 256, ... in fp64, then the CTA adds the 256 sums in a fixed
-// order (a shuffle tree per warp, then the warps in order) and rounds once.  Writes the view's [4, 4] gradient, the
-// last row 0.
-__global__ void __launch_bounds__(POSE_FINISH_THREADS) k_pose_finish(int nblk, const float* __restrict__ partials,
-                                                                    float* __restrict__ g_pose) {
-    __shared__ double s_sum[POSE_FINISH_THREADS / 32][POSE_VALUES];
-    const int c = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    const float* src = partials + (size_t)c * nblk * POSE_VALUES;
-    double acc[POSE_VALUES];
+// Whole CTA of POSE_FINISH_THREADS, one view: thread t adds the partials t, t + 256, ... of src [nblk, NV] in fp64,
+// then a shuffle tree per warp leaves the warps' sums in s_sum; ends with a CTA barrier.  The caller adds the warps in
+// order and rounds once.
+template <int NV>
+__device__ __forceinline__ void finish_partials(int nblk, const float* __restrict__ src, double (*s_sum)[NV]) {
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    double acc[NV];
 #pragma unroll
-    for (int k = 0; k < POSE_VALUES; ++k) acc[k] = 0.0;
+    for (int k = 0; k < NV; ++k) acc[k] = 0.0;
     for (int b = t; b < nblk; b += POSE_FINISH_THREADS) {
-        const float4* row = reinterpret_cast<const float4*>(src + (size_t)b * POSE_VALUES);
+        const float4* row = reinterpret_cast<const float4*>(src + (size_t)b * NV);
 #pragma unroll
-        for (int q = 0; q < POSE_VALUES / 4; ++q) {
+        for (int q = 0; q < NV / 4; ++q) {
             const float4 v = row[q];
             acc[4 * q + 0] += (double)v.x;
             acc[4 * q + 1] += (double)v.y;
@@ -169,13 +218,23 @@ __global__ void __launch_bounds__(POSE_FINISH_THREADS) k_pose_finish(int nblk, c
         }
     }
 #pragma unroll
-    for (int k = 0; k < POSE_VALUES; ++k) {
+    for (int k = 0; k < NV; ++k) {
         double v = acc[k];
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
         if (lane == 0) s_sum[warp][k] = v;
     }
     __syncthreads();
+}
+
+#ifndef GSR_POSE_CAMERA
+// one CTA per view: the fixed-order fp64 sum of the view's partials, rounded once.  Writes the view's [4, 4] gradient,
+// the last row 0.
+__global__ void __launch_bounds__(POSE_FINISH_THREADS) k_pose_finish(int nblk, const float* __restrict__ partials,
+                                                                    float* __restrict__ g_pose) {
+    __shared__ double s_sum[POSE_FINISH_THREADS / 32][POSE_VALUES];
+    const int c = blockIdx.x, t = threadIdx.x;
+    finish_partials<POSE_VALUES>(nblk, partials + (size_t)c * nblk * POSE_VALUES, s_sum);
     if (t < 16) {
         float out = 0.f;
         if (t < POSE_VALUES) {
@@ -186,6 +245,31 @@ __global__ void __launch_bounds__(POSE_FINISH_THREADS) k_pose_finish(int nblk, c
         g_pose[(size_t)c * 16 + t] = out;
     }
 }
+#else
+// the same for rows of NV camera values: g_pose [C, 4, 4] (last row 0), g_intrinsics [C, 4] (fx fy cx cy) and
+// g_lens [C, n_lens]
+template <int NV>
+__global__ void __launch_bounds__(POSE_FINISH_THREADS)
+    k_camera_finish(int nblk, int n_lens, const float* __restrict__ partials, float* __restrict__ g_pose,
+                    float* __restrict__ g_intrinsics, float* __restrict__ g_lens) {
+    __shared__ double s_sum[POSE_FINISH_THREADS / 32][NV];
+    const int c = blockIdx.x, t = threadIdx.x;
+    finish_partials<NV>(nblk, partials + (size_t)c * nblk * NV, s_sum);
+    if (t < POSE_VALUES + 4 + n_lens) {
+        double v = s_sum[0][t];
+        for (int w = 1; w < POSE_FINISH_THREADS / 32; ++w) v += s_sum[w][t];
+        const float out = (float)v;
+        if (t < POSE_VALUES) {
+            g_pose[(size_t)c * 16 + t] = out;
+        } else if (t < POSE_VALUES + 4) {
+            g_pose[(size_t)c * 16 + t] = 0.f;
+            g_intrinsics[(size_t)c * 4 + t - POSE_VALUES] = out;
+        } else {
+            g_lens[(size_t)c * n_lens + t - POSE_VALUES - 4] = out;
+        }
+    }
+}
+#endif
 
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -196,16 +280,35 @@ constexpr int KNOWN_MODES = GSR_MODE_DEPTH_ALPHA | GSR_MODE_ANTIALIASED | GSR_MO
 
 using namespace gsr;
 
+// the values per row of the camera-gradient kernels of a lens (12 pose, 4 intrinsics, the coefficients, padding)
+static int camera_values(int lens) { return lens == GSR_LENS_FISHEYE ? 20 : lens == GSR_LENS_DISTORTION ? 24 : 16; }
+
+static size_t partial_bytes(int values, int C, int N) {
+    const size_t nblk = (size_t)((N > 0 ? N : 0) + PRE_THREADS - 1) / PRE_THREADS;
+    return align256(sizeof(float) * (size_t)values * nblk * (size_t)(C > 0 ? C : 0));
+}
+
+#ifdef GSR_POSE_CAMERA
+constexpr bool CAMERA = true;
+#else
+constexpr bool CAMERA = false;
+#endif
+
+// The entry points of this library (libgsr_pose.so; with GSR_POSE_CAMERA libgsr_calib.so, which also writes the
+// intrinsics and lens-coefficient gradients g_intrinsics [C, 4] and g_lens [C, n], NULL for the pinhole)
 static int pose_backward(bool single, int lens, int mode, int C, int N, int n_sh_rest, const float* xyz,
                          const float* quaternion, const float* scale, const float* opacity_logit, const float* filter3d,
                          const float* camera_T_world, const float* K, const float* camera_centre,
                          const uint8_t* visible, const float* grad_rows, int use_rows_uv,
                          const float* grad_uv_compact, const uint64_t* scan, float* g_xyz, float* g_quaternion,
                          float* g_scale, float* g_opacity_logit, float* g_rgb_dc, float* g_sh_rest,
-                         const float* lens_consts, float* g_pose, void* temp, size_t temp_bytes, void* stream) {
+                         const float* lens_consts, float* g_pose, float* g_intrinsics, float* g_lens, void* temp,
+                         size_t temp_bytes, void* stream) {
     if (C < 1 || N < 0 || (mode & ~KNOWN_MODES) != 0 || g_pose == nullptr) return GSR_ERR_BAD_ARG;
     if (lens != GSR_LENS_PINHOLE && lens != GSR_LENS_FISHEYE && lens != GSR_LENS_DISTORTION) return GSR_ERR_BAD_ARG;
     if ((lens != GSR_LENS_PINHOLE) != (lens_consts != nullptr)) return GSR_ERR_BAD_ARG;
+    if (CAMERA && (g_intrinsics == nullptr || (lens != GSR_LENS_PINHOLE) != (g_lens != nullptr))) return GSR_ERR_BAD_ARG;
+    const int values = CAMERA ? camera_values(lens) : POSE_VALUES;
     if (((mode & GSR_MODE_FILTER3D) != 0) != (filter3d != nullptr)) return GSR_ERR_BAD_ARG;
     cudaStream_t st = (cudaStream_t)stream;
     const int nblk = (N + PRE_THREADS - 1) / PRE_THREADS;
@@ -220,31 +323,72 @@ static int pose_backward(bool single, int lens, int mode, int C, int N, int n_sh
         if (!aligned16(grad_rows)) return GSR_ERR_BAD_ARG;
         if (grad_uv_compact != nullptr && scan == nullptr) return GSR_ERR_BAD_ARG;
         if (n_sh_rest != 0 && n_sh_rest != 3 && n_sh_rest != 8 && n_sh_rest != 15) return GSR_ERR_UNSUPPORTED;
-        if (temp == nullptr || !aligned16(temp) || temp_bytes < gsr_pose_temp_bytes(C, N)) return GSR_ERR_BAD_ARG;
+        if (temp == nullptr || !aligned16(temp) || temp_bytes < partial_bytes(values, C, N)) return GSR_ERR_BAD_ARG;
         const int use_tma = (aligned16(g_xyz) && aligned16(g_quaternion) && aligned16(g_scale) &&
                              aligned16(g_opacity_logit) && aligned16(g_rgb_dc) &&
                              (g_sh_rest == nullptr || aligned16(g_sh_rest)))
                                 ? 1
                                 : 0;
-        const auto launcher = lens == GSR_LENS_FISHEYE      ? gsr_pose_launch_fisheye
-                              : lens == GSR_LENS_DISTORTION ? gsr_pose_launch_distortion
-                                                            : gsr_pose_launch_pinhole;
+        const auto launcher = lens == GSR_LENS_FISHEYE      ? GSR_LAUNCH_FISHEYE
+                              : lens == GSR_LENS_DISTORTION ? GSR_LAUNCH_DISTORTION
+                                                            : GSR_POSE_LAUNCH;
         const int rc = launcher(single, mode, C, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
                                 camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact,
                                 scan, g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, use_tma,
                                 lens_consts, partials, st);
         if (rc != GSR_OK) return rc;
     }
+#ifdef GSR_POSE_CAMERA
+    if (values == 20)
+        k_camera_finish<20><<<C, POSE_FINISH_THREADS, 0, st>>>(nblk, 4, partials, g_pose, g_intrinsics, g_lens);
+    else if (values == 24)
+        k_camera_finish<24><<<C, POSE_FINISH_THREADS, 0, st>>>(nblk, 5, partials, g_pose, g_intrinsics, g_lens);
+    else
+        k_camera_finish<16><<<C, POSE_FINISH_THREADS, 0, st>>>(nblk, 0, partials, g_pose, g_intrinsics, g_lens);
+#else
     k_pose_finish<<<C, POSE_FINISH_THREADS, 0, st>>>(nblk, partials, g_pose);
+#endif
     return (int)cudaGetLastError();
 }
 
 extern "C" {
 
-size_t gsr_pose_temp_bytes(int C, int N) {
-    const size_t nblk = (size_t)((N > 0 ? N : 0) + PRE_THREADS - 1) / PRE_THREADS;
-    return align256(sizeof(float) * POSE_VALUES * nblk * (size_t)(C > 0 ? C : 0));
+#ifdef GSR_POSE_CAMERA
+
+size_t gsr_camera_temp_bytes(int lens, int C, int N) { return partial_bytes(camera_values(lens), C, N); }
+
+int gsr_camera_preprocess_backward(int lens, int mode, int N, int n_sh_rest, const float* xyz,
+                                   const float* quaternion, const float* scale, const float* opacity_logit,
+                                   const float* filter3d, const float* camera_T_world, const float* K,
+                                   const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                                   int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan, float* g_xyz,
+                                   float* g_quaternion, float* g_scale, float* g_opacity_logit, float* g_rgb_dc,
+                                   float* g_sh_rest, const float* lens_consts, float* g_pose, float* g_intrinsics,
+                                   float* g_lens, void* temp, size_t temp_bytes, void* stream) {
+    return pose_backward(true, lens, mode, 1, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
+                         camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
+                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose,
+                         g_intrinsics, g_lens, temp, temp_bytes, stream);
 }
+
+int gsr_camera_batch_preprocess_backward(int lens, int mode, int C, int N, int n_sh_rest, const float* xyz,
+                                         const float* quaternion, const float* scale, const float* opacity_logit,
+                                         const float* filter3d, const float* camera_T_world, const float* K,
+                                         const float* camera_centre, const uint8_t* visible, const float* grad_rows,
+                                         int use_rows_uv, const float* grad_uv_compact, const uint64_t* scan,
+                                         float* g_xyz, float* g_quaternion, float* g_scale, float* g_opacity_logit,
+                                         float* g_rgb_dc, float* g_sh_rest, const float* lens_consts, float* g_pose,
+                                         float* g_intrinsics, float* g_lens, void* temp, size_t temp_bytes,
+                                         void* stream) {
+    return pose_backward(false, lens, mode, C, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
+                         camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
+                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose,
+                         g_intrinsics, g_lens, temp, temp_bytes, stream);
+}
+
+#else
+
+size_t gsr_pose_temp_bytes(int C, int N) { return partial_bytes(POSE_VALUES, C, N); }
 
 int gsr_pose_preprocess_backward(int lens, int mode, int N, int n_sh_rest, const float* xyz, const float* quaternion,
                                  const float* scale, const float* opacity_logit, const float* filter3d,
@@ -256,8 +400,8 @@ int gsr_pose_preprocess_backward(int lens, int mode, int N, int n_sh_rest, const
                                  size_t temp_bytes, void* stream) {
     return pose_backward(true, lens, mode, 1, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
                          camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
-                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose, temp,
-                         temp_bytes, stream);
+                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose,
+                         nullptr, nullptr, temp, temp_bytes, stream);
 }
 
 int gsr_pose_batch_preprocess_backward(int lens, int mode, int C, int N, int n_sh_rest, const float* xyz,
@@ -270,9 +414,11 @@ int gsr_pose_batch_preprocess_backward(int lens, int mode, int C, int N, int n_s
                                        void* temp, size_t temp_bytes, void* stream) {
     return pose_backward(false, lens, mode, C, N, n_sh_rest, xyz, quaternion, scale, opacity_logit, filter3d,
                          camera_T_world, K, camera_centre, visible, grad_rows, use_rows_uv, grad_uv_compact, scan,
-                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose, temp,
-                         temp_bytes, stream);
+                         g_xyz, g_quaternion, g_scale, g_opacity_logit, g_rgb_dc, g_sh_rest, lens_consts, g_pose,
+                         nullptr, nullptr, temp, temp_bytes, stream);
 }
+
+#endif  // GSR_POSE_CAMERA
 
 }  // extern "C"
 

@@ -6,8 +6,9 @@
 // 2-D covariance M Sigma M^T (the packed conic gradient gc after the antialiased rho terms), M = J W, and Sigma the
 // (filtered) world covariance.  The camera centre of the SH view direction is held constant, as for xyz.
 //
-// Each thread holds its gaussian's 12 values (T[:3, :] row-major).  After every view the CTA adds them up in a fixed
-// order (a shuffle tree per warp, then the 4 warps in order) and writes one partial per CTA and view: [C, grid, 12].
+// Each thread holds its gaussian's 12 values (T[:3, :] row-major; NV values with the camera gradient).  After every
+// view the CTA adds them up in a fixed order (a shuffle tree per warp, then the 4 warps in order) and writes one partial
+// per CTA and view: [C, grid, NV].
 // k_pose_finish adds the partials of a view in fp64 in a fixed order and rounds once.  The per-gaussian arithmetic is
 // written with explicit rounding intrinsics, so the single-view and the batched kernels give the same bits for the
 // same rows.
@@ -52,20 +53,22 @@ __device__ __forceinline__ void pose_contribution(const float* __restrict__ J, c
     }
 }
 
-// Whole CTA: the fixed-order sum of every thread's 12 values into out[0..11].  Every thread must call it.  The
+// Whole CTA: the fixed-order sum of every thread's NV values into out[0..NV-1].  Every thread must call it.  The
 // shared scratch may be rewritten by the next call only after a CTA barrier (the batched body has one per view).
+template <int NV>
 __device__ __forceinline__ void pose_cta_reduce(const float* __restrict__ acc, float* __restrict__ out) {
-    __shared__ float s_pose[POSE_CTA_THREADS / 32][POSE_VALUES];
+    static_assert(NV <= POSE_CTA_THREADS, "one thread per value adds the warps' sums");
+    __shared__ float s_pose[POSE_CTA_THREADS / 32][NV];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-    for (int k = 0; k < POSE_VALUES; ++k) {
+    for (int k = 0; k < NV; ++k) {
         float v = acc[k];
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) v = __fadd_rn(v, __shfl_down_sync(0xffffffffu, v, off));
         if (lane == 0) s_pose[warp][k] = v;
     }
     __syncthreads();
-    if (threadIdx.x < POSE_VALUES) {
+    if (threadIdx.x < NV) {
         float v = s_pose[0][threadIdx.x];
 #pragma unroll
         for (int w = 1; w < POSE_CTA_THREADS / 32; ++w) v = __fadd_rn(v, s_pose[w][threadIdx.x]);
@@ -75,10 +78,21 @@ __device__ __forceinline__ void pose_cta_reduce(const float* __restrict__ acc, f
 
 }  // namespace gsr
 
-// The hooks (gsr_preprocess.cuh): the bodies take the partials [C, grid, 12] as one more trailing parameter.
+// The hooks (gsr_preprocess.cuh): the bodies take the partials [C, grid, NV] as one more trailing parameter.  With
+// GSR_POSE_CAMERA (the camera-gradient kernels, gsr_calib.cuh) a row is the 12 pose values followed by
+// CAMERA_VALUES - 12 intrinsics and lens values, added by GSR_CAMERA_VIEW.
 #define GSR_POSE_HOOKS
 #define GSR_POSE_PARAM , float* __restrict__ pose_partials
+#ifdef GSR_POSE_CAMERA
+#define GSR_POSE_DECL float gpose[CAMERA_VALUES] = {};
+#define GSR_POSE_VIEW                                   \
+    pose_contribution(J, W, S9, gc, gp, x, y, z, gpose); \
+    GSR_CAMERA_VIEW(px, py, pz, guv, gJ, gpose + POSE_VALUES);
+#define GSR_POSE_REDUCE(view) \
+    pose_cta_reduce<CAMERA_VALUES>(gpose, pose_partials + ((size_t)(view) * gridDim.x + blockIdx.x) * CAMERA_VALUES);
+#else
 #define GSR_POSE_DECL float gpose[POSE_VALUES] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #define GSR_POSE_VIEW pose_contribution(J, W, S9, gc, gp, x, y, z, gpose);
 #define GSR_POSE_REDUCE(view) \
-    pose_cta_reduce(gpose, pose_partials + ((size_t)(view) * gridDim.x + blockIdx.x) * POSE_VALUES);
+    pose_cta_reduce<POSE_VALUES>(gpose, pose_partials + ((size_t)(view) * gridDim.x + blockIdx.x) * POSE_VALUES);
+#endif

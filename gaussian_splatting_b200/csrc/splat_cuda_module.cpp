@@ -17,6 +17,7 @@
 #include "../../include/gsr_fisheye.h"
 #include "../../include/gsr_distortion.h"
 #include "../../include/gsr_pose.h"
+#include "../../include/gsr_calib.h"
 #include "../../include/gsr_bilagrid.h"
 
 namespace {
@@ -453,6 +454,11 @@ static const float* filter3d_ptr(const c10::optional<torch::Tensor>& filter3d, i
 // theta_max}) or OPENCV radial-tangential distortion (libgsr_distortion.so, {k1, k2, p1, p2, k3, r2_max}).
 enum class Lens { Pinhole, Fisheye, Distortion };
 
+// the lens coefficients that get a gradient (k1..k4; k1 k2 p1 p2 k3): the constants without the cull limit
+static int64_t lens_coefficient_count(Lens lens) {
+    return lens == Lens::Fisheye ? GSR_FISHEYE_CONSTS - 1 : lens == Lens::Distortion ? GSR_DISTORTION_CONSTS - 1 : 0;
+}
+
 // the lens constants of C views (fp32 on xyz's device), or NULL for the pinhole
 static const float* lens_ptr(Lens lens, const c10::optional<torch::Tensor>& consts, int64_t C,
                              const torch::Tensor& xyz) {
@@ -796,7 +802,7 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
                                                       c10::optional<torch::Tensor> scan, bool use_slab_uv,
                                                       int64_t mode, c10::optional<torch::Tensor> filter3d,
                                                       Lens lens, c10::optional<torch::Tensor> lc,
-                                                      bool pose = false) {
+                                                      bool pose = false, bool camera = false) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     const int64_t N = xyz.size(0);
     TORCH_CHECK(slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ", GSR_GRAD_ROW_FLOATS,
@@ -847,8 +853,18 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
         F32PTR(camera_T_world), F32PTR(K), camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,   \
         visible.data_ptr<uint8_t>(), slab.data_ptr<float>(), use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr,            \
         F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    torch::Tensor g_pose;
-    if (pose) {
+    torch::Tensor g_pose, g_intr, g_lens;
+    if (camera) {
+        g_pose = torch::empty({4, 4}, opt);
+        g_intr = torch::empty({4}, opt);
+        g_lens = torch::empty({lens_coefficient_count(lens)}, opt);
+        torch::Tensor temp =
+            torch::empty({(int64_t)gsr_camera_temp_bytes((int)lens, 1, (int)N)}, opt.dtype(torch::kUInt8));
+        check_rc(gsr_camera_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), F32PTR(g_intr),
+                                                g_lens.numel() ? F32PTR(g_lens) : nullptr, temp.data_ptr(),
+                                                (size_t)temp.numel(), cur_stream()),
+                 "gsr_camera_preprocess_backward");
+    } else if (pose) {
         g_pose = torch::empty({4, 4}, opt);
         torch::Tensor temp = torch::empty({(int64_t)gsr_pose_temp_bytes(1, (int)N)}, opt.dtype(torch::kUInt8));
         check_rc(gsr_pose_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), temp.data_ptr(),
@@ -865,7 +881,11 @@ static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch:
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
     out.push_back(flat);  // the allocation all the gaussian gradients are views of
-    if (pose) out.push_back(g_pose);  // last: d loss / d camera_T_world [4,4]
+    if (pose || camera) out.push_back(g_pose);  // d loss / d camera_T_world [4,4]
+    if (camera) {  // last: d loss / d (fx, fy, cx, cy) [4] and d loss / d lens coefficients [n]
+        out.push_back(g_intr);
+        out.push_back(g_lens);
+    }
     return out;
 }
 
@@ -1080,7 +1100,8 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
                                                  c10::optional<torch::Tensor> grad_uv_compact,
                                                  c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
                                                  c10::optional<torch::Tensor> filter3d, Lens lens,
-                                                 c10::optional<torch::Tensor> lc, bool pose = false) {
+                                                 c10::optional<torch::Tensor> lc, bool pose = false,
+                                                 bool camera = false) {
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(visible);
@@ -1138,8 +1159,18 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
         F32PTR(camera_T_world), F32PTR(K), centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab),                    \
         use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o),           \
         F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    torch::Tensor g_pose;
-    if (pose) {
+    torch::Tensor g_pose, g_intr, g_lens;
+    if (camera) {
+        g_pose = torch::empty({C, 4, 4}, opt);
+        g_intr = torch::empty({C, 4}, opt);
+        g_lens = torch::empty({C, lens_coefficient_count(lens)}, opt);
+        torch::Tensor temp =
+            torch::empty({(int64_t)gsr_camera_temp_bytes((int)lens, (int)C, (int)N)}, opt.dtype(torch::kUInt8));
+        check_rc(gsr_camera_batch_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), F32PTR(g_intr),
+                                                      g_lens.numel() ? F32PTR(g_lens) : nullptr, temp.data_ptr(),
+                                                      (size_t)temp.numel(), cur_stream()),
+                 "gsr_camera_batch_preprocess_backward");
+    } else if (pose) {
         g_pose = torch::empty({C, 4, 4}, opt);
         torch::Tensor temp = torch::empty({(int64_t)gsr_pose_temp_bytes((int)C, (int)N)}, opt.dtype(torch::kUInt8));
         check_rc(gsr_pose_batch_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), temp.data_ptr(),
@@ -1157,7 +1188,11 @@ static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tens
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
     out.push_back(flat);
-    if (pose) out.push_back(g_pose);  // last: d loss / d camera_T_world [C,4,4]
+    if (pose || camera) out.push_back(g_pose);  // d loss / d camera_T_world [C,4,4]
+    if (camera) {  // last: [C,4] intrinsics and [C,n] lens-coefficient gradients
+        out.push_back(g_intr);
+        out.push_back(g_lens);
+    }
     return out;
 }
 
@@ -1273,6 +1308,31 @@ std::vector<torch::Tensor> batch_pose_preprocess_backward(
     return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
                           visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
                           lens_consts, true);
+}
+
+// The per-gaussian backward with the pose, intrinsics and lens-coefficient gradients (libgsr_calib.so, gsr_camera_*):
+// the arguments of pose_preprocess_backward / batch_pose_preprocess_backward.  Returns their outputs followed by
+// d loss / d (fx, fy, cx, cy) [4] / [C,4] and d loss / d lens coefficients [n] / [C,n] (n = 0 for the pinhole).
+std::vector<torch::Tensor> camera_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
+    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
+                               lens_consts, false, true);
+}
+
+std::vector<torch::Tensor> batch_camera_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
+    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
+                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
+                          lens_consts, false, true);
 }
 
 // gsr_distortion_r2_max of 5 coefficients k1 k2 p1 p2 k3 (host floats)
@@ -1839,6 +1899,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("batch_pose_preprocess_backward", &batch_pose_preprocess_backward,
           "batch_preprocess_backward plus d loss / d camera_T_world [C,4,4], any lens "
           "(gsr_pose_batch_preprocess_backward)");
+    m.def("camera_preprocess_backward", &camera_preprocess_backward,
+          "pose_preprocess_backward plus d loss / d (fx, fy, cx, cy) [4] and d loss / d lens coefficients [n], any "
+          "lens (gsr_camera_preprocess_backward)");
+    m.def("batch_camera_preprocess_backward", &batch_camera_preprocess_backward,
+          "batch_pose_preprocess_backward plus [C,4] intrinsics and [C,n] lens-coefficient gradients, any lens "
+          "(gsr_camera_batch_preprocess_backward)");
     m.def("distortion_r2_max", &distortion_r2_max,
           "the radial fold limit s = r^2 of 5 coefficients k1 k2 p1 p2 k3 (gsr_distortion_r2_max)");
     m.def("filter3d", &filter3d, "Mip-Splatting's 3-D filter size per gaussian from the training cameras (gsr_filter3d)",

@@ -401,9 +401,47 @@ def _pose_lens(lens):
     return (1 if lens[0] == "fisheye" else 2), lens[1]
 
 
+def _lens_input(fisheye, distortion):
+    """The lens coefficient tensor that takes a gradient: a CPU tensor that requires grad, else None (a sequence of
+    numbers and a tensor that does not require grad stay host constants)."""
+    k = fisheye if fisheye is not None else distortion
+    return k if torch.is_tensor(k) and k.requires_grad else None
+
+
+def _intrinsics_grad(g):
+    """d loss / d K [..., 3, 3] from the kernels' [..., 4] (fx, fy, cx, cy); every other entry (the skew, the last
+    row) is exactly 0: the projection never reads it."""
+    out = g.new_zeros(*g.shape[:-1], 9)
+    out[..., 0], out[..., 4], out[..., 2], out[..., 5] = g[..., 0], g[..., 1], g[..., 2], g[..., 3]
+    return out.view(*g.shape[:-1], 3, 3)
+
+
+def _lens_grad(g, k):
+    """The lens-coefficient gradient [n] / [C,n] on the device, brought to the host in k's shape and dtype: one blocking
+    device->host copy (the coefficients are host constants, DESIGN.md 3.23).  A [C,n] gradient for a shared [n] k is
+    summed over the views in fp64."""
+    g = g.to("cpu").to(torch.float64)
+    if g.dim() == 2 and k.dim() == 1:
+        g = g.sum(0)
+    return g.to(k.dtype)
+
+
+def _camera_backward(ctx, native_fn, args, lens, k_input):
+    """The backward with the camera gradients: (gaussian grads..., g_pose or None, g_K or None, g_k or None).  The
+    intrinsics or the lens coefficients require grad: the camera-gradient kernels (libgsr_calib.so); only the pose:
+    the pose kernels."""
+    *grads, g_pose, g_intr, g_lens = native_fn(*args, *_pose_lens(lens))
+    g_pose = g_pose if ctx.needs_input_grad[6] else None
+    g_K = _intrinsics_grad(g_intr) if ctx.needs_input_grad[7] else None
+    g_k = _lens_grad(g_lens, k_input) if k_input is not None and ctx.needs_input_grad[10] else None
+    return grads, g_pose, g_K, g_k
+
+
 class _ProjectGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg):
+    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg, lens_k=None):
+        # lens_k: the lens coefficient tensor when it requires grad (an input for its gradient only: the forward reads
+        # the constants uploaded to state.lens)
         ext = native()
         # torch.matmul takes another path (other rounding) for an operand that requires grad: the forward's bits must
         # not depend on whether the pose does
@@ -440,8 +478,8 @@ class _ProjectGaussians(torch.autograd.Function):
                 lens, consts = state.lens
                 fwd = ext.fisheye_preprocess_forward if lens == "fisheye" else ext.distortion_preprocess_forward
                 records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
-        # a backward pass can follow (the pose counts: a pose-only refinement needs the masks too)
-        record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:7])
+        # a backward pass can follow (the camera counts: a pose- or intrinsics-only refinement needs the masks too)
+        record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or ctx.needs_input_grad[10])
         background = state.background
 
         def counts(total):
@@ -521,6 +559,7 @@ class _ProjectGaussians(torch.autograd.Function):
         carrier = torch.empty(12 * xyz.shape[0], dtype=xyz.dtype, device=xyz.device)
         ctx.state = state
         ctx.has_sh = sh is not None
+        ctx.lens_k = lens_k
         ctx.save_for_backward(xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre)
         return uv, carrier
 
@@ -543,8 +582,11 @@ class _ProjectGaussians(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            g_pose = None
-            if ctx.needs_input_grad[6]:
+            g_pose = g_K = g_k = None
+            if ctx.needs_input_grad[7] or ctx.needs_input_grad[10]:
+                grads, g_pose, g_K, g_k = _camera_backward(ctx, native().camera_preprocess_backward, args, st.lens,
+                                                           ctx.lens_k)
+            elif ctx.needs_input_grad[6]:
                 # the same kernels' arithmetic plus the pose reduction (libgsr_pose.so)
                 *grads, g_pose = native().pose_preprocess_backward(*args, *_pose_lens(st.lens))
             elif st.lens is None:
@@ -557,7 +599,7 @@ class _ProjectGaussians(torch.autograd.Function):
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
-        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, None, None, None
+        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, g_K, None, None, g_k
 
 
 class _CompositeTiles(torch.autograd.Function):
@@ -697,8 +739,8 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     k = 0 is the equidistant fisheye, not the pinhole.  The 2-D covariance uses the Jacobian of that projection at the
     mean (EWA), and a gaussian at theta >= fisheye_theta_max(k), where the model folds back, is culled on top of the
     near / far / padding rules.  Depth keys, the depth map and the SH view direction keep camera-frame z and the
-    position; uv and uv.grad are the fisheye pixel coordinates and their gradient; K and k get no gradient
-    (DESIGN.md 3.19).  The coefficients are constants of the camera, uploaded once per camera without synchronising
+    position; uv and uv.grad are the fisheye pixel coordinates and their gradient (DESIGN.md 3.19); for K and k
+    requiring grad see camera.K below.  The coefficients are constants of the camera, uploaded once per camera without synchronising
     with the device.  Combines with every other option.  None (the default) is the pinhole.  A CUDA tensor, a wrong
     shape or non-finite coefficients raise ValueError; fp32 and precomputed SH colours only.
 
@@ -720,7 +762,16 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     direction is held constant, as it is for xyz (exact with SH degree 0).  Reduced natively in a fixed order, so the
     same render-stage rows give the same bits (DESIGN.md 3.21).  Everything else is unchanged.  A pose that does not
     require grad runs exactly the kernels without it.  rasterize_unfused (and fp64 / per-pixel SH) gives the pose only
-    what autograd gets through its torch transform of the means."""
+    what autograd gets through its torch transform of the means.
+
+    camera.K: when it requires grad (e.g. calib.IntrinsicsDelta's output), the backward also gives d loss / d K [3,3]
+    for self-calibration: dL/dfx = sum_i (g_u a_d + sum_j gJ[0,j] J[0,j] / fx), dL/dcx = sum_i g_u (fy, cy with row 1),
+    u = fx a_d + cx the lens's projection, g_u the complete gradient on u, gJ the gradient on the Jacobian; every other
+    entry (the skew, the last row) is exactly 0.  Lens coefficients: a CPU tensor that requires grad passed as fisheye=
+    or distortion= gets d loss / d k in its shape and dtype, through one blocking device -> host copy of n floats at the
+    end of the backward (only then; a sequence of numbers gets none).  Cull limits get no gradient.  Every lens and
+    option combine with it; outputs, gaussian gradients and the pose gradient are bit-identical to a run without it
+    (DESIGN.md 3.23)."""
     lens = _lens_arg(fisheye, distortion)
     if lens is not None:
         if gaussians.xyz.dtype != torch.float32:
@@ -804,7 +855,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
         gaussians.xyz.contiguous(), gaussians.quaternion.contiguous(), gaussians.scale.contiguous(),
         gaussians.opacity.contiguous(), gaussians.rgb.contiguous(),
         None if gaussians.sh is None else gaussians.sh.contiguous(),
-        camera_T_world.contiguous(), camera.K.contiguous(), state, cfg)
+        camera_T_world.contiguous(), camera.K.contiguous(), state, cfg, _lens_input(fisheye, distortion))
     state.uv_ref = weakref.ref(uv)
     culling_mask = state.visible == 0
     outs = _CompositeTiles.apply(uv, carrier, state.background, state, features)
@@ -892,7 +943,7 @@ class _BatchState:
 
 class _ProjectBatch(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg):
+    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg, lens_k=None):
         camera_T_world = camera_T_world.detach()  # as in _ProjectGaussians.forward
         ext = native()
         H, W, near, far, pad, mh = cfg
@@ -921,7 +972,7 @@ class _ProjectBatch(torch.autograd.Function):
                 fwd = (ext.batch_fisheye_preprocess_forward if lens == "fisheye"
                        else ext.batch_distortion_preprocess_forward)
                 records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
-        record_masks = USE_CONTRIBUTION_MASKS and any(ctx.needs_input_grad[:7])
+        record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or ctx.needs_input_grad[10])
         background = state.background
         depth_mode = bool(state.mode & ext.MODE_DEPTH_ALPHA)
 
@@ -1004,6 +1055,7 @@ class _ProjectBatch(torch.autograd.Function):
         carrier = torch.empty(C * 12 * N, dtype=xyz.dtype, device=xyz.device)
         ctx.state = state
         ctx.has_sh = sh is not None
+        ctx.lens_k = lens_k
         ctx.save_for_backward(xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre)
         return uv_all, carrier
 
@@ -1023,8 +1075,11 @@ class _ProjectBatch(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            g_pose = None
-            if ctx.needs_input_grad[6]:
+            g_pose = g_K = g_k = None
+            if ctx.needs_input_grad[7] or ctx.needs_input_grad[10]:
+                grads, g_pose, g_K, g_k = _camera_backward(ctx, native().batch_camera_preprocess_backward, args,
+                                                           st.lens, ctx.lens_k)
+            elif ctx.needs_input_grad[6]:
                 *grads, g_pose = native().batch_pose_preprocess_backward(*args, *_pose_lens(st.lens))
             elif st.lens is None:
                 grads = native().batch_preprocess_backward(*args)
@@ -1037,7 +1092,7 @@ class _ProjectBatch(torch.autograd.Function):
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]
-        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, None, None, None
+        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, g_K, None, None, g_k
 
 
 class _CompositeBatch(torch.autograd.Function):
@@ -1152,7 +1207,11 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
 
     fisheye: OPENCV_FISHEYE cameras as in rasterize(), k [4] shared by every view or [C,4] one row per view (host
     values: a sequence or a CPU tensor); view c is then bit-identical to rasterize(..., fisheye=k_c).  distortion:
-    radial-tangential cameras likewise, k [5] or [C,5] (rasterize(..., distortion=k_c))."""
+    radial-tangential cameras likewise, k [5] or [C,5] (rasterize(..., distortion=k_c)).
+
+    A camera.K that requires grad gets d loss / d K as rasterize() defines it, [C,3,3] per view (a shared [3,3]: the sum
+    over the views), and a CPU coefficient tensor that requires grad its gradient in its shape ([n]: summed over the
+    views); view c's values are bit-identical to the single-view kernel's on view c's rows (DESIGN.md 3.23)."""
     C = _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, background_rgb, filter3d, weight_stats,
                           features)
     lens = _lens_arg(fisheye, distortion, C)
@@ -1171,7 +1230,7 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
         gaussians.xyz.contiguous(), gaussians.quaternion.contiguous(), gaussians.scale.contiguous(),
         gaussians.opacity.contiguous(), gaussians.rgb.contiguous(),
         None if gaussians.sh is None else gaussians.sh.contiguous(),
-        camera_T_world.contiguous(), K.contiguous(), state, cfg)
+        camera_T_world.contiguous(), K.contiguous(), state, cfg, _lens_input(fisheye, distortion))
     uvs = torch.split(uv_all, [v.M for v in state.views])
     state.uv_refs = [weakref.ref(u) for u in uvs]
     culling_mask = state.visible == 0
