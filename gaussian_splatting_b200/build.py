@@ -5,7 +5,8 @@
   libgsr_features.so        the feature-channel tile kernels (include/gsr_features.h), same flags
   libgsr_batch.so           the multi-view per-gaussian kernels of rasterize_batch (include/gsr_batch.h), same flags
   libgsr_fisheye.so         the per-gaussian kernels for fisheye cameras (include/gsr_fisheye.h), same flags
-  libgsr_distortion.so      the per-gaussian kernels for radial-tangential lens distortion (include/gsr_distortion.h)
+  libgsr_distortion.so      the per-gaussian kernels for radial-tangential lens distortion (include/gsr_distortion.h);
+                            both built from gsr_lens.cu, once per lens
   libgsr_pose.so            the per-gaussian backward with the camera pose gradient, every lens (include/gsr_pose.h)
   libgsr_calib.so           the same sources compiled with the pose, intrinsics and lens-coefficient gradients
                             (include/gsr_calib.h)
@@ -13,7 +14,8 @@
                             (include/gsr_bilagrid.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all ten; `build(force=False)` is incremental.
+`python -m gaussian_splatting_b200.build` builds all ten (the CUDA libraries from the LIBS table);
+`build(force=False)` is incremental.
 """
 from __future__ import annotations
 
@@ -31,14 +33,6 @@ CSRC = PKG / "csrc"
 OBJ = PKG / "_build"
 EXT_DIR = PKG / "_ext"
 LIB = PKG / "libgsr_b200.so"
-SELECTIVE_LIB = PKG / "libgsr_selective_adam.so"
-FEATURES_LIB = PKG / "libgsr_features.so"
-BATCH_LIB = PKG / "libgsr_batch.so"
-FISHEYE_LIB = PKG / "libgsr_fisheye.so"
-DISTORTION_LIB = PKG / "libgsr_distortion.so"
-POSE_LIB = PKG / "libgsr_pose.so"
-CALIB_LIB = PKG / "libgsr_calib.so"
-BILAGRID_LIB = PKG / "libgsr_bilagrid.so"
 
 CU_SOURCES = [
     "gsr_pergaussian.cu",
@@ -62,40 +56,42 @@ HEADERS = [
     CSRC / "gsr_preprocess.cuh",
     ROOT / "include" / "gsr_b200.h",
 ]
-# A library of its own, so that libgsr_b200.so keeps exactly its kernels (and their SASS).
-SELECTIVE_SOURCES = ["gsr_adam_selective.cu"]
-SELECTIVE_HEADERS = [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h",
-                     ROOT / "include" / "gsr_selective_adam.h"]
-FEATURES_SOURCES = ["gsr_features.cu"]
-FEATURES_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [ROOT / "include" / "gsr_b200.h",
-                                                                  ROOT / "include" / "gsr_features.h"]
-BATCH_SOURCES = ["gsr_batch.cu"]
-BATCH_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [ROOT / "include" / "gsr_b200.h",
-                                                               ROOT / "include" / "gsr_batch.h"]
-FISHEYE_SOURCES = ["gsr_fisheye.cu"]
-FISHEYE_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_fisheye.cuh",
-                                                                 CSRC / "gsr_poly_roots.h",
-                                                                 ROOT / "include" / "gsr_b200.h",
-                                                                 ROOT / "include" / "gsr_fisheye.h"]
-DISTORTION_SOURCES = ["gsr_distortion.cu"]
-DISTORTION_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_distortion.cuh",
-                                                                    CSRC / "gsr_poly_roots.h",
-                                                                    ROOT / "include" / "gsr_b200.h",
-                                                                    ROOT / "include" / "gsr_distortion.h"]
-# gsr_pose.cu once per camera model (GSR_POSE_LENS: 0 pinhole, 1 fisheye, 2 distortion): (source, object, -D flags);
-# libgsr_calib.so compiles the same three with GSR_POSE_CAMERA (the camera-gradient kernels)
-POSE_SOURCES = [("gsr_pose.cu", f"gsr_pose_{i}", [f"-DGSR_POSE_LENS={i}"]) for i in range(3)]
-CALIB_SOURCES = [("gsr_pose.cu", f"gsr_camera_{i}", [f"-DGSR_POSE_LENS={i}", "-DGSR_POSE_CAMERA"]) for i in range(3)]
-POSE_HEADERS = [h for h in HEADERS if h.suffix == ".cuh"] + [CSRC / "gsr_pose.cuh", CSRC / "gsr_calib.cuh",
-                                                             CSRC / "gsr_fisheye.cuh",
-                                                             CSRC / "gsr_distortion.cuh",
-                                                             ROOT / "include" / "gsr_b200.h",
-                                                             ROOT / "include" / "gsr_fisheye.h",
-                                                             ROOT / "include" / "gsr_distortion.h",
-                                                             ROOT / "include" / "gsr_pose.h",
-                                                             ROOT / "include" / "gsr_calib.h"]
-BILAGRID_SOURCES = ["gsr_bilagrid.cu"]
-BILAGRID_HEADERS = [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_bilagrid.h"]
+CUH = [h for h in HEADERS if h.suffix == ".cuh"]
+# The sources of a library are file names, or (file name, object stem, extra nvcc flags) for a file compiled more
+# than once.  gsr_lens.cu is compiled once per lens model (GSR_LENS: 1 fisheye, 2 distortion), gsr_pose.cu once per
+# camera model (GSR_POSE_LENS: 0 pinhole, 1 fisheye, 2 distortion), and again with GSR_POSE_CAMERA for libgsr_calib.so
+# (the camera-gradient kernels).
+LENS_HEADERS = CUH + [CSRC / "gsr_fisheye.cuh", CSRC / "gsr_distortion.cuh", CSRC / "gsr_poly_roots.h",
+                      ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_fisheye.h",
+                      ROOT / "include" / "gsr_distortion.h"]
+POSE_HEADERS = CUH + [CSRC / "gsr_pose.cuh", CSRC / "gsr_calib.cuh", CSRC / "gsr_fisheye.cuh",
+                      CSRC / "gsr_distortion.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_fisheye.h",
+                      ROOT / "include" / "gsr_distortion.h", ROOT / "include" / "gsr_pose.h",
+                      ROOT / "include" / "gsr_calib.h"]
+# (library, sources, headers, stamp): each library apart, so that every library keeps exactly its kernels (and their
+# SASS) when another one changes
+LIBS = [
+    (LIB, CU_SOURCES, HEADERS, "lib.sha256"),
+    (PKG / "libgsr_selective_adam.so", ["gsr_adam_selective.cu"],
+     [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_selective_adam.h"],
+     "selective_lib.sha256"),
+    (PKG / "libgsr_features.so", ["gsr_features.cu"],
+     CUH + [ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_features.h"], "features_lib.sha256"),
+    (PKG / "libgsr_batch.so", ["gsr_batch.cu"],
+     CUH + [ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_batch.h"], "batch_lib.sha256"),
+    (PKG / "libgsr_fisheye.so", [("gsr_lens.cu", "gsr_fisheye", ["-DGSR_LENS=1"])], LENS_HEADERS,
+     "fisheye_lib.sha256"),
+    (PKG / "libgsr_distortion.so", [("gsr_lens.cu", "gsr_distortion", ["-DGSR_LENS=2"])], LENS_HEADERS,
+     "distortion_lib.sha256"),
+    (PKG / "libgsr_pose.so", [("gsr_pose.cu", f"gsr_pose_{i}", [f"-DGSR_POSE_LENS={i}"]) for i in range(3)],
+     POSE_HEADERS, "pose_lib.sha256"),
+    (PKG / "libgsr_calib.so",
+     [("gsr_pose.cu", f"gsr_camera_{i}", [f"-DGSR_POSE_LENS={i}", "-DGSR_POSE_CAMERA"]) for i in range(3)],
+     POSE_HEADERS, "calib_lib.sha256"),
+    (PKG / "libgsr_bilagrid.so", ["gsr_bilagrid.cu"],
+     [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_bilagrid.h"],
+     "bilagrid_lib.sha256"),
+]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -159,44 +155,6 @@ def _build_cuda_lib(lib: Path, sources, headers, stamp_name: str, force: bool, v
     return lib
 
 
-def build_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(LIB, CU_SOURCES, HEADERS, "lib.sha256", force, verbose)
-
-
-def build_selective_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(SELECTIVE_LIB, SELECTIVE_SOURCES, SELECTIVE_HEADERS, "selective_lib.sha256", force,
-                           verbose)
-
-
-def build_features_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(FEATURES_LIB, FEATURES_SOURCES, FEATURES_HEADERS, "features_lib.sha256", force, verbose)
-
-
-def build_batch_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(BATCH_LIB, BATCH_SOURCES, BATCH_HEADERS, "batch_lib.sha256", force, verbose)
-
-
-def build_fisheye_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(FISHEYE_LIB, FISHEYE_SOURCES, FISHEYE_HEADERS, "fisheye_lib.sha256", force, verbose)
-
-
-def build_distortion_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(DISTORTION_LIB, DISTORTION_SOURCES, DISTORTION_HEADERS, "distortion_lib.sha256", force,
-                           verbose)
-
-
-def build_pose_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(POSE_LIB, POSE_SOURCES, POSE_HEADERS, "pose_lib.sha256", force, verbose)
-
-
-def build_calib_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(CALIB_LIB, CALIB_SOURCES, POSE_HEADERS, "calib_lib.sha256", force, verbose)
-
-
-def build_bilagrid_lib(force: bool = False, verbose: bool = False) -> Path:
-    return _build_cuda_lib(BILAGRID_LIB, BILAGRID_SOURCES, BILAGRID_HEADERS, "bilagrid_lib.sha256", force, verbose)
-
-
 def build_ext(force: bool = False) -> Path:
     import torch  # noqa: F401  (needed for include/library paths)
     from torch.utils import cpp_extension as ce
@@ -242,17 +200,10 @@ def build_render_variant(out_dir, flags) -> Path:
 
 
 def build(force: bool = False, verbose: bool = False):
-    lib = build_lib(force=force, verbose=verbose)
-    build_selective_lib(force=force, verbose=verbose)
-    build_features_lib(force=force, verbose=verbose)
-    build_batch_lib(force=force, verbose=verbose)
-    build_fisheye_lib(force=force, verbose=verbose)
-    build_distortion_lib(force=force, verbose=verbose)
-    build_pose_lib(force=force, verbose=verbose)
-    build_calib_lib(force=force, verbose=verbose)
-    build_bilagrid_lib(force=force, verbose=verbose)
+    for lib, sources, headers, stamp in LIBS:
+        _build_cuda_lib(lib, sources, headers, stamp, force, verbose)
     ext = build_ext(force=force)
-    return lib, ext
+    return LIB, ext
 
 
 if __name__ == "__main__":

@@ -108,7 +108,7 @@ __device__ __forceinline__ void distortion_project_bwd(const float* __restrict__
 }  // namespace gsr
 
 // The camera-model hooks of gsr_preprocess.cuh for this lens, for a translation unit that defines GSR_DISTORTION_HOOKS
-// before including this header and then includes gsr_preprocess.cuh (gsr_distortion.cu, gsr_pose.cu).  The lens
+// before including this header and then includes gsr_preprocess.cuh (gsr_lens.cu, gsr_pose.cu).  The lens
 // constants of view `view` are read into shared memory next to the view constants.
 #ifdef GSR_DISTORTION_HOOKS
 #define GSR_PROJECTION_HOOKS

@@ -136,7 +136,7 @@ __device__ __forceinline__ void fisheye_project_bwd(const float* __restrict__ J,
 }  // namespace gsr
 
 // The camera-model hooks of gsr_preprocess.cuh for this lens, for a translation unit that defines GSR_FISHEYE_HOOKS
-// before including this header and then includes gsr_preprocess.cuh (gsr_fisheye.cu, gsr_pose.cu).  The lens
+// before including this header and then includes gsr_preprocess.cuh (gsr_lens.cu, gsr_pose.cu).  The lens
 // constants of view `view` are read into shared memory next to the view constants.
 #ifdef GSR_FISHEYE_HOOKS
 #define GSR_PROJECTION_HOOKS

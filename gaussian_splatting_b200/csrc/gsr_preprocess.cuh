@@ -1,6 +1,6 @@
 // gsr_preprocess.cuh — the per-Gaussian stages of the fused path and the view constants they read, shared by the
 // single-view kernels (gsr_preprocess.cu, libgsr_b200.so), the multi-view kernels (gsr_batch.cu, libgsr_batch.so)
-// the lens kernels (gsr_fisheye.cu, gsr_distortion.cu) and the pose-gradient kernels (gsr_pose.cu).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian;
+// the lens kernels (gsr_lens.cu) and the pose-gradient kernels (gsr_pose.cu).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian;
 // the single-view kernels store its result, the batched kernels add it up over the views.  The camera model enters
 // only through the GSR_PROJECT / GSR_JACOBIAN hooks below.
 #pragma once

@@ -447,64 +447,90 @@ static const float* filter3d_ptr(const c10::optional<torch::Tensor>& filter3d, i
     return f.data_ptr<float>();
 }
 
-// returns [records [N,12], depth_key [N] i32-viewed u32, visible [N] u8, scan [N] i64-viewed u64] and, with_tiles,
-// also [tile_mask [N] i64-viewed u64, tile_win [N] i32-viewed u32].  mode: GSR_MODE_* bits
-// The camera model of the per-gaussian stages: the pinhole (libgsr_b200.so, libgsr_batch.so) or a lens whose
-// per-view constants the lens library's entry points read: OPENCV_FISHEYE (libgsr_fisheye.so, {k1, k2, k3, k4,
-// theta_max}) or OPENCV radial-tangential distortion (libgsr_distortion.so, {k1, k2, p1, p2, k3, r2_max}).
-enum class Lens { Pinhole, Fisheye, Distortion };
-
-// the lens coefficients that get a gradient (k1..k4; k1 k2 p1 p2 k3): the constants without the cull limit
-static int64_t lens_coefficient_count(Lens lens) {
-    return lens == Lens::Fisheye ? GSR_FISHEYE_CONSTS - 1 : lens == Lens::Distortion ? GSR_DISTORTION_CONSTS - 1 : 0;
+// The camera model of the per-gaussian stages, a GSR_LENS_* value (gsr_pose.h): the pinhole (libgsr_b200.so,
+// libgsr_batch.so) or a lens whose per-view constants the lens library's entry points read: OPENCV_FISHEYE
+// (libgsr_fisheye.so, {k1, k2, k3, k4, theta_max}) or OPENCV radial-tangential distortion (libgsr_distortion.so,
+// {k1, k2, p1, p2, k3, r2_max}).  Returns the lens's constants per view (0 for the pinhole); the coefficients that
+// get a gradient are all of them but the last, the cull limit.
+static int64_t lens_consts_per_view(int64_t lens) {
+    TORCH_CHECK(lens == GSR_LENS_PINHOLE || lens == GSR_LENS_FISHEYE || lens == GSR_LENS_DISTORTION,
+                "lens must be 0 (pinhole), 1 (fisheye) or 2 (distortion)");
+    return lens == GSR_LENS_FISHEYE ? GSR_FISHEYE_CONSTS : lens == GSR_LENS_DISTORTION ? GSR_DISTORTION_CONSTS : 0;
 }
 
 // the lens constants of C views (fp32 on xyz's device), or NULL for the pinhole
-static const float* lens_ptr(Lens lens, const c10::optional<torch::Tensor>& consts, int64_t C,
+static const float* lens_ptr(int64_t lens, const c10::optional<torch::Tensor>& consts, int64_t C,
                              const torch::Tensor& xyz) {
-    if (lens == Lens::Pinhole) return nullptr;
+    const int64_t per_view = lens_consts_per_view(lens);
+    if (per_view == 0) {
+        TORCH_CHECK(!consts.has_value(), "the pinhole takes no lens constants");
+        return nullptr;
+    }
     TORCH_CHECK(consts.has_value(), "a lens needs its constants");
     const torch::Tensor& f = *consts;
-    const int64_t per_view = lens == Lens::Fisheye ? GSR_FISHEYE_CONSTS : GSR_DISTORTION_CONSTS;
-    const char* name = lens == Lens::Fisheye ? "fisheye" : "distortion";
+    const char* name = lens == GSR_LENS_FISHEYE ? "fisheye" : "distortion";
     CHECK_VALID_INPUT(f); CHECK_FLOAT_TENSOR(f);
     TORCH_CHECK(f.numel() == C * per_view, name, " constants must hold ", per_view, " floats per view");
     TORCH_CHECK(f.device() == xyz.device(), name, " constants must be on the gaussians' device");
     return f.data_ptr<float>();
 }
 
-// lens: the camera model; lc: its constants (gsr_fisheye_ / gsr_distortion_preprocess_forward), none for the pinhole
+// the number of views: 1 for a single view (camera_T_world [4,4], K [3,3]), else C (camera_T_world [C,4,4], K [C,3,3])
+static int64_t check_views(bool batched, const torch::Tensor& camera_T_world, const torch::Tensor& K) {
+    CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
+    CHECK_FLOAT_TENSOR(camera_T_world); CHECK_FLOAT_TENSOR(K);
+    if (!batched) {
+        TORCH_CHECK(camera_T_world.numel() == 16 && K.numel() == 9, "camera_T_world must be 4x4 and K 3x3");
+        return 1;
+    }
+    const int64_t C = camera_T_world.size(0);
+    TORCH_CHECK(camera_T_world.dim() == 3 && C >= 1 && camera_T_world.size(1) == 4 && camera_T_world.size(2) == 4,
+                "camera_T_world must have shape Cx4x4, C >= 1");
+    TORCH_CHECK(K.dim() == 3 && K.size(0) == C && K.size(1) == 3 && K.size(2) == 3, "K must have shape Cx3x3");
+    return C;
+}
+
+// The per-gaussian forward (gsr_preprocess_forward, or the lens's: lens a GSR_LENS_* value, lc its constants [C, n+1]).
+// One view (batched false): returns [records [N,12], depth_key [N] i32-viewed u32, visible [N] u8, scan [N]
+// i64-viewed u64] and, with_tiles, also [tile_mask [N] i64-viewed u64, tile_win [N] i32-viewed u32].  C views
+// (batched, camera_T_world [C,4,4], K [C,3,3]): the single-view forward of every view into the same outputs with a
+// leading view dimension, each view's own packed inclusive scan; xyz_camera_frame [C,R,3] holds the camera-frame
+// positions of the LAST R gaussians of every view, camera_centre [C,3].  mode: GSR_MODE_* bits.
 static std::vector<torch::Tensor> preprocess_forward(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
+    bool batched, torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion,
+    torch::Tensor scale, torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, Lens lens, c10::optional<torch::Tensor> lc) {
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, int64_t lens,
+    c10::optional<torch::Tensor> lc) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
-    CHECK_VALID_INPUT(rgb_dc); CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
+    CHECK_VALID_INPUT(rgb_dc);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
-    CHECK_FLOAT_TENSOR(opacity_logit); CHECK_FLOAT_TENSOR(rgb_dc); CHECK_FLOAT_TENSOR(camera_T_world);
-    CHECK_FLOAT_TENSOR(K);
+    CHECK_FLOAT_TENSOR(opacity_logit); CHECK_FLOAT_TENSOR(rgb_dc);
+    const int64_t C = check_views(batched, camera_T_world, K);
     const int N = xyz.size(0);
     TORCH_CHECK(xyz.dim() == 2 && xyz.size(1) == 3, "xyz must have shape Nx3");
     TORCH_CHECK(quaternion.size(0) == N && quaternion.size(1) == 4, "quaternion must have shape Nx4");
     TORCH_CHECK(scale.size(0) == N && scale.size(1) == 3, "scale must have shape Nx3");
     TORCH_CHECK(opacity_logit.numel() == N, "opacity must have shape Nx1");
     TORCH_CHECK(rgb_dc.size(0) == N && rgb_dc.size(1) == 3, "rgb must have shape Nx3");
-    TORCH_CHECK(camera_T_world.numel() == 16 && K.numel() == 9, "camera_T_world must be 4x4 and K 3x3");
     const float* cam_ptr = nullptr;
-    int cam_first = 0;
-    if (xyz_camera_frame.has_value()) {  // positions of the LAST xyz_camera_frame.size(0) gaussians
+    int64_t R = 0;
+    if (xyz_camera_frame.has_value()) {  // positions of the LAST R gaussians
         const torch::Tensor& pc = *xyz_camera_frame;
         CHECK_VALID_INPUT(pc); CHECK_FLOAT_TENSOR(pc);
-        TORCH_CHECK(pc.dim() == 2 && pc.size(0) <= N && pc.size(1) == 3, "xyz_camera_frame must have shape Rx3, R <= N");
+        TORCH_CHECK(pc.dim() == (batched ? 3 : 2) && (!batched || pc.size(0) == C) && pc.size(-2) <= N &&
+                        pc.size(-1) == 3,
+                    batched ? "xyz_camera_frame must have shape CxRx3, R <= N"
+                            : "xyz_camera_frame must have shape Rx3, R <= N");
         cam_ptr = pc.data_ptr<float>();
-        cam_first = N - (int)pc.size(0);
+        R = pc.size(-2);
     }
     const float* centre_ptr = nullptr;
     if (camera_centre.has_value()) {
         CHECK_VALID_INPUT((*camera_centre)); CHECK_FLOAT_TENSOR((*camera_centre));
-        TORCH_CHECK(camera_centre->numel() == 3, "camera_centre must have 3 elements");
+        TORCH_CHECK(camera_centre->numel() == 3 * C,
+                    batched ? "camera_centre must have shape Cx3" : "camera_centre must have 3 elements");
         centre_ptr = camera_centre->data_ptr<float>();
     }
     int n_rest = 0;
@@ -517,33 +543,47 @@ static std::vector<torch::Tensor> preprocess_forward(
         TORCH_CHECK(n_rest == 3 || n_rest == 8 || n_rest == 15, "sh must hold 3, 8 or 15 coefficients per channel");
         sh_ptr = sh.data_ptr<float>();
     }
+    const float* f3d = filter3d_ptr(filter3d, N);
+    const float* lens_consts = lens_ptr(lens, lc, C, xyz);
     c10::cuda::CUDAGuard guard(xyz.device());
     auto opt = xyz.options();
-    torch::Tensor records = torch::empty({N, GSR_REC_FLOATS}, opt);
-    torch::Tensor zkey = torch::empty({N}, opt.dtype(torch::kInt32));
-    torch::Tensor visible = torch::empty({N}, opt.dtype(torch::kUInt8));
-    torch::Tensor scan = torch::empty({N}, opt.dtype(torch::kInt64));
-    torch::Tensor tile_mask = torch::empty({with_tiles ? N : 0}, opt.dtype(torch::kInt64));
-    torch::Tensor tile_win = torch::empty({with_tiles ? N : 0}, opt.dtype(torch::kInt32));
+    // one view's outputs have no view dimension
+    auto shape = [&](std::initializer_list<int64_t> s) {
+        std::vector<int64_t> v(s);
+        if (batched) v.insert(v.begin(), C);
+        return v;
+    };
+    torch::Tensor records = torch::empty(shape({N, GSR_REC_FLOATS}), opt);
+    torch::Tensor zkey = torch::empty(shape({N}), opt.dtype(torch::kInt32));
+    torch::Tensor visible = torch::empty(shape({N}), opt.dtype(torch::kUInt8));
+    torch::Tensor scan = torch::empty(shape({N}), opt.dtype(torch::kInt64));
+    torch::Tensor tile_mask = torch::empty(shape({with_tiles ? N : 0}), opt.dtype(torch::kInt64));
+    torch::Tensor tile_win = torch::empty(shape({with_tiles ? N : 0}), opt.dtype(torch::kInt32));
     const size_t tb = gsr_preprocess_temp_bytes(N);
     torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
-    const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = lens_ptr(lens, lc, 1, xyz);
+    const bool tiles = with_tiles && N > 0;
+    // one view calls its entry point also for an empty scene (which only checks the arguments)
+    for (int64_t c = 0; c < C && (N > 0 || !batched); ++c) {
 #define GSR_FWD_ARGS                                                                                                  \
-    (int)mode, N, n_rest, F32PTR(xyz), cam_ptr, cam_first, F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), \
-        f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world), F32PTR(K), centre_ptr, (int)H, (int)W,                   \
-        (float)near_thresh, (float)far_thresh, (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base,        \
-        F32PTR(records), (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),                                \
-        (uint64_t*)scan.data_ptr<int64_t>(), with_tiles && N > 0 ? (uint64_t*)tile_mask.data_ptr<int64_t>() : nullptr, \
-        with_tiles && N > 0 ? (uint32_t*)tile_win.data_ptr<int>() : nullptr, temp.data_ptr(), tb
-    if (lens == Lens::Fisheye)
-        check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, fe, cur_stream()), "gsr_fisheye_preprocess_forward");
-    else if (lens == Lens::Distortion)
-        check_rc(gsr_distortion_preprocess_forward(GSR_FWD_ARGS, fe, cur_stream()),
-                 "gsr_distortion_preprocess_forward");
-    else
-        check_rc(gsr_preprocess_forward(GSR_FWD_ARGS, cur_stream()), "gsr_preprocess_forward");
+    (int)mode, N, n_rest, F32PTR(xyz), cam_ptr ? cam_ptr + c * R * 3 : nullptr, N - (int)R, F32PTR(quaternion),       \
+        F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world) + 16 * c,            \
+        F32PTR(K) + 9 * c, centre_ptr ? centre_ptr + 3 * c : nullptr, (int)H, (int)W, (float)near_thresh,              \
+        (float)far_thresh, (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base,                             \
+        F32PTR(records) + c * N * GSR_REC_FLOATS, (uint32_t*)zkey.data_ptr<int>() + c * N,                             \
+        visible.data_ptr<uint8_t>() + c * N, (uint64_t*)scan.data_ptr<int64_t>() + c * N,                              \
+        tiles ? (uint64_t*)tile_mask.data_ptr<int64_t>() + c * N : nullptr,                                            \
+        tiles ? (uint32_t*)tile_win.data_ptr<int>() + c * N : nullptr, temp.data_ptr(), tb
+        if (lens == GSR_LENS_FISHEYE)
+            check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, lens_consts + GSR_FISHEYE_CONSTS * c, cur_stream()),
+                     "gsr_fisheye_preprocess_forward");
+        else if (lens == GSR_LENS_DISTORTION)
+            check_rc(gsr_distortion_preprocess_forward(GSR_FWD_ARGS, lens_consts + GSR_DISTORTION_CONSTS * c,
+                                                       cur_stream()),
+                     "gsr_distortion_preprocess_forward");
+        else
+            check_rc(gsr_preprocess_forward(GSR_FWD_ARGS, cur_stream()), "gsr_preprocess_forward");
 #undef GSR_FWD_ARGS
+    }
     if (!with_tiles) return {records, zkey, visible, scan};
     return {records, zkey, visible, scan, tile_mask, tile_win};
 }
@@ -553,22 +593,22 @@ std::vector<torch::Tensor> fused_preprocess_forward(
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d) {
-    return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
-                              K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
-                              with_tiles, mode, filter3d, Lens::Pinhole, c10::nullopt);
+    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, int64_t lens,
+    c10::optional<torch::Tensor> lens_consts) {
+    return preprocess_forward(false, xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
+                              camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding,
+                              mh_dist, depth_base, with_tiles, mode, filter3d, lens, lens_consts);
 }
 
-// fused_preprocess_forward for a fisheye camera: fisheye [5] = {k1, k2, k3, k4, theta_max} on xyz's device
-std::vector<torch::Tensor> fisheye_preprocess_forward(
+std::vector<torch::Tensor> batch_preprocess_forward(
     torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
-    return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
-                              K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
-                              with_tiles, mode, filter3d, Lens::Fisheye, fisheye);
+    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
+    return preprocess_forward(true, xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
+                              camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding,
+                              mh_dist, depth_base, true, mode, filter3d, lens, lens_consts);
 }
 
 // (M, P known) -> the sorted pair list the tile renderers read records through, tile ranges [n_tiles+1] i32,
@@ -787,253 +827,185 @@ torch::Tensor fused_render_features_backward(torch::Tensor grad_map, torch::Tens
     return grad_features;
 }
 
-// grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the slab of fused_render_backward:
-// interleaved rows [N,12] by gaussian.  grad_uv_compact [M,2] (optional): gradient on the compact uv,
-// added to — or, with use_slab_uv false, replacing — the slab's uv section.  mode: the GSR_MODE_* bits of the forward
-// (gsr_preprocess_backward): GSR_MODE_DEPTH_ALPHA reads the z gradient of the depth/alpha rows, GSR_MODE_ANTIALIASED
-// takes the rows' opacity slot as the gradient on the compensated opacity, GSR_MODE_FILTER3D needs the forward's filter3d.
-static std::vector<torch::Tensor> preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
-                                                      torch::Tensor scale, torch::Tensor opacity_logit,
-                                                      c10::optional<torch::Tensor> sh_rest,
-                                                      torch::Tensor camera_T_world, torch::Tensor K,
-                                                      c10::optional<torch::Tensor> camera_centre,
-                                                      torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-                                                      c10::optional<torch::Tensor> grad_uv_compact,
-                                                      c10::optional<torch::Tensor> scan, bool use_slab_uv,
-                                                      int64_t mode, c10::optional<torch::Tensor> filter3d,
-                                                      Lens lens, c10::optional<torch::Tensor> lc,
-                                                      bool pose = false, bool camera = false) {
+// The flat parameter / gradient layout: [xyz 3N | quaternion 4N | scale 3N | opacity N | rgb 3N | sh 3*n_sh_rest*N],
+// every section starting on a 16-byte boundary (TMA bulk stores).  width: floats per gaussian of each section; off:
+// each section's start, off[6] the total.
+struct FlatLayout {
+    int64_t width[6];
+    int64_t off[7];
+};
+static FlatLayout flat_layout(int64_t N, int64_t n_sh_rest) {
+    FlatLayout l = {{3, 4, 3, 1, 3, 3 * n_sh_rest}, {0}};
+    for (int i = 0; i < 6; ++i) l.off[i + 1] = (l.off[i] + N * l.width[i] + 3) & ~(int64_t)3;
+    return l;
+}
+
+// The per-gaussian backward: grads of (xyz, quaternion, scale, opacity_logit, rgb_dc[, sh_rest]) from the gradient
+// rows of the render backward, interleaved [N,12] by gaussian.  One view (batched false): slab [N*12] of
+// fused_render_backward, visible / scan [N] of fused_preprocess_forward (gsr_preprocess_backward, or the lens's).
+// C views (batched): slab [C, N*12] of batch_render_backward, visible / scan [C,N] of batch_preprocess_forward,
+// grad_uv_compact [sum M_c, 2], the gradient summed over the views in one pass (gsr_batch_preprocess_backward, or the
+// lens's).  grad_uv_compact [M,2] (optional): gradient on the compact uv, added to — or, with use_slab_uv false,
+// replacing — the slab's uv section.  mode: the GSR_MODE_* bits of the forward: GSR_MODE_DEPTH_ALPHA reads the z
+// gradient of the depth/alpha rows, GSR_MODE_ANTIALIASED takes the rows' opacity slot as the gradient on the
+// compensated opacity, GSR_MODE_FILTER3D needs the forward's filter3d.  lens, lc: the forward's.
+// camera_grads: 0 none; 1 also d loss / d camera_T_world (gsr_pose_*, libgsr_pose.so); 2 also the intrinsics and
+// lens-coefficient gradients (gsr_camera_*, libgsr_calib.so).
+// Returns the gaussian gradients, then `flat` (the one allocation they are views of), then with camera_grads >= 1
+// g_pose [4,4] / [C,4,4] (last row 0), then with camera_grads 2 d loss / d (fx, fy, cx, cy) [4] / [C,4] and d loss /
+// d lens coefficients [n] / [C,n] (n = 0 for the pinhole).
+static std::vector<torch::Tensor> preprocess_backward(
+    bool batched, torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale,
+    torch::Tensor opacity_logit, c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lc, int64_t camera_grads) {
+    TORCH_CHECK(camera_grads >= 0 && camera_grads <= 2,
+                "camera_grads must be 0 (none), 1 (pose) or 2 (pose, intrinsics and lens)");
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
+    CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
+    CHECK_VALID_INPUT(visible);
+    const int64_t C = check_views(batched, camera_T_world, K);
     const int64_t N = xyz.size(0);
-    TORCH_CHECK(slab.numel() == N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ", GSR_GRAD_ROW_FLOATS,
-                " floats per gaussian");
-    c10::cuda::CUDAGuard guard(xyz.device());
-    auto opt = xyz.options();
+    TORCH_CHECK(slab.numel() == C * N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold ",
+                GSR_GRAD_ROW_FLOATS, " floats per gaussian and view");
+    TORCH_CHECK(visible.numel() == C * N && visible.scalar_type() == torch::kUInt8,
+                "visible must hold one uint8 per gaussian and view");
+    const float* centre_ptr = nullptr;
+    if (camera_centre.has_value()) {
+        CHECK_VALID_INPUT((*camera_centre)); CHECK_FLOAT_TENSOR((*camera_centre));
+        TORCH_CHECK(camera_centre->numel() == 3 * C, "camera_centre must hold 3 floats per view");
+        centre_ptr = camera_centre->data_ptr<float>();
+    }
     const int n_rest = sh_rest.has_value() ? (int)sh_rest->size(2) : 0;
     const float* g_uv_compact = nullptr;
     const uint64_t* scan_ptr = nullptr;
     if (grad_uv_compact.has_value() && grad_uv_compact->numel() > 0) {
         CHECK_VALID_INPUT((*grad_uv_compact)); CHECK_FLOAT_TENSOR((*grad_uv_compact));
-        TORCH_CHECK(scan.has_value() && scan->numel() == N && scan->scalar_type() == torch::kInt64,
+        TORCH_CHECK(scan.has_value() && scan->numel() == C * N && scan->scalar_type() == torch::kInt64,
                     "grad_uv_compact needs the packed scan of the forward pass");
+        CHECK_VALID_INPUT((*scan));
         TORCH_CHECK(grad_uv_compact->dim() == 2 && grad_uv_compact->size(1) == 2, "grad_uv_compact must be Mx2");
         g_uv_compact = grad_uv_compact->data_ptr<float>();
         scan_ptr = (const uint64_t*)scan->data_ptr<int64_t>();
     }
-    // All parameter gradients of a view live in ONE allocation, [xyz 3N | quaternion 4N | scale 3N |
-    // opacity N | rgb 3N | sh 3*n_rest*N], every section starting on a 16-byte boundary (TMA bulk stores):
-    // a trainer that sums gradients over views / ranks reduces that one buffer (view_parallel.py).
-    const int64_t widths[6] = {3, 4, 3, 1, 3, 3 * (int64_t)n_rest};
-    int64_t offs[7];
-    offs[0] = 0;
-    for (int i = 0; i < 6; ++i) offs[i + 1] = (offs[i] + N * widths[i] + 3) & ~(int64_t)3;
-    // out_flat: a caller-owned buffer of the same layout (e.g. symmetric memory peers can read, view_parallel.py)
+    const float* f3d = filter3d_ptr(filter3d, N);
+    const float* lens_consts = lens_ptr(lens, lc, C, xyz);
+    c10::cuda::CUDAGuard guard(xyz.device());
+    auto opt = xyz.options();
+    // All parameter gradients live in ONE allocation of the flat layout: a trainer that sums gradients over views /
+    // ranks reduces that one buffer (view_parallel.py).  out_flat: a caller-owned buffer of the same layout (e.g.
+    // symmetric memory peers can read, view_parallel.py)
+    const FlatLayout l = flat_layout(N, n_rest);
     torch::Tensor flat;
     if (out_flat.has_value()) {
         flat = *out_flat;
         CHECK_VALID_INPUT(flat); CHECK_FLOAT_TENSOR(flat);
-        TORCH_CHECK(flat.numel() == offs[6], "out_flat must hold ", offs[6], " floats");
+        TORCH_CHECK(flat.numel() == l.off[6], "out_flat must hold ", l.off[6], " floats");
         TORCH_CHECK((reinterpret_cast<uintptr_t>(flat.data_ptr()) & 15u) == 0, "out_flat must be 16-byte aligned");
     } else {
-        flat = torch::empty({offs[6]}, opt);
+        flat = torch::empty({l.off[6]}, opt);
     }
     for (int i = 0; i < 6; ++i)  // padding between sections (only when N is not a multiple of 4)
-        if (offs[i + 1] > offs[i] + N * widths[i]) flat.narrow(0, offs[i] + N * widths[i], offs[i + 1] - offs[i] - N * widths[i]).zero_();
+        if (l.off[i + 1] > l.off[i] + N * l.width[i])
+            flat.narrow(0, l.off[i] + N * l.width[i], l.off[i + 1] - l.off[i] - N * l.width[i]).zero_();
     auto section = [&](int i, std::vector<int64_t> shape) {
-        return flat.narrow(0, offs[i], N * widths[i]).view(shape);
+        return flat.narrow(0, l.off[i], N * l.width[i]).view(shape);
     };
     torch::Tensor o_xyz = section(0, {N, 3}), o_q = section(1, {N, 4}), o_s = section(2, {N, 3}),
                   o_o = section(3, {N}), o_dc = section(4, {N, 3});
     torch::Tensor g_sh;
     if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
-    const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = lens_ptr(lens, lc, 1, xyz);
+    // the arguments after (mode[, C]) shared by every backward entry point
 #define GSR_BWD_ARGS                                                                                                 \
-    (int)mode, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d,          \
-        F32PTR(camera_T_world), F32PTR(K), camera_centre.has_value() ? camera_centre->data_ptr<float>() : nullptr,   \
-        visible.data_ptr<uint8_t>(), slab.data_ptr<float>(), use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr,            \
-        F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o), F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    torch::Tensor g_pose, g_intr, g_lens;
-    if (camera) {
-        g_pose = torch::empty({4, 4}, opt);
-        g_intr = torch::empty({4}, opt);
-        g_lens = torch::empty({lens_coefficient_count(lens)}, opt);
-        torch::Tensor temp =
-            torch::empty({(int64_t)gsr_camera_temp_bytes((int)lens, 1, (int)N)}, opt.dtype(torch::kUInt8));
-        check_rc(gsr_camera_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), F32PTR(g_intr),
-                                                g_lens.numel() ? F32PTR(g_lens) : nullptr, temp.data_ptr(),
-                                                (size_t)temp.numel(), cur_stream()),
-                 "gsr_camera_preprocess_backward");
-    } else if (pose) {
-        g_pose = torch::empty({4, 4}, opt);
-        torch::Tensor temp = torch::empty({(int64_t)gsr_pose_temp_bytes(1, (int)N)}, opt.dtype(torch::kUInt8));
-        check_rc(gsr_pose_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), temp.data_ptr(),
-                                              (size_t)temp.numel(), cur_stream()),
-                 "gsr_pose_preprocess_backward");
-    } else if (lens == Lens::Fisheye)
-        check_rc(gsr_fisheye_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()), "gsr_fisheye_preprocess_backward");
-    else if (lens == Lens::Distortion)
-        check_rc(gsr_distortion_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
-                 "gsr_distortion_preprocess_backward");
-    else
-        check_rc(gsr_preprocess_backward(GSR_BWD_ARGS, cur_stream()), "gsr_preprocess_backward");
-#undef GSR_BWD_ARGS
+    (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d,                      \
+        F32PTR(camera_T_world), F32PTR(K), centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab),                    \
+        use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o),           \
+        F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
+    const int md = (int)mode, nc = (int)C, ln = (int)lens;
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
-    out.push_back(flat);  // the allocation all the gaussian gradients are views of
-    if (pose || camera) out.push_back(g_pose);  // d loss / d camera_T_world [4,4]
-    if (camera) {  // last: d loss / d (fx, fy, cx, cy) [4] and d loss / d lens coefficients [n]
-        out.push_back(g_intr);
-        out.push_back(g_lens);
+    out.push_back(flat);
+    if (camera_grads == 0) {
+        if (lens == GSR_LENS_FISHEYE)
+            check_rc(batched ? gsr_fisheye_batch_preprocess_backward(md, nc, GSR_BWD_ARGS, lens_consts, cur_stream())
+                             : gsr_fisheye_preprocess_backward(md, GSR_BWD_ARGS, lens_consts, cur_stream()),
+                     batched ? "gsr_fisheye_batch_preprocess_backward" : "gsr_fisheye_preprocess_backward");
+        else if (lens == GSR_LENS_DISTORTION)
+            check_rc(batched
+                         ? gsr_distortion_batch_preprocess_backward(md, nc, GSR_BWD_ARGS, lens_consts, cur_stream())
+                         : gsr_distortion_preprocess_backward(md, GSR_BWD_ARGS, lens_consts, cur_stream()),
+                     batched ? "gsr_distortion_batch_preprocess_backward" : "gsr_distortion_preprocess_backward");
+        else
+            check_rc(batched ? gsr_batch_preprocess_backward(md, nc, GSR_BWD_ARGS, cur_stream())
+                             : gsr_preprocess_backward(md, GSR_BWD_ARGS, cur_stream()),
+                     batched ? "gsr_batch_preprocess_backward" : "gsr_preprocess_backward");
+        return out;
     }
+    // one view's camera gradients have no view dimension
+    auto shape = [&](std::initializer_list<int64_t> s) {
+        std::vector<int64_t> v(s);
+        if (batched) v.insert(v.begin(), C);
+        return v;
+    };
+    torch::Tensor g_pose = torch::empty(shape({4, 4}), opt);
+    out.push_back(g_pose);
+    if (camera_grads == 1) {
+        torch::Tensor temp = torch::empty({(int64_t)gsr_pose_temp_bytes(nc, (int)N)}, opt.dtype(torch::kUInt8));
+        void* tp = temp.data_ptr();
+        const size_t tb = (size_t)temp.numel();
+        check_rc(batched ? gsr_pose_batch_preprocess_backward(ln, md, nc, GSR_BWD_ARGS, lens_consts, F32PTR(g_pose), tp,
+                                                              tb, cur_stream())
+                         : gsr_pose_preprocess_backward(ln, md, GSR_BWD_ARGS, lens_consts, F32PTR(g_pose), tp, tb,
+                                                        cur_stream()),
+                 batched ? "gsr_pose_batch_preprocess_backward" : "gsr_pose_preprocess_backward");
+        return out;
+    }
+    torch::Tensor g_intr = torch::empty(shape({4}), opt);
+    const int64_t n_coeffs = std::max<int64_t>(lens_consts_per_view(lens) - 1, 0);
+    torch::Tensor g_lens = torch::empty(shape({n_coeffs}), opt);
+    torch::Tensor temp = torch::empty({(int64_t)gsr_camera_temp_bytes(ln, nc, (int)N)}, opt.dtype(torch::kUInt8));
+    void* tp = temp.data_ptr();
+    const size_t tb = (size_t)temp.numel();
+    float* gl = g_lens.numel() ? F32PTR(g_lens) : nullptr;
+    check_rc(batched ? gsr_camera_batch_preprocess_backward(ln, md, nc, GSR_BWD_ARGS, lens_consts, F32PTR(g_pose),
+                                                            F32PTR(g_intr), gl, tp, tb, cur_stream())
+                     : gsr_camera_preprocess_backward(ln, md, GSR_BWD_ARGS, lens_consts, F32PTR(g_pose),
+                                                      F32PTR(g_intr), gl, tp, tb, cur_stream()),
+             batched ? "gsr_camera_batch_preprocess_backward" : "gsr_camera_preprocess_backward");
+#undef GSR_BWD_ARGS
+    out.push_back(g_intr);
+    out.push_back(g_lens);
     return out;
 }
 
-std::vector<torch::Tensor> fused_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
-                                                     torch::Tensor scale, torch::Tensor opacity_logit,
-                                                     c10::optional<torch::Tensor> sh_rest,
-                                                     torch::Tensor camera_T_world, torch::Tensor K,
-                                                     c10::optional<torch::Tensor> camera_centre,
-                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-                                                     c10::optional<torch::Tensor> grad_uv_compact,
-                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
-                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
-    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Pinhole,
-                               c10::nullopt);
+std::vector<torch::Tensor> fused_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts,
+    int64_t camera_grads) {
+    return preprocess_backward(false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
+                               camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d,
+                               lens, lens_consts, camera_grads);
 }
 
-// fused_preprocess_backward for a fisheye camera (the forward's fisheye constants)
-std::vector<torch::Tensor> fisheye_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
-                                                       torch::Tensor scale, torch::Tensor opacity_logit,
-                                                       c10::optional<torch::Tensor> sh_rest,
-                                                       torch::Tensor camera_T_world, torch::Tensor K,
-                                                       c10::optional<torch::Tensor> camera_centre,
-                                                       torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-                                                       c10::optional<torch::Tensor> grad_uv_compact,
-                                                       c10::optional<torch::Tensor> scan, bool use_slab_uv,
-                                                       int64_t mode, c10::optional<torch::Tensor> filter3d,
-                                                       torch::Tensor fisheye) {
-    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Fisheye,
-                               fisheye);
+std::vector<torch::Tensor> batch_preprocess_backward(
+    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
+    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
+    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts,
+    int64_t camera_grads) {
+    return preprocess_backward(true, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
+                               camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d,
+                               lens, lens_consts, camera_grads);
 }
 
 // ---------------------------------------------------------------------------------------------
 // multi-view fused path (rasterize_batch): C views of one scene, per-view arrays stacked view-major
 // ---------------------------------------------------------------------------------------------
-static int64_t check_views(const torch::Tensor& camera_T_world, const torch::Tensor& K) {
-    CHECK_VALID_INPUT(camera_T_world); CHECK_VALID_INPUT(K);
-    CHECK_FLOAT_TENSOR(camera_T_world); CHECK_FLOAT_TENSOR(K);
-    const int64_t C = camera_T_world.size(0);
-    TORCH_CHECK(camera_T_world.dim() == 3 && C >= 1 && camera_T_world.size(1) == 4 && camera_T_world.size(2) == 4,
-                "camera_T_world must have shape Cx4x4, C >= 1");
-    TORCH_CHECK(K.dim() == 3 && K.size(0) == C && K.size(1) == 3 && K.size(2) == 3, "K must have shape Cx3x3");
-    return C;
-}
-
-// fused_preprocess_forward of every view into stacked outputs: [records [C,N,12], depth_key [C,N], visible [C,N],
-// scan [C,N] (each view's own packed inclusive scan), tile_mask [C,N], tile_win [C,N]].  xyz_camera_frame [C,R,3]:
-// camera-frame positions of the LAST R gaussians of every view; camera_centre [C,3].
-static std::vector<torch::Tensor> batch_forward(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, Lens lens, c10::optional<torch::Tensor> lc) {
-    CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
-    CHECK_VALID_INPUT(rgb_dc);
-    CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
-    CHECK_FLOAT_TENSOR(opacity_logit); CHECK_FLOAT_TENSOR(rgb_dc);
-    const int64_t C = check_views(camera_T_world, K);
-    const int N = xyz.size(0);
-    TORCH_CHECK(xyz.dim() == 2 && xyz.size(1) == 3, "xyz must have shape Nx3");
-    TORCH_CHECK(quaternion.size(0) == N && quaternion.size(1) == 4, "quaternion must have shape Nx4");
-    TORCH_CHECK(scale.size(0) == N && scale.size(1) == 3, "scale must have shape Nx3");
-    TORCH_CHECK(opacity_logit.numel() == N, "opacity must have shape Nx1");
-    TORCH_CHECK(rgb_dc.size(0) == N && rgb_dc.size(1) == 3, "rgb must have shape Nx3");
-    const float* cam_ptr = nullptr;
-    int64_t R = 0;
-    if (xyz_camera_frame.has_value()) {
-        const torch::Tensor& pc = *xyz_camera_frame;
-        CHECK_VALID_INPUT(pc); CHECK_FLOAT_TENSOR(pc);
-        TORCH_CHECK(pc.dim() == 3 && pc.size(0) == C && pc.size(1) <= N && pc.size(2) == 3,
-                    "xyz_camera_frame must have shape CxRx3, R <= N");
-        cam_ptr = pc.data_ptr<float>();
-        R = pc.size(1);
-    }
-    const float* centre_ptr = nullptr;
-    if (camera_centre.has_value()) {
-        CHECK_VALID_INPUT((*camera_centre)); CHECK_FLOAT_TENSOR((*camera_centre));
-        TORCH_CHECK(camera_centre->numel() == 3 * C, "camera_centre must have shape Cx3");
-        centre_ptr = camera_centre->data_ptr<float>();
-    }
-    int n_rest = 0;
-    const float* sh_ptr = nullptr;
-    if (sh_rest.has_value()) {
-        const torch::Tensor& sh = *sh_rest;
-        CHECK_VALID_INPUT(sh); CHECK_FLOAT_TENSOR(sh);
-        TORCH_CHECK(sh.dim() == 3 && sh.size(0) == N && sh.size(1) == 3, "sh must have shape Nx3xK");
-        n_rest = sh.size(2);
-        TORCH_CHECK(n_rest == 3 || n_rest == 8 || n_rest == 15, "sh must hold 3, 8 or 15 coefficients per channel");
-        sh_ptr = sh.data_ptr<float>();
-    }
-    c10::cuda::CUDAGuard guard(xyz.device());
-    auto opt = xyz.options();
-    torch::Tensor records = torch::empty({C, N, GSR_REC_FLOATS}, opt);
-    torch::Tensor zkey = torch::empty({C, N}, opt.dtype(torch::kInt32));
-    torch::Tensor visible = torch::empty({C, N}, opt.dtype(torch::kUInt8));
-    torch::Tensor scan = torch::empty({C, N}, opt.dtype(torch::kInt64));
-    torch::Tensor tile_mask = torch::empty({C, N}, opt.dtype(torch::kInt64));
-    torch::Tensor tile_win = torch::empty({C, N}, opt.dtype(torch::kInt32));
-    const size_t tb = gsr_preprocess_temp_bytes(N);
-    torch::Tensor temp = torch::empty({(int64_t)tb}, opt.dtype(torch::kUInt8));
-    const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = lens_ptr(lens, lc, C, xyz);
-    for (int64_t c = 0; c < C && N > 0; ++c) {
-#define GSR_FWD_ARGS                                                                                                \
-    (int)mode, N, n_rest, F32PTR(xyz), cam_ptr ? cam_ptr + c * R * 3 : nullptr, N - (int)R, F32PTR(quaternion),     \
-        F32PTR(scale), F32PTR(opacity_logit), f3d, F32PTR(rgb_dc), sh_ptr, F32PTR(camera_T_world) + 16 * c,          \
-        F32PTR(K) + 9 * c, centre_ptr ? centre_ptr + 3 * c : nullptr, (int)H, (int)W, (float)near_thresh,            \
-        (float)far_thresh, (float)cull_mask_padding, (float)mh_dist, (uint32_t)depth_base, F32PTR(records[c]),       \
-        (uint32_t*)zkey[c].data_ptr<int>(), visible[c].data_ptr<uint8_t>(), (uint64_t*)scan[c].data_ptr<int64_t>(),  \
-        (uint64_t*)tile_mask[c].data_ptr<int64_t>(), (uint32_t*)tile_win[c].data_ptr<int>(), temp.data_ptr(), tb
-        if (lens == Lens::Fisheye)
-            check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, fe + GSR_FISHEYE_CONSTS * c, cur_stream()),
-                     "gsr_fisheye_preprocess_forward");
-        else if (lens == Lens::Distortion)
-            check_rc(gsr_distortion_preprocess_forward(GSR_FWD_ARGS, fe + GSR_DISTORTION_CONSTS * c, cur_stream()),
-                     "gsr_distortion_preprocess_forward");
-        else
-            check_rc(gsr_preprocess_forward(GSR_FWD_ARGS, cur_stream()), "gsr_preprocess_forward");
-#undef GSR_FWD_ARGS
-    }
-    return {records, zkey, visible, scan, tile_mask, tile_win};
-}
-
-std::vector<torch::Tensor> batch_preprocess_forward(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
-    c10::optional<torch::Tensor> filter3d) {
-    return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
-                         camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
-                         filter3d, Lens::Pinhole, c10::nullopt);
-}
-
-// batch_preprocess_forward for fisheye cameras: fisheye [C,5] = {k1, k2, k3, k4, theta_max} per view
-std::vector<torch::Tensor> batch_fisheye_preprocess_forward(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
-    return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
-                         camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
-                         filter3d, Lens::Fisheye, fisheye);
-}
-
 // fused_render_backward of every view into one stacked slab [C, N*12]: grad_image [C,H,W,3], per view the forward's
 // pair list (keys_sorted or ids_sorted, the other one empty), ranges, n, w and masks (empty: none); records [C,N,12],
 // background [C,3]; with grad_depth / grad_alpha [C,H,W,1] also depth_key [C,N].
@@ -1089,250 +1061,11 @@ torch::Tensor batch_render_backward(torch::Tensor grad_image, int64_t N, std::ve
     return slab;
 }
 
-// the per-gaussian backward of C views in one pass (gsr_batch_preprocess_backward): slab [C, N*12] of
-// batch_render_backward, visible / scan [C,N] of batch_preprocess_forward, grad_uv_compact [sum M_c, 2] (optional).
-// Same outputs and flat layout as fused_preprocess_backward, holding the gradient summed over the views.
-static std::vector<torch::Tensor> batch_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
-                                                 torch::Tensor scale, torch::Tensor opacity_logit,
-                                                 c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
-                                                 torch::Tensor K, c10::optional<torch::Tensor> camera_centre,
-                                                 torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-                                                 c10::optional<torch::Tensor> grad_uv_compact,
-                                                 c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-                                                 c10::optional<torch::Tensor> filter3d, Lens lens,
-                                                 c10::optional<torch::Tensor> lc, bool pose = false,
-                                                 bool camera = false) {
-    CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
-    CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
-    CHECK_VALID_INPUT(visible);
-    const int64_t C = check_views(camera_T_world, K);
-    const int64_t N = xyz.size(0);
-    TORCH_CHECK(slab.numel() == C * N * (int64_t)GSR_GRAD_ROW_FLOATS, "gradient slab must hold C*N*",
-                GSR_GRAD_ROW_FLOATS, " floats");
-    TORCH_CHECK(visible.numel() == C * N && visible.scalar_type() == torch::kUInt8, "visible must be a CxN uint8 tensor");
-    const float* centre_ptr = nullptr;
-    if (camera_centre.has_value()) {
-        CHECK_VALID_INPUT((*camera_centre)); CHECK_FLOAT_TENSOR((*camera_centre));
-        TORCH_CHECK(camera_centre->numel() == 3 * C, "camera_centre must have shape Cx3");
-        centre_ptr = camera_centre->data_ptr<float>();
-    }
-    c10::cuda::CUDAGuard guard(xyz.device());
-    auto opt = xyz.options();
-    const int n_rest = sh_rest.has_value() ? (int)sh_rest->size(2) : 0;
-    const float* g_uv_compact = nullptr;
-    const uint64_t* scan_ptr = nullptr;
-    if (grad_uv_compact.has_value() && grad_uv_compact->numel() > 0) {
-        CHECK_VALID_INPUT((*grad_uv_compact)); CHECK_FLOAT_TENSOR((*grad_uv_compact));
-        TORCH_CHECK(scan.has_value() && scan->numel() == C * N && scan->scalar_type() == torch::kInt64,
-                    "grad_uv_compact needs the packed scans of the forward pass");
-        CHECK_VALID_INPUT((*scan));
-        TORCH_CHECK(grad_uv_compact->dim() == 2 && grad_uv_compact->size(1) == 2, "grad_uv_compact must be Mx2");
-        g_uv_compact = grad_uv_compact->data_ptr<float>();
-        scan_ptr = (const uint64_t*)scan->data_ptr<int64_t>();
-    }
-    const int64_t widths[6] = {3, 4, 3, 1, 3, 3 * (int64_t)n_rest};
-    int64_t offs[7];
-    offs[0] = 0;
-    for (int i = 0; i < 6; ++i) offs[i + 1] = (offs[i] + N * widths[i] + 3) & ~(int64_t)3;
-    torch::Tensor flat;
-    if (out_flat.has_value()) {
-        flat = *out_flat;
-        CHECK_VALID_INPUT(flat); CHECK_FLOAT_TENSOR(flat);
-        TORCH_CHECK(flat.numel() == offs[6], "out_flat must hold ", offs[6], " floats");
-        TORCH_CHECK((reinterpret_cast<uintptr_t>(flat.data_ptr()) & 15u) == 0, "out_flat must be 16-byte aligned");
-    } else {
-        flat = torch::empty({offs[6]}, opt);
-    }
-    for (int i = 0; i < 6; ++i)
-        if (offs[i + 1] > offs[i] + N * widths[i]) flat.narrow(0, offs[i] + N * widths[i], offs[i + 1] - offs[i] - N * widths[i]).zero_();
-    auto section = [&](int i, std::vector<int64_t> shape) {
-        return flat.narrow(0, offs[i], N * widths[i]).view(shape);
-    };
-    torch::Tensor o_xyz = section(0, {N, 3}), o_q = section(1, {N, 4}), o_s = section(2, {N, 3}),
-                  o_o = section(3, {N}), o_dc = section(4, {N, 3});
-    torch::Tensor g_sh;
-    if (n_rest) g_sh = section(5, {N, 3, (int64_t)n_rest});
-    const float* f3d = filter3d_ptr(filter3d, N);
-    const float* fe = lens_ptr(lens, lc, C, xyz);
-#define GSR_BWD_ARGS                                                                                                \
-    (int)mode, (int)C, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit), f3d,  \
-        F32PTR(camera_T_world), F32PTR(K), centre_ptr, visible.data_ptr<uint8_t>(), F32PTR(slab),                    \
-        use_slab_uv ? 1 : 0, g_uv_compact, scan_ptr, F32PTR(o_xyz), F32PTR(o_q), F32PTR(o_s), F32PTR(o_o),           \
-        F32PTR(o_dc), n_rest ? F32PTR(g_sh) : nullptr
-    torch::Tensor g_pose, g_intr, g_lens;
-    if (camera) {
-        g_pose = torch::empty({C, 4, 4}, opt);
-        g_intr = torch::empty({C, 4}, opt);
-        g_lens = torch::empty({C, lens_coefficient_count(lens)}, opt);
-        torch::Tensor temp =
-            torch::empty({(int64_t)gsr_camera_temp_bytes((int)lens, (int)C, (int)N)}, opt.dtype(torch::kUInt8));
-        check_rc(gsr_camera_batch_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), F32PTR(g_intr),
-                                                      g_lens.numel() ? F32PTR(g_lens) : nullptr, temp.data_ptr(),
-                                                      (size_t)temp.numel(), cur_stream()),
-                 "gsr_camera_batch_preprocess_backward");
-    } else if (pose) {
-        g_pose = torch::empty({C, 4, 4}, opt);
-        torch::Tensor temp = torch::empty({(int64_t)gsr_pose_temp_bytes((int)C, (int)N)}, opt.dtype(torch::kUInt8));
-        check_rc(gsr_pose_batch_preprocess_backward((int)lens, GSR_BWD_ARGS, fe, F32PTR(g_pose), temp.data_ptr(),
-                                                    (size_t)temp.numel(), cur_stream()),
-                 "gsr_pose_batch_preprocess_backward");
-    } else if (lens == Lens::Fisheye)
-        check_rc(gsr_fisheye_batch_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
-                 "gsr_fisheye_batch_preprocess_backward");
-    else if (lens == Lens::Distortion)
-        check_rc(gsr_distortion_batch_preprocess_backward(GSR_BWD_ARGS, fe, cur_stream()),
-                 "gsr_distortion_batch_preprocess_backward");
-    else
-        check_rc(gsr_batch_preprocess_backward(GSR_BWD_ARGS, cur_stream()), "gsr_batch_preprocess_backward");
-#undef GSR_BWD_ARGS
-    std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
-    if (n_rest) out.push_back(g_sh);
-    out.push_back(flat);
-    if (pose || camera) out.push_back(g_pose);  // d loss / d camera_T_world [C,4,4]
-    if (camera) {  // last: [C,4] intrinsics and [C,n] lens-coefficient gradients
-        out.push_back(g_intr);
-        out.push_back(g_lens);
-    }
-    return out;
-}
-
-std::vector<torch::Tensor> batch_preprocess_backward(torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion,
-                                                     torch::Tensor scale, torch::Tensor opacity_logit,
-                                                     c10::optional<torch::Tensor> sh_rest,
-                                                     torch::Tensor camera_T_world, torch::Tensor K,
-                                                     c10::optional<torch::Tensor> camera_centre,
-                                                     torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-                                                     c10::optional<torch::Tensor> grad_uv_compact,
-                                                     c10::optional<torch::Tensor> scan, bool use_slab_uv,
-                                                     int64_t mode, c10::optional<torch::Tensor> filter3d) {
-    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Pinhole,
-                          c10::nullopt);
-}
-
-// batch_preprocess_backward for fisheye cameras (the forward's [C,5] fisheye constants)
-std::vector<torch::Tensor> batch_fisheye_preprocess_backward(
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
-    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, torch::Tensor fisheye) {
-    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Fisheye,
-                          fisheye);
-}
-
 // gsr_fisheye_theta_max of 4 coefficients (host floats)
 double fisheye_theta_max(std::vector<double> k) {
     TORCH_CHECK(k.size() == 4, "fisheye needs 4 coefficients k1 k2 k3 k4");
     const float kf[4] = {(float)k[0], (float)k[1], (float)k[2], (float)k[3]};
     return (double)gsr_fisheye_theta_max(kf);
-}
-
-// The radial-tangential (COLMAP OPENCV) counterparts: distortion [C,6] = {k1, k2, p1, p2, k3, r2_max} per view on
-// xyz's device, C = 1 for the single-view functions.
-std::vector<torch::Tensor> distortion_preprocess_forward(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
-    bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
-    return preprocess_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world,
-                              K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base,
-                              with_tiles, mode, filter3d, Lens::Distortion, distortion);
-}
-
-std::vector<torch::Tensor> distortion_preprocess_backward(
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
-    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
-    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Distortion,
-                               distortion);
-}
-
-std::vector<torch::Tensor> batch_distortion_preprocess_forward(
-    torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion, torch::Tensor scale,
-    torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
-    torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-    double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
-    return batch_forward(xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest, camera_T_world, K,
-                         camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding, mh_dist, depth_base, mode,
-                         filter3d, Lens::Distortion, distortion);
-}
-
-std::vector<torch::Tensor> batch_distortion_preprocess_backward(
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
-    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, torch::Tensor distortion) {
-    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, Lens::Distortion,
-                          distortion);
-}
-
-// The per-gaussian backward with the camera pose gradient (libgsr_pose.so): the arguments of fused_preprocess_backward /
-// batch_preprocess_backward plus the lens (0 pinhole, 1 fisheye, 2 distortion; GSR_LENS_*) and its constants (the
-// forward's, none for the pinhole).  Returns the same outputs followed by d loss / d camera_T_world, [4,4] / [C,4,4]
-// (last row 0).
-static Lens pose_lens(int64_t lens) {
-    TORCH_CHECK(lens == GSR_LENS_PINHOLE || lens == GSR_LENS_FISHEYE || lens == GSR_LENS_DISTORTION,
-                "lens must be 0 (pinhole), 1 (fisheye) or 2 (distortion)");
-    static_assert((int)Lens::Pinhole == GSR_LENS_PINHOLE && (int)Lens::Fisheye == GSR_LENS_FISHEYE &&
-                      (int)Lens::Distortion == GSR_LENS_DISTORTION,
-                  "Lens and GSR_LENS_* agree");
-    return (Lens)lens;
-}
-
-std::vector<torch::Tensor> pose_preprocess_backward(
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
-    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
-    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
-                               lens_consts, true);
-}
-
-std::vector<torch::Tensor> batch_pose_preprocess_backward(
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
-    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
-    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
-                          lens_consts, true);
-}
-
-// The per-gaussian backward with the pose, intrinsics and lens-coefficient gradients (libgsr_calib.so, gsr_camera_*):
-// the arguments of pose_preprocess_backward / batch_pose_preprocess_backward.  Returns their outputs followed by
-// d loss / d (fx, fy, cx, cy) [4] / [C,4] and d loss / d lens coefficients [n] / [C,n] (n = 0 for the pinhole).
-std::vector<torch::Tensor> camera_preprocess_backward(
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
-    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
-    return preprocess_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                               visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
-                               lens_consts, false, true);
-}
-
-std::vector<torch::Tensor> batch_camera_preprocess_backward(
-    torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-    c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
-    c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
-    c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
-    return batch_backward(slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K, camera_centre,
-                          visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d, pose_lens(lens),
-                          lens_consts, false, true);
 }
 
 // gsr_distortion_r2_max of 5 coefficients k1 k2 p1 p2 k3 (host floats)
@@ -1367,13 +1100,10 @@ torch::Tensor filter3d(torch::Tensor xyz, torch::Tensor camera_T_world, torch::T
 
 // sizes of the flat parameter / gradient layout: exclusive end of each section, in elements
 std::vector<int64_t> flat_section_ends(int64_t N, int64_t n_sh_rest) {
-    const int64_t widths[6] = {3, 4, 3, 1, 3, 3 * n_sh_rest};
+    const FlatLayout l = flat_layout(N, n_sh_rest);
     std::vector<int64_t> ends;
-    int64_t off = 0;
-    for (int i = 0; i < 6; ++i) {
-        off = (off + N * widths[i] + 3) & ~(int64_t)3;
-        if (widths[i] > 0) ends.push_back(off);
-    }
+    for (int i = 0; i < 6; ++i)
+        if (l.width[i] > 0) ends.push_back(l.off[i + 1]);
     return ends;
 }
 
@@ -1838,12 +1568,14 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("render_depth_cuda", &render_depth_cuda, "Render depth CUDA");
     // fused path
     m.def("fused_preprocess_forward", &fused_preprocess_forward,
-          "fused per-gaussian stage (with_tiles: also every gaussian's tile-hit mask and window; mode: MODE_* bits)",
+          "fused per-gaussian stage (with_tiles: also every gaussian's tile-hit mask and window; mode: MODE_* bits; "
+          "lens: LENS_*, lens_consts its [n+1] constants)",
           py::arg("xyz"), py::arg("xyz_camera_frame"), py::arg("quaternion"), py::arg("scale"),
           py::arg("opacity_logit"), py::arg("rgb_dc"), py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"),
           py::arg("camera_centre"), py::arg("H"), py::arg("W"), py::arg("near_thresh"), py::arg("far_thresh"),
           py::arg("cull_mask_padding"), py::arg("mh_dist"), py::arg("depth_base"), py::arg("with_tiles") = false,
-          py::arg("mode") = 0, py::arg("filter3d") = py::none());
+          py::arg("mode") = 0, py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE,
+          py::arg("lens_consts") = py::none());
     m.def("fused_bin", &fused_bin, "pair emission + radix sort + tile ranges");
     m.def("fused_render_forward", &fused_render_forward,
           "tile renderer forward (with depth_key: also the depth and alpha maps; with weight_sum / weight_max / "
@@ -1866,45 +1598,33 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("fused_render_features_backward", &fused_render_features_backward,
           "feature backward: grad_features [N, stride], and the geometry part added into the slab");
     m.def("fused_preprocess_backward", &fused_preprocess_backward,
-          "fused per-gaussian backward (mode: MODE_* bits; filter3d: the forward's, with MODE_FILTER3D)",
+          "fused per-gaussian backward (mode: MODE_* bits; filter3d, lens, lens_consts: the forward's; camera_grads: "
+          "0 none, 1 also d loss / d camera_T_world [4,4], 2 also d loss / d (fx, fy, cx, cy) [4] and d loss / d lens "
+          "coefficients [n])",
           py::arg("slab"), py::arg("xyz"), py::arg("quaternion"), py::arg("scale"), py::arg("opacity_logit"),
           py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"), py::arg("camera_centre"), py::arg("visible"),
           py::arg("out_flat"), py::arg("grad_uv_compact"), py::arg("scan"), py::arg("use_slab_uv"), py::arg("mode"),
-          py::arg("filter3d") = py::none());
+          py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE, py::arg("lens_consts") = py::none(),
+          py::arg("camera_grads") = 0);
     m.def("batch_preprocess_forward", &batch_preprocess_forward,
-          "per-gaussian forward of C views into stacked records / keys / visibility / scans (rasterize_batch)");
+          "per-gaussian forward of C views into stacked records / keys / visibility / scans (rasterize_batch; "
+          "lens_consts [C,n+1])",
+          py::arg("xyz"), py::arg("xyz_camera_frame"), py::arg("quaternion"), py::arg("scale"),
+          py::arg("opacity_logit"), py::arg("rgb_dc"), py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"),
+          py::arg("camera_centre"), py::arg("H"), py::arg("W"), py::arg("near_thresh"), py::arg("far_thresh"),
+          py::arg("cull_mask_padding"), py::arg("mh_dist"), py::arg("depth_base"), py::arg("mode"),
+          py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE, py::arg("lens_consts") = py::none());
     m.def("batch_render_backward", &batch_render_backward,
           "render backward of C views into one stacked gradient slab [C, N*12]");
     m.def("batch_preprocess_backward", &batch_preprocess_backward,
-          "per-gaussian backward of C views in one pass: the gradient summed over the views (gsr_batch)");
-    m.def("fisheye_preprocess_forward", &fisheye_preprocess_forward,
-          "fused_preprocess_forward for an OPENCV_FISHEYE camera (gsr_fisheye_preprocess_forward)");
-    m.def("fisheye_preprocess_backward", &fisheye_preprocess_backward,
-          "fused_preprocess_backward for an OPENCV_FISHEYE camera (gsr_fisheye_preprocess_backward)");
-    m.def("batch_fisheye_preprocess_forward", &batch_fisheye_preprocess_forward,
-          "batch_preprocess_forward for OPENCV_FISHEYE cameras, [C,5] constants");
-    m.def("batch_fisheye_preprocess_backward", &batch_fisheye_preprocess_backward,
-          "batch_preprocess_backward for OPENCV_FISHEYE cameras (gsr_fisheye_batch_preprocess_backward)");
+          "per-gaussian backward of C views in one pass: the gradient summed over the views; the camera gradients "
+          "of fused_preprocess_backward per view, [C,4,4], [C,4] and [C,n]",
+          py::arg("slab"), py::arg("xyz"), py::arg("quaternion"), py::arg("scale"), py::arg("opacity_logit"),
+          py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"), py::arg("camera_centre"), py::arg("visible"),
+          py::arg("out_flat"), py::arg("grad_uv_compact"), py::arg("scan"), py::arg("use_slab_uv"), py::arg("mode"),
+          py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE, py::arg("lens_consts") = py::none(),
+          py::arg("camera_grads") = 0);
     m.def("fisheye_theta_max", &fisheye_theta_max, "the fisheye cull limit of 4 coefficients (gsr_fisheye_theta_max)");
-    m.def("distortion_preprocess_forward", &distortion_preprocess_forward,
-          "fused_preprocess_forward for an OPENCV (radial-tangential) camera (gsr_distortion_preprocess_forward)");
-    m.def("distortion_preprocess_backward", &distortion_preprocess_backward,
-          "fused_preprocess_backward for an OPENCV (radial-tangential) camera (gsr_distortion_preprocess_backward)");
-    m.def("batch_distortion_preprocess_forward", &batch_distortion_preprocess_forward,
-          "batch_preprocess_forward for OPENCV (radial-tangential) cameras, [C,6] constants");
-    m.def("batch_distortion_preprocess_backward", &batch_distortion_preprocess_backward,
-          "batch_preprocess_backward for OPENCV cameras (gsr_distortion_batch_preprocess_backward)");
-    m.def("pose_preprocess_backward", &pose_preprocess_backward,
-          "fused_preprocess_backward plus d loss / d camera_T_world [4,4], any lens (gsr_pose_preprocess_backward)");
-    m.def("batch_pose_preprocess_backward", &batch_pose_preprocess_backward,
-          "batch_preprocess_backward plus d loss / d camera_T_world [C,4,4], any lens "
-          "(gsr_pose_batch_preprocess_backward)");
-    m.def("camera_preprocess_backward", &camera_preprocess_backward,
-          "pose_preprocess_backward plus d loss / d (fx, fy, cx, cy) [4] and d loss / d lens coefficients [n], any "
-          "lens (gsr_camera_preprocess_backward)");
-    m.def("batch_camera_preprocess_backward", &batch_camera_preprocess_backward,
-          "batch_pose_preprocess_backward plus [C,4] intrinsics and [C,n] lens-coefficient gradients, any lens "
-          "(gsr_camera_batch_preprocess_backward)");
     m.def("distortion_r2_max", &distortion_r2_max,
           "the radial fold limit s = r^2 of 5 coefficients k1 k2 p1 p2 k3 (gsr_distortion_r2_max)");
     m.def("filter3d", &filter3d, "Mip-Splatting's 3-D filter size per gaussian from the training cameras (gsr_filter3d)",
@@ -1914,6 +1634,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.attr("MODE_ANTIALIASED") = GSR_MODE_ANTIALIASED;
     m.attr("MODE_ABSGRAD") = GSR_MODE_ABSGRAD;
     m.attr("MODE_FILTER3D") = GSR_MODE_FILTER3D;
+    m.attr("LENS_PINHOLE") = GSR_LENS_PINHOLE;
+    m.attr("LENS_FISHEYE") = GSR_LENS_FISHEYE;
+    m.attr("LENS_DISTORTION") = GSR_LENS_DISTORTION;
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");

@@ -286,7 +286,7 @@ class _ViewState:
         # per-gaussian stages: filter3d [N], a constant)
         self.mode = 0
         self.filter3d = None
-        self.lens = None        # a lens model: (name, its constants on the device) (_lens_constants)
+        self.lens = None        # a lens model: (its LENS_* value, its constants on the device) (_lens_state)
         self.depth = self.alpha = None
         self.uv_absgrad = None  # MODE_ABSGRAD: [M,2], set by every render backward
         self.weight_stats = None  # optional densify.WeightStats the render forward accumulates into
@@ -312,8 +312,9 @@ class _stage:
 
 
 # ---- lens models: fisheye and radial-tangential distortion -------------------------------------------------------------
-# name -> (coefficient names, the native cull limit of one row of coefficients)
-_LENSES = {"fisheye": ("k1 k2 k3 k4", "fisheye_theta_max"), "distortion": ("k1 k2 p1 p2 k3", "distortion_r2_max")}
+# name -> (coefficient names, the native cull limit of one row of coefficients, the native LENS_* value)
+_LENSES = {"fisheye": ("k1 k2 k3 k4", "fisheye_theta_max", "LENS_FISHEYE"),
+           "distortion": ("k1 k2 p1 p2 k3", "distortion_r2_max", "LENS_DISTORTION")}
 
 
 def fisheye_theta_max(k) -> float:
@@ -394,11 +395,17 @@ def _lens_constants(lens, k, device):
     return t
 
 
-def _pose_lens(lens):
-    """(lens enum, constants) of the pose bindings for a state's lens (None: the pinhole)"""
+def _lens_state(lens, device):
+    """state.lens for _lens_arg's result: None (the pinhole), or (the native LENS_* value, its device constants)"""
     if lens is None:
-        return 0, None
-    return (1 if lens[0] == "fisheye" else 2), lens[1]
+        return None
+    return getattr(native(), _LENSES[lens[0]][2]), _lens_constants(*lens, device)
+
+
+def _lens_kwargs(lens):
+    """The lens arguments of the per-gaussian bindings for a state's lens"""
+    lens, consts = lens or (native().LENS_PINHOLE, None)
+    return dict(lens=lens, lens_consts=consts)
 
 
 def _lens_input(fisheye, distortion):
@@ -426,14 +433,18 @@ def _lens_grad(g, k):
     return g.to(k.dtype)
 
 
-def _camera_backward(ctx, native_fn, args, lens, k_input):
-    """The backward with the camera gradients: (gaussian grads..., g_pose or None, g_K or None, g_k or None).  The
+def _preprocess_backward(ctx, native_fn, args):
+    """The per-gaussian backward: (gaussian grads..., flat), g_pose, g_K, g_k (None where no gradient is wanted).  The
     intrinsics or the lens coefficients require grad: the camera-gradient kernels (libgsr_calib.so); only the pose:
-    the pose kernels."""
-    *grads, g_pose, g_intr, g_lens = native_fn(*args, *_pose_lens(lens))
-    g_pose = g_pose if ctx.needs_input_grad[6] else None
-    g_K = _intrinsics_grad(g_intr) if ctx.needs_input_grad[7] else None
-    g_k = _lens_grad(g_lens, k_input) if k_input is not None and ctx.needs_input_grad[10] else None
+    the pose kernels (libgsr_pose.so); neither: the plain kernels."""
+    need = ctx.needs_input_grad
+    camera_grads = 2 if need[7] or need[10] else 1 if need[6] else 0
+    out = native_fn(*args, **_lens_kwargs(ctx.state.lens), camera_grads=camera_grads)
+    n = 6 + ctx.has_sh  # the gaussian gradients and the flat allocation, then the camera gradients
+    grads, cam = out[:n], out[n:]
+    g_pose = cam[0] if need[6] else None
+    g_K = _intrinsics_grad(cam[1]) if need[7] else None
+    g_k = _lens_grad(cam[2], ctx.lens_k) if ctx.lens_k is not None and need[10] else None
     return grads, g_pose, g_K, g_k
 
 
@@ -470,14 +481,9 @@ class _ProjectGaussians(torch.autograd.Function):
                 centre = torch.linalg.inv_ex(camera_T_world)[0][:3, 3].contiguous()
         with _stage(state, "preprocess_fwd"):
             # tile_mask / tile_win: the tiles each gaussian hits, tested once here and only expanded by the pair emission
-            args = (xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
-                    pad, mh, depth_base, True, state.mode, state.filter3d)
-            if state.lens is None:
-                records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(*args)
-            else:
-                lens, consts = state.lens
-                fwd = ext.fisheye_preprocess_forward if lens == "fisheye" else ext.distortion_preprocess_forward
-                records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
+            records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(
+                xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far, pad,
+                mh, depth_base, True, state.mode, state.filter3d, **_lens_kwargs(state.lens))
         # a backward pass can follow (the camera counts: a pose- or intrinsics-only refinement needs the masks too)
         record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or ctx.needs_input_grad[10])
         background = state.background
@@ -582,20 +588,7 @@ class _ProjectGaussians(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            g_pose = g_K = g_k = None
-            if ctx.needs_input_grad[7] or ctx.needs_input_grad[10]:
-                grads, g_pose, g_K, g_k = _camera_backward(ctx, native().camera_preprocess_backward, args, st.lens,
-                                                           ctx.lens_k)
-            elif ctx.needs_input_grad[6]:
-                # the same kernels' arithmetic plus the pose reduction (libgsr_pose.so)
-                *grads, g_pose = native().pose_preprocess_backward(*args, *_pose_lens(st.lens))
-            elif st.lens is None:
-                grads = native().fused_preprocess_backward(*args)
-            else:
-                lens, consts = st.lens
-                ext = native()
-                bwd = ext.fisheye_preprocess_backward if lens == "fisheye" else ext.distortion_preprocess_backward
-                grads = bwd(*args, consts)
+            grads, g_pose, g_K, g_k = _preprocess_backward(ctx, native().fused_preprocess_backward, args)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
@@ -846,7 +839,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
-    state.lens = None if lens is None else (lens[0], _lens_constants(*lens, gaussians.xyz.device))
+    state.lens = _lens_state(lens, gaussians.xyz.device)
     state.weight_stats = weight_stats
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
@@ -936,7 +929,7 @@ class _BatchState:
         self.speculation_overflowed = False
         self.mode = 0
         self.filter3d = None
-        self.lens = None         # a lens model: (name, [C, n+1] constants on the device) (_lens_constants)
+        self.lens = None         # a lens model: (its LENS_* value, [C, n+1] constants on the device) (_lens_state)
         self.views = []
         self.images = self.depth = self.alpha = None
 
@@ -963,15 +956,9 @@ class _ProjectBatch(torch.autograd.Function):
             else:
                 centre = torch.stack([torch.linalg.inv_ex(camera_T_world[c])[0][:3, 3] for c in range(C)])
         with _stage(state, "preprocess_fwd"):
-            args = (xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
-                    pad, mh, depth_base, state.mode, state.filter3d)
-            if state.lens is None:
-                records, zkey, visible, scan, tile_mask, tile_win = ext.batch_preprocess_forward(*args)
-            else:
-                lens, consts = state.lens
-                fwd = (ext.batch_fisheye_preprocess_forward if lens == "fisheye"
-                       else ext.batch_distortion_preprocess_forward)
-                records, zkey, visible, scan, tile_mask, tile_win = fwd(*args, consts)
+            records, zkey, visible, scan, tile_mask, tile_win = ext.batch_preprocess_forward(
+                xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far, pad,
+                mh, depth_base, state.mode, state.filter3d, **_lens_kwargs(state.lens))
         record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or ctx.needs_input_grad[10])
         background = state.background
         depth_mode = bool(state.mode & ext.MODE_DEPTH_ALPHA)
@@ -1075,20 +1062,7 @@ class _ProjectBatch(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            g_pose = g_K = g_k = None
-            if ctx.needs_input_grad[7] or ctx.needs_input_grad[10]:
-                grads, g_pose, g_K, g_k = _camera_backward(ctx, native().batch_camera_preprocess_backward, args,
-                                                           st.lens, ctx.lens_k)
-            elif ctx.needs_input_grad[6]:
-                *grads, g_pose = native().batch_pose_preprocess_backward(*args, *_pose_lens(st.lens))
-            elif st.lens is None:
-                grads = native().batch_preprocess_backward(*args)
-            else:
-                lens, consts = st.lens
-                ext = native()
-                bwd = (ext.batch_fisheye_preprocess_backward if lens == "fisheye"
-                       else ext.batch_distortion_preprocess_backward)
-                grads = bwd(*args, consts)
+            grads, g_pose, g_K, g_k = _preprocess_backward(ctx, native().batch_preprocess_backward, args)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]
@@ -1222,7 +1196,7 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
     state.mode = ((ext.MODE_DEPTH_ALPHA if render_depth_alpha else 0) | (ext.MODE_ANTIALIASED if antialiased else 0)
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
-    state.lens = None if lens is None else (lens[0], _lens_constants(*lens, gaussians.xyz.device))
+    state.lens = _lens_state(lens, gaussians.xyz.device)
     state.background = (background_rgb if background_rgb.dim() == 2 else background_rgb.expand(C, 3)).contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))

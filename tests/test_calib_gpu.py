@@ -156,7 +156,7 @@ def test_pinhole_gauge_identities_at_the_headline_size():
 def test_everything_else_is_bit_identical(lens, opts):
     """The forward's outputs (image, mask, uv, depth / alpha, feature map, weight maxima and pixel counts; the weight
     sums, fp32 atomics, to 1e-5) with K and k requiring grad or not.  The gradients are compared on the same rows in
-    test_camera_kernels_repeat_match_the_pose_kernels_and_the_batch_matches_single_views."""
+    test_camera_grads_2_repeat_match_camera_grads_1_and_the_batch_matches_single_views."""
     sc = scene(3)
     outs, sums = [], []
     for want in (False, True):
@@ -194,14 +194,15 @@ def test_everything_else_is_bit_identical(lens, opts):
 
 # ---- 4. determinism, batching and edge cases ---------------------------------------------------------------------------
 def _lens_args(st, c=None):
+    """The lens keyword arguments of the per-gaussian bindings for a state's lens, view c's constants alone for c"""
     if st.lens is None:
-        return 0, None
-    consts = st.lens[1]
-    return (1 if st.lens[0] == "fisheye" else 2), (consts if c is None else consts[c:c + 1].contiguous())
+        return dict(lens=native().LENS_PINHOLE, lens_consts=None)
+    enum, consts = st.lens
+    return dict(lens=enum, lens_consts=consts if c is None else consts[c:c + 1].contiguous())
 
 
 @pytest.mark.parametrize("lens", LENSES)
-def test_camera_kernels_repeat_match_the_pose_kernels_and_the_batch_matches_single_views(lens):
+def test_camera_grads_2_repeat_match_camera_grads_1_and_the_batch_matches_single_views(lens):
     """On the same rows: two calls give the same bits; the gaussian gradients and the pose gradient equal the pose
     kernels' bit for bit; batched view c equals the single-view call on view c's rows; the rasterize_batch gradients
     are the binding's (a shared K: the sum over the views)."""
@@ -224,14 +225,14 @@ def test_camera_kernels_repeat_match_the_pose_kernels_and_the_batch_matches_sing
     Kd = K.detach()
     Ks = Kd.expand(C, 3, 3).contiguous()
     centre = torch.stack([ext.camera_centre(Td[c]) for c in range(C)])
-    enum, consts = _lens_args(st)
+    lk = _lens_args(st)
     args = (slab, xyz, q, s, o.reshape(-1), sh, Td, Ks, centre, st.visible, None, None, None, True, st.mode,
             flags.get("filter3d"))
-    a = ext.batch_camera_preprocess_backward(*args, enum, consts)
-    b = ext.batch_camera_preprocess_backward(*args, enum, consts)
+    a = ext.batch_preprocess_backward(*args, **lk, camera_grads=2)
+    b = ext.batch_preprocess_backward(*args, **lk, camera_grads=2)
     for x, y in zip(a, b):
         assert np.array_equal(bits(x), bits(y))
-    pose = ext.batch_pose_preprocess_backward(*args, enum, consts)
+    pose = ext.batch_preprocess_backward(*args, **lk, camera_grads=1)
     assert len(a) == len(pose) + 2
     for x, y in zip(a[:len(pose)], pose):  # gaussian gradients, the flat allocation and g_pose
         assert np.array_equal(bits(x), bits(y))
@@ -242,41 +243,38 @@ def test_camera_kernels_repeat_match_the_pose_kernels_and_the_batch_matches_sing
     if k is not None:
         assert torch.equal(k.grad, g_lens.cpu().double().sum(0).float())
     for c in range(C):
-        e, cc = _lens_args(st, c)
-        single = ext.camera_preprocess_backward(slab.view(C, -1)[c].contiguous(), xyz, q, s, o.reshape(-1), sh,
-                                                Td[c].contiguous(), Kd, centre[c].contiguous(),
-                                                st.visible[c].contiguous(), None, None, None, True, st.mode,
-                                                flags.get("filter3d"), e, cc)
+        one = (slab.view(C, -1)[c].contiguous(), xyz, q, s, o.reshape(-1), sh, Td[c].contiguous(), Kd,
+               centre[c].contiguous(), st.visible[c].contiguous(), None, None, None, True, st.mode,
+               flags.get("filter3d"))
+        single = ext.fused_preprocess_backward(*one, **_lens_args(st, c), camera_grads=2)
         assert np.array_equal(bits(single[-3]), bits(g_pose[c])), c
         assert np.array_equal(bits(single[-2]), bits(g_intr[c])), c
         assert np.array_equal(bits(single[-1]), bits(g_lens[c])), c
-        pose1 = ext.pose_preprocess_backward(slab.view(C, -1)[c].contiguous(), xyz, q, s, o.reshape(-1), sh,
-                                             Td[c].contiguous(), Kd, centre[c].contiguous(),
-                                             st.visible[c].contiguous(), None, None, None, True, st.mode,
-                                             flags.get("filter3d"), e, cc)
+        pose1 = ext.fused_preprocess_backward(*one, **_lens_args(st, c), camera_grads=1)
         for x, y in zip(single[:len(pose1)], pose1):
             assert np.array_equal(bits(x), bits(y)), c
 
 
 @pytest.mark.parametrize("lens", LENSES)
-def test_empty_scene_and_all_culled_give_zero(lens):
+def test_camera_grads_of_empty_and_all_culled_scenes_are_zero(lens):
     sc = scene(0)
     K = to_t(sc["K"])
     ext = native()
     z = lambda *shape: torch.zeros(shape, device=dev())  # noqa: E731
-    enum = LENSES.index(lens)
+    enum = getattr(ext, "LENS_" + lens.upper())
     lc = None
     if lens != "pinhole":
         lim = (ext.fisheye_theta_max if lens == "fisheye" else ext.distortion_r2_max)(list(LENS_K[lens]))
         lc = to_t(np.array(list(LENS_K[lens]) + [lim], np.float32))
     args = (z(0), z(0, 3), z(0, 4), z(0, 3), z(0), None, to_t(sc["T"]), K, None,
             torch.zeros(0, dtype=torch.uint8, device=dev()), None, None, None, True, 0, None)
-    for t in ext.camera_preprocess_backward(*args, enum, lc)[-3:]:
+    for t in ext.fused_preprocess_backward(*args, lens=enum, lens_consts=lc, camera_grads=2)[-3:]:
         assert (t == 0).all()
     T2 = to_t(np.stack([sc["T"], sc["T"]]))
     args = (z(0),) + args[1:6] + (T2, K.expand(2, 3, 3).contiguous(), None,
                                   torch.zeros(2, 0, dtype=torch.uint8, device=dev())) + args[10:]
-    outs = ext.batch_camera_preprocess_backward(*args, enum, None if lc is None else torch.cat([lc, lc]))[-3:]
+    outs = ext.batch_preprocess_backward(*args, lens=enum, lens_consts=None if lc is None else torch.cat([lc, lc]),
+                                         camera_grads=2)[-3:]
     assert tuple(outs[1].shape) == (2, 4)
     for t in outs:
         assert (t == 0).all()
@@ -290,6 +288,40 @@ def test_empty_scene_and_all_culled_give_zero(lens):
     assert bool(out[1].all())
     out[0].sum().backward()
     assert (Kg.grad == 0).all() and (k is None or (k.grad == 0).all())
+
+
+def test_lens_and_camera_grads_arguments_reject_bad_values():
+    """The per-gaussian bindings raise for an unknown lens, a lens without its constants (or the pinhole with some) and
+    camera_grads outside 0..2, one view and a batch, forward and backward."""
+    sc = scene(0)
+    ext = native()
+    z = lambda *shape: torch.zeros(shape, device=dev())  # noqa: E731
+    T, K = to_t(sc["T"]), to_t(sc["K"])
+    T2, K2 = T.expand(2, 4, 4).contiguous(), K.expand(2, 3, 3).contiguous()
+    lc = to_t(np.array(list(LENS_K["fisheye"]) + [ext.fisheye_theta_max(list(LENS_K["fisheye"]))], np.float32))
+    gauss = (z(0, 3), None, z(0, 4), z(0, 3), z(0), z(0, 3), None)
+    cfg = (None, sc["H"], sc["W"], 0.3, 500.0, 100.0, 3.0, 0)
+    fwds = (lambda **kw: ext.fused_preprocess_forward(*gauss, T, K, *cfg, True, 0, None, **kw),
+            lambda **kw: ext.batch_preprocess_forward(*gauss, T2, K2, *cfg, 0, None, **kw))
+    tail = (None, None, None, True, 0, None)
+    bwds = (lambda **kw: ext.fused_preprocess_backward(z(0), z(0, 3), z(0, 4), z(0, 3), z(0), None, T, K, None,
+                                                       torch.zeros(0, dtype=torch.uint8, device=dev()), *tail, **kw),
+            lambda **kw: ext.batch_preprocess_backward(z(0), z(0, 3), z(0, 4), z(0, 3), z(0), None, T2, K2, None,
+                                                       torch.zeros(2, 0, dtype=torch.uint8, device=dev()), *tail,
+                                                       **kw))
+    for fn in fwds + bwds:
+        for lens in (-1, 3):
+            with pytest.raises(RuntimeError, match="lens must be 0"):
+                fn(lens=lens)
+        with pytest.raises(RuntimeError, match="a lens needs its constants"):
+            fn(lens=ext.LENS_FISHEYE)
+        with pytest.raises(RuntimeError, match="the pinhole takes no lens constants"):
+            fn(lens=ext.LENS_PINHOLE, lens_consts=lc)
+    for fn in bwds:
+        for camera_grads in (-1, 3):
+            with pytest.raises(RuntimeError, match="camera_grads must be 0"):
+                fn(camera_grads=camera_grads)
+        assert len(fn(camera_grads=2)) == 6 + 3  # the valid values still run: flat and the camera gradients
 
 
 @pytest.mark.parametrize("lens", LENSES)

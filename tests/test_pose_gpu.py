@@ -194,7 +194,7 @@ def test_everything_else_is_bit_identical(lens, opts):
     """The forward's outputs (image, mask, uv, depth / alpha, feature map, weight maxima and pixel counts; the weight
     sums, fp32 atomics, to 1e-5) with the pose requiring grad or not.  The gradients come from the render backward's rows, which use atomics and so need not repeat bit for
     bit between two steps; they are compared on the same rows in
-    test_pose_reduction_is_deterministic_and_the_batch_matches_single_views."""
+    test_pose_camera_grads_are_deterministic_and_the_batch_matches_single_views."""
     sc = scene(3)
     outs, sums = [], []
     for pose_grad in (False, True):
@@ -259,14 +259,15 @@ def test_batched_everything_else_is_bit_identical(lens):
 
 # ---- 4. determinism and edge cases -----------------------------------------------------------------------------------
 def _lens_args(st, c=None):
+    """The lens keyword arguments of the per-gaussian bindings for a state's lens, view c's constants alone for c"""
     if st.lens is None:
-        return 0, None
-    consts = st.lens[1]
-    return (1 if st.lens[0] == "fisheye" else 2), (consts if c is None else consts[c:c + 1].contiguous())
+        return dict(lens=native().LENS_PINHOLE, lens_consts=None)
+    enum, consts = st.lens
+    return dict(lens=enum, lens_consts=consts if c is None else consts[c:c + 1].contiguous())
 
 
 @pytest.mark.parametrize("lens", po.LENSES)
-def test_pose_reduction_is_deterministic_and_the_batch_matches_single_views(lens):
+def test_pose_camera_grads_are_deterministic_and_the_batch_matches_single_views(lens):
     ext = native()
     C = 3
     scs = [scenes.np_scene(5000, "tiny", 3, view=c, sigma_px=(0.8, 0.8, 0.15, 8.0)) for c in range(C)]
@@ -285,37 +286,30 @@ def test_pose_reduction_is_deterministic_and_the_batch_matches_single_views(lens
     Td = T.detach().contiguous()
     Ks = K.expand(C, 3, 3).contiguous()
     centre = torch.stack([ext.camera_centre(Td[c]) for c in range(C)])
-    enum, consts = _lens_args(st)
+    lk = _lens_args(st)
     args = (slab, xyz, q, s, o.reshape(-1), sh, Td, Ks, centre, st.visible, None, None, None, True, st.mode,
             flags.get("filter3d"))
-    a = ext.batch_pose_preprocess_backward(*args, enum, consts)[-1]
-    b = ext.batch_pose_preprocess_backward(*args, enum, consts)[-1]
+    a = ext.batch_preprocess_backward(*args, **lk, camera_grads=1)[-1]
+    b = ext.batch_preprocess_backward(*args, **lk, camera_grads=1)[-1]
     assert np.array_equal(bits(a), bits(b))
     assert np.array_equal(bits(a), bits(T.grad))
     for c in range(C):
-        e, cc = _lens_args(st, c)
-        single = ext.pose_preprocess_backward(slab.view(C, -1)[c].contiguous(), xyz, q, s, o.reshape(-1), sh,
-                                              Td[c].contiguous(), K, centre[c].contiguous(),
-                                              st.visible[c].contiguous(), None, None, None, True, st.mode,
-                                              flags.get("filter3d"), e, cc)
+        one = (slab.view(C, -1)[c].contiguous(), xyz, q, s, o.reshape(-1), sh, Td[c].contiguous(), K,
+               centre[c].contiguous(), st.visible[c].contiguous(), None, None, None, True, st.mode,
+               flags.get("filter3d"))
+        single = ext.fused_preprocess_backward(*one, **_lens_args(st, c), camera_grads=1)
         assert np.array_equal(bits(single[-1]), bits(a[c])), c
         # the gaussian gradients of the pose kernel are the plain kernel's, bit for bit
-        plain_fn = {"pinhole": ext.fused_preprocess_backward, "fisheye": ext.fisheye_preprocess_backward,
-                    "distortion": ext.distortion_preprocess_backward}[lens]
-        plain = plain_fn(slab.view(C, -1)[c].contiguous(), xyz, q, s, o.reshape(-1), sh, Td[c].contiguous(), K,
-                         centre[c].contiguous(), st.visible[c].contiguous(), None, None, None, True, st.mode,
-                         flags.get("filter3d"), *(() if cc is None else (cc,)))
+        plain = ext.fused_preprocess_backward(*one, **_lens_args(st, c))
         assert np.array_equal(bits(plain[-1]), bits(single[-2])), c
-    plain_fn = {"pinhole": ext.batch_preprocess_backward, "fisheye": ext.batch_fisheye_preprocess_backward,
-                "distortion": ext.batch_distortion_preprocess_backward}[lens]
-    plain = plain_fn(*args, *(() if consts is None else (consts,)))
-    pose = ext.batch_pose_preprocess_backward(*args, enum, consts)
+    plain = ext.batch_preprocess_backward(*args, **lk)
+    pose = ext.batch_preprocess_backward(*args, **lk, camera_grads=1)
     assert np.array_equal(bits(plain[-1]), bits(pose[-2]))
     assert N == xyz.shape[0]
 
 
 @pytest.mark.parametrize("lens", po.LENSES)
-def test_empty_scene_and_all_culled_give_zero(lens):
+def test_pose_camera_grads_of_empty_and_all_culled_scenes_are_zero(lens):
     sc = scene(0)
     K = to_t(sc["K"])
     # empty: the bindings directly (the render stage has nothing to run), one view and a batch of two
@@ -323,16 +317,17 @@ def test_empty_scene_and_all_culled_give_zero(lens):
     z = lambda *shape: torch.zeros(shape, device=dev())  # noqa: E731
     consts = None if lens == "pinhole" else (ext.fisheye_theta_max(list(LENS_K[lens])) if lens == "fisheye"
                                              else ext.distortion_r2_max(list(LENS_K[lens])))
-    enum = po.LENSES.index(lens)
+    enum = getattr(ext, "LENS_" + lens.upper())
     lc = None if consts is None else to_t(np.array(list(LENS_K[lens]) + [consts], np.float32))
     args = (z(0), z(0, 3), z(0, 4), z(0, 3), z(0), None, to_t(sc["T"]), K, None,
             torch.zeros(0, dtype=torch.uint8, device=dev()), None, None, None, True, 0, None)
-    g = ext.pose_preprocess_backward(*args, enum, lc)[-1]
+    g = ext.fused_preprocess_backward(*args, lens=enum, lens_consts=lc, camera_grads=1)[-1]
     assert tuple(g.shape) == (4, 4) and (g == 0).all()
     T2 = to_t(np.stack([sc["T"], sc["T"]]))
     args = (z(0),) + args[1:6] + (T2, K.expand(2, 3, 3).contiguous(), None,
                                   torch.zeros(2, 0, dtype=torch.uint8, device=dev())) + args[10:]
-    g = ext.batch_pose_preprocess_backward(*args, enum, None if lc is None else torch.cat([lc, lc]))[-1]
+    g = ext.batch_preprocess_backward(*args, lens=enum, lens_consts=None if lc is None else torch.cat([lc, lc]),
+                                      camera_grads=1)[-1]
     assert tuple(g.shape) == (2, 4, 4) and (g == 0).all()
     # every gaussian behind the camera
     sc2 = dict(sc)
