@@ -10,11 +10,13 @@
   libgsr_pose.so            the per-gaussian backward with the camera pose gradient, every lens (include/gsr_pose.h)
   libgsr_calib.so           the same sources compiled with the pose, intrinsics and lens-coefficient gradients
                             (include/gsr_calib.h)
+  libgsr_shutter.so         the per-gaussian stages for rolling-shutter cameras, every lens, with the pose and
+                            readout-motion gradients (include/gsr_shutter.h)
   libgsr_bilagrid.so        bilateral-grid appearance correction: slice forward / backward, total variation
                             (include/gsr_bilagrid.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all ten (the CUDA libraries from the LIBS table);
+`python -m gaussian_splatting_b200.build` builds all eleven (the CUDA libraries from the LIBS table);
 `build(force=False)` is incremental.
 """
 from __future__ import annotations
@@ -60,7 +62,7 @@ CUH = [h for h in HEADERS if h.suffix == ".cuh"]
 # The sources of a library are file names, or (file name, object stem, extra nvcc flags) for a file compiled more
 # than once.  gsr_lens.cu is compiled once per lens model (GSR_LENS: 1 fisheye, 2 distortion), gsr_pose.cu once per
 # camera model (GSR_POSE_LENS: 0 pinhole, 1 fisheye, 2 distortion), and again with GSR_POSE_CAMERA for libgsr_calib.so
-# (the camera-gradient kernels).
+# (the camera-gradient kernels); gsr_shutter.cu once per camera model (GSR_SHUTTER_LENS).
 LENS_HEADERS = CUH + [CSRC / "gsr_fisheye.cuh", CSRC / "gsr_distortion.cuh", CSRC / "gsr_poly_roots.h",
                       ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_fisheye.h",
                       ROOT / "include" / "gsr_distortion.h"]
@@ -88,6 +90,8 @@ LIBS = [
     (PKG / "libgsr_calib.so",
      [("gsr_pose.cu", f"gsr_camera_{i}", [f"-DGSR_POSE_LENS={i}", "-DGSR_POSE_CAMERA"]) for i in range(3)],
      POSE_HEADERS, "calib_lib.sha256"),
+    (PKG / "libgsr_shutter.so", [("gsr_shutter.cu", f"gsr_shutter_{i}", [f"-DGSR_SHUTTER_LENS={i}"]) for i in range(3)],
+     POSE_HEADERS + [CSRC / "gsr_shutter.cuh", ROOT / "include" / "gsr_shutter.h"], "shutter_lib.sha256"),
     (PKG / "libgsr_bilagrid.so", ["gsr_bilagrid.cu"],
      [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_bilagrid.h"],
      "bilagrid_lib.sha256"),
@@ -168,7 +172,7 @@ def build_ext(force: bool = False) -> Path:
                     ROOT / "include" / "gsr_features.h", ROOT / "include" / "gsr_batch.h",
                     ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h",
                     ROOT / "include" / "gsr_pose.h", ROOT / "include" / "gsr_bilagrid.h",
-                    ROOT / "include" / "gsr_calib.h"], torch.__version__)
+                    ROOT / "include" / "gsr_calib.h", ROOT / "include" / "gsr_shutter.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -180,7 +184,7 @@ def build_ext(force: bool = False) -> Path:
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
         f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", "-lgsr_fisheye",
-        "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid", "-lgsr_calib",
+        "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid", "-lgsr_calib", "-lgsr_shutter",
         f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",

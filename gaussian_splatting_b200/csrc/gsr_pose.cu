@@ -195,38 +195,6 @@ GSR_POSE_LAUNCH_DECL(GSR_LAUNCH_DISTORTION);
 
 namespace gsr {
 
-constexpr int POSE_FINISH_THREADS = 256;
-
-// Whole CTA of POSE_FINISH_THREADS, one view: thread t adds the partials t, t + 256, ... of src [nblk, NV] in fp64,
-// then a shuffle tree per warp leaves the warps' sums in s_sum; ends with a CTA barrier.  The caller adds the warps in
-// order and rounds once.
-template <int NV>
-__device__ __forceinline__ void finish_partials(int nblk, const float* __restrict__ src, double (*s_sum)[NV]) {
-    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-    double acc[NV];
-#pragma unroll
-    for (int k = 0; k < NV; ++k) acc[k] = 0.0;
-    for (int b = t; b < nblk; b += POSE_FINISH_THREADS) {
-        const float4* row = reinterpret_cast<const float4*>(src + (size_t)b * NV);
-#pragma unroll
-        for (int q = 0; q < NV / 4; ++q) {
-            const float4 v = row[q];
-            acc[4 * q + 0] += (double)v.x;
-            acc[4 * q + 1] += (double)v.y;
-            acc[4 * q + 2] += (double)v.z;
-            acc[4 * q + 3] += (double)v.w;
-        }
-    }
-#pragma unroll
-    for (int k = 0; k < NV; ++k) {
-        double v = acc[k];
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) v += __shfl_down_sync(0xffffffffu, v, off);
-        if (lane == 0) s_sum[warp][k] = v;
-    }
-    __syncthreads();
-}
-
 #ifndef GSR_POSE_CAMERA
 // one CTA per view: the fixed-order fp64 sum of the view's partials, rounded once.  Writes the view's [4, 4] gradient,
 // the last row 0.

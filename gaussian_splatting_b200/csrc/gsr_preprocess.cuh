@@ -1,6 +1,7 @@
 // gsr_preprocess.cuh — the per-Gaussian stages of the fused path and the view constants they read, shared by the
 // single-view kernels (gsr_preprocess.cu, libgsr_b200.so), the multi-view kernels (gsr_batch.cu, libgsr_batch.so)
-// the lens kernels (gsr_lens.cu) and the pose-gradient kernels (gsr_pose.cu).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian;
+// the lens kernels (gsr_lens.cu), the pose-gradient kernels (gsr_pose.cu) and the rolling-shutter kernels
+// (gsr_shutter.cu).  GSR_PRE_BWD_VIEW is one view's VJP for one gaussian;
 // the single-view kernels store its result, the batched kernels add it up over the views.  The camera model enters
 // only through the GSR_PROJECT / GSR_JACOBIAN hooks below.
 #pragma once
@@ -140,6 +141,29 @@ __device__ __forceinline__ void coop_copy(float* __restrict__ dst, const float* 
 #define GSR_POSE_REDUCE(view)
 #endif
 
+// Rolling-shutter hooks, empty by default: every kernel that does not define GSR_SHUTTER_HOOKS keeps its instructions.
+// gsr_shutter.cuh defines them (gsr_shutter.cu, libgsr_shutter.so).
+//   GSR_SHUTTER_PARAM           extra trailing parameters of the bodies (after GSR_VIEW_PARAM)
+//   GSR_SHUTTER_LOAD(view)      per-thread shutter constants of view `view`, after GSR_LOAD_VIEW
+//   GSR_SHUTTER_POINT(px, py, pz)  replaces the camera-frame mean p0 by p(tau*), the mean at its own line's time
+//   GSR_SHUTTER_CULL            extra `| (...)` terms of the forward's cull
+//   GSR_SHUTTER_W(W)            W <- W(tau*), once W holds the rotation of camera_T_world
+//   GSR_SHUTTER_JACOBIAN(J)     after GSR_JACOBIAN: forms the Jacobian the covariance uses, GSR_SHUTTER_J
+//   GSR_SHUTTER_J               that Jacobian (J: the lens's)
+//   GSR_SHUTTER_BWD_J(gJ)       after conic_bwd: gJ <- the gradient on the lens's J
+//   GSR_SHUTTER_GP(gp)          once gp holds the gradient on p: adds the terms of the shutter time
+#ifndef GSR_SHUTTER_HOOKS
+#define GSR_SHUTTER_PARAM
+#define GSR_SHUTTER_LOAD(view)
+#define GSR_SHUTTER_POINT(px, py, pz)
+#define GSR_SHUTTER_CULL
+#define GSR_SHUTTER_W(W)
+#define GSR_SHUTTER_JACOBIAN(J)
+#define GSR_SHUTTER_J J
+#define GSR_SHUTTER_BWD_J(gJ)
+#define GSR_SHUTTER_GP(gp)
+#endif
+
 // One view's fused VJP for one visible gaussian, as a statement block: it reads the view constants `vc`, the
 // parameters x y z qw qx qy qz s0 s1 s2 opl (f: the 3-D filter) and the view's gradient row (grv rgb, gov opacity,
 // guv uv, gcv conic, gzc camera-frame z; gov and gcv are modified) and assigns gx gq gs go gdc and the SH rest
@@ -157,6 +181,7 @@ __device__ __forceinline__ void coop_copy(float* __restrict__ dst, const float* 
     {                                                                                                                    \
         float px, py, pz;                                                                                                \
         transform_point<float>(vc.T, x, y, z, px, py, pz);                                                               \
+        GSR_SHUTTER_POINT(px, py, pz)                                                                                    \
         float S6[6], S9[9], J[6], W[9];                                                                                  \
         /* 3-D filter: the forward's variances and opacity factor, re-formed (gsr_record.cuh f3d_filter) */              \
         float e[3], v[3], vp[3], t[3], F = 0.f, coef = 1.f;                                                              \
@@ -172,9 +197,11 @@ _Pragma("unroll")                                                               
         }                                                                                                                \
         sym6_to_full(S6, S9);                                                                                            \
         GSR_JACOBIAN(px, py, pz, J);                                                                                     \
+        GSR_SHUTTER_JACOBIAN(J)                                                                                          \
         W[0] = vc.T[0]; W[1] = vc.T[1]; W[2] = vc.T[2];                                                                  \
         W[3] = vc.T[4]; W[4] = vc.T[5]; W[5] = vc.T[6];                                                                  \
         W[6] = vc.T[8]; W[7] = vc.T[9]; W[8] = vc.T[10];                                                                 \
+        GSR_SHUTTER_W(W)                                                                                                 \
                                                                                                                          \
         float rho = 1.0f;                                                                                                \
         if (ANTIALIAS) {                                                                                                 \
@@ -185,7 +212,7 @@ _Pragma("unroll")                                                               
             /* (c2 - rho^2 C = (c2 C + bh^2) / (4 det), 1 - rho^2 = (A + C - 1/4) / (4 det)).  Where rho == 0 the */     \
             /* gradient is infinite but the splat never contributed (g' == 0): no gradient goes through rho there. */    \
             float cn[3];                                                                                                 \
-            conic_from<float>(S9, J, W, cn, nullptr);                                                                    \
+            conic_from<float>(S9, GSR_SHUTTER_J, W, cn, nullptr);                                                        \
             rho = aa_rho(cn[0], cn[1], cn[2]);                                                                           \
             const float A = cn[0] + 0.25f, C = cn[2] + 0.25f, bh = 0.5f * cn[1];                                         \
             const float rd = 1.0f / (A * C - bh * bh);                                                                   \
@@ -198,7 +225,8 @@ _Pragma("unroll")                                                               
         }                                                                                                                \
         const float gc[3] = {gcv[0], gcv[1], gcv[2]};                                                                    \
         float gS[9], gJ[6];                                                                                              \
-        conic_bwd<float>(S9, J, W, gc, gS, gJ);                                                                          \
+        conic_bwd<float>(S9, GSR_SHUTTER_J, W, gc, gS, gJ);                                                              \
+        GSR_SHUTTER_BWD_J(gJ)                                                                                            \
         if (FILTER3D) {                                                                                                  \
             sigma_world_bwd_f3d<float>(qw, qx, qy, qz, e, v, vp, F, gS, gq, gs);                                         \
         } else {                                                                                                         \
@@ -209,6 +237,7 @@ _Pragma("unroll")                                                               
         GSR_PROJECT_BWD(px, py, pz, guv[0], guv[1], gp_uv);                                                              \
         float gp[3] = {gp_j[0] + gp_uv[0], gp_j[1] + gp_uv[1], gp_j[2] + gp_uv[2]};                                      \
         if (DEPTH) gp[2] += gzc;                                                                                         \
+        GSR_SHUTTER_GP(gp)                                                                                               \
         GSR_POSE_VIEW                                                                                                    \
         /* xyz_cam = W xyz + t  =>  grad_xyz = W^T grad_xyz_cam */                                                       \
 _Pragma("unroll")                                                                                                        \
@@ -256,7 +285,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
                      const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
                      float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa,
                      float* __restrict__ o_dc, float* __restrict__ o_sh, int use_tma,
-                     const float* __restrict__ filter3d GSR_VIEW_PARAM GSR_POSE_PARAM) {
+                     const float* __restrict__ filter3d GSR_VIEW_PARAM GSR_SHUTTER_PARAM GSR_POSE_PARAM) {
     constexpr int NR = N_SH - 1;
     constexpr int NR3 = HAS_SH ? 3 * NR : 1;
     // all outputs of the CTA's 128 gaussians are staged in shared memory and leave as six bulk stores
@@ -313,6 +342,7 @@ __device__ __forceinline__ void preprocess_bwd(int N, const float* __restrict__ 
         }
     }
     GSR_LOAD_VIEW(Tdev, Kdev, camdev, 0);
+    GSR_SHUTTER_LOAD(0)
     if (vis) GSR_PRE_BWD_VIEW else if (HAS_SH) {
 #pragma unroll
         for (int k = 0; k < NR3; ++k) my_sh[k] = 0.f;
@@ -383,7 +413,7 @@ __device__ __forceinline__ void sh_rgb_fused(const float* __restrict__ dc, const
 // FILTER3D: Mip-Splatting's 3-D filter, f = filter3d[i]: Sigma_world is formed from the variances exp(s)^2 + f^2 and
 // the opacity is multiplied by coef before rho (gsr_record.cuh f3d_filter)
 template <int N_SH, bool HAS_SH, bool ANTIALIAS, bool FILTER3D>
-__device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* __restrict__ filter3d GSR_VIEW_PARAM) {
+__device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* __restrict__ filter3d GSR_VIEW_PARAM GSR_SHUTTER_PARAM) {
     constexpr int NR3 = HAS_SH ? 3 * (N_SH - 1) : 1;
     __shared__ ViewConsts vc;
     GSR_VIEW_DECL
@@ -415,6 +445,7 @@ __device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* 
         dc0 = rgb_dc[i * 3 + 0]; dc1 = rgb_dc[i * 3 + 1]; dc2 = rgb_dc[i * 3 + 2];
     }
     GSR_LOAD_VIEW(Tdev, Kdev, camdev, 0);
+    GSR_SHUTTER_LOAD(0)
     float rec[REC];
 #pragma unroll
     for (int k = 0; k < REC; ++k) rec[k] = 0.0f;
@@ -426,10 +457,11 @@ __device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* 
         } else {
             transform_point<float>(vc.T, x, y, z, px, py, pz);
         }
+        GSR_SHUTTER_POINT(px, py, pz)
         GSR_PROJECT(px, py, pz, u, v);
         // splat_py/rasterize.py:38-49 (strict compares, fp32)
         const bool culled = (pz < near_t) | (pz > far_t) | (u < -pad) | (u > width + pad) | (v < -pad) |
-                            (v > height + pad) GSR_CULL_MORE;
+                            (v > height + pad) GSR_CULL_MORE GSR_SHUTTER_CULL;
         // visible => pz >= near > 0: float bits are monotone, and relative to bits(near) only a few low
         // bits are significant (shorter radix sort)
         zkey[i] = depth_base ? (__float_as_uint(pz) - depth_base) : depth_key(pz);
@@ -453,10 +485,12 @@ __device__ __forceinline__ void preprocess_fwd(GSR_PRE_FWD_PARAMS, const float* 
             }
             sym6_to_full(S6, S9);
             GSR_JACOBIAN(px, py, pz, J);
+            GSR_SHUTTER_JACOBIAN(J)
             W[0] = vc.T[0]; W[1] = vc.T[1]; W[2] = vc.T[2];
             W[3] = vc.T[4]; W[4] = vc.T[5]; W[5] = vc.T[6];
             W[6] = vc.T[8]; W[7] = vc.T[9]; W[8] = vc.T[10];
-            conic_from<float>(S9, J, W, conic, nullptr);
+            GSR_SHUTTER_W(W)
+            conic_from<float>(S9, GSR_SHUTTER_J, W, conic, nullptr);
 
             float opa = sigmoid_torch(opl);
             if (FILTER3D) opa = __fmul_rn(opa, coef);
@@ -536,7 +570,7 @@ __device__ __forceinline__ void batch_preprocess_bwd(
     const float* __restrict__ camdev, const uint8_t* __restrict__ visible, const float* __restrict__ g_rows,
     int rows_uv, const float* __restrict__ g_uv_compact, const uint64_t* __restrict__ scan, float* __restrict__ o_xyz,
     float* __restrict__ o_quat, float* __restrict__ o_scale, float* __restrict__ o_opa, float* __restrict__ o_dc,
-    float* __restrict__ o_sh, int use_tma, const float* __restrict__ filter3d GSR_VIEW_PARAM GSR_POSE_PARAM) {
+    float* __restrict__ o_sh, int use_tma, const float* __restrict__ filter3d GSR_VIEW_PARAM GSR_SHUTTER_PARAM GSR_POSE_PARAM) {
     constexpr int NR = N_SH - 1;
     constexpr int NR3 = HAS_SH ? 3 * NR : 1;
     __shared__ ViewConsts vc;
@@ -602,6 +636,7 @@ __device__ __forceinline__ void batch_preprocess_bwd(
         if (g_uv_compact != nullptr) uv_base += (size_t)(scan[(size_t)c * N + N - 1] >> 32);
         if (c > 0) __syncthreads();  // every thread is done with the previous view's constants
         GSR_LOAD_VIEW(Tdev + 16 * c, Kdev + 9 * c, camdev != nullptr ? camdev + 3 * c : nullptr, c);
+        GSR_SHUTTER_LOAD(c)
         if (vis) {
             float gx[3], gq[4], gs[3], go, gdc[3], v_sh[NR3];
             float* my_sh = v_sh;

@@ -19,6 +19,7 @@
 #include "../../include/gsr_pose.h"
 #include "../../include/gsr_calib.h"
 #include "../../include/gsr_bilagrid.h"
+#include "../../include/gsr_shutter.h"
 
 namespace {
 
@@ -490,19 +491,33 @@ static int64_t check_views(bool batched, const torch::Tensor& camera_T_world, co
     return C;
 }
 
+// Rolling-shutter twists xi of C views (gsr_shutter.h): fp32 [6] for one view, [C,6] for C views, on xyz's device; or
+// NULL (a global shutter)
+static const float* shutter_ptr(const c10::optional<torch::Tensor>& xi, int64_t C, bool batched,
+                                const torch::Tensor& xyz) {
+    if (!xi.has_value()) return nullptr;
+    const torch::Tensor& t = *xi;
+    CHECK_VALID_INPUT(t); CHECK_FLOAT_TENSOR(t);
+    TORCH_CHECK(batched ? (t.dim() == 2 && t.size(0) == C && t.size(1) == 6) : (t.dim() == 1 && t.size(0) == 6),
+                batched ? "rolling_shutter must have shape Cx6" : "rolling_shutter must have shape 6");
+    TORCH_CHECK(t.device() == xyz.device(), "rolling_shutter must be on the gaussians' device");
+    return t.data_ptr<float>();
+}
+
 // The per-gaussian forward (gsr_preprocess_forward, or the lens's: lens a GSR_LENS_* value, lc its constants [C, n+1]).
 // One view (batched false): returns [records [N,12], depth_key [N] i32-viewed u32, visible [N] u8, scan [N]
 // i64-viewed u64] and, with_tiles, also [tile_mask [N] i64-viewed u64, tile_win [N] i32-viewed u32].  C views
 // (batched, camera_T_world [C,4,4], K [C,3,3]): the single-view forward of every view into the same outputs with a
 // leading view dimension, each view's own packed inclusive scan; xyz_camera_frame [C,R,3] holds the camera-frame
-// positions of the LAST R gaussians of every view, camera_centre [C,3].  mode: GSR_MODE_* bits.
+// positions of the LAST R gaussians of every view, camera_centre [C,3].  mode: GSR_MODE_* bits.  shutter: the views'
+// rolling-shutter twists ([6] / [C,6], gsr_shutter_preprocess_forward with `readout`), or none.
 static std::vector<torch::Tensor> preprocess_forward(
     bool batched, torch::Tensor xyz, c10::optional<torch::Tensor> xyz_camera_frame, torch::Tensor quaternion,
     torch::Tensor scale, torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
     bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, int64_t lens,
-    c10::optional<torch::Tensor> lc) {
+    c10::optional<torch::Tensor> lc, c10::optional<torch::Tensor> shutter, int64_t readout) {
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(rgb_dc);
     CHECK_FLOAT_TENSOR(xyz); CHECK_FLOAT_TENSOR(quaternion); CHECK_FLOAT_TENSOR(scale);
@@ -545,6 +560,8 @@ static std::vector<torch::Tensor> preprocess_forward(
     }
     const float* f3d = filter3d_ptr(filter3d, N);
     const float* lens_consts = lens_ptr(lens, lc, C, xyz);
+    const float* xi = shutter_ptr(shutter, C, batched, xyz);
+    const int64_t lens_per_view = lens_consts_per_view(lens);
     c10::cuda::CUDAGuard guard(xyz.device());
     auto opt = xyz.options();
     // one view's outputs have no view dimension
@@ -573,7 +590,12 @@ static std::vector<torch::Tensor> preprocess_forward(
         visible.data_ptr<uint8_t>() + c * N, (uint64_t*)scan.data_ptr<int64_t>() + c * N,                              \
         tiles ? (uint64_t*)tile_mask.data_ptr<int64_t>() + c * N : nullptr,                                            \
         tiles ? (uint32_t*)tile_win.data_ptr<int>() + c * N : nullptr, temp.data_ptr(), tb
-        if (lens == GSR_LENS_FISHEYE)
+        if (xi != nullptr)
+            check_rc(gsr_shutter_preprocess_forward((int)lens, GSR_FWD_ARGS,
+                                                    lens_consts ? lens_consts + lens_per_view * c : nullptr,
+                                                    xi + 6 * c, (int)readout, cur_stream()),
+                     "gsr_shutter_preprocess_forward");
+        else if (lens == GSR_LENS_FISHEYE)
             check_rc(gsr_fisheye_preprocess_forward(GSR_FWD_ARGS, lens_consts + GSR_FISHEYE_CONSTS * c, cur_stream()),
                      "gsr_fisheye_preprocess_forward");
         else if (lens == GSR_LENS_DISTORTION)
@@ -594,10 +616,11 @@ std::vector<torch::Tensor> fused_preprocess_forward(
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base,
     bool with_tiles, int64_t mode, c10::optional<torch::Tensor> filter3d, int64_t lens,
-    c10::optional<torch::Tensor> lens_consts) {
+    c10::optional<torch::Tensor> lens_consts, c10::optional<torch::Tensor> rolling_shutter, int64_t readout) {
     return preprocess_forward(false, xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
                               camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding,
-                              mh_dist, depth_base, with_tiles, mode, filter3d, lens, lens_consts);
+                              mh_dist, depth_base, with_tiles, mode, filter3d, lens, lens_consts, rolling_shutter,
+                              readout);
 }
 
 std::vector<torch::Tensor> batch_preprocess_forward(
@@ -605,10 +628,11 @@ std::vector<torch::Tensor> batch_preprocess_forward(
     torch::Tensor opacity_logit, torch::Tensor rgb_dc, c10::optional<torch::Tensor> sh_rest,
     torch::Tensor camera_T_world, torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
     double near_thresh, double far_thresh, double cull_mask_padding, double mh_dist, int64_t depth_base, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts) {
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts,
+    c10::optional<torch::Tensor> rolling_shutter, int64_t readout) {
     return preprocess_forward(true, xyz, xyz_camera_frame, quaternion, scale, opacity_logit, rgb_dc, sh_rest,
                               camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, cull_mask_padding,
-                              mh_dist, depth_base, true, mode, filter3d, lens, lens_consts);
+                              mh_dist, depth_base, true, mode, filter3d, lens, lens_consts, rolling_shutter, readout);
 }
 
 // (M, P known) -> the sorted pair list the tile renderers read records through, tile ranges [n_tiles+1] i32,
@@ -850,18 +874,23 @@ static FlatLayout flat_layout(int64_t N, int64_t n_sh_rest) {
 // gradient of the depth/alpha rows, GSR_MODE_ANTIALIASED takes the rows' opacity slot as the gradient on the
 // compensated opacity, GSR_MODE_FILTER3D needs the forward's filter3d.  lens, lc: the forward's.
 // camera_grads: 0 none; 1 also d loss / d camera_T_world (gsr_pose_*, libgsr_pose.so); 2 also the intrinsics and
-// lens-coefficient gradients (gsr_camera_*, libgsr_calib.so).
+// lens-coefficient gradients (gsr_camera_*, libgsr_calib.so).  shutter, readout, H, W: the forward's rolling shutter
+// (gsr_shutter_*, libgsr_shutter.so), where camera_grads 1 also gives the gradient on the twists and 2 is refused.
 // Returns the gaussian gradients, then `flat` (the one allocation they are views of), then with camera_grads >= 1
 // g_pose [4,4] / [C,4,4] (last row 0), then with camera_grads 2 d loss / d (fx, fy, cx, cy) [4] / [C,4] and d loss /
-// d lens coefficients [n] / [C,n] (n = 0 for the pinhole).
+// d lens coefficients [n] / [C,n] (n = 0 for the pinhole); with a shutter and camera_grads 1: g_pose, then g_xi
+// [6] / [C,6].
 static std::vector<torch::Tensor> preprocess_backward(
     bool batched, torch::Tensor slab, torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale,
     torch::Tensor opacity_logit, c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world, torch::Tensor K,
     c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
     c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
-    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lc, int64_t camera_grads) {
+    c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lc, int64_t camera_grads,
+    c10::optional<torch::Tensor> shutter, int64_t readout, int64_t H, int64_t W) {
     TORCH_CHECK(camera_grads >= 0 && camera_grads <= 2,
                 "camera_grads must be 0 (none), 1 (pose) or 2 (pose, intrinsics and lens)");
+    TORCH_CHECK(!(shutter.has_value() && camera_grads == 2),
+                "intrinsics and lens-coefficient gradients are not available with a rolling shutter");
     CHECK_VALID_INPUT(slab); CHECK_FLOAT_TENSOR(slab);
     CHECK_VALID_INPUT(xyz); CHECK_VALID_INPUT(quaternion); CHECK_VALID_INPUT(scale); CHECK_VALID_INPUT(opacity_logit);
     CHECK_VALID_INPUT(visible);
@@ -891,6 +920,7 @@ static std::vector<torch::Tensor> preprocess_backward(
     }
     const float* f3d = filter3d_ptr(filter3d, N);
     const float* lens_consts = lens_ptr(lens, lc, C, xyz);
+    const float* xi = shutter_ptr(shutter, C, batched, xyz);
     c10::cuda::CUDAGuard guard(xyz.device());
     auto opt = xyz.options();
     // All parameter gradients live in ONE allocation of the flat layout: a trainer that sums gradients over views /
@@ -926,6 +956,28 @@ static std::vector<torch::Tensor> preprocess_backward(
     std::vector<torch::Tensor> out = {o_xyz, o_q, o_s, o_o, o_dc};
     if (n_rest) out.push_back(g_sh);
     out.push_back(flat);
+    if (xi != nullptr) {
+        torch::Tensor g_pose, g_xi, temp;
+        if (camera_grads == 1) {
+            g_pose = torch::empty(batched ? std::vector<int64_t>{C, 4, 4} : std::vector<int64_t>{4, 4}, opt);
+            g_xi = torch::empty(batched ? std::vector<int64_t>{C, 6} : std::vector<int64_t>{6}, opt);
+            temp = torch::empty({(int64_t)gsr_shutter_temp_bytes(nc, (int)N)}, opt.dtype(torch::kUInt8));
+        }
+        float* gp = camera_grads == 1 ? F32PTR(g_pose) : nullptr;
+        float* gx = camera_grads == 1 ? F32PTR(g_xi) : nullptr;
+        void* tp = camera_grads == 1 ? temp.data_ptr() : nullptr;
+        const size_t tb = camera_grads == 1 ? (size_t)temp.numel() : 0;
+        check_rc(batched ? gsr_shutter_batch_preprocess_backward(ln, md, nc, GSR_BWD_ARGS, lens_consts, xi, (int)readout,
+                                                                 (int)H, (int)W, gp, gx, tp, tb, cur_stream())
+                         : gsr_shutter_preprocess_backward(ln, md, GSR_BWD_ARGS, lens_consts, xi, (int)readout, (int)H,
+                                                           (int)W, gp, gx, tp, tb, cur_stream()),
+                 batched ? "gsr_shutter_batch_preprocess_backward" : "gsr_shutter_preprocess_backward");
+        if (camera_grads == 1) {
+            out.push_back(g_pose);
+            out.push_back(g_xi);
+        }
+        return out;
+    }
     if (camera_grads == 0) {
         if (lens == GSR_LENS_FISHEYE)
             check_rc(batched ? gsr_fisheye_batch_preprocess_backward(md, nc, GSR_BWD_ARGS, lens_consts, cur_stream())
@@ -985,10 +1037,10 @@ std::vector<torch::Tensor> fused_preprocess_backward(
     c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
     c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
     c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts,
-    int64_t camera_grads) {
+    int64_t camera_grads, c10::optional<torch::Tensor> rolling_shutter, int64_t readout, int64_t H, int64_t W) {
     return preprocess_backward(false, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
                                camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d,
-                               lens, lens_consts, camera_grads);
+                               lens, lens_consts, camera_grads, rolling_shutter, readout, H, W);
 }
 
 std::vector<torch::Tensor> batch_preprocess_backward(
@@ -997,10 +1049,10 @@ std::vector<torch::Tensor> batch_preprocess_backward(
     c10::optional<torch::Tensor> camera_centre, torch::Tensor visible, c10::optional<torch::Tensor> out_flat,
     c10::optional<torch::Tensor> grad_uv_compact, c10::optional<torch::Tensor> scan, bool use_slab_uv, int64_t mode,
     c10::optional<torch::Tensor> filter3d, int64_t lens, c10::optional<torch::Tensor> lens_consts,
-    int64_t camera_grads) {
+    int64_t camera_grads, c10::optional<torch::Tensor> rolling_shutter, int64_t readout, int64_t H, int64_t W) {
     return preprocess_backward(true, slab, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world, K,
                                camera_centre, visible, out_flat, grad_uv_compact, scan, use_slab_uv, mode, filter3d,
-                               lens, lens_consts, camera_grads);
+                               lens, lens_consts, camera_grads, rolling_shutter, readout, H, W);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1575,7 +1627,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("camera_centre"), py::arg("H"), py::arg("W"), py::arg("near_thresh"), py::arg("far_thresh"),
           py::arg("cull_mask_padding"), py::arg("mh_dist"), py::arg("depth_base"), py::arg("with_tiles") = false,
           py::arg("mode") = 0, py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE,
-          py::arg("lens_consts") = py::none());
+          py::arg("lens_consts") = py::none(),
+          py::arg("rolling_shutter") = py::none(), py::arg("readout") = GSR_READOUT_TOP_TO_BOTTOM);
     m.def("fused_bin", &fused_bin, "pair emission + radix sort + tile ranges");
     m.def("fused_render_forward", &fused_render_forward,
           "tile renderer forward (with depth_key: also the depth and alpha maps; with weight_sum / weight_max / "
@@ -1605,7 +1658,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"), py::arg("camera_centre"), py::arg("visible"),
           py::arg("out_flat"), py::arg("grad_uv_compact"), py::arg("scan"), py::arg("use_slab_uv"), py::arg("mode"),
           py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE, py::arg("lens_consts") = py::none(),
-          py::arg("camera_grads") = 0);
+          py::arg("camera_grads") = 0, py::arg("rolling_shutter") = py::none(),
+          py::arg("readout") = GSR_READOUT_TOP_TO_BOTTOM, py::arg("height") = 0, py::arg("width") = 0);
     m.def("batch_preprocess_forward", &batch_preprocess_forward,
           "per-gaussian forward of C views into stacked records / keys / visibility / scans (rasterize_batch; "
           "lens_consts [C,n+1])",
@@ -1613,7 +1667,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("opacity_logit"), py::arg("rgb_dc"), py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"),
           py::arg("camera_centre"), py::arg("H"), py::arg("W"), py::arg("near_thresh"), py::arg("far_thresh"),
           py::arg("cull_mask_padding"), py::arg("mh_dist"), py::arg("depth_base"), py::arg("mode"),
-          py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE, py::arg("lens_consts") = py::none());
+          py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE, py::arg("lens_consts") = py::none(),
+          py::arg("rolling_shutter") = py::none(), py::arg("readout") = GSR_READOUT_TOP_TO_BOTTOM);
     m.def("batch_render_backward", &batch_render_backward,
           "render backward of C views into one stacked gradient slab [C, N*12]");
     m.def("batch_preprocess_backward", &batch_preprocess_backward,
@@ -1623,7 +1678,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("sh_rest"), py::arg("camera_T_world"), py::arg("K"), py::arg("camera_centre"), py::arg("visible"),
           py::arg("out_flat"), py::arg("grad_uv_compact"), py::arg("scan"), py::arg("use_slab_uv"), py::arg("mode"),
           py::arg("filter3d") = py::none(), py::arg("lens") = GSR_LENS_PINHOLE, py::arg("lens_consts") = py::none(),
-          py::arg("camera_grads") = 0);
+          py::arg("camera_grads") = 0, py::arg("rolling_shutter") = py::none(),
+          py::arg("readout") = GSR_READOUT_TOP_TO_BOTTOM, py::arg("height") = 0, py::arg("width") = 0);
     m.def("fisheye_theta_max", &fisheye_theta_max, "the fisheye cull limit of 4 coefficients (gsr_fisheye_theta_max)");
     m.def("distortion_r2_max", &distortion_r2_max,
           "the radial fold limit s = r^2 of 5 coefficients k1 k2 p1 p2 k3 (gsr_distortion_r2_max)");
@@ -1637,6 +1693,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.attr("LENS_PINHOLE") = GSR_LENS_PINHOLE;
     m.attr("LENS_FISHEYE") = GSR_LENS_FISHEYE;
     m.attr("LENS_DISTORTION") = GSR_LENS_DISTORTION;
+    m.attr("READOUT_TOP_TO_BOTTOM") = GSR_READOUT_TOP_TO_BOTTOM;
+    m.attr("READOUT_BOTTOM_TO_TOP") = GSR_READOUT_BOTTOM_TO_TOP;
+    m.attr("READOUT_LEFT_TO_RIGHT") = GSR_READOUT_LEFT_TO_RIGHT;
+    m.attr("READOUT_RIGHT_TO_LEFT") = GSR_READOUT_RIGHT_TO_LEFT;
     m.def("flat_section_ends", &flat_section_ends, "section ends of the flat parameter/gradient layout");
     m.def("adam_step_flat", &adam_step_flat, "Adam on the flat parameter buffer");
     m.def("adam_step_sharded", &adam_step_sharded, "reduce-scatter + Adam + all-gather over peer memory");

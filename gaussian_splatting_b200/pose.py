@@ -6,8 +6,9 @@ applied on the left (a perturbation in the camera frame):
 
     T' = se3_exp(xi) @ T
 
-so the pose stays rigid whatever the optimiser does, and xi = 0 is the identity.  Plain torch, differentiable,
-any dtype and device.
+so the pose stays rigid whatever the optimiser does, and xi = 0 is the identity.  se3_log inverts se3_exp, and
+shutter_from_endpoints turns a rolling shutter's first-line and last-line poses into rasterize's (camera_T_world,
+rolling_shutter).  Plain torch, differentiable, any dtype and device.
 """
 from __future__ import annotations
 
@@ -46,6 +47,41 @@ def se3_exp(xi):
     bottom = torch.zeros(xi.shape[:-1] + (1, 4), dtype=xi.dtype, device=xi.device)
     bottom[..., 0, 3] = 1
     return torch.cat([top, bottom], -2)
+
+
+def se3_log(T):
+    """The inverse of se3_exp: rigid transforms T [..., 4, 4] -> twists xi = (rho, omega) [..., 6] with |omega| < pi.
+    The angle is atan2(|vee(R - R^T)| / 2, (tr R - 1) / 2), which keeps its precision near 0; below th^2 = 1e-4 the
+    coefficients th / (2 sin th) and (1 - th sin th / (2 (1 - cos th))) / th^2 of omega = coef vee(R - R^T) and
+    rho = V^-1 t come from their Taylor series, so the result and its gradient are finite at the identity.  Near
+    |omega| = pi the rotation's axis is ill-conditioned (as for any logarithm)."""
+    R, t = T[..., :3, :3], T[..., :3, 3]
+    v = torch.stack([R[..., 2, 1] - R[..., 1, 2], R[..., 0, 2] - R[..., 2, 0], R[..., 1, 0] - R[..., 0, 1]], -1)
+    s = 0.5 * torch.linalg.vector_norm(v, dim=-1)
+    c = 0.5 * (R[..., 0, 0] + R[..., 1, 1] + R[..., 2, 2] - 1)
+    th = torch.atan2(s, c)
+    th2 = th * th
+    small = th2 < 1e-4
+    th_safe = torch.where(small, torch.ones_like(th), th)
+    s_safe = torch.where(small, torch.ones_like(s), s)
+    half = torch.where(small, 0.5 + th2 / 12 + 7 * th2 * th2 / 720, th_safe / (2 * s_safe))
+    w = half[..., None] * v
+    d = torch.where(small, 1.0 / 12 + th2 / 720 + th2 * th2 / 30240,
+                    (1 - th_safe * s_safe / (2 * (1 - torch.cos(th_safe)))) / (th_safe * th_safe))
+    Wx = _hat(w)
+    eye = torch.eye(3, dtype=T.dtype, device=T.device).expand(Wx.shape)
+    Vinv = eye - 0.5 * Wx + d[..., None, None] * (Wx @ Wx)
+    rho = (Vinv @ t[..., None])[..., 0]
+    return torch.cat([rho, w], -1)
+
+
+def shutter_from_endpoints(T_start, T_end):
+    """(camera_T_world of the middle line, xi) for rasterize(..., rolling_shutter=xi) from the poses of a rolling
+    shutter's first and last lines ([..., 4, 4] each): xi = se3_log(T_end @ inverse(T_start)), the motion over the
+    readout applied on the left, and T_mid = se3_exp(xi / 2) @ T_start, so that se3_exp((tau - 1/2) xi) @ T_mid is
+    T_start at tau = 0 and T_end at tau = 1."""
+    xi = se3_log(T_end @ torch.linalg.inv(T_start))
+    return se3_exp(0.5 * xi) @ T_start, xi
 
 
 class PoseDelta(torch.nn.Module):

@@ -253,7 +253,7 @@ class _ViewState:
                  "records", "keys_sorted", "id_bits",
                  "n_per_pixel", "w_per_pixel", "background", "profile", "grad_flat", "grad_out", "vis_idx32", "scan", "masks", "uv_ref", "uv_grad_emitted", "image", "speculation_overflowed",
                  "mode", "zkey", "depth_base", "depth_bits", "depth", "alpha", "uv_absgrad", "filter3d",
-                 "weight_stats", "lens")
+                 "weight_stats", "lens", "shutter")
 
     @property
     def ids_sorted(self):
@@ -287,6 +287,7 @@ class _ViewState:
         self.mode = 0
         self.filter3d = None
         self.lens = None        # a lens model: (its LENS_* value, its constants on the device) (_lens_state)
+        self.shutter = None     # a rolling shutter: (its twist [6] on the device, its READOUT_* value)
         self.depth = self.alpha = None
         self.uv_absgrad = None  # MODE_ABSGRAD: [M,2], set by every render backward
         self.weight_stats = None  # optional densify.WeightStats the render forward accumulates into
@@ -433,26 +434,74 @@ def _lens_grad(g, k):
     return g.to(k.dtype)
 
 
+READOUTS = ("top_to_bottom", "bottom_to_top", "left_to_right", "right_to_left")
+
+
+def _shutter_arg(xi, readout, K, lens_k, device, H, W, C=None):
+    """Checks rasterize's / rasterize_batch's rolling_shutter and readout (before any launch); returns
+    (twists [6] or [C,6] for the kernels, the native READOUT_* value), or None for a global shutter."""
+    if readout not in READOUTS:
+        raise ValueError(f"readout must be one of {READOUTS}, got {readout!r}")
+    if xi is None:
+        return None
+    if not torch.is_tensor(xi):
+        raise TypeError("rolling_shutter must be a torch tensor [6] (a twist (rho, omega), pose.se3_exp's convention)")
+    if xi.dtype != torch.float32:
+        raise TypeError(f"rolling_shutter must be float32, got {xi.dtype}")
+    shapes = ((6,),) if C is None else ((6,), (C, 6))
+    if tuple(xi.shape) not in shapes:
+        raise ValueError(f"rolling_shutter has shape {tuple(xi.shape)} but must be "
+                         + (" or ".join(str(list(t)) for t in shapes)))
+    if xi.device != device:
+        raise ValueError("rolling_shutter must be on the gaussians' device")
+    if (H if readout in READOUTS[:2] else W) < 2:
+        raise ValueError(f"a {readout} readout needs at least 2 lines")
+    if K.requires_grad or lens_k is not None:
+        raise ValueError("intrinsics and lens-coefficient gradients are not available with rolling_shutter: pass "
+                         "camera.K.detach() and constant lens coefficients")
+    xi = xi.detach()
+    if C is not None and xi.dim() == 1:
+        xi = xi.expand(C, 6)
+    return xi.contiguous(), getattr(native(), "READOUT_" + readout.upper())
+
+
+def _shutter_kwargs(shutter):
+    """The rolling-shutter arguments of the per-gaussian forward bindings for a state's shutter"""
+    return {} if shutter is None else dict(rolling_shutter=shutter[0], readout=shutter[1])
+
+
 def _preprocess_backward(ctx, native_fn, args):
-    """The per-gaussian backward: (gaussian grads..., flat), g_pose, g_K, g_k (None where no gradient is wanted).  The
-    intrinsics or the lens coefficients require grad: the camera-gradient kernels (libgsr_calib.so); only the pose:
-    the pose kernels (libgsr_pose.so); neither: the plain kernels."""
+    """The per-gaussian backward: (gaussian grads..., flat), g_pose, g_K, g_k, g_xi (None where no gradient is
+    wanted).  The intrinsics or the lens coefficients require grad: the camera-gradient kernels (libgsr_calib.so); only
+    the pose: the pose kernels (libgsr_pose.so); neither: the plain kernels.  With a rolling shutter the shutter
+    kernels (libgsr_shutter.so), with the camera row when the pose or the twists require grad."""
     need = ctx.needs_input_grad
+    st = ctx.state
+    if st.shutter is not None:
+        camera_grads = 1 if need[6] or need[11] else 0
+        out = native_fn(*args, **_lens_kwargs(st.lens), camera_grads=camera_grads, **_shutter_kwargs(st.shutter),
+                        height=st.H, width=st.W)
+        n = 6 + ctx.has_sh
+        grads, cam = out[:n], out[n:]
+        g_xi = None
+        if need[11]:
+            g_xi = cam[1] if ctx.xi_shape == tuple(cam[1].shape) else cam[1].sum(0)
+        return grads, cam[0] if need[6] else None, None, None, g_xi
     camera_grads = 2 if need[7] or need[10] else 1 if need[6] else 0
-    out = native_fn(*args, **_lens_kwargs(ctx.state.lens), camera_grads=camera_grads)
+    out = native_fn(*args, **_lens_kwargs(st.lens), camera_grads=camera_grads)
     n = 6 + ctx.has_sh  # the gaussian gradients and the flat allocation, then the camera gradients
     grads, cam = out[:n], out[n:]
     g_pose = cam[0] if need[6] else None
     g_K = _intrinsics_grad(cam[1]) if need[7] else None
     g_k = _lens_grad(cam[2], ctx.lens_k) if ctx.lens_k is not None and need[10] else None
-    return grads, g_pose, g_K, g_k
+    return grads, g_pose, g_K, g_k, None
 
 
 class _ProjectGaussians(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg, lens_k=None):
+    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg, lens_k=None, xi=None):
         # lens_k: the lens coefficient tensor when it requires grad (an input for its gradient only: the forward reads
-        # the constants uploaded to state.lens)
+        # the constants uploaded to state.lens); xi likewise the rolling-shutter twist (state.shutter)
         ext = native()
         # torch.matmul takes another path (other rounding) for an operand that requires grad: the forward's bits must
         # not depend on whether the pose does
@@ -483,9 +532,11 @@ class _ProjectGaussians(torch.autograd.Function):
             # tile_mask / tile_win: the tiles each gaussian hits, tested once here and only expanded by the pair emission
             records, zkey, visible, scan, tile_mask, tile_win = ext.fused_preprocess_forward(
                 xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far, pad,
-                mh, depth_base, True, state.mode, state.filter3d, **_lens_kwargs(state.lens))
-        # a backward pass can follow (the camera counts: a pose- or intrinsics-only refinement needs the masks too)
-        record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or ctx.needs_input_grad[10])
+                mh, depth_base, True, state.mode, state.filter3d, **_lens_kwargs(state.lens),
+                **_shutter_kwargs(state.shutter))
+        # a backward pass can follow (the camera counts: a pose-, intrinsics- or shutter-only refinement needs the
+        # masks too)
+        record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or any(ctx.needs_input_grad[10:]))
         background = state.background
 
         def counts(total):
@@ -566,6 +617,7 @@ class _ProjectGaussians(torch.autograd.Function):
         ctx.state = state
         ctx.has_sh = sh is not None
         ctx.lens_k = lens_k
+        ctx.xi_shape = None if xi is None else tuple(xi.shape)
         ctx.save_for_backward(xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre)
         return uv, carrier
 
@@ -588,11 +640,11 @@ class _ProjectGaussians(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            grads, g_pose, g_K, g_k = _preprocess_backward(ctx, native().fused_preprocess_backward, args)
+            grads, g_pose, g_K, g_k, g_xi = _preprocess_backward(ctx, native().fused_preprocess_backward, args)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]  # the one allocation all parameter gradients of this view are views of
-        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, g_K, None, None, g_k
+        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, g_K, None, None, g_k, g_xi
 
 
 class _CompositeTiles(torch.autograd.Function):
@@ -672,7 +724,7 @@ class _CompositeTiles(torch.autograd.Function):
 def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
               use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
               render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
-              features=None, fisheye=None, distortion=None):
+              features=None, fisheye=None, distortion=None, rolling_shutter=None, readout="top_to_bottom"):
     """render_depth_alpha=True: also the per-pixel depth and alpha maps, differentiable, from the same tile walk —
     returns (image, culling_mask, uv, depth [H,W,1], alpha [H,W,1]) (+ state with return_state).  alpha is the
     accumulated blend weight before the background; depth = sum of w_i * z_i over the same splats and weights as the
@@ -764,8 +816,34 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
     or distortion= gets d loss / d k in its shape and dtype, through one blocking device -> host copy of n floats at the
     end of the backward (only then; a sequence of numbers gets none).  Cull limits get no gradient.  Every lens and
     option combine with it; outputs, gaussian gradients and the pose gradient are bit-identical to a run without it
-    (DESIGN.md 3.23)."""
+    (DESIGN.md 3.23).
+
+    rolling_shutter: a rolling-shutter camera whose lines are read out one after another while it moves.
+    camera_T_world is then the pose of the image's middle line, and rolling_shutter an fp32 tensor xi = (rho, omega)
+    [6] on the gaussians' device (pose.se3_exp's convention, e.g. a row of an nn.Parameter of zeros [n_images, 6]): the
+    camera's motion over the whole readout, applied on the left, T(tau) = se3_exp((tau - 1/2) xi) @ camera_T_world for
+    the line read at time tau in [0, 1].  readout gives the line time of a pixel: "top_to_bottom" (the default,
+    tau = v / (H - 1)), "bottom_to_top", "left_to_right" (u / (W - 1)) or "right_to_left"; pose.shutter_from_endpoints
+    turns first-line / last-line poses into (camera_T_world, xi).  Each gaussian is projected at its own line's time
+    tau* = clamp(r(u(tau*)), 0, 1) (a fixed number of Newton steps), with the pose, depth and lens Jacobian of that
+    time; its 2-D covariance includes the time's dependence on image position, A J W Sigma W^T J^T A^T with
+    A = I + f e^T / (1 - lambda), f = du/dtau and lambda the point's speed along the readout (a shear for a pan across
+    the lines, a stretch for motion along them).  A gaussian with lambda >= 3/4 or an unconverged time is culled.  The
+    SH view direction keeps the centre of camera_T_world.  xi = 0 renders bit-identically to the call without it.
+    Gradients are exact derivatives of this model (tau* an implicit function of the inputs): to the gaussians, to
+    camera_T_world when it requires grad, and to xi when it requires grad (DESIGN.md 3.24).  The values of xi are read
+    by the kernels without a host synchronisation and are not checked.  Combines with every lens and option above
+    except K or lens-coefficient gradients (ValueError).  A wrong shape, device (ValueError) or dtype (TypeError) of
+    xi, an unknown readout or a 1-line image raise before any launch; None (the default) runs exactly the kernels
+    without it.  fp32 and precomputed SH colours only."""
     lens = _lens_arg(fisheye, distortion)
+    if rolling_shutter is not None:
+        if gaussians.xyz.dtype != torch.float32:
+            raise TypeError("rolling_shutter needs fp32 inputs (the fused rasterizer's per-gaussian stages apply it)")
+        if gaussians.sh is not None and not use_sh_precompute:
+            raise ValueError("rolling_shutter needs use_sh_precompute=True (per-pixel SH colours are not supported)")
+    shutter = _shutter_arg(rolling_shutter, readout, camera.K, _lens_input(fisheye, distortion), gaussians.xyz.device,
+                           int(camera.height), int(camera.width))
     if lens is not None:
         if gaussians.xyz.dtype != torch.float32:
             raise TypeError(f"{lens[0]} needs fp32 inputs (the fused rasterizer's per-gaussian stages project through "
@@ -840,6 +918,7 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
     state.lens = _lens_state(lens, gaussians.xyz.device)
+    state.shutter = shutter
     state.weight_stats = weight_stats
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
@@ -848,7 +927,8 @@ def rasterize(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_m
         gaussians.xyz.contiguous(), gaussians.quaternion.contiguous(), gaussians.scale.contiguous(),
         gaussians.opacity.contiguous(), gaussians.rgb.contiguous(),
         None if gaussians.sh is None else gaussians.sh.contiguous(),
-        camera_T_world.contiguous(), camera.K.contiguous(), state, cfg, _lens_input(fisheye, distortion))
+        camera_T_world.contiguous(), camera.K.contiguous(), state, cfg, _lens_input(fisheye, distortion),
+        rolling_shutter if shutter is not None and rolling_shutter.requires_grad else None)
     state.uv_ref = weakref.ref(uv)
     culling_mask = state.visible == 0
     outs = _CompositeTiles.apply(uv, carrier, state.background, state, features)
@@ -930,13 +1010,14 @@ class _BatchState:
         self.mode = 0
         self.filter3d = None
         self.lens = None         # a lens model: (its LENS_* value, [C, n+1] constants on the device) (_lens_state)
+        self.shutter = None      # a rolling shutter: (the views' twists [C,6] on the device, a READOUT_* value)
         self.views = []
         self.images = self.depth = self.alpha = None
 
 
 class _ProjectBatch(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg, lens_k=None):
+    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg, lens_k=None, xi=None):
         camera_T_world = camera_T_world.detach()  # as in _ProjectGaussians.forward
         ext = native()
         H, W, near, far, pad, mh = cfg
@@ -958,8 +1039,8 @@ class _ProjectBatch(torch.autograd.Function):
         with _stage(state, "preprocess_fwd"):
             records, zkey, visible, scan, tile_mask, tile_win = ext.batch_preprocess_forward(
                 xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far, pad,
-                mh, depth_base, state.mode, state.filter3d, **_lens_kwargs(state.lens))
-        record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or ctx.needs_input_grad[10])
+                mh, depth_base, state.mode, state.filter3d, **_lens_kwargs(state.lens), **_shutter_kwargs(state.shutter))
+        record_masks = USE_CONTRIBUTION_MASKS and (any(ctx.needs_input_grad[:8]) or any(ctx.needs_input_grad[10:]))
         background = state.background
         depth_mode = bool(state.mode & ext.MODE_DEPTH_ALPHA)
 
@@ -1043,6 +1124,7 @@ class _ProjectBatch(torch.autograd.Function):
         ctx.state = state
         ctx.has_sh = sh is not None
         ctx.lens_k = lens_k
+        ctx.xi_shape = None if xi is None else tuple(xi.shape)
         ctx.save_for_backward(xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre)
         return uv_all, carrier
 
@@ -1062,11 +1144,11 @@ class _ProjectBatch(torch.autograd.Function):
         with _stage(st, "preprocess_bwd"):
             args = (slab, xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre, st.visible, st.grad_out,
                     guv, st.scan if guv is not None else None, not st.uv_grad_emitted, st.mode, st.filter3d)
-            grads, g_pose, g_K, g_k = _preprocess_backward(ctx, native().batch_preprocess_backward, args)
+            grads, g_pose, g_K, g_k, g_xi = _preprocess_backward(ctx, native().batch_preprocess_backward, args)
         g_xyz, g_q, g_s, g_o, g_dc = grads[:5]
         g_sh = grads[5] if ctx.has_sh else None
         st.grad_flat = grads[-1]
-        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, g_K, None, None, g_k
+        return g_xyz, g_q, g_s, g_o.view(-1, 1), g_dc, g_sh, g_pose, g_K, None, None, g_k, g_xi
 
 
 class _CompositeBatch(torch.autograd.Function):
@@ -1153,7 +1235,7 @@ def _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, back
 def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
                     use_sh_precompute, background_rgb, return_state=False, profile=None, grad_out=None,
                     render_depth_alpha=False, antialiased=False, absgrad=False, filter3d=None, weight_stats=None,
-                    features=None, fisheye=None, distortion=None):
+                    features=None, fisheye=None, distortion=None, rolling_shutter=None, readout="top_to_bottom"):
     """C cameras of one scene in one call: rasterize()'s nine positional arguments with camera_T_world [C,4,4]
     (C >= 1), camera.K [3,3] (shared) or [C,3,3], camera.height / width shared, background_rgb [3] or [C,3].
 
@@ -1185,10 +1267,16 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
 
     A camera.K that requires grad gets d loss / d K as rasterize() defines it, [C,3,3] per view (a shared [3,3]: the sum
     over the views), and a CPU coefficient tensor that requires grad its gradient in its shape ([n]: summed over the
-    views); view c's values are bit-identical to the single-view kernel's on view c's rows (DESIGN.md 3.23)."""
+    views); view c's values are bit-identical to the single-view kernel's on view c's rows (DESIGN.md 3.23).
+
+    rolling_shutter: rolling-shutter cameras as in rasterize(), xi [6] shared by every view or [C,6] one row per view,
+    with one readout for all views; view c is bit-identical to rasterize(..., rolling_shutter=xi_c).  A shared [6] that
+    requires grad gets the views' summed gradient, a [C,6] one row per view (DESIGN.md 3.24)."""
     C = _check_batch_args(gaussians, camera_T_world, camera, use_sh_precompute, background_rgb, filter3d, weight_stats,
                           features)
     lens = _lens_arg(fisheye, distortion, C)
+    shutter = _shutter_arg(rolling_shutter, readout, camera.K, _lens_input(fisheye, distortion), gaussians.xyz.device,
+                           int(camera.height), int(camera.width), C)
     ext = native()
     K = camera.K if camera.K.dim() == 3 else camera.K.expand(C, 3, 3)
     state = _BatchState(profile)
@@ -1197,6 +1285,7 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
                   | (ext.MODE_ABSGRAD if absgrad else 0) | (ext.MODE_FILTER3D if filter3d is not None else 0))
     state.filter3d = None if filter3d is None else filter3d.reshape(-1).contiguous()
     state.lens = _lens_state(lens, gaussians.xyz.device)
+    state.shutter = shutter
     state.background = (background_rgb if background_rgb.dim() == 2 else background_rgb.expand(C, 3)).contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh),
            float(cull_mask_padding), float(mh_dist))
@@ -1204,7 +1293,8 @@ def rasterize_batch(gaussians, camera_T_world, camera, near_thresh, far_thresh, 
         gaussians.xyz.contiguous(), gaussians.quaternion.contiguous(), gaussians.scale.contiguous(),
         gaussians.opacity.contiguous(), gaussians.rgb.contiguous(),
         None if gaussians.sh is None else gaussians.sh.contiguous(),
-        camera_T_world.contiguous(), K.contiguous(), state, cfg, _lens_input(fisheye, distortion))
+        camera_T_world.contiguous(), K.contiguous(), state, cfg, _lens_input(fisheye, distortion),
+        rolling_shutter if shutter is not None and rolling_shutter.requires_grad else None)
     uvs = torch.split(uv_all, [v.M for v in state.views])
     state.uv_refs = [weakref.ref(u) for u in uvs]
     culling_mask = state.visible == 0
