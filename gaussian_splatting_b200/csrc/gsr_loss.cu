@@ -11,19 +11,34 @@
 //   - L1 = mean |p - t| over all B*C*H*W elements, gradient sign(p - t) / numel with sign(0) = 0.
 // loss = l1_weight * L1 + ssim_weight * (1 - SSIM).  Gradients flow to pred only.
 //
+// Accuracy: late in training the render nearly equals the target (1 - S of 1e-2 down to 1e-5 and below, flat regions
+// equal to within one 8-bit step), where the textbook arithmetic cancels: E[x^2] - mu^2 when the variance is much
+// smaller than mu^2, 1 - S with S rounded per window, and D_mu + 2p D_pp + t D_pt, whose terms are of size 2 / C2.
+// So both kernels stage d = p - t and t' = t - k (k one target value per CTA and channel) instead of p and t, and form
+// every variance from local deviations:
+//     mu_t = k W + mu_t',  mu_d,  mu_p = mu_t + mu_d,
+//     s_tt = s_t't' + k (1 - W)(mu_t' + mu_t),  s_td = s_t'd + k (1 - W) mu_d,  s_dd,
+// where W = (sum of the taps)^2 is the window's total weight (the fp32 taps do not sum to exactly 1, and the definition
+// keeps them as they are).  Then b1 - a1 = mu_d^2 and b2 - a2 = s_dd, so per window
+//     1 - S = (mu_d^2 b2 + a1 s_dd) / (b1 b2)
+// is summed and SSIM = 1 - mean(1 - S), and with D_pt = -2 D_pp + E, E = 2 a1 s_dd / (b1 b2^2),
+//     D_mu + 2p D_pp + t D_pt = G + 2 d D_pp + t' E,  G = dS/dmu_p|_sigma - 2 mu_d D_pp - (mu_t - k) E,
+// dS/dmu_p|_sigma = -2 a2 mu_d (mu_t (mu_p + mu_t) + C1) / (b1^2 b2).  Identical images give d = 0 exactly, hence
+// 1 - S = 0, G = E = 0 and a gradient of exactly 0.
+//
 // Forward: one CTA per 32x16 tile of window origins / pixels, all channels (staged LOSS_CG at a time).  The tile
-// plus its 10-pixel halo to the right and below is staged in shared memory for pred and target, the five moments are
-// blurred horizontally then vertically, S is summed over the CTA's valid origins and |p - t| over the CTA's own
-// pixels (each pixel counts once).  Each CTA writes an fp64 (sum S, sum |p - t|) pair; the last CTA to finish (an
+// plus its 10-pixel halo to the right and below is staged in shared memory as t' and d, the five moments are
+// blurred horizontally then vertically, 1 - S is summed over the CTA's valid origins and |d| over the CTA's own
+// pixels (each pixel counts once).  Each CTA writes an fp64 (sum 1 - S, sum |p - t|) pair; the last CTA to finish (an
 // atomic ticket) adds the pairs up in a fixed order and writes out[3] = {loss, L1, SSIM} on the device.  No host
 // sync, no atomics on the result: bit-identical from run to run.
 //
 // Backward: recomputes instead of storing intermediate maps (an evaluation under no_grad pays for the forward
 // only).  A 32x16 pixel tile needs dS/dmu_p, dS/dE[p^2], dS/dE[pt] at the window origins y in [x-10, x] (zero at
 // origins outside the valid range), which need the images over [x-10, x+10]: that 52x36 region is staged, the
-// moments and the three derivative maps are formed over the 42x26 origins, and the maps are blurred with the
-// flipped window (separably) back onto the pixels:
-//     grad(x) = g_out * (l1_weight / numel * sign(p - t) - ssim_weight / n_valid * (D_mu + 2 p D_pp + t D_pt)).
+// moments and the three derivative maps G, D_pp, E are formed over the 42x26 origins, and the maps are blurred with
+// the flipped window (separably) back onto the pixels:
+//     grad(x) = g_out * (l1_weight / numel * sign(d) - ssim_weight / n_valid * (G + 2 d D_pp + t' E)).
 //
 // Layouts: every image is a base pointer plus four element strides (B, C, H, W), so the rasterizer's [H,W,3] image,
 // the trainer's image.unsqueeze(0).permute(0,3,1,2) view of it and a contiguous NCHW tensor go through the same code
@@ -52,15 +67,16 @@ struct LossArgs {
     int B, C, H, W;
     T w[SSIM_TAPS];
     T c1, c2;
+    T eps;  // 1 - W, W = (sum of the taps)^2 the 2-D window's total weight
 };
 
-// forward shared memory: pred + target [CG][TH+10][TW+10], horizontal moments [5][TH+10][TW]
+// forward shared memory: t' + d [CG][TH+10][TW+10], horizontal moments [5][TH+10][TW]
 constexpr int FWD_IH = LOSS_TH + SSIM_HALO, FWD_IW = LOSS_TW + SSIM_HALO;
 template <typename T>
 constexpr size_t fwd_smem_bytes() {
     return sizeof(T) * (2 * LOSS_CG * FWD_IH * FWD_IW + 5 * FWD_IH * LOSS_TW);
 }
-// backward shared memory: pred + target [CG][TH+20][TW+20], horizontal moments [5][TH+20][TW+10] (reused for the
+// backward shared memory: t' + d [CG][TH+20][TW+20], horizontal moments [5][TH+20][TW+10] (reused for the
 // transposed horizontal pass [3][TH+10][TW]), derivative maps [3][TH+10][TW+10], gradient [CG][TH][TW]
 constexpr int BWD_RH = LOSS_TH + 2 * SSIM_HALO, BWD_RW = LOSS_TW + 2 * SSIM_HALO;
 constexpr int BWD_OH = LOSS_TH + SSIM_HALO, BWD_OW = LOSS_TW + SSIM_HALO;
@@ -70,13 +86,27 @@ constexpr size_t bwd_smem_bytes() {
                         LOSS_CG * LOSS_TH * LOSS_TW);
 }
 
-// Stage channels [c0, c0 + cg) of image b, rows [y0, y0 + nr), cols [x0, x0 + nc) into s[c][r][col]; zero outside
-// the image.  The element each thread takes follows the smaller of the channel / column strides (coalescing only).
+// The shift k of channel c0 + c into shared k[c]: the target at the tile's centre pixel (clamped into the image), the
+// same element whatever the layout.  Read after the next barrier.
 template <typename T>
-__device__ __forceinline__ void stage_region(T* __restrict__ s, const T* __restrict__ src, const long long* st, int b,
-                                             int c0, int cg, int y0, int x0, int nr, int nc, int H, int W) {
-    const bool interleaved = st[1] < st[3];
-    const long long base = (long long)b * st[0] + (long long)c0 * st[1];
+__device__ __forceinline__ void tile_shifts(const LossArgs<T>& A, int b, int c0, int cg, int ty0, int tx0, T* k) {
+    const int y = min(ty0 + LOSS_TH / 2, A.H - 1), x = min(tx0 + LOSS_TW / 2, A.W - 1);
+    const int c = threadIdx.x;
+    if (c < cg) k[c] = A.target[b * A.ts[0] + (c0 + c) * A.ts[1] + y * A.ts[2] + x * A.ts[3]];
+}
+
+// Stage channels [c0, c0 + cg) of image b, rows [y0, y0 + nr), cols [x0, x0 + nc) as st[c][r][col] = t - k[c] and
+// sd[c][r][col] = p - t; zero outside the image.  The element each thread takes follows the smaller of pred's channel
+// / column strides (coalescing only).
+template <typename T>
+__device__ __forceinline__ void stage_region(T* __restrict__ st, T* __restrict__ sd, const LossArgs<T>& A, int b,
+                                             int c0, int cg, int y0, int x0, int nr, int nc, const T* k) {
+    const int H = A.H, W = A.W;
+    const long long* ps = A.ps;
+    const long long* ts = A.ts;
+    const bool interleaved = ps[1] < ps[3];
+    const long long pbase = (long long)b * ps[0] + (long long)c0 * ps[1];
+    const long long tbase = (long long)b * ts[0] + (long long)c0 * ts[1];
     const int n = cg * nr * nc;
     for (int e = threadIdx.x; e < n; e += LOSS_THREADS) {
         int c, r, col;
@@ -92,20 +122,26 @@ __device__ __forceinline__ void stage_region(T* __restrict__ s, const T* __restr
             c = rc / nr;
         }
         const int y = y0 + r, x = x0 + col;
-        T v = T(0);
-        if (y >= 0 && y < H && x >= 0 && x < W) v = src[base + c * st[1] + y * st[2] + x * st[3]];
-        s[(c * nr + r) * nc + col] = v;
+        T tv = T(0), dv = T(0);
+        if (y >= 0 && y < H && x >= 0 && x < W) {
+            const T p = A.pred[pbase + c * ps[1] + y * ps[2] + x * ps[3]];
+            const T t = A.target[tbase + c * ts[1] + y * ts[2] + x * ts[3]];
+            tv = t - k[c];
+            dv = p - t;
+        }
+        st[(c * nr + r) * nc + col] = tv;
+        sd[(c * nr + r) * nc + col] = dv;
     }
 }
 
-// Five horizontal window sums of row r starting at column u: p, t, p^2, t^2, pt.
+// Five horizontal window sums of row r starting at column u: t', d, t'^2, d^2, t'd.
 template <typename T>
-__device__ __forceinline__ void hsum5(const T* __restrict__ p, const T* __restrict__ t, int off, const T* w, T& m0,
+__device__ __forceinline__ void hsum5(const T* __restrict__ t, const T* __restrict__ d, int off, const T* w, T& m0,
                                       T& m1, T& m2, T& m3, T& m4) {
     m0 = m1 = m2 = m3 = m4 = T(0);
 #pragma unroll
     for (int k = 0; k < SSIM_TAPS; ++k) {
-        const T a = p[off + k], c = t[off + k];
+        const T a = t[off + k], c = d[off + k];
         m0 = fma(w[k], a, m0);
         m1 = fma(w[k], c, m1);
         m2 = fma(w[k], a * a, m2);
@@ -128,17 +164,23 @@ __device__ __forceinline__ void vsum5(const T* __restrict__ hb, int ps, int rs, 
 
 template <typename T>
 struct SsimTerms {
-    T a1, a2, b1, b2;
+    T mu_t, mu_p, mu_d, s_dd, a1, a2, b1, b2;
 };
 
+// The window's terms from the moments m = (mu_t', mu_d, E[t'^2], E[d^2], E[t'd]) of t' = t - k and d = p - t.
 template <typename T>
-__device__ __forceinline__ SsimTerms<T> ssim_terms(const T m[5], T c1, T c2) {
-    const T mp = m[0], mt = m[1], mpt = mp * mt, mpp = mp * mp, mtt = mt * mt;
+__device__ __forceinline__ SsimTerms<T> ssim_terms(const T m[5], T k, T eps, T c1, T c2) {
     SsimTerms<T> s;
-    s.a1 = T(2) * mpt + c1;
-    s.a2 = T(2) * (m[4] - mpt) + c2;
-    s.b1 = mpp + mtt + c1;
-    s.b2 = (m[2] - mpp) + (m[3] - mtt) + c2;
+    s.mu_d = m[1];
+    s.mu_t = (k - k * eps) + m[0];
+    s.mu_p = s.mu_t + s.mu_d;
+    const T s_tt = (m[2] - m[0] * m[0]) + k * eps * (m[0] + s.mu_t);
+    const T s_td = (m[4] - m[0] * m[1]) + k * eps * m[1];
+    s.s_dd = m[3] - m[1] * m[1];
+    s.a1 = T(2) * s.mu_p * s.mu_t + c1;
+    s.b1 = s.a1 + s.mu_d * s.mu_d;
+    s.a2 = T(2) * (s_tt + s_td) + c2;
+    s.b2 = s.a2 + s.s_dd;
     return s;
 }
 
@@ -171,27 +213,29 @@ __global__ void __launch_bounds__(LOSS_THREADS)
     k_photometric_loss_fwd(LossArgs<T> A, double2* __restrict__ partials, unsigned int* __restrict__ ticket,
                            T* __restrict__ out, double l1_weight, double ssim_weight) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    T* sp = reinterpret_cast<T*>(smem_raw);
-    T* st = sp + LOSS_CG * FWD_IH * FWD_IW;
-    T* hb = st + LOSS_CG * FWD_IH * FWD_IW;  // [5][IH][TW]
+    T* st = reinterpret_cast<T*>(smem_raw);
+    T* sd = st + LOSS_CG * FWD_IH * FWD_IW;
+    T* hb = sd + LOSS_CG * FWD_IH * FWD_IW;  // [5][IH][TW]
     __shared__ double red[2 * LOSS_THREADS / 32];
     __shared__ bool is_last;
+    __shared__ T k[LOSS_CG];  // the channel group's shifts
 
     const int tx0 = blockIdx.x * LOSS_TW, ty0 = blockIdx.y * LOSS_TH, b = blockIdx.z;
     const int H = A.H, W = A.W;
     double acc_s = 0.0, acc_l1 = 0.0;
     for (int c0 = 0; c0 < A.C; c0 += LOSS_CG) {
         const int cg = min(LOSS_CG, A.C - c0);
-        stage_region(sp, A.pred, A.ps, b, c0, cg, ty0, tx0, FWD_IH, FWD_IW, H, W);
-        stage_region(st, A.target, A.ts, b, c0, cg, ty0, tx0, FWD_IH, FWD_IW, H, W);
+        tile_shifts(A, b, c0, cg, ty0, tx0, k);
+        __syncthreads();
+        stage_region(st, sd, A, b, c0, cg, ty0, tx0, FWD_IH, FWD_IW, k);
         __syncthreads();
         for (int c = 0; c < cg; ++c) {
-            const T* p = sp + c * FWD_IH * FWD_IW;
             const T* t = st + c * FWD_IH * FWD_IW;
+            const T* d = sd + c * FWD_IH * FWD_IW;
             for (int e = threadIdx.x; e < FWD_IH * LOSS_TW; e += LOSS_THREADS) {
                 const int r = e / LOSS_TW, j = e % LOSS_TW;
                 T m0, m1, m2, m3, m4;
-                hsum5(p, t, r * FWD_IW + j, A.w, m0, m1, m2, m3, m4);
+                hsum5(t, d, r * FWD_IW + j, A.w, m0, m1, m2, m3, m4);
                 constexpr int PL = FWD_IH * LOSS_TW;
                 hb[e] = m0;
                 hb[PL + e] = m1;
@@ -203,15 +247,15 @@ __global__ void __launch_bounds__(LOSS_THREADS)
             for (int e = threadIdx.x; e < LOSS_TH * LOSS_TW; e += LOSS_THREADS) {
                 const int i = e / LOSS_TW, j = e % LOSS_TW;
                 const int y = ty0 + i, x = tx0 + j;
-                if (y < H && x < W) acc_l1 += (double)fabs(p[i * FWD_IW + j] - t[i * FWD_IW + j]);
+                if (y < H && x < W) acc_l1 += (double)fabs(d[i * FWD_IW + j]);
                 if (y < H - SSIM_HALO && x < W - SSIM_HALO) {
                     T m[5];
                     vsum5(hb, FWD_IH * LOSS_TW, LOSS_TW, i, j, A.w, m);
-                    const SsimTerms<T> s = ssim_terms(m, A.c1, A.c2);
-                    acc_s += (double)((s.a1 * s.a2) / (s.b1 * s.b2));
+                    const SsimTerms<T> s = ssim_terms(m, k[c], A.eps, A.c1, A.c2);
+                    acc_s += (double)((s.mu_d * s.mu_d * s.b2 + s.a1 * s.s_dd) / (s.b1 * s.b2));
                 }
             }
-            __syncthreads();  // hb / sp / st are rewritten next
+            __syncthreads();  // hb / st / sd are rewritten next
         }
     }
 
@@ -236,10 +280,10 @@ __global__ void __launch_bounds__(LOSS_THREADS)
     if (threadIdx.x == 0) {
         const double numel = (double)A.B * A.C * H * W;
         const double n_valid = (double)A.B * A.C * (H - SSIM_HALO) * (W - SSIM_HALO);
-        const double l1 = l / numel, ssim = s / n_valid;
-        out[0] = (T)(l1_weight * l1 + ssim_weight * (1.0 - ssim));
+        const double l1 = l / numel, one_minus_ssim = s / n_valid;
+        out[0] = (T)(l1_weight * l1 + ssim_weight * one_minus_ssim);
         out[1] = (T)l1;
-        out[2] = (T)ssim;
+        out[2] = (T)(1.0 - one_minus_ssim);
         *ticket = 0u;  // ready for the next launch on the same buffer
     }
 }
@@ -249,11 +293,12 @@ __global__ void __launch_bounds__(LOSS_THREADS)
     k_photometric_loss_bwd(LossArgs<T> A, const T* __restrict__ grad_loss, T* __restrict__ grad, long long gs0,
                            long long gs1, long long gs2, long long gs3, T l1_scale, T ssim_scale) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    T* sp = reinterpret_cast<T*>(smem_raw);
-    T* st = sp + LOSS_CG * BWD_RH * BWD_RW;
-    T* hb = st + LOSS_CG * BWD_RH * BWD_RW;  // [5][RH][OW], then [3][OH][TW]
+    T* st = reinterpret_cast<T*>(smem_raw);
+    T* sd = st + LOSS_CG * BWD_RH * BWD_RW;
+    T* hb = sd + LOSS_CG * BWD_RH * BWD_RW;  // [5][RH][OW], then [3][OH][TW]
     T* db = hb + 5 * BWD_RH * BWD_OW;        // [3][OH][OW]
     T* gb = db + 3 * BWD_OH * BWD_OW;        // [CG][TH][TW]
+    __shared__ T k[LOSS_CG];                  // the channel group's shifts
 
     const int tx0 = blockIdx.x * LOSS_TW, ty0 = blockIdx.y * LOSS_TH, b = blockIdx.z;
     const int H = A.H, W = A.W;
@@ -262,17 +307,18 @@ __global__ void __launch_bounds__(LOSS_THREADS)
     const long long gs[4] = {gs0, gs1, gs2, gs3};
     for (int c0 = 0; c0 < A.C; c0 += LOSS_CG) {
         const int cg = min(LOSS_CG, A.C - c0);
-        stage_region(sp, A.pred, A.ps, b, c0, cg, ry0, rx0, BWD_RH, BWD_RW, H, W);
-        stage_region(st, A.target, A.ts, b, c0, cg, ry0, rx0, BWD_RH, BWD_RW, H, W);
+        tile_shifts(A, b, c0, cg, ty0, tx0, k);
+        __syncthreads();
+        stage_region(st, sd, A, b, c0, cg, ry0, rx0, BWD_RH, BWD_RW, k);
         __syncthreads();
         for (int c = 0; c < cg; ++c) {
-            const T* p = sp + c * BWD_RH * BWD_RW;
             const T* t = st + c * BWD_RH * BWD_RW;
+            const T* d = sd + c * BWD_RH * BWD_RW;
             constexpr int PL = BWD_RH * BWD_OW;
             for (int e = threadIdx.x; e < PL; e += LOSS_THREADS) {
                 const int r = e / BWD_OW, u = e % BWD_OW;
                 T m0, m1, m2, m3, m4;
-                hsum5(p, t, r * BWD_RW + u, A.w, m0, m1, m2, m3, m4);
+                hsum5(t, d, r * BWD_RW + u, A.w, m0, m1, m2, m3, m4);
                 hb[e] = m0;
                 hb[PL + e] = m1;
                 hb[2 * PL + e] = m2;
@@ -284,21 +330,22 @@ __global__ void __launch_bounds__(LOSS_THREADS)
             for (int e = threadIdx.x; e < DL; e += LOSS_THREADS) {
                 const int v = e / BWD_OW, u = e % BWD_OW;
                 const int oy = ry0 + v, ox = rx0 + u;
-                T d_mu = T(0), d_pp = T(0), d_pt = T(0);
+                T d_g = T(0), d_pp = T(0), d_e = T(0);
                 if (oy >= 0 && oy < H - SSIM_HALO && ox >= 0 && ox < W - SSIM_HALO) {
                     T m[5];
                     vsum5(hb, PL, BWD_OW, v, u, A.w, m);
-                    const SsimTerms<T> s = ssim_terms(m, A.c1, A.c2);
+                    const T kc = k[c];
+                    const SsimTerms<T> s = ssim_terms(m, kc, A.eps, A.c1, A.c2);
                     const T den = s.b1 * s.b2;
                     const T S = (s.a1 * s.a2) / den;
-                    const T inv = T(1) / den;
-                    d_mu = (T(2) * m[1] * (s.a2 - s.a1) - S * (T(2) * m[0] * (s.b2 - s.b1))) * inv;
                     d_pp = -S / s.b2;
-                    d_pt = T(2) * s.a1 * inv;
+                    d_e = T(2) * s.a1 * s.s_dd / (den * s.b2);
+                    const T ds_dmu = T(-2) * s.a2 * s.mu_d * (s.mu_t * (s.mu_p + s.mu_t) + A.c1) / (s.b1 * den);
+                    d_g = ds_dmu - T(2) * s.mu_d * d_pp - (m[0] - kc * A.eps) * d_e;
                 }
-                db[e] = d_mu;
+                db[e] = d_g;
                 db[DL + e] = d_pp;
-                db[2 * DL + e] = d_pt;
+                db[2 * DL + e] = d_e;
             }
             __syncthreads();
             // transposed horizontal pass: pixel column j collects origins j + 10 - k (local origin coordinates)
@@ -324,11 +371,10 @@ __global__ void __launch_bounds__(LOSS_THREADS)
                     for (int k = 0; k < SSIM_TAPS; ++k) s = fma(A.w[k], hb[q * TL + (i + SSIM_HALO - k) * LOSS_TW + j], s);
                     dq[q] = s;
                 }
-                const T pv = p[(i + SSIM_HALO) * BWD_RW + j + SSIM_HALO];
+                const T dv = d[(i + SSIM_HALO) * BWD_RW + j + SSIM_HALO];
                 const T tv = t[(i + SSIM_HALO) * BWD_RW + j + SSIM_HALO];
-                const T diff = pv - tv;
-                const T sgn = diff > T(0) ? T(1) : (diff < T(0) ? T(-1) : T(0));
-                const T ssim_part = dq[0] + T(2) * pv * dq[1] + tv * dq[2];
+                const T sgn = dv > T(0) ? T(1) : (dv < T(0) ? T(-1) : T(0));
+                const T ssim_part = dq[0] + T(2) * dv * dq[1] + tv * dq[2];
                 gb[c * LOSS_TH * LOSS_TW + e] = g * (l1_scale * sgn - ssim_scale * ssim_part);
             }
             __syncthreads();  // hb is rewritten by the next channel
@@ -353,7 +399,7 @@ __global__ void __launch_bounds__(LOSS_THREADS)
             const int y = ty0 + i, x = tx0 + j;
             if (y < H && x < W) grad[base + c * gs[1] + y * gs[2] + x * gs[3]] = gb[(c * LOSS_TH + i) * LOSS_TW + j];
         }
-        __syncthreads();  // gb / sp / st are rewritten by the next channel group
+        __syncthreads();  // gb / st / sd are rewritten by the next channel group
     }
 }
 
@@ -379,9 +425,14 @@ static LossArgs<T> loss_args(int B, int C, int H, int W, const void* pred, const
     A.C = C;
     A.H = H;
     A.W = W;
-    for (int k = 0; k < SSIM_TAPS; ++k) A.w[k] = (T)window[k];
+    double sum = 0.0;
+    for (int k = 0; k < SSIM_TAPS; ++k) {
+        A.w[k] = (T)window[k];
+        sum += (double)A.w[k];
+    }
     A.c1 = (T)c1;
     A.c2 = (T)c2;
+    A.eps = (T)(1.0 - sum * sum);
     return A;
 }
 

@@ -39,14 +39,25 @@ def _moments(p, t):
 
 
 def forward(pred, target, ssim_frac, data_range=1.0):
-    """(loss, L1, SSIM) as python floats; pred / target [H,W,C] or [B,C,H,W]."""
+    """(loss, L1, SSIM) as python floats; pred / target [H,W,C] or [B,C,H,W].
+
+    1 - S is formed per window from the moments of d = p - t, (mu_d^2 b2 + a1 s_dd) / (b1 b2), since b1 - a1 = mu_d^2
+    and b2 - a2 = s_dd: 1 - a1 a2 / (b1 b2) would cancel most digits where the images nearly agree."""
     p, t = _nchw(pred), _nchw(target)
+    C = p.shape[1]
     c1, c2 = (K1 * data_range) ** 2, (K2 * data_range) ** 2
     mp, mt, epp, ett, ept = _moments(p, t)
-    s = ((2 * mp * mt + c1) * (2 * (ept - mp * mt) + c2)) / ((mp * mp + mt * mt + c1) * ((epp - mp * mp) + (ett - mt * mt) + c2))
-    l1 = float((p - t).abs().mean())
-    ssim = float(s.mean())
-    return (1.0 - ssim_frac) * l1 + ssim_frac * (1.0 - ssim), l1, ssim
+    k = _window2d(C, p.device)
+    d = p - t
+    mu_d = F.conv2d(d, k, groups=C)
+    s_dd = F.conv2d(d * d, k, groups=C) - mu_d * mu_d
+    a1 = 2 * mp * mt + c1
+    b1 = mp * mp + mt * mt + c1
+    b2 = (epp - mp * mp) + (ett - mt * mt) + c2
+    one_minus_s = (mu_d * mu_d * b2 + a1 * s_dd) / (b1 * b2)
+    l1 = float(d.abs().mean())
+    one_minus_ssim = float(one_minus_s.mean())
+    return (1.0 - ssim_frac) * l1 + ssim_frac * one_minus_ssim, l1, 1.0 - one_minus_ssim
 
 
 def grad(pred, target, ssim_frac, data_range=1.0, grad_loss=1.0):
