@@ -14,9 +14,11 @@
                             readout-motion gradients (include/gsr_shutter.h)
   libgsr_bilagrid.so        bilateral-grid appearance correction: slice forward / backward, total variation
                             (include/gsr_bilagrid.h)
+  libgsr_surfels.so         2-D Gaussian surfels: per-gaussian and tile kernels of rasterize_surfels
+                            (include/gsr_surfels.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all eleven (the CUDA libraries from the LIBS table);
+`python -m gaussian_splatting_b200.build` builds all twelve (the CUDA libraries from the LIBS table);
 `build(force=False)` is incremental.
 """
 from __future__ import annotations
@@ -95,6 +97,8 @@ LIBS = [
     (PKG / "libgsr_bilagrid.so", ["gsr_bilagrid.cu"],
      [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_bilagrid.h"],
      "bilagrid_lib.sha256"),
+    (PKG / "libgsr_surfels.so", ["gsr_surfels.cu"],
+     CUH + [ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_surfels.h"], "surfels_lib.sha256"),
 ]
 
 NVCC_FLAGS = [
@@ -172,7 +176,8 @@ def build_ext(force: bool = False) -> Path:
                     ROOT / "include" / "gsr_features.h", ROOT / "include" / "gsr_batch.h",
                     ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h",
                     ROOT / "include" / "gsr_pose.h", ROOT / "include" / "gsr_bilagrid.h",
-                    ROOT / "include" / "gsr_calib.h", ROOT / "include" / "gsr_shutter.h"], torch.__version__)
+                    ROOT / "include" / "gsr_calib.h", ROOT / "include" / "gsr_shutter.h",
+                    ROOT / "include" / "gsr_surfels.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -184,7 +189,7 @@ def build_ext(force: bool = False) -> Path:
         f"-D_GLIBCXX_USE_CXX11_ABI={int(torch._C._GLIBCXX_USE_CXX11_ABI)}",
         *incs, str(src), "-o", str(out),
         f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", "-lgsr_fisheye",
-        "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid", "-lgsr_calib", "-lgsr_shutter",
+        "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid", "-lgsr_calib", "-lgsr_shutter", "-lgsr_surfels",
         f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",

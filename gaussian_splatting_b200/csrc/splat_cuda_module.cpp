@@ -20,6 +20,7 @@
 #include "../../include/gsr_calib.h"
 #include "../../include/gsr_bilagrid.h"
 #include "../../include/gsr_shutter.h"
+#include "../../include/gsr_surfels.h"
 
 namespace {
 
@@ -1593,6 +1594,172 @@ torch::Tensor bilagrid_tv_backward(torch::Tensor grids, torch::Tensor grad_tv) {
     return grad;
 }
 
+// ---- 2-D Gaussian surfels (libgsr_surfels.so) -------------------------------------------------------------------------
+static const float* opt_f32(const c10::optional<torch::Tensor>& t) {
+    if (!t.has_value()) return nullptr;
+    CHECK_VALID_INPUT((*t)); CHECK_FLOAT_TENSOR((*t));
+    return t->data_ptr<float>();
+}
+
+// returns (surfels [N,20], bin_records [N,12], depth_key, visible, scan, tile_mask, tile_win): the inputs of fused_bin
+// (with bin_records as its records) and of the surfel tile kernels
+std::vector<torch::Tensor> surfel_forward(torch::Tensor xyz, c10::optional<torch::Tensor> xyz_cam,
+                                          torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+                                          torch::Tensor rgb, c10::optional<torch::Tensor> sh_rest,
+                                          torch::Tensor camera_T_world, torch::Tensor K,
+                                          c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+                                          double near_thresh, double far_thresh, double pad, double mh_dist,
+                                          int64_t depth_base) {
+    for (const torch::Tensor* t : {&xyz, &quaternion, &scale, &opacity_logit, &rgb, &camera_T_world, &K}) {
+        CHECK_VALID_INPUT((*t)); CHECK_FLOAT_TENSOR((*t));
+    }
+    const int64_t N = xyz.size(0);
+    const int n_rest = sh_rest.has_value() ? (int)sh_rest->size(2) : 0;
+    const float* cam = opt_f32(xyz_cam);
+    const int cam_first = xyz_cam.has_value() ? (int)(N - xyz_cam->size(0)) : 0;
+    c10::cuda::CUDAGuard guard(xyz.device());
+    auto opt = xyz.options();
+    torch::Tensor surfels = torch::empty({N, GSR_SURFEL_REC_FLOATS}, opt);
+    torch::Tensor bins = torch::empty({N, GSR_REC_FLOATS}, opt);
+    torch::Tensor zkey = torch::empty({N}, opt.dtype(torch::kInt32));
+    torch::Tensor visible = torch::empty({N}, opt.dtype(torch::kUInt8));
+    torch::Tensor scan = torch::empty({N}, opt.dtype(torch::kInt64));
+    torch::Tensor tile_mask = torch::empty({N}, opt.dtype(torch::kInt64));
+    torch::Tensor tile_win = torch::empty({N}, opt.dtype(torch::kInt32));
+    torch::Tensor temp = torch::empty({(int64_t)gsr_surfel_temp_bytes((int)N)}, opt.dtype(torch::kUInt8));
+    check_rc(gsr_surfel_preprocess_forward(
+                 (int)N, n_rest, F32PTR(xyz), cam, cam_first, F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit),
+                 F32PTR(rgb), opt_f32(sh_rest), F32PTR(camera_T_world), F32PTR(K), opt_f32(camera_centre), (int)H,
+                 (int)W, (float)near_thresh, (float)far_thresh, (float)pad, (float)mh_dist, (uint32_t)depth_base,
+                 F32PTR(surfels), F32PTR(bins), (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),
+                 (uint64_t*)scan.data_ptr<int64_t>(), (uint64_t*)tile_mask.data_ptr<int64_t>(),
+                 (uint32_t*)tile_win.data_ptr<int>(), temp.data_ptr(), (size_t)temp.numel(), cur_stream()),
+             "gsr_surfel_preprocess_forward");
+    return {surfels, bins, zkey, visible, scan, tile_mask, tile_win};
+}
+
+// returns (image [H,W,3], depth [H,W,1], alpha [H,W,1], normal [H,W,3], distortion [H,W,1], last [H,W] i32,
+// totals [H,W,3])
+std::vector<torch::Tensor> surfel_render_forward(torch::Tensor surfels, torch::Tensor ranges, torch::Tensor background,
+                                                 int64_t H, int64_t W, int64_t P,
+                                                 c10::optional<torch::Tensor> keys_sorted,
+                                                 c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                                 double near_thresh, double m_scale, double mh_dist) {
+    CHECK_VALID_INPUT(surfels); CHECK_FLOAT_TENSOR(surfels);
+    CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
+    TORCH_CHECK(background.numel() == 3, "Background RGB must have 3 elements");
+    c10::cuda::CUDAGuard guard(surfels.device());
+    auto opt = surfels.options();
+    torch::Tensor image = torch::empty({H, W, 3}, opt), depth = torch::empty({H, W, 1}, opt),
+                  alpha = torch::empty({H, W, 1}, opt), normal = torch::empty({H, W, 3}, opt),
+                  dist = torch::empty({H, W, 1}, opt), last = torch::empty({H, W}, opt.dtype(torch::kInt32)),
+                  totals = torch::empty({H, W, 3}, opt);
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    const bool keys = ps.keys != nullptr;  // else ids (with P == 0 a placeholder the kernels never read)
+    check_rc(gsr_surfel_render_forward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0, keys ? nullptr : ps.ids,
+                                       ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W, (float)near_thresh,
+                                       (float)m_scale, (float)mh_dist, F32PTR(image), F32PTR(depth), F32PTR(alpha),
+                                       F32PTR(normal), F32PTR(dist), last.data_ptr<int>(), F32PTR(totals),
+                                       cur_stream()),
+             "gsr_surfel_render_forward");
+    return {image, depth, alpha, normal, dist, last, totals};
+}
+
+// the surfel gradient rows [N, 20] (zero-filled, accumulated by the tile backward)
+torch::Tensor surfel_render_backward(int64_t N, torch::Tensor surfels, torch::Tensor ranges, torch::Tensor background,
+                                     int64_t H, int64_t W, int64_t P, c10::optional<torch::Tensor> keys_sorted,
+                                     c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, double near_thresh,
+                                     double m_scale, double mh_dist, torch::Tensor alpha, torch::Tensor last,
+                                     torch::Tensor totals, torch::Tensor g_image, torch::Tensor g_depth,
+                                     torch::Tensor g_alpha, torch::Tensor g_normal, torch::Tensor g_distortion) {
+    for (const torch::Tensor* t : {&surfels, &background, &alpha, &totals, &g_image, &g_depth, &g_alpha, &g_normal,
+                                   &g_distortion}) {
+        CHECK_VALID_INPUT((*t)); CHECK_FLOAT_TENSOR((*t));
+    }
+    TORCH_CHECK(g_image.numel() == H * W * 3 && g_normal.numel() == H * W * 3 && g_depth.numel() == H * W &&
+                    g_alpha.numel() == H * W && g_distortion.numel() == H * W,
+                "upstream gradients must match the maps' shapes");
+    c10::cuda::CUDAGuard guard(surfels.device());
+    torch::Tensor rows = torch::zeros({N, GSR_SURFEL_GRAD_FLOATS}, surfels.options());
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    const bool keys = ps.keys != nullptr;
+    check_rc(gsr_surfel_render_backward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0, keys ? nullptr : ps.ids,
+                                        ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
+                                        (float)near_thresh, (float)m_scale, (float)mh_dist, F32PTR(alpha),
+                                        last.data_ptr<int>(), F32PTR(totals), F32PTR(g_image), F32PTR(g_depth),
+                                        F32PTR(g_alpha), F32PTR(g_normal), F32PTR(g_distortion), F32PTR(rows),
+                                        cur_stream()),
+             "gsr_surfel_render_backward");
+    return rows;
+}
+
+// uv.grad [M,2] of the visible gaussians vis_idx from the gradient rows
+torch::Tensor surfel_uv_grad(torch::Tensor vis_idx, torch::Tensor surfels, torch::Tensor rows) {
+    CHECK_VALID_INPUT(vis_idx); CHECK_INT_TENSOR(vis_idx);
+    CHECK_VALID_INPUT(surfels); CHECK_VALID_INPUT(rows);
+    c10::cuda::CUDAGuard guard(surfels.device());
+    const int64_t M = vis_idx.numel();
+    torch::Tensor out = torch::empty({M, 2}, surfels.options());
+    check_rc(gsr_surfel_uv_grad((int)M, vis_idx.data_ptr<int>(), F32PTR(surfels), F32PTR(rows), F32PTR(out),
+                                cur_stream()),
+             "gsr_surfel_uv_grad");
+    return out;
+}
+
+// the per-gaussian backward into the flat layout of fused_preprocess_backward (out_flat: a caller-owned buffer of it);
+// returns the gaussian gradients (xyz, quaternion, scale, opacity, rgb[, sh]) and then `flat`
+std::vector<torch::Tensor> surfel_backward(torch::Tensor rows, torch::Tensor xyz, torch::Tensor quaternion,
+                                           torch::Tensor scale, torch::Tensor opacity_logit,
+                                           c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
+                                           torch::Tensor K, c10::optional<torch::Tensor> camera_centre,
+                                           torch::Tensor visible, torch::Tensor surfels,
+                                           c10::optional<torch::Tensor> out_flat,
+                                           c10::optional<torch::Tensor> grad_uv_compact,
+                                           c10::optional<torch::Tensor> scan, bool uv_grad_emitted) {
+    for (const torch::Tensor* t : {&rows, &xyz, &quaternion, &scale, &opacity_logit, &camera_T_world, &K, &surfels}) {
+        CHECK_VALID_INPUT((*t)); CHECK_FLOAT_TENSOR((*t));
+    }
+    CHECK_VALID_INPUT(visible);
+    const int64_t N = xyz.size(0);
+    TORCH_CHECK(rows.numel() == N * GSR_SURFEL_GRAD_FLOATS && surfels.numel() == N * GSR_SURFEL_REC_FLOATS &&
+                    visible.numel() == N,
+                "surfel rows, records and visible must hold one entry per gaussian");
+    const int n_rest = sh_rest.has_value() ? (int)sh_rest->size(2) : 0;
+    const float* guv = nullptr;
+    const uint64_t* scan_ptr = nullptr;
+    if (grad_uv_compact.has_value() && grad_uv_compact->numel() > 0) {
+        guv = opt_f32(grad_uv_compact);
+        TORCH_CHECK(scan.has_value() && scan->numel() == N, "grad_uv_compact needs the forward's scan");
+        scan_ptr = (const uint64_t*)scan->data_ptr<int64_t>();
+    }
+    c10::cuda::CUDAGuard guard(xyz.device());
+    const FlatLayout l = flat_layout(N, n_rest);
+    torch::Tensor flat;
+    if (out_flat.has_value()) {
+        flat = *out_flat;
+        CHECK_VALID_INPUT(flat); CHECK_FLOAT_TENSOR(flat);
+        TORCH_CHECK(flat.numel() == l.off[6], "out_flat must hold ", l.off[6], " floats");
+    } else {
+        flat = torch::empty({l.off[6]}, xyz.options());
+    }
+    for (int i = 0; i < 6; ++i)
+        if (l.off[i + 1] > l.off[i] + N * l.width[i])
+            flat.narrow(0, l.off[i] + N * l.width[i], l.off[i + 1] - l.off[i] - N * l.width[i]).zero_();
+    auto section = [&](int i, std::vector<int64_t> shape) { return flat.narrow(0, l.off[i], N * l.width[i]).view(shape); };
+    std::vector<torch::Tensor> out = {section(0, {N, 3}), section(1, {N, 4}), section(2, {N, 3}), section(3, {N}),
+                                      section(4, {N, 3})};
+    if (n_rest) out.push_back(section(5, {N, 3, (int64_t)n_rest}));
+    check_rc(gsr_surfel_preprocess_backward((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
+                                            F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
+                                            opt_f32(camera_centre), visible.data_ptr<uint8_t>(), F32PTR(surfels),
+                                            F32PTR(rows), guv, scan_ptr, uv_grad_emitted ? 1 : 0, F32PTR(out[0]),
+                                            F32PTR(out[1]), F32PTR(out[2]), F32PTR(out[3]), F32PTR(out[4]),
+                                            n_rest ? F32PTR(out[5]) : nullptr, cur_stream()),
+             "gsr_surfel_preprocess_backward");
+    out.push_back(flat);
+    return out;
+}
+
 std::string version() { return gsr_version(); }
 
 }  // namespace
@@ -1727,6 +1894,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("need_grids"));
     m.def("bilagrid_tv_forward", &bilagrid_tv_forward, "total variation of the grids, on the device");
     m.def("bilagrid_tv_backward", &bilagrid_tv_backward, "total variation backward -> gradient on the grids");
+    m.def("surfel_forward", &surfel_forward, "2-D surfels: per-gaussian forward (gsr_surfel_preprocess_forward)");
+    m.def("surfel_render_forward", &surfel_render_forward, "2-D surfels: tile forward (gsr_surfel_render_forward)");
+    m.def("surfel_render_backward", &surfel_render_backward, "2-D surfels: tile backward (gsr_surfel_render_backward)");
+    m.def("surfel_uv_grad", &surfel_uv_grad, "2-D surfels: uv.grad of the visible gaussians (gsr_surfel_uv_grad)");
+    m.def("surfel_backward", &surfel_backward, "2-D surfels: per-gaussian backward (gsr_surfel_preprocess_backward)");
     m.def("version", &version, "library version string");
     m.def("contribution_mask_words",
           [](int64_t P, int64_t H, int64_t W) { return (int64_t)gsr_contribution_mask_words(P, (int)H, (int)W); },

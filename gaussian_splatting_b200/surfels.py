@@ -1,0 +1,203 @@
+"""rasterize_surfels(): 2-D Gaussian surfels (2DGS, Huang et al., SIGGRAPH 2024) in the fused rasterizer.
+
+The scene is the 3DGS scene (mean, quaternion, scales, opacity logit, SH) and binning is the 3DGS binning; each gaussian
+is rendered as a flat disk whose two tangent axes are scale[:, 0] and scale[:, 1] (scale[:, 2] is not used and gets an
+exact 0 gradient).  Per pixel the ray meets the surfel at a point (a, b) of its plane, so depth lies on the surface and
+every surfel has a normal.  The model is DESIGN.md 3.25; the kernels are libgsr_surfels.so (include/gsr_surfels.h).
+
+Two autograd nodes, as in rasterize():
+
+    _ProjectSurfels    params -> uv [M,2], carrier          (gsr_surfel_preprocess_forward, binning, tile forward)
+    _CompositeSurfels  uv, carrier -> image, depth, alpha, normal, distortion
+
+``carrier`` only carries the tile backward's per-surfel gradient rows [N,20] to the per-gaussian backward, which writes
+the flat gradient layout of rasterize() (state.grad_flat, or grad_out), so FlatAdam, DensificationStats,
+AdaptiveDensityControl and MCMCDensityControl drive a surfel scene unchanged.
+"""
+from __future__ import annotations
+
+import math
+import weakref
+
+import torch
+
+from . import native
+from .rasterize import (IN_KERNEL_TRANSFORM, IN_KERNEL_TRANSFORM_MIN_N, _depth_key_params, in_kernel_transform_ok,
+                        native_centre_ok, tail_positions)
+from .utils import transform_points_torch
+
+
+class _SurfelState:
+    """Per-view buffers shared by the two autograd nodes (return_state=True hands it out).  vis_idx / vis_idx32: the
+    visible gaussians, ascending (the order of uv); grad_flat: the flat gradient of the last backward."""
+
+    __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "vis_idx32", "scan", "surfels", "ranges", "keys_sorted",
+                 "ids_sorted", "id_bits", "maps", "last", "totals", "background", "near", "m_scale", "mh", "grad_flat",
+                 "grad_out", "uv_ref", "uv_grad_emitted", "uv_absgrad")
+
+    def __init__(self):
+        self.grad_flat = self.grad_out = self.uv_ref = self.uv_absgrad = None
+        self.uv_grad_emitted = False
+
+
+class _ProjectSurfels(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, xyz, quaternion, scale, opacity, rgb, sh, camera_T_world, K, state, cfg):
+        ext = native()
+        H, W, near, far, pad, mh = cfg
+        depth_base, depth_bits = _depth_key_params(near, far)
+        opacity_flat = opacity.reshape(-1)
+        N = xyz.shape[0]
+        # camera-frame positions and camera centre exactly as rasterize() forms them, so that uv and the culling mask
+        # are bit-identical to rasterize's
+        if IN_KERNEL_TRANSFORM and N >= IN_KERNEL_TRANSFORM_MIN_N and in_kernel_transform_ok(xyz.device):
+            xyz_cam = tail_positions(xyz, camera_T_world)
+        else:
+            xyz_cam = transform_points_torch(xyz, camera_T_world)
+        centre = None
+        if sh is not None:
+            if native_centre_ok(xyz.device):
+                centre = ext.camera_centre(camera_T_world)
+            else:
+                centre = torch.linalg.inv_ex(camera_T_world)[0][:3, 3].contiguous()
+        surfels, bins, zkey, visible, scan, tile_mask, tile_win = ext.surfel_forward(
+            xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far, pad,
+            mh, depth_base)
+        total = int(scan[-1].item()) if N > 0 else 0
+        M, P = total >> 32, total & 0xFFFFFFFF
+        if M > N or P >= 2**31:
+            raise RuntimeError(f"rasterize_surfels: {P} (gaussian, tile) pairs / {M} visible of {N} gaussians exceed "
+                               "the int32 pair index of the native path (P must be < 2^31)")
+        ids_sorted, ranges, vis_idx, uv, keys_sorted, id_bits = ext.fused_bin(
+            bins, zkey, visible, scan, M, P, H, W, mh, depth_bits, False, tile_mask, tile_win)
+        m_scale = far / (far - near) if math.isfinite(far) else 1.0
+        rendered = ext.surfel_render_forward(surfels, ranges, state.background, H, W, P, keys_sorted, ids_sorted,
+                                             int(id_bits), near, m_scale, mh)
+        state.N, state.M, state.P, state.H, state.W = N, M, P, H, W
+        state.visible, state.vis_idx, state.vis_idx32, state.scan = visible, vis_idx, vis_idx, scan
+        state.surfels, state.ranges, state.keys_sorted, state.ids_sorted, state.id_bits = (
+            surfels, ranges, keys_sorted, ids_sorted, int(id_bits))
+        state.maps, state.last, state.totals = rendered[:5], rendered[5], rendered[6]
+        state.near, state.m_scale, state.mh = near, m_scale, mh
+        ctx.state = state
+        ctx.has_sh = sh is not None
+        ctx.opacity_shape = opacity.shape
+        ctx.save_for_backward(xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre)
+        carrier = torch.empty(20 * N, dtype=xyz.dtype, device=xyz.device)
+        return uv, carrier
+
+    @staticmethod
+    def backward(ctx, grad_uv, grad_carrier):
+        xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre = ctx.saved_tensors
+        st = ctx.state
+        if grad_carrier is None:
+            grad_carrier = torch.zeros(20 * st.N, dtype=xyz.dtype, device=xyz.device)
+        guv = grad_uv.contiguous() if grad_uv is not None and st.M > 0 else None
+        out = native().surfel_backward(grad_carrier.contiguous(), xyz, quaternion, scale, opacity_flat, sh,
+                                       camera_T_world, K, centre, st.visible, st.surfels, st.grad_out, guv,
+                                       st.scan if guv is not None else None, st.uv_grad_emitted)
+        g_xyz, g_q, g_s, g_o, g_dc = out[:5]
+        g_sh = out[5] if ctx.has_sh else None
+        st.grad_flat = out[-1]
+        return g_xyz, g_q, g_s, g_o.view(ctx.opacity_shape), g_dc, g_sh, None, None, None, None
+
+
+class _CompositeSurfels(torch.autograd.Function):
+    """uv, carrier -> (image, depth, alpha, normal, distortion); the tile forward already ran in _ProjectSurfels."""
+
+    @staticmethod
+    def forward(ctx, uv, carrier, state):
+        ctx.state = state
+        maps = state.maps
+        state.maps = None
+        ctx.save_for_backward(maps[2])  # alpha: the backward's total weight and final transmittance
+        return tuple(maps)
+
+    @staticmethod
+    def backward(ctx, g_image, g_depth, g_alpha, g_normal, g_dist):
+        st = ctx.state
+        (alpha,) = ctx.saved_tensors
+
+        def grad(g, k):
+            return torch.zeros(st.H, st.W, k, device=alpha.device) if g is None else g.contiguous()
+
+        rows = native().surfel_render_backward(
+            st.N, st.surfels, st.ranges, st.background, st.H, st.W, st.P, st.keys_sorted, st.ids_sorted, st.id_bits,
+            st.near, st.m_scale, st.mh, alpha, st.last, st.totals, grad(g_image, 3), grad(g_depth, 1),
+            grad(g_alpha, 1), grad(g_normal, 3), grad(g_dist, 1))
+        # uv.grad (d loss / d footprint translation) is formed only when somebody can observe it, as in rasterize()
+        uv_t = st.uv_ref() if st.uv_ref is not None else None
+        watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
+        st.uv_grad_emitted = bool(watched)
+        grad_uv = native().surfel_uv_grad(st.vis_idx, st.surfels, rows) if watched else None
+        return grad_uv, rows.view(-1), None
+
+
+def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
+                      background_rgb, return_state=False, grad_out=None):
+    """Render the gaussians as 2-D surfels.  Arguments as rasterize() with use_sh_precompute=True; mh_dist is the
+    cutoff radius r in the surfel's own units (a pixel takes part where rho <= r^2) and must be > 0.
+
+    Returns (image [H,W,3], culling_mask [N] bool, uv [M,2], depth [H,W,1], alpha [H,W,1], normal [H,W,3],
+    distortion [H,W,1]) and the state with return_state.  Per pixel, with the blend weights w_i = T_i alpha_i of the
+    colour: alpha = sum w_i; depth = sum w_i z_i (z_i the camera z of the ray-surfel intersection, or p_z where the
+    low-pass filter decides; expected depth is depth / alpha); normal = sum w_i n_i (camera frame, each n_i facing the
+    camera, not normalised); distortion = sum_i w_i sum_{j<i} w_j (m_i - m_j)^2 with m = (f / (f - n)) (1 - n / z),
+    n, f = near_thresh, far_thresh (2DGS's depth-distortion term).  Every output is differentiable; gradients reach
+    xyz, quaternion, scale[:, :2], opacity, rgb and sh (the colour is the SH colour at the centre's view direction,
+    held constant for xyz as in rasterize).  uv.grad is d loss / d delta, delta a pixel translation of the surfel's
+    whole footprint (DESIGN.md 3.25), for densification.  The backward writes rasterize()'s flat gradient layout
+    (state.grad_flat, or grad_out when given).
+
+    fp32 CUDA tensors only (TypeError otherwise); a camera_T_world or K that requires grad raises ValueError: no pose
+    or intrinsics gradient is formed for surfels."""
+    g = gaussians
+    tensors = [g.xyz, g.quaternion, g.scale, g.opacity, g.rgb, camera_T_world, camera.K, background_rgb]
+    if g.sh is not None:
+        tensors.append(g.sh)
+    for t in tensors:
+        if not torch.is_tensor(t) or t.dtype != torch.float32:
+            raise TypeError("rasterize_surfels takes fp32 tensors only, got "
+                            + (str(t.dtype) if torch.is_tensor(t) else type(t).__name__))
+    if camera_T_world.requires_grad or camera.K.requires_grad:
+        raise ValueError("rasterize_surfels forms no camera gradient: pass camera_T_world.detach() and "
+                         "camera.K.detach()")
+    if any(t.device.type != "cuda" or t.device != g.xyz.device for t in tensors):
+        raise ValueError("rasterize_surfels needs every tensor on the gaussians' CUDA device")
+    if not float(mh_dist) > 0.0:
+        raise ValueError(f"mh_dist must be > 0, got {mh_dist}")
+    if background_rgb.numel() != 3:
+        raise ValueError("background_rgb must hold 3 values")
+    state = _SurfelState()
+    state.grad_out = grad_out
+    state.background = background_rgb.contiguous()
+    cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh), float(cull_mask_padding),
+           float(mh_dist))
+    uv, carrier = _ProjectSurfels.apply(
+        g.xyz.contiguous(), g.quaternion.contiguous(), g.scale.contiguous(), g.opacity.contiguous(), g.rgb.contiguous(),
+        None if g.sh is None else g.sh.contiguous(), camera_T_world.contiguous(), camera.K.contiguous(), state, cfg)
+    state.uv_ref = weakref.ref(uv)
+    culling_mask = state.visible == 0
+    image, depth, alpha, normal, distortion = _CompositeSurfels.apply(uv, carrier, state)
+    result = (image, culling_mask, uv, depth, alpha, normal, distortion)
+    return (*result, state) if return_state else result
+
+
+def depth_normals(depth, alpha, camera, eps=1e-6):
+    """Normals of the rendered surface [H,W,3] for 2DGS's normal-consistency loss 1 - n . N: the expected depth
+    depth / alpha.clamp_min(eps) is back-projected through K^-1, and each interior pixel gets the normalised cross
+    product of the central differences along x and y, turned towards the camera.  Border pixels are 0."""
+    H, W = depth.shape[0], depth.shape[1]
+    d = (depth / alpha.clamp_min(eps)).reshape(H, W, 1)
+    ys, xs = torch.meshgrid(torch.arange(H, device=d.device, dtype=d.dtype),
+                            torch.arange(W, device=d.device, dtype=d.dtype), indexing="ij")
+    pix = torch.stack((xs, ys, torch.ones_like(xs)), -1)
+    rays = pix @ torch.linalg.inv(camera.K.to(d.dtype)).T
+    pts = rays * d
+    out = torch.zeros_like(pts)
+    dx = pts[1:-1, 2:] - pts[1:-1, :-2]
+    dy = pts[2:, 1:-1] - pts[:-2, 1:-1]
+    n = torch.nn.functional.normalize(torch.cross(dx, dy, dim=-1), dim=-1)
+    facing = (n * pts[1:-1, 1:-1]).sum(-1, keepdim=True) > 0
+    out[1:-1, 1:-1] = torch.where(facing, -n, n)
+    return out
