@@ -16,9 +16,11 @@
                             (include/gsr_bilagrid.h)
   libgsr_surfels.so         2-D Gaussian surfels: per-gaussian and tile kernels of rasterize_surfels
                             (include/gsr_surfels.h)
+  libgsr_surfels_lens.so    the same through fisheye and radial-tangential lenses, with the ray-map kernel
+                            (include/gsr_surfels_lens.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all twelve (the CUDA libraries from the LIBS table);
+`python -m gaussian_splatting_b200.build` builds all thirteen (the CUDA libraries from the LIBS table);
 `build(force=False)` is incremental.
 """
 from __future__ import annotations
@@ -72,6 +74,10 @@ POSE_HEADERS = CUH + [CSRC / "gsr_pose.cuh", CSRC / "gsr_calib.cuh", CSRC / "gsr
                       CSRC / "gsr_distortion.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_fisheye.h",
                       ROOT / "include" / "gsr_distortion.h", ROOT / "include" / "gsr_pose.h",
                       ROOT / "include" / "gsr_calib.h"]
+# the surfel kernels' bodies (gsr_surfels.cuh) are shared by the pinhole and the lens library
+SURFEL_HEADERS = CUH + [CSRC / "gsr_surfels.cuh", CSRC / "gsr_surfels_lens.cuh", CSRC / "gsr_fisheye.cuh",
+                        CSRC / "gsr_distortion.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_surfels.h",
+                        ROOT / "include" / "gsr_surfels_lens.h"]
 # (library, sources, headers, stamp): each library apart, so that every library keeps exactly its kernels (and their
 # SASS) when another one changes
 LIBS = [
@@ -97,8 +103,10 @@ LIBS = [
     (PKG / "libgsr_bilagrid.so", ["gsr_bilagrid.cu"],
      [CSRC / "gsr_common.cuh", ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_bilagrid.h"],
      "bilagrid_lib.sha256"),
-    (PKG / "libgsr_surfels.so", ["gsr_surfels.cu"],
-     CUH + [ROOT / "include" / "gsr_b200.h", ROOT / "include" / "gsr_surfels.h"], "surfels_lib.sha256"),
+    (PKG / "libgsr_surfels.so", ["gsr_surfels.cu"], SURFEL_HEADERS, "surfels_lib.sha256"),
+    (PKG / "libgsr_surfels_lens.so", ["gsr_surfels_lens.cu"],
+     SURFEL_HEADERS + [ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h"],
+     "surfels_lens_lib.sha256"),
 ]
 
 NVCC_FLAGS = [
@@ -177,7 +185,7 @@ def build_ext(force: bool = False) -> Path:
                     ROOT / "include" / "gsr_fisheye.h", ROOT / "include" / "gsr_distortion.h",
                     ROOT / "include" / "gsr_pose.h", ROOT / "include" / "gsr_bilagrid.h",
                     ROOT / "include" / "gsr_calib.h", ROOT / "include" / "gsr_shutter.h",
-                    ROOT / "include" / "gsr_surfels.h"], torch.__version__)
+                    ROOT / "include" / "gsr_surfels.h", ROOT / "include" / "gsr_surfels_lens.h"], torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -190,6 +198,7 @@ def build_ext(force: bool = False) -> Path:
         *incs, str(src), "-o", str(out),
         f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", "-lgsr_fisheye",
         "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid", "-lgsr_calib", "-lgsr_shutter", "-lgsr_surfels",
+        "-lgsr_surfels_lens",
         f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",

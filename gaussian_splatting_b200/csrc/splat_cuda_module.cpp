@@ -21,6 +21,7 @@
 #include "../../include/gsr_bilagrid.h"
 #include "../../include/gsr_shutter.h"
 #include "../../include/gsr_surfels.h"
+#include "../../include/gsr_surfels_lens.h"
 
 namespace {
 
@@ -1603,13 +1604,15 @@ static const float* opt_f32(const c10::optional<torch::Tensor>& t) {
 
 // returns (surfels [N,20], bin_records [N,12], depth_key, visible, scan, tile_mask, tile_win): the inputs of fused_bin
 // (with bin_records as its records) and of the surfel tile kernels
-std::vector<torch::Tensor> surfel_forward(torch::Tensor xyz, c10::optional<torch::Tensor> xyz_cam,
-                                          torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
-                                          torch::Tensor rgb, c10::optional<torch::Tensor> sh_rest,
-                                          torch::Tensor camera_T_world, torch::Tensor K,
-                                          c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
-                                          double near_thresh, double far_thresh, double pad, double mh_dist,
-                                          int64_t depth_base) {
+// lens 0: the pinhole (gsr_surfel_preprocess_forward), else GSR_SURFEL_LENS_* with its constants lens_consts
+std::vector<torch::Tensor> surfel_forward_any(int64_t lens, const c10::optional<torch::Tensor>& lens_consts,
+                                              torch::Tensor xyz, c10::optional<torch::Tensor> xyz_cam,
+                                              torch::Tensor quaternion, torch::Tensor scale,
+                                              torch::Tensor opacity_logit, torch::Tensor rgb,
+                                              c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
+                                              torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H,
+                                              int64_t W, double near_thresh, double far_thresh, double pad,
+                                              double mh_dist, int64_t depth_base) {
     for (const torch::Tensor* t : {&xyz, &quaternion, &scale, &opacity_logit, &rgb, &camera_T_world, &K}) {
         CHECK_VALID_INPUT((*t)); CHECK_FLOAT_TENSOR((*t));
     }
@@ -1627,24 +1630,74 @@ std::vector<torch::Tensor> surfel_forward(torch::Tensor xyz, c10::optional<torch
     torch::Tensor tile_mask = torch::empty({N}, opt.dtype(torch::kInt64));
     torch::Tensor tile_win = torch::empty({N}, opt.dtype(torch::kInt32));
     torch::Tensor temp = torch::empty({(int64_t)gsr_surfel_temp_bytes((int)N)}, opt.dtype(torch::kUInt8));
-    check_rc(gsr_surfel_preprocess_forward(
-                 (int)N, n_rest, F32PTR(xyz), cam, cam_first, F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit),
-                 F32PTR(rgb), opt_f32(sh_rest), F32PTR(camera_T_world), F32PTR(K), opt_f32(camera_centre), (int)H,
-                 (int)W, (float)near_thresh, (float)far_thresh, (float)pad, (float)mh_dist, (uint32_t)depth_base,
-                 F32PTR(surfels), F32PTR(bins), (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(),
-                 (uint64_t*)scan.data_ptr<int64_t>(), (uint64_t*)tile_mask.data_ptr<int64_t>(),
-                 (uint32_t*)tile_win.data_ptr<int>(), temp.data_ptr(), (size_t)temp.numel(), cur_stream()),
-             "gsr_surfel_preprocess_forward");
+    if (lens == 0) {
+        check_rc(gsr_surfel_preprocess_forward(
+                     (int)N, n_rest, F32PTR(xyz), cam, cam_first, F32PTR(quaternion), F32PTR(scale),
+                     F32PTR(opacity_logit), F32PTR(rgb), opt_f32(sh_rest), F32PTR(camera_T_world), F32PTR(K),
+                     opt_f32(camera_centre), (int)H, (int)W, (float)near_thresh, (float)far_thresh, (float)pad,
+                     (float)mh_dist, (uint32_t)depth_base, F32PTR(surfels), F32PTR(bins),
+                     (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(), (uint64_t*)scan.data_ptr<int64_t>(),
+                     (uint64_t*)tile_mask.data_ptr<int64_t>(), (uint32_t*)tile_win.data_ptr<int>(), temp.data_ptr(),
+                     (size_t)temp.numel(), cur_stream()),
+                 "gsr_surfel_preprocess_forward");
+    } else {
+        check_rc(gsr_surfel_lens_preprocess_forward(
+                     (int)lens, (int)N, n_rest, F32PTR(xyz), cam, cam_first, F32PTR(quaternion), F32PTR(scale),
+                     F32PTR(opacity_logit), F32PTR(rgb), opt_f32(sh_rest), F32PTR(camera_T_world), F32PTR(K),
+                     opt_f32(camera_centre), (int)H, (int)W, (float)near_thresh, (float)far_thresh, (float)pad,
+                     (float)mh_dist, (uint32_t)depth_base, F32PTR(surfels), F32PTR(bins),
+                     (uint32_t*)zkey.data_ptr<int>(), visible.data_ptr<uint8_t>(), (uint64_t*)scan.data_ptr<int64_t>(),
+                     (uint64_t*)tile_mask.data_ptr<int64_t>(), (uint32_t*)tile_win.data_ptr<int>(), temp.data_ptr(),
+                     (size_t)temp.numel(), opt_f32(lens_consts), cur_stream()),
+                 "gsr_surfel_lens_preprocess_forward");
+    }
     return {surfels, bins, zkey, visible, scan, tile_mask, tile_win};
+}
+
+std::vector<torch::Tensor> surfel_forward(torch::Tensor xyz, c10::optional<torch::Tensor> xyz_cam,
+                                          torch::Tensor quaternion, torch::Tensor scale, torch::Tensor opacity_logit,
+                                          torch::Tensor rgb, c10::optional<torch::Tensor> sh_rest,
+                                          torch::Tensor camera_T_world, torch::Tensor K,
+                                          c10::optional<torch::Tensor> camera_centre, int64_t H, int64_t W,
+                                          double near_thresh, double far_thresh, double pad, double mh_dist,
+                                          int64_t depth_base) {
+    return surfel_forward_any(0, c10::nullopt, xyz, xyz_cam, quaternion, scale, opacity_logit, rgb, sh_rest,
+                              camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, pad, mh_dist,
+                              depth_base);
+}
+
+std::vector<torch::Tensor> surfel_lens_forward(int64_t lens, torch::Tensor lens_consts, torch::Tensor xyz,
+                                               c10::optional<torch::Tensor> xyz_cam, torch::Tensor quaternion,
+                                               torch::Tensor scale, torch::Tensor opacity_logit, torch::Tensor rgb,
+                                               c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
+                                               torch::Tensor K, c10::optional<torch::Tensor> camera_centre, int64_t H,
+                                               int64_t W, double near_thresh, double far_thresh, double pad,
+                                               double mh_dist, int64_t depth_base) {
+    TORCH_CHECK(lens == GSR_SURFEL_LENS_FISHEYE || lens == GSR_SURFEL_LENS_DISTORTION, "unknown surfel lens ", lens);
+    return surfel_forward_any(lens, lens_consts, xyz, xyz_cam, quaternion, scale, opacity_logit, rgb, sh_rest,
+                              camera_T_world, K, camera_centre, H, W, near_thresh, far_thresh, pad, mh_dist,
+                              depth_base);
+}
+
+// the ray map [H, W, 3] of a lens (gsr_surfel_rays)
+torch::Tensor surfel_rays(int64_t lens, torch::Tensor lens_consts, torch::Tensor K, int64_t H, int64_t W) {
+    CHECK_VALID_INPUT(K); CHECK_FLOAT_TENSOR(K);
+    CHECK_VALID_INPUT(lens_consts); CHECK_FLOAT_TENSOR(lens_consts);
+    c10::cuda::CUDAGuard guard(K.device());
+    torch::Tensor rays = torch::empty({H, W, 3}, K.options());
+    check_rc(gsr_surfel_rays((int)lens, (int)H, (int)W, F32PTR(K), F32PTR(lens_consts), F32PTR(rays), cur_stream()),
+             "gsr_surfel_rays");
+    return rays;
 }
 
 // returns (image [H,W,3], depth [H,W,1], alpha [H,W,1], normal [H,W,3], distortion [H,W,1], last [H,W] i32,
 // totals [H,W,3])
-std::vector<torch::Tensor> surfel_render_forward(torch::Tensor surfels, torch::Tensor ranges, torch::Tensor background,
-                                                 int64_t H, int64_t W, int64_t P,
-                                                 c10::optional<torch::Tensor> keys_sorted,
-                                                 c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
-                                                 double near_thresh, double m_scale, double mh_dist) {
+// rays: the lens's ray map (gsr_surfel_lens_render_forward), or none for the pinhole
+std::vector<torch::Tensor> surfel_render_forward_any(const c10::optional<torch::Tensor>& rays, torch::Tensor surfels,
+                                                     torch::Tensor ranges, torch::Tensor background, int64_t H,
+                                                     int64_t W, int64_t P, c10::optional<torch::Tensor> keys_sorted,
+                                                     c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                                     double near_thresh, double m_scale, double mh_dist) {
     CHECK_VALID_INPUT(surfels); CHECK_FLOAT_TENSOR(surfels);
     CHECK_VALID_INPUT(background); CHECK_FLOAT_TENSOR(background);
     TORCH_CHECK(background.numel() == 3, "Background RGB must have 3 elements");
@@ -1656,22 +1709,53 @@ std::vector<torch::Tensor> surfel_render_forward(torch::Tensor surfels, torch::T
                   totals = torch::empty({H, W, 3}, opt);
     const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
     const bool keys = ps.keys != nullptr;  // else ids (with P == 0 a placeholder the kernels never read)
-    check_rc(gsr_surfel_render_forward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0, keys ? nullptr : ps.ids,
-                                       ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W, (float)near_thresh,
-                                       (float)m_scale, (float)mh_dist, F32PTR(image), F32PTR(depth), F32PTR(alpha),
-                                       F32PTR(normal), F32PTR(dist), last.data_ptr<int>(), F32PTR(totals),
-                                       cur_stream()),
-             "gsr_surfel_render_forward");
+    if (!rays.has_value()) {
+        check_rc(gsr_surfel_render_forward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0, keys ? nullptr : ps.ids,
+                                           ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
+                                           (float)near_thresh, (float)m_scale, (float)mh_dist, F32PTR(image),
+                                           F32PTR(depth), F32PTR(alpha), F32PTR(normal), F32PTR(dist),
+                                           last.data_ptr<int>(), F32PTR(totals), cur_stream()),
+                 "gsr_surfel_render_forward");
+    } else {
+        TORCH_CHECK(rays->numel() == H * W * 3, "rays must be [H, W, 3]");
+        check_rc(gsr_surfel_lens_render_forward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0,
+                                                keys ? nullptr : ps.ids, ranges.data_ptr<int>(), F32PTR(background),
+                                                (int)H, (int)W, (float)near_thresh, (float)m_scale, (float)mh_dist,
+                                                opt_f32(rays), F32PTR(image), F32PTR(depth), F32PTR(alpha),
+                                                F32PTR(normal), F32PTR(dist), last.data_ptr<int>(), F32PTR(totals),
+                                                cur_stream()),
+                 "gsr_surfel_lens_render_forward");
+    }
     return {image, depth, alpha, normal, dist, last, totals};
 }
 
+std::vector<torch::Tensor> surfel_render_forward(torch::Tensor surfels, torch::Tensor ranges, torch::Tensor background,
+                                                 int64_t H, int64_t W, int64_t P,
+                                                 c10::optional<torch::Tensor> keys_sorted,
+                                                 c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                                 double near_thresh, double m_scale, double mh_dist) {
+    return surfel_render_forward_any(c10::nullopt, surfels, ranges, background, H, W, P, keys_sorted, ids_sorted,
+                                     id_bits, near_thresh, m_scale, mh_dist);
+}
+
+std::vector<torch::Tensor> surfel_lens_render_forward(torch::Tensor rays, torch::Tensor surfels, torch::Tensor ranges,
+                                                      torch::Tensor background, int64_t H, int64_t W, int64_t P,
+                                                      c10::optional<torch::Tensor> keys_sorted,
+                                                      c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                                      double near_thresh, double m_scale, double mh_dist) {
+    return surfel_render_forward_any(rays, surfels, ranges, background, H, W, P, keys_sorted, ids_sorted, id_bits,
+                                     near_thresh, m_scale, mh_dist);
+}
+
 // the surfel gradient rows [N, 20] (zero-filled, accumulated by the tile backward)
-torch::Tensor surfel_render_backward(int64_t N, torch::Tensor surfels, torch::Tensor ranges, torch::Tensor background,
-                                     int64_t H, int64_t W, int64_t P, c10::optional<torch::Tensor> keys_sorted,
-                                     c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, double near_thresh,
-                                     double m_scale, double mh_dist, torch::Tensor alpha, torch::Tensor last,
-                                     torch::Tensor totals, torch::Tensor g_image, torch::Tensor g_depth,
-                                     torch::Tensor g_alpha, torch::Tensor g_normal, torch::Tensor g_distortion) {
+torch::Tensor surfel_render_backward_any(const c10::optional<torch::Tensor>& rays, int64_t N, torch::Tensor surfels,
+                                         torch::Tensor ranges, torch::Tensor background, int64_t H, int64_t W,
+                                         int64_t P, c10::optional<torch::Tensor> keys_sorted,
+                                         c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                         double near_thresh, double m_scale, double mh_dist, torch::Tensor alpha,
+                                         torch::Tensor last, torch::Tensor totals, torch::Tensor g_image,
+                                         torch::Tensor g_depth, torch::Tensor g_alpha, torch::Tensor g_normal,
+                                         torch::Tensor g_distortion) {
     for (const torch::Tensor* t : {&surfels, &background, &alpha, &totals, &g_image, &g_depth, &g_alpha, &g_normal,
                                    &g_distortion}) {
         CHECK_VALID_INPUT((*t)); CHECK_FLOAT_TENSOR((*t));
@@ -1683,14 +1767,49 @@ torch::Tensor surfel_render_backward(int64_t N, torch::Tensor surfels, torch::Te
     torch::Tensor rows = torch::zeros({N, GSR_SURFEL_GRAD_FLOATS}, surfels.options());
     const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
     const bool keys = ps.keys != nullptr;
-    check_rc(gsr_surfel_render_backward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0, keys ? nullptr : ps.ids,
-                                        ranges.data_ptr<int>(), F32PTR(background), (int)H, (int)W,
-                                        (float)near_thresh, (float)m_scale, (float)mh_dist, F32PTR(alpha),
-                                        last.data_ptr<int>(), F32PTR(totals), F32PTR(g_image), F32PTR(g_depth),
-                                        F32PTR(g_alpha), F32PTR(g_normal), F32PTR(g_distortion), F32PTR(rows),
-                                        cur_stream()),
-             "gsr_surfel_render_backward");
+    if (!rays.has_value()) {
+        check_rc(gsr_surfel_render_backward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0,
+                                            keys ? nullptr : ps.ids, ranges.data_ptr<int>(), F32PTR(background),
+                                            (int)H, (int)W, (float)near_thresh, (float)m_scale, (float)mh_dist,
+                                            F32PTR(alpha), last.data_ptr<int>(), F32PTR(totals), F32PTR(g_image),
+                                            F32PTR(g_depth), F32PTR(g_alpha), F32PTR(g_normal), F32PTR(g_distortion),
+                                            F32PTR(rows), cur_stream()),
+                 "gsr_surfel_render_backward");
+    } else {
+        TORCH_CHECK(rays->numel() == H * W * 3, "rays must be [H, W, 3]");
+        check_rc(gsr_surfel_lens_render_backward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0,
+                                                 keys ? nullptr : ps.ids, ranges.data_ptr<int>(), F32PTR(background),
+                                                 (int)H, (int)W, (float)near_thresh, (float)m_scale, (float)mh_dist,
+                                                 opt_f32(rays), F32PTR(alpha), last.data_ptr<int>(), F32PTR(totals),
+                                                 F32PTR(g_image), F32PTR(g_depth), F32PTR(g_alpha), F32PTR(g_normal),
+                                                 F32PTR(g_distortion), F32PTR(rows), cur_stream()),
+                 "gsr_surfel_lens_render_backward");
+    }
     return rows;
+}
+
+torch::Tensor surfel_render_backward(int64_t N, torch::Tensor surfels, torch::Tensor ranges, torch::Tensor background,
+                                     int64_t H, int64_t W, int64_t P, c10::optional<torch::Tensor> keys_sorted,
+                                     c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, double near_thresh,
+                                     double m_scale, double mh_dist, torch::Tensor alpha, torch::Tensor last,
+                                     torch::Tensor totals, torch::Tensor g_image, torch::Tensor g_depth,
+                                     torch::Tensor g_alpha, torch::Tensor g_normal, torch::Tensor g_distortion) {
+    return surfel_render_backward_any(c10::nullopt, N, surfels, ranges, background, H, W, P, keys_sorted, ids_sorted,
+                                      id_bits, near_thresh, m_scale, mh_dist, alpha, last, totals, g_image, g_depth,
+                                      g_alpha, g_normal, g_distortion);
+}
+
+torch::Tensor surfel_lens_render_backward(torch::Tensor rays, int64_t N, torch::Tensor surfels, torch::Tensor ranges,
+                                          torch::Tensor background, int64_t H, int64_t W, int64_t P,
+                                          c10::optional<torch::Tensor> keys_sorted,
+                                          c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                          double near_thresh, double m_scale, double mh_dist, torch::Tensor alpha,
+                                          torch::Tensor last, torch::Tensor totals, torch::Tensor g_image,
+                                          torch::Tensor g_depth, torch::Tensor g_alpha, torch::Tensor g_normal,
+                                          torch::Tensor g_distortion) {
+    return surfel_render_backward_any(rays, N, surfels, ranges, background, H, W, P, keys_sorted, ids_sorted, id_bits,
+                                      near_thresh, m_scale, mh_dist, alpha, last, totals, g_image, g_depth, g_alpha,
+                                      g_normal, g_distortion);
 }
 
 // uv.grad [M,2] of the visible gaussians vis_idx from the gradient rows
@@ -1706,16 +1825,31 @@ torch::Tensor surfel_uv_grad(torch::Tensor vis_idx, torch::Tensor surfels, torch
     return out;
 }
 
+// uv.grad [M,2] of a lens surfel view (gsr_surfel_lens_uv_grad)
+torch::Tensor surfel_lens_uv_grad(int64_t lens, torch::Tensor lens_consts, torch::Tensor K, torch::Tensor vis_idx,
+                                  torch::Tensor surfels, torch::Tensor rows) {
+    CHECK_VALID_INPUT(vis_idx); CHECK_INT_TENSOR(vis_idx);
+    CHECK_VALID_INPUT(surfels); CHECK_VALID_INPUT(rows); CHECK_VALID_INPUT(K); CHECK_VALID_INPUT(lens_consts);
+    c10::cuda::CUDAGuard guard(surfels.device());
+    const int64_t M = vis_idx.numel();
+    torch::Tensor out = torch::empty({M, 2}, surfels.options());
+    check_rc(gsr_surfel_lens_uv_grad((int)lens, (int)M, vis_idx.data_ptr<int>(), F32PTR(surfels), F32PTR(rows),
+                                     F32PTR(K), F32PTR(lens_consts), F32PTR(out), cur_stream()),
+             "gsr_surfel_lens_uv_grad");
+    return out;
+}
+
 // the per-gaussian backward into the flat layout of fused_preprocess_backward (out_flat: a caller-owned buffer of it);
 // returns the gaussian gradients (xyz, quaternion, scale, opacity, rgb[, sh]) and then `flat`
-std::vector<torch::Tensor> surfel_backward(torch::Tensor rows, torch::Tensor xyz, torch::Tensor quaternion,
-                                           torch::Tensor scale, torch::Tensor opacity_logit,
-                                           c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
-                                           torch::Tensor K, c10::optional<torch::Tensor> camera_centre,
-                                           torch::Tensor visible, torch::Tensor surfels,
-                                           c10::optional<torch::Tensor> out_flat,
-                                           c10::optional<torch::Tensor> grad_uv_compact,
-                                           c10::optional<torch::Tensor> scan, bool uv_grad_emitted) {
+std::vector<torch::Tensor> surfel_backward_any(int64_t lens, const c10::optional<torch::Tensor>& lens_consts,
+                                               torch::Tensor rows, torch::Tensor xyz, torch::Tensor quaternion,
+                                               torch::Tensor scale, torch::Tensor opacity_logit,
+                                               c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
+                                               torch::Tensor K, c10::optional<torch::Tensor> camera_centre,
+                                               torch::Tensor visible, torch::Tensor surfels,
+                                               c10::optional<torch::Tensor> out_flat,
+                                               c10::optional<torch::Tensor> grad_uv_compact,
+                                               c10::optional<torch::Tensor> scan, bool uv_grad_emitted) {
     for (const torch::Tensor* t : {&rows, &xyz, &quaternion, &scale, &opacity_logit, &camera_T_world, &K, &surfels}) {
         CHECK_VALID_INPUT((*t)); CHECK_FLOAT_TENSOR((*t));
     }
@@ -1749,15 +1883,51 @@ std::vector<torch::Tensor> surfel_backward(torch::Tensor rows, torch::Tensor xyz
     std::vector<torch::Tensor> out = {section(0, {N, 3}), section(1, {N, 4}), section(2, {N, 3}), section(3, {N}),
                                       section(4, {N, 3})};
     if (n_rest) out.push_back(section(5, {N, 3, (int64_t)n_rest}));
-    check_rc(gsr_surfel_preprocess_backward((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
-                                            F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
-                                            opt_f32(camera_centre), visible.data_ptr<uint8_t>(), F32PTR(surfels),
-                                            F32PTR(rows), guv, scan_ptr, uv_grad_emitted ? 1 : 0, F32PTR(out[0]),
-                                            F32PTR(out[1]), F32PTR(out[2]), F32PTR(out[3]), F32PTR(out[4]),
-                                            n_rest ? F32PTR(out[5]) : nullptr, cur_stream()),
-             "gsr_surfel_preprocess_backward");
+    if (lens == 0) {
+        check_rc(gsr_surfel_preprocess_backward((int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale),
+                                                F32PTR(opacity_logit), F32PTR(camera_T_world), F32PTR(K),
+                                                opt_f32(camera_centre), visible.data_ptr<uint8_t>(), F32PTR(surfels),
+                                                F32PTR(rows), guv, scan_ptr, uv_grad_emitted ? 1 : 0, F32PTR(out[0]),
+                                                F32PTR(out[1]), F32PTR(out[2]), F32PTR(out[3]), F32PTR(out[4]),
+                                                n_rest ? F32PTR(out[5]) : nullptr, cur_stream()),
+                 "gsr_surfel_preprocess_backward");
+    } else {
+        check_rc(gsr_surfel_lens_preprocess_backward(
+                     (int)lens, (int)N, n_rest, F32PTR(xyz), F32PTR(quaternion), F32PTR(scale), F32PTR(opacity_logit),
+                     F32PTR(camera_T_world), F32PTR(K), opt_f32(camera_centre), visible.data_ptr<uint8_t>(),
+                     F32PTR(surfels), F32PTR(rows), guv, scan_ptr, uv_grad_emitted ? 1 : 0, F32PTR(out[0]),
+                     F32PTR(out[1]), F32PTR(out[2]), F32PTR(out[3]), F32PTR(out[4]), n_rest ? F32PTR(out[5]) : nullptr,
+                     opt_f32(lens_consts), cur_stream()),
+                 "gsr_surfel_lens_preprocess_backward");
+    }
     out.push_back(flat);
     return out;
+}
+
+std::vector<torch::Tensor> surfel_backward(torch::Tensor rows, torch::Tensor xyz, torch::Tensor quaternion,
+                                           torch::Tensor scale, torch::Tensor opacity_logit,
+                                           c10::optional<torch::Tensor> sh_rest, torch::Tensor camera_T_world,
+                                           torch::Tensor K, c10::optional<torch::Tensor> camera_centre,
+                                           torch::Tensor visible, torch::Tensor surfels,
+                                           c10::optional<torch::Tensor> out_flat,
+                                           c10::optional<torch::Tensor> grad_uv_compact,
+                                           c10::optional<torch::Tensor> scan, bool uv_grad_emitted) {
+    return surfel_backward_any(0, c10::nullopt, rows, xyz, quaternion, scale, opacity_logit, sh_rest, camera_T_world,
+                               K, camera_centre, visible, surfels, out_flat, grad_uv_compact, scan, uv_grad_emitted);
+}
+
+std::vector<torch::Tensor> surfel_lens_backward(int64_t lens, torch::Tensor lens_consts, torch::Tensor rows,
+                                                torch::Tensor xyz, torch::Tensor quaternion, torch::Tensor scale,
+                                                torch::Tensor opacity_logit, c10::optional<torch::Tensor> sh_rest,
+                                                torch::Tensor camera_T_world, torch::Tensor K,
+                                                c10::optional<torch::Tensor> camera_centre, torch::Tensor visible,
+                                                torch::Tensor surfels, c10::optional<torch::Tensor> out_flat,
+                                                c10::optional<torch::Tensor> grad_uv_compact,
+                                                c10::optional<torch::Tensor> scan, bool uv_grad_emitted) {
+    TORCH_CHECK(lens == GSR_SURFEL_LENS_FISHEYE || lens == GSR_SURFEL_LENS_DISTORTION, "unknown surfel lens ", lens);
+    return surfel_backward_any(lens, lens_consts, rows, xyz, quaternion, scale, opacity_logit, sh_rest,
+                               camera_T_world, K, camera_centre, visible, surfels, out_flat, grad_uv_compact, scan,
+                               uv_grad_emitted);
 }
 
 std::string version() { return gsr_version(); }
@@ -1899,6 +2069,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("surfel_render_backward", &surfel_render_backward, "2-D surfels: tile backward (gsr_surfel_render_backward)");
     m.def("surfel_uv_grad", &surfel_uv_grad, "2-D surfels: uv.grad of the visible gaussians (gsr_surfel_uv_grad)");
     m.def("surfel_backward", &surfel_backward, "2-D surfels: per-gaussian backward (gsr_surfel_preprocess_backward)");
+    m.attr("SURFEL_LENS_FISHEYE") = (int)GSR_SURFEL_LENS_FISHEYE;
+    m.attr("SURFEL_LENS_DISTORTION") = (int)GSR_SURFEL_LENS_DISTORTION;
+    m.def("surfel_rays", &surfel_rays, "2-D surfels through a lens: the ray map [H,W,3] (gsr_surfel_rays)");
+    m.def("surfel_lens_forward", &surfel_lens_forward,
+          "2-D surfels through a lens: per-gaussian forward (gsr_surfel_lens_preprocess_forward)");
+    m.def("surfel_lens_render_forward", &surfel_lens_render_forward,
+          "2-D surfels through a lens: tile forward along the ray map (gsr_surfel_lens_render_forward)");
+    m.def("surfel_lens_render_backward", &surfel_lens_render_backward,
+          "2-D surfels through a lens: tile backward along the ray map (gsr_surfel_lens_render_backward)");
+    m.def("surfel_lens_uv_grad", &surfel_lens_uv_grad,
+          "2-D surfels through a lens: uv.grad of the visible gaussians (gsr_surfel_lens_uv_grad)");
+    m.def("surfel_lens_backward", &surfel_lens_backward,
+          "2-D surfels through a lens: per-gaussian backward (gsr_surfel_lens_preprocess_backward)");
     m.def("version", &version, "library version string");
     m.def("contribution_mask_words",
           [](int64_t P, int64_t H, int64_t W) { return (int64_t)gsr_contribution_mask_words(P, (int)H, (int)W); },

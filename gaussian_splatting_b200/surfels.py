@@ -4,6 +4,8 @@ The scene is the 3DGS scene (mean, quaternion, scales, opacity logit, SH) and bi
 is rendered as a flat disk whose two tangent axes are scale[:, 0] and scale[:, 1] (scale[:, 2] is not used and gets an
 exact 0 gradient).  Per pixel the ray meets the surfel at a point (a, b) of its plane, so depth lies on the surface and
 every surfel has a normal.  The model is DESIGN.md 3.25; the kernels are libgsr_surfels.so (include/gsr_surfels.h).
+Through a fisheye or OPENCV lens (DESIGN.md 3.26) each pixel intersects its own undistorted ray, from a ray map, with
+the surfel; those kernels are libgsr_surfels_lens.so (include/gsr_surfels_lens.h).
 
 Two autograd nodes, as in rasterize():
 
@@ -22,21 +24,23 @@ import weakref
 import torch
 
 from . import native
-from .rasterize import (IN_KERNEL_TRANSFORM, IN_KERNEL_TRANSFORM_MIN_N, _depth_key_params, in_kernel_transform_ok,
-                        native_centre_ok, tail_positions)
+from .rasterize import (IN_KERNEL_TRANSFORM, IN_KERNEL_TRANSFORM_MIN_N, _depth_key_params, _lens_arg,
+                        _lens_constants, in_kernel_transform_ok, native_centre_ok, tail_positions)
 from .utils import transform_points_torch
 
 
 class _SurfelState:
     """Per-view buffers shared by the two autograd nodes (return_state=True hands it out).  vis_idx / vis_idx32: the
-    visible gaussians, ascending (the order of uv); grad_flat: the flat gradient of the last backward."""
+    visible gaussians, ascending (the order of uv); grad_flat: the flat gradient of the last backward; lens: None (the
+    pinhole) or (the native SURFEL_LENS_* value, its device constants); rays: the lens's ray map [H,W,3] (0 where a
+    pixel has no ray)."""
 
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "vis_idx32", "scan", "surfels", "ranges", "keys_sorted",
                  "ids_sorted", "id_bits", "maps", "last", "totals", "background", "near", "m_scale", "mh", "grad_flat",
-                 "grad_out", "uv_ref", "uv_grad_emitted", "uv_absgrad")
+                 "grad_out", "uv_ref", "uv_grad_emitted", "uv_absgrad", "lens", "rays", "K")
 
     def __init__(self):
-        self.grad_flat = self.grad_out = self.uv_ref = self.uv_absgrad = None
+        self.grad_flat = self.grad_out = self.uv_ref = self.uv_absgrad = self.lens = self.rays = None
         self.uv_grad_emitted = False
 
 
@@ -60,9 +64,13 @@ class _ProjectSurfels(torch.autograd.Function):
                 centre = ext.camera_centre(camera_T_world)
             else:
                 centre = torch.linalg.inv_ex(camera_T_world)[0][:3, 3].contiguous()
-        surfels, bins, zkey, visible, scan, tile_mask, tile_win = ext.surfel_forward(
-            xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far, pad,
-            mh, depth_base)
+        args = (xyz, xyz_cam, quaternion, scale, opacity_flat, rgb, sh, camera_T_world, K, centre, H, W, near, far,
+                pad, mh, depth_base)
+        if state.lens is None:
+            surfels, bins, zkey, visible, scan, tile_mask, tile_win = ext.surfel_forward(*args)
+        else:
+            state.rays = ext.surfel_rays(*state.lens, K, H, W)
+            surfels, bins, zkey, visible, scan, tile_mask, tile_win = ext.surfel_lens_forward(*state.lens, *args)
         total = int(scan[-1].item()) if N > 0 else 0
         M, P = total >> 32, total & 0xFFFFFFFF
         if M > N or P >= 2**31:
@@ -71,14 +79,15 @@ class _ProjectSurfels(torch.autograd.Function):
         ids_sorted, ranges, vis_idx, uv, keys_sorted, id_bits = ext.fused_bin(
             bins, zkey, visible, scan, M, P, H, W, mh, depth_bits, False, tile_mask, tile_win)
         m_scale = far / (far - near) if math.isfinite(far) else 1.0
-        rendered = ext.surfel_render_forward(surfels, ranges, state.background, H, W, P, keys_sorted, ids_sorted,
-                                             int(id_bits), near, m_scale, mh)
+        rargs = (surfels, ranges, state.background, H, W, P, keys_sorted, ids_sorted, int(id_bits), near, m_scale, mh)
+        rendered = (ext.surfel_render_forward(*rargs) if state.lens is None
+                    else ext.surfel_lens_render_forward(state.rays, *rargs))
         state.N, state.M, state.P, state.H, state.W = N, M, P, H, W
         state.visible, state.vis_idx, state.vis_idx32, state.scan = visible, vis_idx, vis_idx, scan
         state.surfels, state.ranges, state.keys_sorted, state.ids_sorted, state.id_bits = (
             surfels, ranges, keys_sorted, ids_sorted, int(id_bits))
         state.maps, state.last, state.totals = rendered[:5], rendered[5], rendered[6]
-        state.near, state.m_scale, state.mh = near, m_scale, mh
+        state.near, state.m_scale, state.mh, state.K = near, m_scale, mh, K
         ctx.state = state
         ctx.has_sh = sh is not None
         ctx.opacity_shape = opacity.shape
@@ -93,9 +102,10 @@ class _ProjectSurfels(torch.autograd.Function):
         if grad_carrier is None:
             grad_carrier = torch.zeros(20 * st.N, dtype=xyz.dtype, device=xyz.device)
         guv = grad_uv.contiguous() if grad_uv is not None and st.M > 0 else None
-        out = native().surfel_backward(grad_carrier.contiguous(), xyz, quaternion, scale, opacity_flat, sh,
-                                       camera_T_world, K, centre, st.visible, st.surfels, st.grad_out, guv,
-                                       st.scan if guv is not None else None, st.uv_grad_emitted)
+        args = (grad_carrier.contiguous(), xyz, quaternion, scale, opacity_flat, sh, camera_T_world, K, centre,
+                st.visible, st.surfels, st.grad_out, guv, st.scan if guv is not None else None, st.uv_grad_emitted)
+        out = (native().surfel_backward(*args) if st.lens is None
+               else native().surfel_lens_backward(*st.lens, *args))
         g_xyz, g_q, g_s, g_o, g_dc = out[:5]
         g_sh = out[5] if ctx.has_sh else None
         st.grad_flat = out[-1]
@@ -121,20 +131,35 @@ class _CompositeSurfels(torch.autograd.Function):
         def grad(g, k):
             return torch.zeros(st.H, st.W, k, device=alpha.device) if g is None else g.contiguous()
 
-        rows = native().surfel_render_backward(
-            st.N, st.surfels, st.ranges, st.background, st.H, st.W, st.P, st.keys_sorted, st.ids_sorted, st.id_bits,
-            st.near, st.m_scale, st.mh, alpha, st.last, st.totals, grad(g_image, 3), grad(g_depth, 1),
-            grad(g_alpha, 1), grad(g_normal, 3), grad(g_dist, 1))
+        args = (st.N, st.surfels, st.ranges, st.background, st.H, st.W, st.P, st.keys_sorted, st.ids_sorted,
+                st.id_bits, st.near, st.m_scale, st.mh, alpha, st.last, st.totals, grad(g_image, 3), grad(g_depth, 1),
+                grad(g_alpha, 1), grad(g_normal, 3), grad(g_dist, 1))
+        ext = native()
+        rows = (ext.surfel_render_backward(*args) if st.lens is None
+                else ext.surfel_lens_render_backward(st.rays, *args))
         # uv.grad (d loss / d footprint translation) is formed only when somebody can observe it, as in rasterize()
         uv_t = st.uv_ref() if st.uv_ref is not None else None
         watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
         st.uv_grad_emitted = bool(watched)
-        grad_uv = native().surfel_uv_grad(st.vis_idx, st.surfels, rows) if watched else None
+        grad_uv = None
+        if watched:
+            grad_uv = (ext.surfel_uv_grad(st.vis_idx, st.surfels, rows) if st.lens is None
+                       else ext.surfel_lens_uv_grad(*st.lens, st.K, st.vis_idx, st.surfels, rows))
         return grad_uv, rows.view(-1), None
 
 
+def _surfel_lens(fisheye, distortion, device):
+    """(native SURFEL_LENS_* value, [n+1] device constants) for the lens arguments, or None for the pinhole"""
+    lens = _lens_arg(fisheye, distortion)
+    if lens is None:
+        return None
+    ext = native()
+    code = ext.SURFEL_LENS_FISHEYE if lens[0] == "fisheye" else ext.SURFEL_LENS_DISTORTION
+    return code, _lens_constants(*lens, device).reshape(-1)
+
+
 def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
-                      background_rgb, return_state=False, grad_out=None):
+                      background_rgb, return_state=False, grad_out=None, fisheye=None, distortion=None):
     """Render the gaussians as 2-D surfels.  Arguments as rasterize() with use_sh_precompute=True; mh_dist is the
     cutoff radius r in the surfel's own units (a pixel takes part where rho <= r^2) and must be > 0.
 
@@ -149,8 +174,16 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
     whole footprint (DESIGN.md 3.25), for densification.  The backward writes rasterize()'s flat gradient layout
     (state.grad_flat, or grad_out when given).
 
-    fp32 CUDA tensors only (TypeError otherwise); a camera_T_world or K that requires grad raises ValueError: no pose
-    or intrinsics gradient is formed for surfels."""
+    fisheye=k (COLMAP's OPENCV_FISHEYE, k1 k2 k3 k4) or distortion=k (COLMAP's OPENCV, k1 k2 p1 p2 k3) renders through
+    that lens, with the coefficients as rasterize() takes them (host values; the two are exclusive).  Each pixel then
+    meets the surfel along its own undistorted ray (state.rays; DESIGN.md 3.26), which is exact for the central lens;
+    uv, the depth keys and the culling mask are rasterize()'s with the same lens, and a pixel with no ray on the lens's
+    monotone branch (beyond fisheye_theta_max or distortion_r2_max) shows the background.  uv.grad is then
+    J_n^-T g_n + g_c, the gradient on a translation of the footprint in the normalised plane mapped to pixels through
+    the lens Jacobian at the centre; its sum is d loss / d(cx, cy) for the pinhole only.
+
+    fp32 CUDA tensors only (TypeError otherwise); a camera_T_world, K or lens-coefficient tensor that requires grad
+    raises ValueError: no camera gradient is formed for surfels."""
     g = gaussians
     tensors = [g.xyz, g.quaternion, g.scale, g.opacity, g.rgb, camera_T_world, camera.K, background_rgb]
     if g.sh is not None:
@@ -162,6 +195,9 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
     if camera_T_world.requires_grad or camera.K.requires_grad:
         raise ValueError("rasterize_surfels forms no camera gradient: pass camera_T_world.detach() and "
                          "camera.K.detach()")
+    if any(torch.is_tensor(k) and k.requires_grad for k in (fisheye, distortion)):
+        raise ValueError("rasterize_surfels forms no camera gradient: pass lens coefficients that do not require grad")
+    lens = _lens_arg(fisheye, distortion)
     if any(t.device.type != "cuda" or t.device != g.xyz.device for t in tensors):
         raise ValueError("rasterize_surfels needs every tensor on the gaussians' CUDA device")
     if not float(mh_dist) > 0.0:
@@ -169,6 +205,8 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
     if background_rgb.numel() != 3:
         raise ValueError("background_rgb must hold 3 values")
     state = _SurfelState()
+    if lens is not None:
+        state.lens = _surfel_lens(fisheye, distortion, g.xyz.device)
     state.grad_out = grad_out
     state.background = background_rgb.contiguous()
     cfg = (int(camera.height), int(camera.width), float(near_thresh), float(far_thresh), float(cull_mask_padding),
@@ -183,21 +221,37 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
     return (*result, state) if return_state else result
 
 
-def depth_normals(depth, alpha, camera, eps=1e-6):
+def depth_normals(depth, alpha, camera, eps=1e-6, fisheye=None, distortion=None):
     """Normals of the rendered surface [H,W,3] for 2DGS's normal-consistency loss 1 - n . N: the expected depth
-    depth / alpha.clamp_min(eps) is back-projected through K^-1, and each interior pixel gets the normalised cross
-    product of the central differences along x and y, turned towards the camera.  Border pixels are 0."""
+    z = depth / alpha.clamp_min(eps) is back-projected along each pixel's ray, and each interior pixel gets the
+    normalised cross product of the central differences along x and y, turned towards the camera.  Border pixels are 0.
+    The ray is K^-1 (x, y, 1) for the pinhole, and with fisheye=k / distortion=k the lens's ray d of rasterize_surfels
+    (point = d z / d_z, CUDA tensors only); pixels next to one without a ray are 0 as well."""
     H, W = depth.shape[0], depth.shape[1]
     d = (depth / alpha.clamp_min(eps)).reshape(H, W, 1)
-    ys, xs = torch.meshgrid(torch.arange(H, device=d.device, dtype=d.dtype),
-                            torch.arange(W, device=d.device, dtype=d.dtype), indexing="ij")
-    pix = torch.stack((xs, ys, torch.ones_like(xs)), -1)
-    rays = pix @ torch.linalg.inv(camera.K.to(d.dtype)).T
+    valid = None
+    if fisheye is None and distortion is None:
+        ys, xs = torch.meshgrid(torch.arange(H, device=d.device, dtype=d.dtype),
+                                torch.arange(W, device=d.device, dtype=d.dtype), indexing="ij")
+        pix = torch.stack((xs, ys, torch.ones_like(xs)), -1)
+        rays = pix @ torch.linalg.inv(camera.K.to(d.dtype)).T
+    else:
+        if d.device.type != "cuda":
+            raise ValueError("depth_normals with a lens needs CUDA tensors: the rays come from the native ray kernel")
+        code, consts = _surfel_lens(fisheye, distortion, d.device)
+        ray = native().surfel_rays(code, consts, camera.K.to(d.device, torch.float32).contiguous(), H, W)
+        ray = ray.to(d.dtype)
+        valid = ray[..., 2:] > 0
+        rays = torch.where(valid, ray / torch.where(valid, ray[..., 2:], torch.ones_like(ray[..., 2:])), 0.0)
     pts = rays * d
     out = torch.zeros_like(pts)
     dx = pts[1:-1, 2:] - pts[1:-1, :-2]
     dy = pts[2:, 1:-1] - pts[:-2, 1:-1]
     n = torch.nn.functional.normalize(torch.cross(dx, dy, dim=-1), dim=-1)
     facing = (n * pts[1:-1, 1:-1]).sum(-1, keepdim=True) > 0
-    out[1:-1, 1:-1] = torch.where(facing, -n, n)
+    inner = torch.where(facing, -n, n)
+    if valid is not None:
+        ok = valid[1:-1, 2:] & valid[1:-1, :-2] & valid[2:, 1:-1] & valid[:-2, 1:-1] & valid[1:-1, 1:-1]
+        inner = torch.where(ok, inner, 0.0)
+    out[1:-1, 1:-1] = inner
     return out
