@@ -22,6 +22,7 @@
 #include "../../include/gsr_shutter.h"
 #include "../../include/gsr_surfels.h"
 #include "../../include/gsr_surfels_lens.h"
+#include "../../include/gsr_surfels_features.h"
 
 namespace {
 
@@ -1812,6 +1813,73 @@ torch::Tensor surfel_lens_render_backward(torch::Tensor rays, int64_t N, torch::
                                       g_normal, g_distortion);
 }
 
+// the feature kernels' common checks: features [N, stride] (stride = D rounded up to a multiple of 4, the padding
+// columns 0) next to the surfel records, and the ray map of a lens
+static void check_surfel_features(const torch::Tensor& surfels, const torch::Tensor& features, int64_t D,
+                                  const c10::optional<torch::Tensor>& rays, int64_t H, int64_t W) {
+    CHECK_VALID_INPUT(surfels); CHECK_FLOAT_TENSOR(surfels);
+    CHECK_VALID_INPUT(features); CHECK_FLOAT_TENSOR(features);
+    TORCH_CHECK(features.dim() == 2 && features.size(0) == surfels.size(0), "features must be [N, stride]");
+    TORCH_CHECK(features.device() == surfels.device(), "features must be on the surfels' device");
+    TORCH_CHECK(D >= 1 && features.size(1) >= D, "features must hold D >= 1 columns");
+    if (rays.has_value()) {
+        CHECK_VALID_INPUT((*rays)); CHECK_FLOAT_TENSOR((*rays));
+        TORCH_CHECK(rays->numel() == H * W * 3, "rays must be [H, W, 3]");
+    }
+}
+
+// feature_map [H,W,D]: features blended with the surfel colour forward's weights, up to its `last` contributor
+// (gsr_surfel_render_features_forward); rays: the lens's ray map, or none for the pinhole
+torch::Tensor surfel_features_forward(const c10::optional<torch::Tensor>& rays, torch::Tensor surfels,
+                                      torch::Tensor ranges, int64_t H, int64_t W, int64_t P,
+                                      c10::optional<torch::Tensor> keys_sorted, c10::optional<torch::Tensor> ids_sorted,
+                                      int64_t id_bits, double mh_dist, torch::Tensor last, torch::Tensor features,
+                                      int64_t D) {
+    check_surfel_features(surfels, features, D, rays, H, W);
+    CHECK_VALID_INPUT(last); CHECK_INT_TENSOR(last);
+    TORCH_CHECK(last.numel() == H * W, "last must be [H, W]");
+    c10::cuda::CUDAGuard guard(surfels.device());
+    torch::Tensor fmap = torch::empty({H, W, D}, surfels.options());
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    const bool keys = ps.keys != nullptr;
+    check_rc(gsr_surfel_render_features_forward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0,
+                                                keys ? nullptr : ps.ids, ranges.data_ptr<int>(), (int)H, (int)W,
+                                                (float)mh_dist, opt_f32(rays), last.data_ptr<int>(), F32PTR(features),
+                                                (int)features.size(1), (int)D, F32PTR(fmap), cur_stream()),
+             "gsr_surfel_render_features_forward");
+    return fmap;
+}
+
+// the feature backward (gsr_surfel_render_features_backward): adds the feature loss's part of d alpha into the surfel
+// gradient rows [N, 20] of surfel_render_backward (in place) and returns grad_features [N, stride]
+torch::Tensor surfel_features_backward(const c10::optional<torch::Tensor>& rays, torch::Tensor surfels,
+                                       torch::Tensor ranges, int64_t H, int64_t W, int64_t P,
+                                       c10::optional<torch::Tensor> keys_sorted,
+                                       c10::optional<torch::Tensor> ids_sorted, int64_t id_bits, double mh_dist,
+                                       torch::Tensor last, torch::Tensor totals, torch::Tensor features, int64_t D,
+                                       torch::Tensor grad_map, torch::Tensor rows) {
+    check_surfel_features(surfels, features, D, rays, H, W);
+    CHECK_VALID_INPUT(last); CHECK_INT_TENSOR(last);
+    CHECK_VALID_INPUT(totals); CHECK_FLOAT_TENSOR(totals);
+    CHECK_VALID_INPUT(grad_map); CHECK_FLOAT_TENSOR(grad_map);
+    CHECK_VALID_INPUT(rows); CHECK_FLOAT_TENSOR(rows);
+    TORCH_CHECK(last.numel() == H * W && totals.numel() == H * W * 3, "last and totals must be [H, W] and [H, W, 3]");
+    TORCH_CHECK(grad_map.numel() == H * W * D, "grad_map must be [H, W, D]");
+    TORCH_CHECK(rows.numel() == surfels.size(0) * (int64_t)GSR_SURFEL_GRAD_FLOATS, "rows must hold ",
+                GSR_SURFEL_GRAD_FLOATS, " floats per gaussian");
+    c10::cuda::CUDAGuard guard(surfels.device());
+    torch::Tensor grad_features = torch::zeros_like(features);
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    const bool keys = ps.keys != nullptr;
+    check_rc(gsr_surfel_render_features_backward(
+                 F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0, keys ? nullptr : ps.ids, ranges.data_ptr<int>(),
+                 (int)H, (int)W, (float)mh_dist, opt_f32(rays), last.data_ptr<int>(), F32PTR(totals),
+                 F32PTR(features), (int)features.size(1), (int)D, F32PTR(grad_map), F32PTR(grad_features),
+                 F32PTR(rows), cur_stream()),
+             "gsr_surfel_render_features_backward");
+    return grad_features;
+}
+
 // uv.grad [M,2] of the visible gaussians vis_idx from the gradient rows
 torch::Tensor surfel_uv_grad(torch::Tensor vis_idx, torch::Tensor surfels, torch::Tensor rows) {
     CHECK_VALID_INPUT(vis_idx); CHECK_INT_TENSOR(vis_idx);
@@ -2082,6 +2150,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           "2-D surfels through a lens: uv.grad of the visible gaussians (gsr_surfel_lens_uv_grad)");
     m.def("surfel_lens_backward", &surfel_lens_backward,
           "2-D surfels through a lens: per-gaussian backward (gsr_surfel_lens_preprocess_backward)");
+    m.def("surfel_features_forward", &surfel_features_forward,
+          "2-D surfels: feature map [H,W,D] with the colour's weights (gsr_surfel_render_features_forward)");
+    m.def("surfel_features_backward", &surfel_features_backward,
+          "2-D surfels: feature backward into the gradient rows -> grad_features "
+          "(gsr_surfel_render_features_backward)");
     m.def("version", &version, "library version string");
     m.def("contribution_mask_words",
           [](int64_t P, int64_t H, int64_t W) { return (int64_t)gsr_contribution_mask_words(P, (int)H, (int)W); },

@@ -5,12 +5,13 @@ is rendered as a flat disk whose two tangent axes are scale[:, 0] and scale[:, 1
 exact 0 gradient).  Per pixel the ray meets the surfel at a point (a, b) of its plane, so depth lies on the surface and
 every surfel has a normal.  The model is DESIGN.md 3.25; the kernels are libgsr_surfels.so (include/gsr_surfels.h).
 Through a fisheye or OPENCV lens (DESIGN.md 3.26) each pixel intersects its own undistorted ray, from a ray map, with
-the surfel; those kernels are libgsr_surfels_lens.so (include/gsr_surfels_lens.h).
+the surfel; those kernels are libgsr_surfels_lens.so (include/gsr_surfels_lens.h).  Per-gaussian feature channels
+blended with the colour's weights (DESIGN.md 3.27) are libgsr_surfels_features.so's (include/gsr_surfels_features.h).
 
 Two autograd nodes, as in rasterize():
 
     _ProjectSurfels    params -> uv [M,2], carrier          (gsr_surfel_preprocess_forward, binning, tile forward)
-    _CompositeSurfels  uv, carrier -> image, depth, alpha, normal, distortion
+    _CompositeSurfels  uv, carrier[, features] -> image, depth, alpha, normal, distortion[, feature map]
 
 ``carrier`` only carries the tile backward's per-surfel gradient rows [N,20] to the per-gaussian backward, which writes
 the flat gradient layout of rasterize() (state.grad_flat, or grad_out), so FlatAdam, DensificationStats,
@@ -113,20 +114,39 @@ class _ProjectSurfels(torch.autograd.Function):
 
 
 class _CompositeSurfels(torch.autograd.Function):
-    """uv, carrier -> (image, depth, alpha, normal, distortion); the tile forward already ran in _ProjectSurfels."""
+    """uv, carrier[, features] -> (image, depth, alpha, normal, distortion[, feature map]); the tile forward already
+    ran in _ProjectSurfels, the feature forward (DESIGN.md 3.27) runs here on its pair list, `last` and ray map."""
 
     @staticmethod
-    def forward(ctx, uv, carrier, state):
+    def forward(ctx, uv, carrier, state, features=None):
         ctx.state = state
+        ctx.set_materialize_grads(False)  # an output without a gradient comes as None: no feature backward for it
         maps = state.maps
         state.maps = None
-        ctx.save_for_backward(maps[2])  # alpha: the backward's total weight and final transmittance
-        return tuple(maps)
+        outs = tuple(maps)
+        fpad = None
+        ctx.n_features = 0
+        if features is not None:
+            # the feature kernels read 4 channels per CTA with 16-byte copies: rows padded to a multiple of 4 columns
+            D = features.shape[1]
+            stride = (D + 3) // 4 * 4
+            fpad = features
+            if stride != D:
+                fpad = torch.nn.functional.pad(features, (0, stride - D))
+            elif features.data_ptr() % 16 != 0:
+                fpad = features.clone()
+            fmap = native().surfel_features_forward(state.rays, state.surfels, state.ranges, state.H, state.W, state.P,
+                                                    state.keys_sorted, state.ids_sorted, state.id_bits, state.mh,
+                                                    state.last, fpad, D)
+            ctx.n_features = D
+            outs = outs + (fmap,)
+        ctx.save_for_backward(maps[2], fpad)  # alpha: the backward's total weight and final transmittance
+        return outs
 
     @staticmethod
-    def backward(ctx, g_image, g_depth, g_alpha, g_normal, g_dist):
+    def backward(ctx, g_image, g_depth, g_alpha, g_normal, g_dist, *g_features):
         st = ctx.state
-        (alpha,) = ctx.saved_tensors
+        alpha, fpad = ctx.saved_tensors
 
         def grad(g, k):
             return torch.zeros(st.H, st.W, k, device=alpha.device) if g is None else g.contiguous()
@@ -137,6 +157,15 @@ class _CompositeSurfels(torch.autograd.Function):
         ext = native()
         rows = (ext.surfel_render_backward(*args) if st.lens is None
                 else ext.surfel_lens_render_backward(st.rays, *args))
+        grad_features = None
+        if ctx.n_features and g_features[0] is not None:
+            # into the same rows, before uv.grad and the per-gaussian backward read them: the feature loss's part of
+            # d alpha
+            gpad = ext.surfel_features_backward(st.rays, st.surfels, st.ranges, st.H, st.W, st.P, st.keys_sorted,
+                                                st.ids_sorted, st.id_bits, st.mh, st.last, st.totals, fpad,
+                                                ctx.n_features, g_features[0].contiguous(), rows)
+            if ctx.needs_input_grad[3]:
+                grad_features = gpad if gpad.shape[1] == ctx.n_features else gpad[:, :ctx.n_features]
         # uv.grad (d loss / d footprint translation) is formed only when somebody can observe it, as in rasterize()
         uv_t = st.uv_ref() if st.uv_ref is not None else None
         watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
@@ -145,7 +174,7 @@ class _CompositeSurfels(torch.autograd.Function):
         if watched:
             grad_uv = (ext.surfel_uv_grad(st.vis_idx, st.surfels, rows) if st.lens is None
                        else ext.surfel_lens_uv_grad(*st.lens, st.K, st.vis_idx, st.surfels, rows))
-        return grad_uv, rows.view(-1), None
+        return grad_uv, rows.view(-1), None, grad_features
 
 
 def _surfel_lens(fisheye, distortion, device):
@@ -159,13 +188,13 @@ def _surfel_lens(fisheye, distortion, device):
 
 
 def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
-                      background_rgb, return_state=False, grad_out=None, fisheye=None, distortion=None):
+                      background_rgb, return_state=False, grad_out=None, fisheye=None, distortion=None, features=None):
     """Render the gaussians as 2-D surfels.  Arguments as rasterize() with use_sh_precompute=True; mh_dist is the
     cutoff radius r in the surfel's own units (a pixel takes part where rho <= r^2) and must be > 0.
 
     Returns (image [H,W,3], culling_mask [N] bool, uv [M,2], depth [H,W,1], alpha [H,W,1], normal [H,W,3],
-    distortion [H,W,1]) and the state with return_state.  Per pixel, with the blend weights w_i = T_i alpha_i of the
-    colour: alpha = sum w_i; depth = sum w_i z_i (z_i the camera z of the ray-surfel intersection, or p_z where the
+    distortion [H,W,1]), then the feature map [H,W,D] with features, and the state with return_state.  Per pixel,
+    with the blend weights w_i = T_i alpha_i of the colour: alpha = sum w_i; depth = sum w_i z_i (z_i the camera z of the ray-surfel intersection, or p_z where the
     low-pass filter decides; expected depth is depth / alpha); normal = sum w_i n_i (camera frame, each n_i facing the
     camera, not normalised); distortion = sum_i w_i sum_{j<i} w_j (m_i - m_j)^2 with m = (f / (f - n)) (1 - n / z),
     n, f = near_thresh, far_thresh (2DGS's depth-distortion term).  Every output is differentiable; gradients reach
@@ -182,6 +211,13 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
     J_n^-T g_n + g_c, the gradient on a translation of the footprint in the normalised plane mapped to pixels through
     the lens Jacobian at the centre; its sum is d loss / d(cx, cy) for the pinhole only.
 
+    features: an fp32 CUDA tensor [N, D] (D >= 1, contiguous, on the gaussians' device; it may require grad) of
+    per-gaussian channels (semantics, instance ids, distilled features, any attribute).  The feature map [H,W,D],
+    feature_map[p, c] = sum_i w_i F[i, c] with exactly the colour's surfels, order and fp32 weights w_i and no
+    background term, is then returned after the distortion (DESIGN.md 3.27).  Its gradient reaches F (returned through
+    autograd, not part of the flat layout) and, through the blend weights, the geometry: the feature loss lands in the
+    same gradient rows as the maps', so uv.grad, state.grad_flat / grad_out and everything that reads them see it.
+
     fp32 CUDA tensors only (TypeError otherwise); a camera_T_world, K or lens-coefficient tensor that requires grad
     raises ValueError: no camera gradient is formed for surfels."""
     g = gaussians
@@ -197,6 +233,17 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
                          "camera.K.detach()")
     if any(torch.is_tensor(k) and k.requires_grad for k in (fisheye, distortion)):
         raise ValueError("rasterize_surfels forms no camera gradient: pass lens coefficients that do not require grad")
+    if features is not None:
+        if not torch.is_tensor(features):
+            raise TypeError("features must be a torch tensor [N, D]")
+        if features.dtype != torch.float32:
+            raise TypeError(f"features must be float32, got {features.dtype}")
+        n = g.xyz.shape[0]
+        if features.dim() != 2 or features.shape[0] != n or features.shape[1] < 1:
+            raise ValueError(f"features has shape {tuple(features.shape)} but must be [{n}, D] with D >= 1 (one row "
+                             "per gaussian)")
+        if features.device != g.xyz.device or not features.is_contiguous():
+            raise ValueError("features must be contiguous and on the gaussians' device")
     lens = _lens_arg(fisheye, distortion)
     if any(t.device.type != "cuda" or t.device != g.xyz.device for t in tensors):
         raise ValueError("rasterize_surfels needs every tensor on the gaussians' CUDA device")
@@ -216,8 +263,9 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
         None if g.sh is None else g.sh.contiguous(), camera_T_world.contiguous(), camera.K.contiguous(), state, cfg)
     state.uv_ref = weakref.ref(uv)
     culling_mask = state.visible == 0
-    image, depth, alpha, normal, distortion = _CompositeSurfels.apply(uv, carrier, state)
-    result = (image, culling_mask, uv, depth, alpha, normal, distortion)
+    maps = _CompositeSurfels.apply(uv, carrier, state, features)
+    image, depth, alpha, normal, distortion = maps[:5]
+    result = (image, culling_mask, uv, depth, alpha, normal, distortion) + tuple(maps[5:])
     return (*result, state) if return_state else result
 
 
