@@ -20,9 +20,10 @@
                             (include/gsr_surfels_lens.h)
   libgsr_surfels_features.so  per-gaussian feature channels blended with the surfel colour's weights, every lens
                             (include/gsr_surfels_features.h)
+  libgsr_surfels_median.so  the median depth of the surfel blend, every lens (include/gsr_surfels_median.h)
   _ext/splat_cuda.*.so      torch binding exporting the reference's `splat_cuda` surface
 
-`python -m gaussian_splatting_b200.build` builds all fourteen (the CUDA libraries from the LIBS table);
+`python -m gaussian_splatting_b200.build` builds all fifteen (the CUDA libraries from the LIBS table);
 `build(force=False)` is incremental.
 """
 from __future__ import annotations
@@ -111,6 +112,8 @@ LIBS = [
      "surfels_lens_lib.sha256"),
     (PKG / "libgsr_surfels_features.so", ["gsr_surfels_features.cu"],
      SURFEL_HEADERS + [ROOT / "include" / "gsr_surfels_features.h"], "surfels_features_lib.sha256"),
+    (PKG / "libgsr_surfels_median.so", ["gsr_surfels_median.cu"],
+     SURFEL_HEADERS + [ROOT / "include" / "gsr_surfels_median.h"], "surfels_median_lib.sha256"),
 ]
 
 NVCC_FLAGS = [
@@ -190,7 +193,8 @@ def build_ext(force: bool = False) -> Path:
                     ROOT / "include" / "gsr_pose.h", ROOT / "include" / "gsr_bilagrid.h",
                     ROOT / "include" / "gsr_calib.h", ROOT / "include" / "gsr_shutter.h",
                     ROOT / "include" / "gsr_surfels.h", ROOT / "include" / "gsr_surfels_lens.h",
-                    ROOT / "include" / "gsr_surfels_features.h"], torch.__version__)
+                    ROOT / "include" / "gsr_surfels_features.h", ROOT / "include" / "gsr_surfels_median.h"],
+                   torch.__version__)
     if not force and out.exists() and stamp.exists() and stamp.read_text() == want:
         return out
     incs = [f"-I{p}" for p in ce.include_paths("cuda")] + [f"-I{sysconfig.get_paths()['include']}"]
@@ -203,7 +207,7 @@ def build_ext(force: bool = False) -> Path:
         *incs, str(src), "-o", str(out),
         f"-L{PKG}", "-lgsr_b200", "-lgsr_selective_adam", "-lgsr_features", "-lgsr_batch", "-lgsr_fisheye",
         "-lgsr_distortion", "-lgsr_pose", "-lgsr_bilagrid", "-lgsr_calib", "-lgsr_shutter", "-lgsr_surfels",
-        "-lgsr_surfels_lens", "-lgsr_surfels_features",
+        "-lgsr_surfels_lens", "-lgsr_surfels_features", "-lgsr_surfels_median",
         f"-L{torch_lib}", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10",
         "-lc10_cuda", "-ltorch_python", f"-L{cuda_lib}", "-lcudart",
         "-Wl,-rpath,$ORIGIN/..", f"-Wl,-rpath,{torch_lib}", f"-Wl,-rpath,{cuda_lib}",

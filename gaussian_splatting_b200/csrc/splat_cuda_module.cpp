@@ -23,6 +23,7 @@
 #include "../../include/gsr_surfels.h"
 #include "../../include/gsr_surfels_lens.h"
 #include "../../include/gsr_surfels_features.h"
+#include "../../include/gsr_surfels_median.h"
 
 namespace {
 
@@ -1880,6 +1881,56 @@ torch::Tensor surfel_features_backward(const c10::optional<torch::Tensor>& rays,
     return grad_features;
 }
 
+// (median [H,W,1], median_id [H,W] int32): each pixel's median contributor of the surfel colour forward, up to its
+// `last` (gsr_surfel_render_median_forward); rays: the lens's ray map, or none for the pinhole
+std::vector<torch::Tensor> surfel_median_forward(const c10::optional<torch::Tensor>& rays, torch::Tensor surfels,
+                                                 torch::Tensor ranges, int64_t H, int64_t W, int64_t P,
+                                                 c10::optional<torch::Tensor> keys_sorted,
+                                                 c10::optional<torch::Tensor> ids_sorted, int64_t id_bits,
+                                                 double mh_dist, torch::Tensor last) {
+    CHECK_VALID_INPUT(surfels); CHECK_FLOAT_TENSOR(surfels);
+    CHECK_VALID_INPUT(ranges); CHECK_INT_TENSOR(ranges);
+    CHECK_VALID_INPUT(last); CHECK_INT_TENSOR(last);
+    TORCH_CHECK(last.numel() == H * W, "last must be [H, W]");
+    if (rays.has_value()) {
+        CHECK_VALID_INPUT((*rays)); CHECK_FLOAT_TENSOR((*rays));
+        TORCH_CHECK(rays->numel() == H * W * 3, "rays must be [H, W, 3]");
+    }
+    c10::cuda::CUDAGuard guard(surfels.device());
+    torch::Tensor median = torch::empty({H, W, 1}, surfels.options());
+    torch::Tensor median_id = torch::empty({H, W}, last.options());
+    const PairSource ps = pair_source(keys_sorted, ids_sorted, P);
+    const bool keys = ps.keys != nullptr;
+    check_rc(gsr_surfel_render_median_forward(F32PTR(surfels), ps.keys, keys ? (int)id_bits : 0,
+                                              keys ? nullptr : ps.ids, ranges.data_ptr<int>(), (int)H, (int)W,
+                                              (float)mh_dist, opt_f32(rays), last.data_ptr<int>(), F32PTR(median),
+                                              median_id.data_ptr<int>(), cur_stream()),
+             "gsr_surfel_render_median_forward");
+    return {median, median_id};
+}
+
+// the median backward (gsr_surfel_render_median_backward): adds d loss / d median through each pixel's median surfel's
+// z into the surfel gradient rows [N, 20] of surfel_render_backward, in place
+void surfel_median_backward(const c10::optional<torch::Tensor>& rays, torch::Tensor surfels, int64_t H, int64_t W,
+                            double mh_dist, torch::Tensor median_id, torch::Tensor grad_median, torch::Tensor rows) {
+    CHECK_VALID_INPUT(surfels); CHECK_FLOAT_TENSOR(surfels);
+    CHECK_VALID_INPUT(median_id); CHECK_INT_TENSOR(median_id);
+    CHECK_VALID_INPUT(grad_median); CHECK_FLOAT_TENSOR(grad_median);
+    CHECK_VALID_INPUT(rows); CHECK_FLOAT_TENSOR(rows);
+    TORCH_CHECK(median_id.numel() == H * W && grad_median.numel() == H * W, "median_id and grad_median must be [H, W]");
+    TORCH_CHECK(rows.numel() == surfels.size(0) * (int64_t)GSR_SURFEL_GRAD_FLOATS, "rows must hold ",
+                GSR_SURFEL_GRAD_FLOATS, " floats per gaussian");
+    if (rays.has_value()) {
+        CHECK_VALID_INPUT((*rays)); CHECK_FLOAT_TENSOR((*rays));
+        TORCH_CHECK(rays->numel() == H * W * 3, "rays must be [H, W, 3]");
+    }
+    c10::cuda::CUDAGuard guard(surfels.device());
+    check_rc(gsr_surfel_render_median_backward(F32PTR(surfels), (int)H, (int)W, (float)mh_dist, opt_f32(rays),
+                                               median_id.data_ptr<int>(), F32PTR(grad_median), F32PTR(rows),
+                                               cur_stream()),
+             "gsr_surfel_render_median_backward");
+}
+
 // uv.grad [M,2] of the visible gaussians vis_idx from the gradient rows
 torch::Tensor surfel_uv_grad(torch::Tensor vis_idx, torch::Tensor surfels, torch::Tensor rows) {
     CHECK_VALID_INPUT(vis_idx); CHECK_INT_TENSOR(vis_idx);
@@ -2155,6 +2206,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("surfel_features_backward", &surfel_features_backward,
           "2-D surfels: feature backward into the gradient rows -> grad_features "
           "(gsr_surfel_render_features_backward)");
+    m.def("surfel_median_forward", &surfel_median_forward,
+          "2-D surfels: median depth [H,W,1] and median surfel [H,W] (gsr_surfel_render_median_forward)");
+    m.def("surfel_median_backward", &surfel_median_backward,
+          "2-D surfels: median backward into the gradient rows (gsr_surfel_render_median_backward)");
     m.def("version", &version, "library version string");
     m.def("contribution_mask_words",
           [](int64_t P, int64_t H, int64_t W) { return (int64_t)gsr_contribution_mask_words(P, (int)H, (int)W); },

@@ -6,12 +6,13 @@ exact 0 gradient).  Per pixel the ray meets the surfel at a point (a, b) of its 
 every surfel has a normal.  The model is DESIGN.md 3.25; the kernels are libgsr_surfels.so (include/gsr_surfels.h).
 Through a fisheye or OPENCV lens (DESIGN.md 3.26) each pixel intersects its own undistorted ray, from a ray map, with
 the surfel; those kernels are libgsr_surfels_lens.so (include/gsr_surfels_lens.h).  Per-gaussian feature channels
-blended with the colour's weights (DESIGN.md 3.27) are libgsr_surfels_features.so's (include/gsr_surfels_features.h).
+blended with the colour's weights (DESIGN.md 3.27) are libgsr_surfels_features.so's (include/gsr_surfels_features.h),
+the median depth (DESIGN.md 3.28) libgsr_surfels_median.so's (include/gsr_surfels_median.h).
 
 Two autograd nodes, as in rasterize():
 
     _ProjectSurfels    params -> uv [M,2], carrier          (gsr_surfel_preprocess_forward, binning, tile forward)
-    _CompositeSurfels  uv, carrier[, features] -> image, depth, alpha, normal, distortion[, feature map]
+    _CompositeSurfels  uv, carrier[, features] -> image, depth, alpha, normal, distortion[, median][, feature map]
 
 ``carrier`` only carries the tile backward's per-surfel gradient rows [N,20] to the per-gaussian backward, which writes
 the flat gradient layout of rasterize() (state.grad_flat, or grad_out), so FlatAdam, DensificationStats,
@@ -34,14 +35,14 @@ class _SurfelState:
     """Per-view buffers shared by the two autograd nodes (return_state=True hands it out).  vis_idx / vis_idx32: the
     visible gaussians, ascending (the order of uv); grad_flat: the flat gradient of the last backward; lens: None (the
     pinhole) or (the native SURFEL_LENS_* value, its device constants); rays: the lens's ray map [H,W,3] (0 where a
-    pixel has no ray)."""
+    pixel has no ray); median_ids: each pixel's median surfel [H,W] int32 (-1: none), with median_depth."""
 
     __slots__ = ("N", "M", "P", "H", "W", "visible", "vis_idx", "vis_idx32", "scan", "surfels", "ranges", "keys_sorted",
                  "ids_sorted", "id_bits", "maps", "last", "totals", "background", "near", "m_scale", "mh", "grad_flat",
-                 "grad_out", "uv_ref", "uv_grad_emitted", "uv_absgrad", "lens", "rays", "K")
+                 "grad_out", "uv_ref", "uv_grad_emitted", "uv_absgrad", "lens", "rays", "K", "median_ids")
 
     def __init__(self):
-        self.grad_flat = self.grad_out = self.uv_ref = self.uv_absgrad = self.lens = self.rays = None
+        self.grad_flat = self.grad_out = self.uv_ref = self.uv_absgrad = self.lens = self.rays = self.median_ids = None
         self.uv_grad_emitted = False
 
 
@@ -114,16 +115,23 @@ class _ProjectSurfels(torch.autograd.Function):
 
 
 class _CompositeSurfels(torch.autograd.Function):
-    """uv, carrier[, features] -> (image, depth, alpha, normal, distortion[, feature map]); the tile forward already
-    ran in _ProjectSurfels, the feature forward (DESIGN.md 3.27) runs here on its pair list, `last` and ray map."""
+    """uv, carrier[, features] -> (image, depth, alpha, normal, distortion[, median][, feature map]); the tile forward
+    already ran in _ProjectSurfels, the median (DESIGN.md 3.28) and feature (DESIGN.md 3.27) forwards run here on its
+    pair list, `last` and ray map."""
 
     @staticmethod
-    def forward(ctx, uv, carrier, state, features=None):
+    def forward(ctx, uv, carrier, state, features=None, median_depth=False):
         ctx.state = state
-        ctx.set_materialize_grads(False)  # an output without a gradient comes as None: no feature backward for it
+        ctx.set_materialize_grads(False)  # an output without a gradient comes as None: no feature / median backward
         maps = state.maps
         state.maps = None
         outs = tuple(maps)
+        ctx.median_depth = median_depth
+        if median_depth:
+            median, state.median_ids = native().surfel_median_forward(
+                state.rays, state.surfels, state.ranges, state.H, state.W, state.P, state.keys_sorted,
+                state.ids_sorted, state.id_bits, state.mh, state.last)
+            outs = outs + (median,)
         fpad = None
         ctx.n_features = 0
         if features is not None:
@@ -144,8 +152,10 @@ class _CompositeSurfels(torch.autograd.Function):
         return outs
 
     @staticmethod
-    def backward(ctx, g_image, g_depth, g_alpha, g_normal, g_dist, *g_features):
+    def backward(ctx, g_image, g_depth, g_alpha, g_normal, g_dist, *g_rest):
         st = ctx.state
+        g_median = g_rest[0] if ctx.median_depth else None
+        g_features = g_rest[1:] if ctx.median_depth else g_rest
         alpha, fpad = ctx.saved_tensors
 
         def grad(g, k):
@@ -166,6 +176,11 @@ class _CompositeSurfels(torch.autograd.Function):
                                                 ctx.n_features, g_features[0].contiguous(), rows)
             if ctx.needs_input_grad[3]:
                 grad_features = gpad if gpad.shape[1] == ctx.n_features else gpad[:, :ctx.n_features]
+        if g_median is not None:
+            # into the same rows, after the colour and feature backwards and before uv.grad and the per-gaussian backward
+            # read them: the median loss through each pixel's median surfel's z
+            ext.surfel_median_backward(st.rays, st.surfels, st.H, st.W, st.mh, st.median_ids, g_median.contiguous(),
+                                       rows)
         # uv.grad (d loss / d footprint translation) is formed only when somebody can observe it, as in rasterize()
         uv_t = st.uv_ref() if st.uv_ref is not None else None
         watched = uv_t is None or uv_t.retains_grad or bool(uv_t._backward_hooks)
@@ -174,7 +189,7 @@ class _CompositeSurfels(torch.autograd.Function):
         if watched:
             grad_uv = (ext.surfel_uv_grad(st.vis_idx, st.surfels, rows) if st.lens is None
                        else ext.surfel_lens_uv_grad(*st.lens, st.K, st.vis_idx, st.surfels, rows))
-        return grad_uv, rows.view(-1), None, grad_features
+        return grad_uv, rows.view(-1), None, grad_features, None
 
 
 def _surfel_lens(fisheye, distortion, device):
@@ -188,12 +203,14 @@ def _surfel_lens(fisheye, distortion, device):
 
 
 def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh, cull_mask_padding, mh_dist,
-                      background_rgb, return_state=False, grad_out=None, fisheye=None, distortion=None, features=None):
+                      background_rgb, return_state=False, grad_out=None, fisheye=None, distortion=None, features=None,
+                      median_depth=False):
     """Render the gaussians as 2-D surfels.  Arguments as rasterize() with use_sh_precompute=True; mh_dist is the
     cutoff radius r in the surfel's own units (a pixel takes part where rho <= r^2) and must be > 0.
 
     Returns (image [H,W,3], culling_mask [N] bool, uv [M,2], depth [H,W,1], alpha [H,W,1], normal [H,W,3],
-    distortion [H,W,1]), then the feature map [H,W,D] with features, and the state with return_state.  Per pixel,
+    distortion [H,W,1]), then the median [H,W,1] with median_depth, the feature map [H,W,D] with features, and the
+    state with return_state.  Per pixel,
     with the blend weights w_i = T_i alpha_i of the colour: alpha = sum w_i; depth = sum w_i z_i (z_i the camera z of the ray-surfel intersection, or p_z where the
     low-pass filter decides; expected depth is depth / alpha); normal = sum w_i n_i (camera frame, each n_i facing the
     camera, not normalised); distortion = sum_i w_i sum_{j<i} w_j (m_i - m_j)^2 with m = (f / (f - n)) (1 - n / z),
@@ -217,6 +234,13 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
     background term, is then returned after the distortion (DESIGN.md 3.27).  Its gradient reaches F (returned through
     autograd, not part of the flat layout) and, through the blend weights, the geometry: the feature loss lands in the
     same gradient rows as the maps', so uv.grad, state.grad_flat / grad_out and everything that reads them see it.
+
+    median_depth=True also returns the median depth [H,W,1] after the distortion, before the feature map (2DGS's
+    median; DESIGN.md 3.28): per pixel the camera z (as depth blends it) of the last of the colour's surfels whose
+    transmittance in front of it, 1 - A in fp32, is above 0.5; 0 where no surfel contributes.  state.median_ids holds
+    those surfels' indices [H,W] (-1: none).  Its gradient goes to that surfel's z only (its position, orientation and
+    the surfel plane; not its opacity, colour or the choice of surfel), into the same gradient rows as the maps'.
+    2DGS's bounded-scene depth is (1 - r) depth / alpha + r median (INTEGRATION.md B23).
 
     fp32 CUDA tensors only (TypeError otherwise); a camera_T_world, K or lens-coefficient tensor that requires grad
     raises ValueError: no camera gradient is formed for surfels."""
@@ -263,7 +287,7 @@ def rasterize_surfels(gaussians, camera_T_world, camera, near_thresh, far_thresh
         None if g.sh is None else g.sh.contiguous(), camera_T_world.contiguous(), camera.K.contiguous(), state, cfg)
     state.uv_ref = weakref.ref(uv)
     culling_mask = state.visible == 0
-    maps = _CompositeSurfels.apply(uv, carrier, state, features)
+    maps = _CompositeSurfels.apply(uv, carrier, state, features, bool(median_depth))
     image, depth, alpha, normal, distortion = maps[:5]
     result = (image, culling_mask, uv, depth, alpha, normal, distortion) + tuple(maps[5:])
     return (*result, state) if return_state else result
