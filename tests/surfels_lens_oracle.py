@@ -1,7 +1,7 @@
 """fp64 oracle of rasterize_surfels(..., fisheye=k / distortion=k) (tests/surfels_lens_oracle.c): every pixel's ray
 against every visible surfel in depth order, no tiles, with the analytic backward.  TEST INFRASTRUCTURE.
 
-    o = render(scene, bg, lens, kc)              # as tests/surfels_oracle.render, plus o.rays [H,W,3]
+    o = render(scene, bg, lens, kc)              # as tests/surfels_oracle.render (o.near, o.ill), plus o.rays [H,W,3]
     o = render(scene, bg, lens, kc, grads=G)     # + o.g, o.rows (dL/dM'), o.uv_grad, o.mass
 
 lens: "fisheye" (kc = k1 k2 k3 k4) or "distortion" (kc = k1 k2 p1 p2 k3); the cull limit is appended here as the
@@ -86,6 +86,8 @@ def render(scene, bg, lens, kc, grads=None, near=0.3, far=500.0, pad=100.0, mh=3
     kcd = _f64(lens_constants(lens, kc, limit))
     keep = [_f64(scene["xyz"]), _f64(scene["quaternion"]), _f64(scene["scale"]), _f64(np.reshape(scene["opacity"], -1)),
             _f64(scene["T"]), _f64(scene["K"]), _f64(bg)]
+    o.ill = np.zeros((H, W), np.uint8)
+    lib().surfel_lens_oracle_ill(_p(o.ill))
     o.M = lib().surfel_lens_oracle(
         C.c_int(LENS_ID[lens]), _p(kcd), C.c_int(N), *[_p(a) for a in keep[:4]], _p(colour), _p(keep[4]),
         _p(keep[5]), C.c_int(H), C.c_int(W), C.c_double(near), C.c_double(far), C.c_double(pad), C.c_double(mh),
@@ -93,6 +95,7 @@ def render(scene, bg, lens, kc, grads=None, near=0.3, far=500.0, pad=100.0, mh=3
         _p(o.alpha), _p(o.normal), _p(o.dist), _p(o.visible), _p(o.uv), og("xyz"), og("quaternion"), og("scale"),
         og("opacity"), og("colour"), None if G is None else _p(o.rows), None if G is None else _p(o.uv_grad),
         None if G is None else _p(o.mass), _p(o.near), _p(zs), _p(o.rays))
+    lib().surfel_lens_oracle_ill(None)
     if G is not None:
         gc = o.g.pop("colour")
         gcoef = gc[:, :, None] * Y[:, None, :]

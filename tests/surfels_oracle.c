@@ -106,6 +106,21 @@ static int intersect(const Surfel* s, double x, double y, double r2, Hit* h, int
     return 1;
 }
 
+/* ill (NULL unless surfel_oracle_ill set it; [H,W], zeroed by the caller): the pixels where a contributing surfel's
+ * ray-plane intersection is ill-conditioned, |c2| < |hx| |hy| / ILL_KAPPA with a = c0 / c2, b = c1 / c2.  The gradient
+ * of (a, b) carries 1 / c2^2: an input rounded to fp32 (eps = 6e-8) moves that pixel's gradient terms by about
+ * eps kappa^2 of themselves, 2.4e-4 at kappa = 64.  Such pixels are nearly edge-on surfels whose intersection branch
+ * is taken. */
+#define ILL_KAPPA 64.0
+static unsigned char* g_ill;
+void surfel_oracle_ill(unsigned char* ill) { g_ill = ill; }
+
+static int ill_conditioned(const Hit* h) {
+    const double nx = sqrt(h->hx[0] * h->hx[0] + h->hx[1] * h->hx[1] + h->hx[2] * h->hx[2]);
+    const double ny = sqrt(h->hy[0] * h->hy[0] + h->hy[1] * h->hy[1] + h->hy[2] * h->hy[2]);
+    return h->use3 && fabs(h->c2) * ILL_KAPPA < nx * ny;
+}
+
 static const double* g_sort_z;
 static int by_depth(const void* pa, const void* pb) {
     const int a = *(const int*)pa, b = *(const int*)pb;
@@ -155,6 +170,7 @@ int surfel_oracle(int N, const double* xyz, const double* quat, const double* sc
                 if (A > 0.9999) break;
                 const Surfel* s = &S[order[k]];
                 if (!intersect(s, x, y, r2, &h, &nr)) continue;
+                if (g_ill != NULL && ill_conditioned(&h)) g_ill[pix] = 1;
                 const double w = h.alpha * (1 - A);
                 for (int c = 0; c < 3; ++c) {
                     img[c] += w * colour[3 * order[k] + c];

@@ -5,6 +5,7 @@ no tiles, with the analytic backward.  TEST INFRASTRUCTURE.
     o = render(scene, bg, grads=G)               # + o.g (xyz, quaternion, scale, opacity, rgb, sh), o.rows, o.uv_grad,
                                                  #   o.mass (per-pixel magnitudes summed into each row entry)
 o.near [H,W]: pixels with a branch of the blend within 1e-4 of its threshold (surfels_oracle.c).
+o.ill [H,W]: pixels where a contributing surfel's ray-plane intersection is ill-conditioned (nearly edge-on; surfels_oracle.c).
 
 scene: dict of numpy arrays as tests/scenes.np_scene makes (xyz, quaternion, scale, opacity, rgb, sh, T, K, H, W).
 The SH colour is formed here at the centre's view direction; view_dirs [N,3] replaces that direction (held constant,
@@ -113,6 +114,8 @@ def render(scene, bg, grads=None, near=0.3, far=500.0, pad=100.0, mh=3.0, dirs=N
     zs = None if sort_z is None else _f64(sort_z)
     keep = [_f64(scene["xyz"]), _f64(scene["quaternion"]), _f64(scene["scale"]), _f64(np.reshape(scene["opacity"], -1)),
             _f64(scene["T"]), _f64(scene["K"]), _f64(bg)]
+    o.ill = np.zeros((H, W), np.uint8)
+    lib().surfel_oracle_ill(_p(o.ill))
     o.M = lib().surfel_oracle(
         C.c_int(N), *[_p(a) for a in keep[:4]], _p(colour), _p(keep[4]), _p(keep[5]), C.c_int(H), C.c_int(W),
         C.c_double(near), C.c_double(far), C.c_double(pad), C.c_double(mh), _p(keep[6]), gp("image"), gp("depth"),
@@ -120,6 +123,7 @@ def render(scene, bg, grads=None, near=0.3, far=500.0, pad=100.0, mh=3.0, dirs=N
         _p(o.visible), _p(o.uv), og("xyz"), og("quaternion"), og("scale"), og("opacity"), og("colour"),
         None if G is None else _p(o.rows), None if G is None else _p(o.uv_grad), None if G is None else _p(o.mass),
         _p(o.near), _p(zs))
+    lib().surfel_oracle_ill(None)
     if G is not None:
         gc = o.g.pop("colour")
         gcoef = gc[:, :, None] * Y[:, None, :]   # colour = sum_k Y_k coef_k
